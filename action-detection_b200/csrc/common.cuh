@@ -1,4 +1,4 @@
-// Shared declarations for libssn_b200 (sm_100a only).
+// Shared declarations for libssn_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>

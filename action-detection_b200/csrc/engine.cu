@@ -85,15 +85,15 @@ struct Op {
   size_t argmax_off = 0;
   int grad_accumulate = 0;  // backward: dIn += (another consumer wrote first)
   int wsplits = 1, wrows = 0;
-  int tsplits = 1;                // upper bound of the split count the tcgen05 weight-gradient planner may pick (sizes `partial`)
+  int tsplits = 1;                // upper bound of the split count the tensor-core weight-gradient planner may pick (sizes `partial`)
   size_t partial_off = 0, bias_partial_off = 0;   // this layer's split-K partials (own region: finalised in one batch)
-  UmmaConvPlan umma;        // tcgen05 forward plan (FAST mode, stride-1 layers)
-  UmmaConvPlan umma_dgrad;  // tcgen05 data-gradient plan
-  UmmaWgradPlan umma_wgrad; // tcgen05 weight-gradient plan
+  UmmaConvPlan umma;        // tensor-core forward plan (FAST mode, stride-1 layers)
+  UmmaConvPlan umma_dgrad;  // tensor-core data-gradient plan
+  UmmaWgradPlan umma_wgrad; // tensor-core weight-gradient plan
   int pool_consumer = -1;   // conv whose only consumer is a k3/s2 max pool: that pool's op index (backward gather is folded in)
   bool folded_into_conv = false;   // max pool whose backward runs inside its producer conv's mask+bias pass
   bool dgrad_masks = false; // this op's data gradient is the LAST writer of d(in_val): it applies the ReLU mask of in_val
-  bool bias_in_wgrad = false;// conv: bias gradient comes out of the tcgen05 weight-gradient kernel (ones operand)
+  bool bias_in_wgrad = false;// conv: bias gradient comes out of the tensor-core weight-gradient kernel (ones operand)
   bool dy_premasked = false;// conv: d(out) arrives already masked, the backward pass only needs the bias column sums
   bool raw = false;         // conv whose BatchNorm runs unfused in training mode: no fold, no ReLU in the epilogue, no ReLU mask in backward
   int fuse_role = 0;        // sibling 1x1 fusion: 1 = leader (launches the fused kernels), 2 = follower
@@ -118,7 +118,7 @@ struct ssnb_engine {
   ssnb_config cfg;
   int F = 0;
   bool fp16 = false;
-  bool tc = false;                  // SSNB_EXACT_TC: fp32 storage + glue, convolutions as split-operand (hi/lo fp16) tcgen05 MMAs
+  bool tc = false;                  // SSNB_EXACT_TC: fp32 storage + glue, convolutions as split-operand (hi/lo fp16) tensor-core MMAs
   size_t esz = 4;
   size_t up_plane = 0, s2d_plane = 0, s2d_w_plane = 0;
   int* tc_flag = nullptr;           // device int: set when a split pass saw |x * grad_scale| beyond the fp16 range
@@ -179,6 +179,16 @@ static bool profiled_op(const char* env, const std::string& id) {
   const std::string list = std::string(",") + e + ",";
   return list.find("," + id + ",") != std::string::npos;
 }
+// SM count of the current device (the H100 SXM's 132 where none is visible: planning without a GPU)
+static int device_sms() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) {
+    cudaGetLastError();
+    return 132;
+  }
+  return sms;
+}
+
 static int pool_out(int h, int k, int s, int p) {   // ceil_mode (layer_factory.py:46-50)
   int o = (h + 2 * p - k + s - 1) / s + 1;
   if ((o - 1) * s >= h + p) --o;
@@ -319,13 +329,13 @@ static void plan(ssnb_engine* e) {
         rows = (rows + 15) / 16 * 16;
         splits = (M + rows - 1) / rows;
         o.wsplits = (int)splits; o.wrows = (int)rows;
-        // tcgen05 path: one CTA per SM is resident, so the planner wants num_sms / (M tiles x N tiles x tap groups) pixel
-        // splits; the SIMT heuristic above used to cap it and left 57-75 % of the SMs busy on most 3x3 layers
+        // tensor-core path: one CTA per SM is resident, so the planner wants num_sms / (M tiles x N tiles x tap groups) pixel
+        // splits; the SIMT heuristic above used to cap it and left most SMs idle on most 3x3 layers
         {
           const int chunks = (c.cin + 63) / 64, n_tiles = (chunks + 3) / 4, block_n = ((chunks + n_tiles - 1) / n_tiles) * 64;
           const int tpc = std::max(1, 4 / (block_n / 64));
           const int ctas = ((c.cout + 127) / 128) * n_tiles * ((taps + tpc - 1) / tpc);
-          o.tsplits = std::max(o.wsplits, std::min(128, std::max(1, 148 / ctas)));
+          o.tsplits = std::max(o.wsplits, std::min(128, std::max(1, device_sms() / ctas)));
         }
         if (e->fp16 || e->tc) splits = std::max<long long>(splits, o.tsplits);
         const size_t need = (size_t)splits * taps * c.cout * c.cin * 4;
@@ -451,7 +461,7 @@ static int tc_split_value(ssnb_engine* e, int val, bool grad, float scale, cudaS
 static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s);
 static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s) {
   if (e->tc && o.kind == OP_CONV && o.umma.enabled) {
-    // split-operand tcgen05 convolution: reads the input's hi/lo planes, writes fp32 + the output's planes
+    // split-operand tensor-core convolution: reads the input's hi/lo planes, writes fp32 + the output's planes
     if (o.conv == 0 && !e->s2d_ready)
       if (int rc = launch_nhwc_to_s2d_split(e->view(o.in_val, false), e->F, (__half*)(e->ws + e->s2d_off), (long long)e->s2d_plane, e->Cs, s)) return rc;
     tag_next(0, conv_flops(e, o));
@@ -684,7 +694,7 @@ int engine_tail_view(ssnb_handle h, View* v, int* F, int* fp16) {
 // ---- C ABI -----------------------------------------------------------------------------------------
 extern "C" {
 
-const char* ssnb_version(void) { return "libssn_b200 0.2 (sm_100a)"; }
+const char* ssnb_version(void) { return "libssn_b200 0.3 (sm_90a)"; }
 
 const char* ssnb_last_error(ssnb_handle h) { return h ? h->error.c_str() : ssnb::thread_error().c_str(); }
 
@@ -765,7 +775,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
         rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, h->planes(o.out_val, false), h->F, Ck, c.cout, 4, dy, dx,
                                  (const __half*)(h->ws + h->s2d_w_off), (const float*)(h->ws + pk.bias), o.raw ? 0 : 1, &t);
         if (rc) return h->fail(rc, "tc conv1 bind: " + ssnb::thread_error());
-        if (!o.umma.p.v2) o.umma.enabled = false;
+        if (!o.umma.p.tc_ok) o.umma.enabled = false;
         if (use_wgrad_tc) {
           rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->planes(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
                                     (float*)(h->ws + o.partial_off), 128);
@@ -787,7 +797,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, dxp, h->F, c.cin, c.cout, c.k, c.pad, (const __half*)(h->ws + pk.wf16),
                                 o.grad_accumulate, &tg);
       if (rc) return h->fail(rc, "tc bind_dgrad(" + c.id + "): " + ssnb::thread_error());
-      if (!o.umma_dgrad.p.v2) o.umma_dgrad.enabled = false;
+      if (!o.umma_dgrad.p.tc_ok) o.umma_dgrad.enabled = false;
       if (use_wgrad_tc) {
         rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->planes(o.out_val, true), h->planes(o.in_val, false), h->F, c.cin, c.cout, c.k, c.pad,
                              (float*)(h->ws + o.partial_off), o.tsplits, c.stride);
@@ -821,7 +831,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
                                   (const float*)(h->ws + fb.bias), &t);
         }
         if (rc) return h->fail(rc, "tc fused fwd bind(" + o3.id + "): " + ssnb::thread_error());
-        if (!fb.fwd.p.v2) continue;
+        if (!fb.fwd.p.tc_ok) continue;
         if (h->cfg.training) {
           View dredp = h->planes(o3.out_val, true); dredp.C = fb.c3r + fb.cdr;
           View d1p = fb.op1 >= 0 ? h->planes(h->ops[fb.op1].out_val, true) : dredp;
@@ -830,7 +840,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
           rc = umma_conv_bind_fused_dgrad(h->umma_ctx, fb.dgrad, d1p, dredp, dxp, h->F, fb.cx, fb.c1, fb.c3r + fb.cdr, (const __half*)(h->ws + fb.w_dg),
                                           od.grad_accumulate, &tg);
           if (rc) return h->fail(rc, "tc fused dgrad bind(" + o3.id + "): " + ssnb::thread_error());
-          if (!fb.dgrad.p.v2) continue;
+          if (!fb.dgrad.p.tc_ok) continue;
           // zero the K padding of the concatenated data-gradient weights once (both planes); split_all_kernel never writes it
           if (cudaMemset(h->ws + fb.w_dg, 0, 2 * fb.w_dg_plane) != cudaSuccess) cudaGetLastError();
         }
@@ -875,12 +885,12 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
             if (h->vals[v].buf == ov.buf && h->vals[v].coff == 0 && h->vals[v].C == h->bufs[ov.buf].C && first_consumer[v] >= 0) { w = (int)v; break; }
         }
         if (first_consumer[w] >= 0 && h->ops[first_consumer[w]].dgrad_masks) o.dy_premasked = true;
-        o.bias_in_wgrad = o.dy_premasked && o.conv != 0 && o.umma_wgrad.enabled && o.umma_wgrad.p.taps_per_cta * o.umma_wgrad.p.mma_n + 16 <= 512;
+        o.bias_in_wgrad = o.dy_premasked && o.conv != 0 && o.umma_wgrad.enabled;
       }
     }
     return SSNB_OK;
   }
-  // bind tcgen05 plans (tensor maps need final addresses); SSNB_DISABLE_UMMA=1 keeps FAST mode on the SIMT kernels
+  // bind tensor-core plans (tensor maps need final addresses); SSNB_DISABLE_UMMA=1 keeps FAST mode on the SIMT kernels
   const char* dis = getenv("SSNB_DISABLE_UMMA");
   const bool use_umma = h->fp16 && !(dis && dis[0] == '1');
   for (Op& o : h->ops) {
@@ -955,7 +965,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       if (j >= 0) { h->ops[j].fuse_block = (int)bi; h->ops[j].fuse_role = (j == leader) ? 1 : 2; }
   }
   // ReLU-mask fusion: the consumer with the smallest forward index is the last writer of a value's gradient in the
-  // reverse schedule (sibling followers are folded into their leader); if that writer is a tcgen05 data gradient or the
+  // reverse schedule (sibling followers are folded into their leader); if that writer is a tensor-core data gradient or the
   // global pool, it applies dz = dy * (y > 0) in its epilogue and the producing conv skips its own mask pass.
   for (Op& o : h->ops) { o.dgrad_masks = false; o.dy_premasked = false; }
   if (use_umma && h->cfg.training) {
@@ -973,7 +983,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       else if (c.kind == OP_CONV && (c.fuse_role == 1 ? h->fused[c.fuse_block].enabled : (c.fuse_role == 0 && c.umma_dgrad.enabled))) {
         c.dgrad_masks = true;
         const View yv = h->view((int)v, false);
-        if (c.fuse_role == 1) umma_conv_set_mask(h->umma_ctx, h->fused[c.fuse_block].dgrad, yv); else umma_conv_set_mask(h->umma_ctx, c.umma_dgrad, yv);
+        if (c.fuse_role == 1) umma_conv_set_mask(h->fused[c.fuse_block].dgrad, yv); else umma_conv_set_mask(c.umma_dgrad, yv);
       }
     }
     for (Op& o : h->ops) {
@@ -985,7 +995,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
           if (h->vals[v].buf == ov.buf && h->vals[v].coff == 0 && h->vals[v].C == h->bufs[ov.buf].C && first_consumer[v] >= 0) { w = (int)v; break; }
       }
       if (first_consumer[w] >= 0 && h->ops[first_consumer[w]].dgrad_masks) o.dy_premasked = true;
-      o.bias_in_wgrad = o.dy_premasked && o.conv != 0 && o.umma_wgrad.enabled && o.umma_wgrad.p.taps_per_cta * o.umma_wgrad.p.mma_n + 16 <= 512;
+      o.bias_in_wgrad = o.dy_premasked && o.conv != 0 && o.umma_wgrad.enabled;
     }
   }
   return SSNB_OK;

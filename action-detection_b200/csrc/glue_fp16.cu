@@ -166,8 +166,7 @@ __global__ void maxpool_bwd_h8(__half* __restrict__ dsrc, int H, int W, int C, i
 
 // 3x3 stride-1 pad-1 average (count_include_pad: always /9; its own adjoint), 8 channels per thread, walking down a
 // column with a rolling window of row sums.  Two adjacent columns per thread share the loads, the fp16->fp32
-// conversions and the middle partial sum b + c: ~65 instead of ~100 instructions per output (the kernel is issue-bound;
-// measured on B200 in round 2 against the one-column version: 9.71 vs 10.00 ms per training step).
+// conversions and the middle partial sum b + c: ~65 instead of ~100 instructions per output (the kernel is issue-bound).
 __global__ void avgpool3_pair_h8(const __half* __restrict__ src, int H, int W, int C, int spitch, int scoff,
                                  __half* __restrict__ dst, int dpitch, int dcoff, int F, int accumulate) {
   const int G = C / 8, W2 = (W + 1) / 2;

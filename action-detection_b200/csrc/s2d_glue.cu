@@ -1,4 +1,4 @@
-// FAST-mode helpers that let every convolution of BNInception run on the stride-1 tcgen05 kernels:
+// FAST-mode helpers that let every convolution of BNInception run on the stride-1 tensor-core kernels:
 //  * conv1 (7x7 stride 2 pad 3, bn_inception.yaml:3-5) as a 4x4 stride-1 convolution over the
 //    space-to-depth input  xs[f, i, j, (a*2+b)*Cin + c] = x[f, 2i+a, 2j+b, c]   (r = 2*dr + a - 1)
 //  * stride-2 3x3 layers (inception_3c/4e): backward through a zero-upsampled output gradient.

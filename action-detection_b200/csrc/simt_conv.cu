@@ -2,7 +2,7 @@
 // as implicit GEMMs over NHWC tensors.  This is the EXACT-precision engine of libssn_b200
 // (SSNB_EXACT_FP32: fp32 storage, end-to-end parity with the reference's fp32 PyTorch path,
 // ssn_models.py:266 / model_zoo/bninception/pytorch_load.py:37-61) and the generic-geometry kernel
-// for the layers the tcgen05 path does not cover.
+// for the layers the tensor-core path does not cover.
 #include "common.cuh"
 
 namespace ssnb {

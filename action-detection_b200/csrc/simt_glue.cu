@@ -198,8 +198,8 @@ __global__ void pack_conv_kernel(const float* __restrict__ w, const float* __res
   }
 }
 
-// all layers of the network in a few launches (the 69 per-layer launches cost ~1.1 ms per training step, mostly launch
-// latency: the weights are re-packed after every optimizer step)
+// all layers of the network in a few launches (69 per-layer launches would be mostly launch latency: the weights are
+// re-packed after every optimizer step)
 template <typename T>
 __global__ void pack_all_kernel(const __grid_constant__ PackTable t) {
   int ei = 0;
@@ -212,7 +212,7 @@ __global__ void pack_all_kernel(const __grid_constant__ PackTable t) {
   if (taps <= PACK_TILE_TAPS) {
     // tiled path: a CTA owns PACK_TILE output x PACK_TILE input channels x taps.  The source rows ([ci][tap] runs of one output
     // channel) are read contiguously into shared memory, wf is then written with the output channel and wd with the input channel
-    // as the lane index, so all three streams are coalesced (the element-wise path scatters both stores: 0.32 ms per step)
+    // as the lane index, so all three streams are coalesced (the element-wise path scatters both stores)
     __shared__ float tile[PACK_TILE][PACK_TILE * PACK_TILE_TAPS + 1];
     const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int ci_tiles = (q.cin + PACK_TILE - 1) / PACK_TILE;

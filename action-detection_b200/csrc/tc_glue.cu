@@ -1,10 +1,10 @@
 // SSNB_EXACT_TC glue: error-compensated fp16 operand planes of fp32 tensors.
 //
 // The reference computes every convolution in fp32 (model_zoo/bninception/layer_factory.py:25-39, no AMP in
-// ssn_train.py:81).  tcgen05 has no fp32 MMA; an fp32 value x is instead carried as TWO fp16 numbers
+// ssn_train.py:81).  tensor-core has no fp32 MMA; an fp32 value x is instead carried as TWO fp16 numbers
 //     hi = fp16(x),  lo = fp16(x - float(hi))          (hi + lo == x to ~2^-22 relative, fp16 range permitting)
 // and a product a*b is evaluated as a_lo*b_hi + a_hi*b_lo + a_hi*b_hi on the tensor cores with fp32 accumulation
-// (umma_conv_v2.cu / umma_conv.cu / umma_wgrad.cu, nseg = 3).  The kernels here produce those planes for tensors that
+// (umma_conv.cu / umma_wgrad.cu, nseg = 3).  The kernels here produce those planes for tensors that
 // do not come out of a convolution epilogue (pool outputs, the network input, masked output gradients, weights).
 #include "common.cuh"
 
@@ -50,7 +50,7 @@ __global__ void split_flat_kernel(const float* __restrict__ src, long long n, __
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   // power-of-two scale (exact in fp): the largest weight lands in [4096, 8192), so hi's ulp is >= 4 and lo >= 2^-... stays
   // a NORMAL fp16 number down to weights 2^-13 below the maximum.  Unscaled, a BN-folded weight of ~1e-3 (conv1: inputs
-  // are +-128, the fold divides by sigma ~ 100) has a subnormal lo with 3 significant bits: measured 1.4e-5 error.
+  // are +-128, the fold divides by sigma ~ 100) has a subnormal lo with 3 significant bits.
   float sc = 1.0f;
   if (absmax) {
     int e = 0;

@@ -1,14 +1,15 @@
-// tcgen05 implicit-GEMM convolution (sm_100a): host-side planning for both kernel generations, and the first-generation
-// kernel (per-tap A boxes), which still runs the four stride-2 forward layers (TMA element-stride boxes) and everything
-// under SSNB_V2=0.  All stride-1 layers run on umma_conv_v2.cu (halo boxes, CTA pairs, warp-uniform role loops).
+// wgmma implicit-GEMM convolution (sm_90a): host-side planning and the kernel that runs every tensor-core convolution
+// (forward, data gradient, fused sibling 1x1 forward / data gradient, stride-2 forward through TMA element strides).
 //
-//   warp 0      : TMA producer   (A: 4-D activation box, B: 3-D weight box, SWIZZLE_128B)
-//   warp 1      : TMEM allocator + MMA issuer (tcgen05.mma.cta_group::1.kind::f16, M=128, N=block_n)
-//   warps 2..9  : epilogue       (tcgen05.ld 32x32b -> bias/ReLU or accumulate/mask -> fp16 NHWC store); two warps per
-//                 TMEM lane quadrant take alternating 32-column groups (memory-level parallelism of the stores/loads)
+//   warpgroup 0     : TMA producer (one thread; A: 4-D activation box, B: 3-D weight box, SWIZZLE_128B)
+//   warpgroups 1, 2 : consumers -- rows [64 * (wg - 1), +64) of the 128-row tile, one m64nNk16 wgmma (N = block_n) per 16 channels,
+//                     fp32 accumulators in registers; then the epilogue: each 64-column slice of the accumulator goes
+//                     through shared memory so that every thread owns one output row (bias/ReLU or accumulate/mask ->
+//                     fp16 NHWC stores, or the SSNB_EXACT_TC fp32 epilogue of umma_epi32.cuh)
 //
 // Rows of the M tile are the pixels of one TMA box (bw x bh x bf); taps shift the box origin and
-// rely on TMA's out-of-bounds zero fill for the convolution padding.
+// rely on TMA's out-of-bounds zero fill for the convolution padding.  The producer runs ahead into the next tile
+// while the consumers drain the current one.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -24,13 +25,14 @@ namespace {
 
 using namespace umma;
 constexpr int MAX_STAGES = 8;
-constexpr int PIPE_BYTES = 4 * (BLOCK_M * BLOCK_K * 2 + 256 * BLOCK_K * 2);   // 192 KiB of operand staging
+constexpr int PIPE_BYTES = 180 * 1024;             // operand staging
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;     // 16 KiB
-constexpr int NUM_THREADS = 320;
-constexpr int EPI_WARPS = 8;
-constexpr int TMEM_COLS = 512;
-constexpr int BAR_BYTES = 1024;                    // barriers
-constexpr int SMEM_BYTES = PIPE_BYTES + 1024 /*align slack*/ + BAR_BYTES;
+constexpr int NUM_THREADS = 384;
+constexpr int EPI_PITCH = 68;                      // floats per staged accumulator row (64 + 4: 16-byte aligned, banks rotate)
+constexpr int EPI_BYTES = BLOCK_M * EPI_PITCH * 4;
+constexpr int BAR_BYTES = 256;
+constexpr int SMEM_BYTES = PIPE_BYTES + EPI_BYTES + BAR_BYTES + 1024 /*align slack*/;
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
 struct TileCoord { int w0, h0, f0, n0; };
 __device__ __forceinline__ TileCoord decode_tile(const UmmaConvParams& p, int tile) {
@@ -87,131 +89,89 @@ __device__ __forceinline__ void epilogue_chunk(const UmmaConvParams& p, const ui
   dst[0] = q0; dst[1] = q1;
 }
 
-// Direct variant of the epilogue (SSNB_EPI=0): every thread stores its own accumulator row, 32 bytes per 16 columns.
-// Epilogue role shared by the kernels: for every tile of this CTA wait for the accumulator, then TMEM -> registers ->
-// bias/ReLU (forward) or accumulate/mask (data gradient) -> fp16 NHWC stores.  Row r of the tile is pixel
-// (x, y, f) = (r % bw, (r / bw) % bh, r / (bw*bh)) in the classic layout and (r % bw, r / (bw*bf), (r / bw) % bf) in
-// the halo layout (rows ordered y-major, then frame, so that tap views have one uniform group stride).
-__device__ __forceinline__ void epilogue_loop_direct(const UmmaConvParams& p, uint32_t tmem_base, uint64_t* tfull_bar, uint64_t* tempty_bar,
-                                              int warp, int lane, int total_tiles, int tile0, int tstep) {
-  const int quad = warp & 3;
-  const int cpar = (warp - 2) >> 2;
-  const int row = quad * 32 + lane;
-  int rw, rh, rf;
-  if (p.halo) { rw = row % p.bw; rf = (row / p.bw) % p.bf; rh = row / (p.bw * p.bf); }
-  else { rw = row % p.bw; rh = (row / p.bw) % p.bh; rf = row / (p.bw * p.bh); }
-  uint32_t acc = 0, acc_phase = 0;
-  for (int tile = tile0; tile < total_tiles; tile += tstep) {
-    const TileCoord t = decode_tile(p, tile);
-    const int w = t.w0 + rw, h = t.h0 + rh, f = t.f0 + rf;
-    const int os = p.out_stride;
-    const bool valid = (rf < p.bf) && (rh < p.bh) && (w < p.W) && (h < p.H) && (f < p.F) && (w % os == 0) && (h % os == 0);
-    const long long opix = (long long)(f * p.OH + h / os) * p.OW + w / os;
-    __half* orow = p.out + opix * p.out_pitch + p.out_coff;
-    __half* orow2 = p.out2 + opix * p.out2_pitch + p.out2_coff - p.n_split;
-    mbar_wait(&tfull_bar[acc], acc_phase);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + acc * 256 + ((uint32_t)(quad * 32) << 16);
-    if (p.out_f32) {
-      // SSNB_EXACT_TC: fp32 epilogue + the result's fp16 hi / lo operand planes (umma_epi32.cuh)
-      float* orow32 = p.out32 + opix * p.out_pitch + p.out_coff;
-      __half* hrow = p.out_hi ? p.out_hi + opix * p.out_pitch + p.out_coff : nullptr;
-      const float alpha = p.alpha * (p.alpha_dev ? __ldg(p.alpha_dev) : 1.0f);
-      const float* mrow32 = p.mask32 ? p.mask32 + opix * p.mask32_pitch + p.mask32_coff : nullptr;
-      for (int c0 = cpar * 32; c0 < p.block_n; c0 += 64) {
-        const bool two = c0 + 16 < p.block_n;
-        const int cola = t.n0 + c0, colb = cola + 16;
-        uint32_t ra[16], rb[16];
-        tmem_ld16(taddr + c0, ra);
-        if (two) tmem_ld16(taddr + c0 + 16, rb);
-        tmem_ld_wait();
-        if (valid && cola < p.Cout) store_chunk32(p, alpha, ra, p.bias + cola, orow32 + cola, hrow ? hrow + cola : nullptr, mrow32 ? mrow32 + cola : nullptr, p.out_lo_off);
-        if (two && valid && colb < p.Cout) store_chunk32(p, alpha, rb, p.bias + colb, orow32 + colb, hrow ? hrow + colb : nullptr, mrow32 ? mrow32 + colb : nullptr, p.out_lo_off);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      continue;
-    }
-    // two 16-column chunks per iteration: the global loads of both (accumulate / mask operands) and both TMEM
-    // loads are in flight before the first use
-    for (int c0 = cpar * 32; c0 < p.block_n; c0 += 64) {
-      const bool two = c0 + 16 < p.block_n;                       // warp-uniform
-      const int cola = t.n0 + c0, colb = cola + 16;
-      const bool va = valid && cola < p.Cout, vb = two && valid && colb < p.Cout;
-      uint4* da = reinterpret_cast<uint4*>((cola < p.n_split ? orow : orow2) + cola);
-      uint4* db2 = reinterpret_cast<uint4*>((colb < p.n_split ? orow : orow2) + colb);
-      uint4 oa0 = {}, oa1 = {}, ob0 = {}, ob1 = {}, ya0 = {}, ya1 = {}, yb0 = {}, yb1 = {};
-      if (p.accumulate) {
-        if (va) { oa0 = da[0]; oa1 = da[1]; }
-        if (vb) { ob0 = db2[0]; ob1 = db2[1]; }
-      }
-      if (p.mask_y) {
-        const uint4* my = reinterpret_cast<const uint4*>(p.mask_y + opix * p.mask_pitch + p.mask_coff + cola);
-        if (va) { ya0 = __ldg(my); ya1 = __ldg(my + 1); }
-        if (vb) { yb0 = __ldg(my + 2); yb1 = __ldg(my + 3); }
-      }
-      uint32_t ra[16], rb[16];
-      tmem_ld16(taddr + c0, ra);
-      if (two) tmem_ld16(taddr + c0 + 16, rb);
-      tmem_ld_wait();
-      if (va) epilogue_chunk(p, ra, cola, da, oa0, oa1, ya0, ya1);
-      if (vb) epilogue_chunk(p, rb, colb, db2, ob0, ob1, yb0, yb1);
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      mbar_arrive(&tempty_bar[acc]);     // 8 arrivals (one per epilogue warp) release it
-    }
-    if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+// One 16-column chunk (tile columns [c, c + 16)) of accumulator row `row`, read from the staged slice `st`.
+// Row r of the tile is pixel (x, y, f) = (r % bw, (r / bw) % bh, r / (bw*bh)).
+__device__ __forceinline__ void epilogue_row_chunk(const UmmaConvParams& p, const TileCoord& t, int row, int col, const float* st) {
+  const int rw = row % p.bw, rh = (row / p.bw) % p.bh, rf = row / (p.bw * p.bh);
+  const int w = t.w0 + rw, h = t.h0 + rh, f = t.f0 + rf;
+  const int os = p.out_stride;
+  const bool valid = (rf < p.bf) && (w < p.W) && (h < p.H) && (f < p.F) && (w % os == 0) && (h % os == 0);
+  if (!valid || col >= p.Cout) return;
+  const long long opix = (long long)(f * p.OH + h / os) * p.OW + w / os;
+  uint32_t r[16];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 q = reinterpret_cast<const float4*>(st)[j];
+    r[4 * j] = __float_as_uint(q.x); r[4 * j + 1] = __float_as_uint(q.y); r[4 * j + 2] = __float_as_uint(q.z); r[4 * j + 3] = __float_as_uint(q.w);
   }
+  const bool d1 = col < p.n_split;
+  if (p.out_f32) {
+    // SSNB_EXACT_TC: fp32 epilogue + the result's fp16 hi / lo operand planes (umma_epi32.cuh); a fused sibling forward sends
+    // columns >= n_split to the second destination (its own pitch / channel offset)
+    const float alpha = p.alpha * (p.alpha_dev ? __ldg(p.alpha_dev) : 1.0f);
+    float* o32 = d1 ? p.out32 + opix * p.out_pitch + p.out_coff + col : p.out32_2 + opix * p.out2_pitch + p.out2_coff - p.n_split + col;
+    __half* hi = d1 ? p.out_hi : p.out_hi2;
+    if (hi) hi += d1 ? opix * p.out_pitch + p.out_coff + col : opix * p.out2_pitch + p.out2_coff - p.n_split + col;
+    const float* m32 = p.mask32 ? p.mask32 + opix * p.mask32_pitch + p.mask32_coff + col : nullptr;
+    store_chunk32(p, alpha, r, p.bias + col, o32, hi, m32, d1 ? p.out_lo_off : p.out_lo_off2);
+    return;
+  }
+  uint4* dst = reinterpret_cast<uint4*>(d1 ? p.out + opix * p.out_pitch + p.out_coff + col : p.out2 + opix * p.out2_pitch + p.out2_coff - p.n_split + col);
+  uint4 o0 = {}, o1 = {}, y0 = {}, y1 = {};
+  if (p.accumulate) { o0 = dst[0]; o1 = dst[1]; }
+  if (p.mask_y) {
+    const uint4* my = reinterpret_cast<const uint4*>(p.mask_y + opix * p.mask_pitch + p.mask_coff + col);
+    y0 = __ldg(my); y1 = __ldg(my + 1);
+  }
+  epilogue_chunk(p, r, col, dst, o0, o1, y0, y1);
 }
 
+// the first NK 16-channel steps of a staged K chunk: A rows [sa, +64 rows) x B rows [sb, +64 NSUB rows), both K-major
+template <int NSUB, int NK>
+__device__ __forceinline__ void mma_k(float* d, uint32_t sa, uint32_t sb) {
+#pragma unroll
+  for (int k = 0; k < NK; ++k) wgmma<NSUB * MMA_N, 0, 0>(d, make_desc_sw128(sa + k * MMA_K * 2), make_desc_sw128(sb + k * MMA_K * 2));
+}
+
+// NSUB = block_n / 64 accumulator slices per consumer warpgroup
+template <int NSUB>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                  const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a_lo,
-                 const __grid_constant__ CUtensorMap tmap_a2_lo, const __grid_constant__ CUtensorMap tmap_b_lo, const UmmaConvParams p) {
+                 const __grid_constant__ CUtensorMap tmap_a2_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
+                 const __grid_constant__ UmmaConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operand tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  // pipeline depth adapts to the tile: narrow-N layers get up to 8 stages in the same 192 KiB
+  // pipeline depth adapts to the tile: narrow-N layers get more stages in the same staging area
   const int STAGES = p.stages, STAGE_BYTES = p.stage_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES);
+  float* epi = reinterpret_cast<float*>(smem + PIPE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES + EPI_BYTES);
   uint64_t* full_bar = bars;                     // [MAX_STAGES]
   uint64_t* empty_bar = bars + MAX_STAGES;       // [MAX_STAGES]
-  uint64_t* tfull_bar = bars + 2 * MAX_STAGES;   // [2] accumulator ready
-  uint64_t* tempty_bar = bars + 2 * MAX_STAGES + 2;  // [2] accumulator drained
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 4);
 
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const int wg = threadIdx.x / 128;
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_f * p.n_tiles;
   const int nseg = p.nseg > 1 ? p.nseg : 1;          // SSNB_EXACT_TC: (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi) per (tap, K chunk)
   const int ksteps = p.ntaps * p.kchunks * nseg;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a2)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], EPI_WARPS); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }   // one release per consumer warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    producer_regs();
+    if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       // bytes the two TMA boxes deliver (zero-filled out-of-bounds elements count; a 7x1x18 box has 126 rows)
-      const uint32_t tx_bytes = (uint32_t)(p.bw * p.bh * p.bf + p.block_n) * BLOCK_K * 2;
+      const uint32_t a_bytes = (uint32_t)(p.bw * p.bh * p.bf) * BLOCK_K * 2;
+      const uint32_t tx_bytes = a_bytes + (uint32_t)p.block_n * BLOCK_K * 2;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile(p, tile);
         for (int seg = 3 - nseg; seg < 3; ++seg)
@@ -223,62 +183,75 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sa = smem + stage * STAGE_BYTES;
             uint8_t* sb = sa + A_BYTES;
-            const uint32_t a_bytes = (uint32_t)(p.bw * p.bh * p.bf) * BLOCK_K * 2;
-            mbar_expect_tx(&full_bar[stage], ((p.ablate & 32) ? 0u : a_bytes) + ((p.ablate & 16) ? 0u : tx_bytes - a_bytes));
-            if (p.ablate & 32) {}
-            else if (kc < p.kchunks_a1) tma_load_4d(sa, ma, &full_bar[stage], kc * BLOCK_K, t.w0 * p.a_stride + p.tap_dx[tap], t.h0 * p.a_stride + p.tap_dy[tap], t.f0);
+            mbar_expect_tx(&full_bar[stage], tx_bytes);
+            if (kc < p.kchunks_a1) tma_load_4d(sa, ma, &full_bar[stage], kc * BLOCK_K, t.w0 * p.a_stride + p.tap_dx[tap], t.h0 * p.a_stride + p.tap_dy[tap], t.f0);
             else tma_load_4d(sa, ma2, &full_bar[stage], (kc - p.kchunks_a1) * BLOCK_K, t.w0 + p.tap_dx[tap], t.h0 + p.tap_dy[tap], t.f0);
-            if (!(p.ablate & 16)) tma_load_3d(sb, mb, &full_bar[stage], kc * BLOCK_K, t.n0, tap);
+            tma_load_3d(sb, mb, &full_bar[stage], kc * BLOCK_K, t.n0, tap);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(p.block_n);
-      uint32_t stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        int kc = 0;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
-          const uint32_t sb = sa + A_BYTES;
-          // K chunks whose tail is TMA zero fill (Cin % 64 != 0) skip the all-zero MMAs
-          const int kvalid = kc < p.kchunks_a1 ? p.K1 - kc * BLOCK_K : p.K - p.K1 - (kc - p.kchunks_a1) * BLOCK_K;
-          if (p.ablate & 8) {
-          } else if (kvalid >= BLOCK_K) {
+  } else {
+    // ===== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64) =====
+    consumer_regs();
+    const int cw = wg - 1, ct = threadIdx.x - 128;
+    const int warp = (threadIdx.x / 32) & 3, lane = threadIdx.x & 31;
+    uint32_t stage = 0, phase = 0, prev = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile);
+      float acc[NSUB][32];
 #pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_f16(d_tmem, make_desc_k_sw128(sa + k * UMMA_K * 2), make_desc_k_sw128(sb + k * UMMA_K * 2), idesc, (ks | k) ? 1u : 0u);
-          } else {
-            const int nk = (kvalid + UMMA_K - 1) / UMMA_K;
-            for (int k = 0; k < nk; ++k)
-              umma_f16(d_tmem, make_desc_k_sw128(sa + k * UMMA_K * 2), make_desc_k_sw128(sb + k * UMMA_K * 2), idesc, (ks | k) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);               // frees the smem slot when these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          if (++kc == p.kchunks) kc = 0;
+      for (int j = 0; j < NSUB; ++j)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+      int kc = 0;
+      for (int ks = 0; ks < ksteps; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * (64 * 128);
+        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+        // K chunks whose tail is TMA zero fill (Cin % 64 != 0) skip the all-zero MMAs
+        const int kvalid = kc < p.kchunks_a1 ? p.K1 - kc * BLOCK_K : p.K - p.K1 - (kc - p.kchunks_a1) * BLOCK_K;
+        const int nk = kvalid >= BLOCK_K ? BLOCK_K / MMA_K : (kvalid + MMA_K - 1) / MMA_K;
+        // one m64n(64 NSUB)k16 MMA per 16 channels: the A rows are read from shared memory once for all columns of the
+        // tile.  Every path issues a compile-time number of MMAs (no predicated wgmma inside a sequence).
+        wgmma_fence();
+        float* d = &acc[0][0];
+        switch (nk) {
+          case 1: mma_k<NSUB, 1>(d, sa, sb); break;
+          case 2: mma_k<NSUB, 2>(d, sa, sb); break;
+          case 3: mma_k<NSUB, 3>(d, sa, sb); break;
+          default: mma_k<NSUB, BLOCK_K / MMA_K>(d, sa, sb); break;
         }
-        umma_commit(&tfull_bar[acc]);                   // accumulator complete
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+        wgmma_commit();
+        // one group stays in flight: the previous stage's MMAs have retired, its smem slot goes back to the producer
+        wgmma_wait<1>();
+        if (ks > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        if (++kc == p.kchunks) kc = 0;
+      }
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      // epilogue, one 64-column slice at a time: fragments -> shared memory -> one row per thread, 32 columns per thread
+      const int row = ct & 127, half = ct >> 7;
+#pragma unroll
+      for (int j = 0; j < NSUB; ++j) {
+        consumer_sync();                             // the previous slice has been read
+#pragma unroll
+        for (int i = 0; i < 32; i += 2) {
+          const int r = cw * 64 + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+          const int c = 8 * (i >> 2) + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(epi + r * EPI_PITCH + c) = make_float2(acc[j][i], acc[j][i + 1]);
+        }
+        consumer_sync();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int c = half * 32 + h * 16;
+          epilogue_row_chunk(p, t, row, t.n0 + j * MMA_N + c, epi + row * EPI_PITCH + c);
+        }
       }
     }
-  } else {
-    // ===== epilogue warps 2..9; TMEM lane quadrant = warp % 4, column-group parity = (warp - 2) / 4 =====
-    epilogue_loop_direct(p, tmem_base, tfull_bar, tempty_bar, warp, lane, total_tiles, blockIdx.x, gridDim.x);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -297,7 +270,7 @@ int resolve_encode(UmmaContext& ctx) {
     return 2;
   }
   ctx.encode_tiled = fn;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   ctx.num_sms = sms;
   return 0;
@@ -357,10 +330,10 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   p.W = a.W; p.H = a.H; p.F = F;
   pick_box(a.W, p.bw, p.bh, p.bf);
   p.tiles_w = (a.W + p.bw - 1) / p.bw; p.tiles_h = (a.H + p.bh - 1) / p.bh; p.tiles_f = (F + p.bf - 1) / p.bf;
-  // N split: equal tiles of block_n <= 256 (multiple of 16); the last tile may overhang N (TMA zero-fills the
+  // N split: equal tiles of block_n <= 256 (multiple of 64); the last tile may overhang N (TMA zero-fills the
   // missing weight rows, the epilogue masks the columns)
   p.n_tiles = (N + 255) / 256;
-  p.block_n = (((N + p.n_tiles - 1) / p.n_tiles) + 15) / 16 * 16;
+  p.block_n = (((N + p.n_tiles - 1) / p.n_tiles) + MMA_N - 1) / MMA_N * MMA_N;
   p.kchunks = (K + BLOCK_K - 1) / BLOCK_K;
   p.K = K;
   p.stage_bytes = (A_BYTES + p.block_n * BLOCK_K * 2 + 1023) / 1024 * 1024;
@@ -383,13 +356,10 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
     cuuint64_t str[2] = {(cuuint64_t)K * 2, (cuuint64_t)N * K * 2};
     cuuint32_t box[3] = {(cuuint32_t)BLOCK_K, (cuuint32_t)p.block_n, 1};
     if (int rc = encode(ctx, &plan.tmap_b, 3, const_cast<__half*>(w), dims, str, box)) return rc;
-    plan.b_ptr = w;
     plan.b_lo_off = tc ? tc->w_lo_off : 0;
     plan.tmap_b_lo = plan.tmap_b;
     if (plan.b_lo_off)
       if (int rc = encode(ctx, &plan.tmap_b_lo, 3, reinterpret_cast<__half*>(reinterpret_cast<char*>(const_cast<__half*>(w)) + plan.b_lo_off), dims, str, box)) return rc;
-    for (int i = 0; i < 3; ++i) plan.b_dims[i] = dims[i];
-    for (int i = 0; i < 2; ++i) plan.b_strides[i] = str[i];
   }
   plan.tmap_a2 = plan.tmap_a; plan.tmap_a2_lo = plan.tmap_a_lo;
   // SSNB_EXACT_TC: three operand segments per K chunk, fp32 epilogue (+ fp16 operand planes of the result)
@@ -402,135 +372,18 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   return 0;
 }
 
-// Route a bound stride-1 plan to the second-generation kernel (umma_conv_v2.cu): halo layout (one A box per K chunk
-// covers the tile plus the filter border, taps = shifted UMMA descriptor views; a 1x1 layer is the halo-free case),
-// several taps per weight stage, CTA pairs.
-//   SSNB_V2=0            keep every layer on the first-generation kernel of this file
-//   SSNB_PAIR=0          single-CTA MMAs (cta_group::1) instead of CTA pairs
-//   SSNB_HALO_MODE=m     how horizontal shifts are realised: 2 (default) halo rows at their exact pitch (bw + halo pixels);
-//                        1 rows padded to a 16-pixel pitch; 4 one box per horizontal shift (every view 1024-byte aligned).
-//                        Measured on B200 (tools/halo_probe.sh): the UMMA unit applies the 128-byte swizzle to absolute
-//                        shared-memory address bits, so views that start at any 128-byte row of a TMA-written tile read
-//                        correctly with descriptor base_offset 0 (a non-zero base_offset gives wrong data).
-//   SSNB_HALO_MIN_W=w    smallest image width that uses it (default 7: every stride-1 layer)
-// `a2` is the second activation source of a fused sibling data gradient (K chunks >= kchunks_a1), or nullptr.
-constexpr int V2_STAGES_MAX = 8;
-int try_halo(UmmaContext& ctx, UmmaConvPlan& plan, View a, int F, const View* a2 = nullptr) {
+// Which plans the split-operand (EXACT_TC) schedule runs on the tensor cores (UmmaConvParams::tc_ok): stride-1 layers of
+// 1, 4 or 9 taps on images at least 7 pixels wide whose outputs are 32-byte aligned NHWC slices; a fused sibling data
+// gradient (two K sources) only as a 1x1 layer.
+void mark_tc_ok(UmmaConvPlan& plan, int W, bool two_sources) {
   UmmaConvParams& p = plan.p;
-  p.halo = 0; p.pair = 0; p.v2 = 0;
-  const char* ve = getenv("SSNB_V2");
-  if ((ve && ve[0] == '0') || !umma_conv_v2_supported(p.ntaps)) return 0;
-  const char* pe = getenv("SSNB_PAIR");
-  const bool pair = !(pe && pe[0] == '0');
-  if (!plan.enabled || p.a_stride != 1 || p.out_stride != 1) return 0;
-  if (p.kchunks_a1 != p.kchunks && (p.ntaps != 1 || !a2)) return 0;
-  // the v2 epilogue moves 16 fp16 columns per 256-bit access: rows and channel slices must be 32-byte aligned; its
-  // shared-memory bias table holds 1024 columns
-  if (p.out_pitch % 16 || p.out_coff % 16 || p.out2_pitch % 16 || p.out2_coff % 16 || p.n_split % 16 || (p.bias && p.n_tiles * p.block_n > 1024)) return 0;
-  if (plan.mask_y && (plan.mask_pitch % 16 || plan.mask_coff % 16)) return 0;
-  const char* mw = getenv("SSNB_HALO_MIN_W");
-  if (a.W < (mw ? atoi(mw) : 7)) return 0;
-  const char* md = getenv("SSNB_HALO_MODE");
-  const int mode = md ? atoi(md) : 2;
-  int x0 = 0, x1 = 0, y0 = 0, y1 = 0;
-  for (int t = 0; t < p.ntaps; ++t) {
-    x0 = std::min(x0, p.tap_dx[t]); x1 = std::max(x1, p.tap_dx[t]);
-    y0 = std::min(y0, p.tap_dy[t]); y1 = std::max(y1, p.tap_dy[t]);
-  }
-  const int xh = x1 - x0, yh = y1 - y0;
-  int bh = 8;
-  while (bh > 1 && a.H % bh) bh >>= 1;
-  const int bw = 8, bf = BLOCK_M / (bw * bh);
-  int loads = 1, pw;
-  if (xh == 0) pw = bw;
-  else if (mode == 4) { loads = xh + 1; pw = bw; }
-  else if (mode >= 2) pw = bw + xh;
-  else pw = 16;
-  const int bhh = bh + yh;
-  if (loads > 4 || bhh > 256 || bf > 256) return 0;
-  // TMA-fed epilogue for data gradients (default; SSNB_EPI_TMA=0 keeps the register-prefetch epilogue -- measured on B200,
-  // round 2: 9.82 vs 10.00 ms per training step, 0 mismatching launches in tools/umma_diag.py): a ring of 3 x (old-gradient + activation chunk) at the
-  // top of the staging area; the operand rings get what is left
-  const char* te = getenv("SSNB_EPI_TMA");
-  const bool want_ring = !(te && te[0] == '0') && !p.bias && !p.relu && !p.out_f32;
-  constexpr int EPI_STAGE = 2 * 128 * 128, EPI_STAGES = 3;
-  int pipe = UMMA_V2_PIPE_BYTES - (want_ring ? EPI_STAGES * EPI_STAGE : 0);
-  bool ring = want_ring;
-retry_without_ring:
-  const int b_rows = pair ? p.block_n / 2 : p.block_n;      // weight rows each CTA stages per (tap, K chunk)
-  const int a_load_bytes = pw * bf * bhh * BLOCK_K * 2;
-  const int a_stage = (loads * a_load_bytes + 1023) / 1024 * 1024;
-  const int slab = b_rows * BLOCK_K * 2;                    // one tap of the weight stage (multiple of 1024: rows % 8 == 0)
-  int b_taps = 1;
-  if (p.ntaps > 1) {                                        // several taps per weight stage: fewer barrier hand-offs per K chunk
-    for (int g = p.ntaps; g >= 1; --g)
-      if (p.ntaps % g == 0 && g * slab <= 48 * 1024 && 2 * a_stage + 3 * g * slab <= pipe) { b_taps = g; break; }
-  }
-  const int b_stage = (b_taps * slab + 1023) / 1024 * 1024;
-  int a_stages, b_stages;
-  if (p.ntaps == 1) {                                       // one box + one slab per step: equal ring depths
-    a_stages = b_stages = std::min(V2_STAGES_MAX, pipe / (a_stage + b_stage));
-    if (a_stages < 3) { if (ring) { ring = false; pipe = UMMA_V2_PIPE_BYTES; goto retry_without_ring; } return 0; }
-  } else {
-    a_stages = 3;
-    if ((pipe - 3 * a_stage) / b_stage < 3) a_stages = 2;
-    b_stages = (pipe - a_stages * a_stage) / b_stage;
-    if (b_stages < 2) { if (ring) { ring = false; pipe = UMMA_V2_PIPE_BYTES; goto retry_without_ring; } return 0; }   // does not fit: stay on the first-generation kernel
-    if (b_stages > V2_STAGES_MAX) b_stages = V2_STAGES_MAX;
-  }
-  p.v2 = 1; p.b_taps = b_taps;
-  p.halo = 1; p.pair = pair ? 1 : 0;
-  p.bw = bw; p.bh = bh; p.bf = bf;
-  p.tiles_w = (a.W + bw - 1) / bw; p.tiles_h = (a.H + bh - 1) / bh; p.tiles_f = (F + bf - 1) / bf;
-  p.tiles_q = pair ? (p.tiles_f + 1) / 2 : p.tiles_f;
-  p.a_stages = a_stages; p.b_stages = b_stages; p.a_stage_bytes = a_stage; p.b_stage_bytes = b_stage;
-  p.a_loads = loads; p.a_load_bytes = a_load_bytes; p.halo_x0 = x0; p.halo_y0 = y0; p.a_sbo = pw * BLOCK_K * 2;
-  for (int l = 0; l < 4; ++l) p.a_load_dx[l] = loads > 1 ? l : 0;
-  for (int t = 0; t < p.ntaps; ++t) {
-    const int l = loads > 1 ? p.tap_dx[t] - x0 : 0;
-    const int dxl = loads > 1 ? 0 : p.tap_dx[t] - x0;
-    p.tap_aoff[t] = l * a_load_bytes + ((p.tap_dy[t] - y0) * bf * pw + dxl) * BLOCK_K * 2;
-  }
-  // halo box: dims {C, W, F, H} so that shared memory holds [y][frame][x][64 ch]
-  auto encode_a = [&](CUtensorMap* m, const View& v, int channels) -> int {
-    cuuint64_t dims[4] = {(cuuint64_t)channels, (cuuint64_t)v.W, (cuuint64_t)F, (cuuint64_t)v.H};
-    cuuint64_t str[3] = {(cuuint64_t)v.pitch * 2, (cuuint64_t)v.H * v.W * v.pitch * 2, (cuuint64_t)v.W * v.pitch * 2};
-    cuuint32_t box[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)pw, (cuuint32_t)bf, (cuuint32_t)bhh};
-    return encode(ctx, m, 4, reinterpret_cast<__half*>(v.base) + v.coff, dims, str, box);
-  };
-  auto lo_of = [](View v) { v.base = reinterpret_cast<char*>(v.base) + v.lo_off; return v; };
-  if (int rc = encode_a(&plan.tmap_a, a, p.K1)) { plan.enabled = false; return rc; }
-  plan.tmap_a_lo = plan.tmap_a;
-  if (a.lo_off) if (int rc = encode_a(&plan.tmap_a_lo, lo_of(a), p.K1)) { plan.enabled = false; return rc; }
-  if (p.kchunks_a1 != p.kchunks) {
-    if (int rc = encode_a(&plan.tmap_a2, *a2, p.K - p.K1)) { plan.enabled = false; return rc; }
-    plan.tmap_a2_lo = plan.tmap_a2;
-    if (a2->lo_off) if (int rc = encode_a(&plan.tmap_a2_lo, lo_of(*a2), p.K - p.K1)) { plan.enabled = false; return rc; }
-  } else { plan.tmap_a2 = plan.tmap_a; plan.tmap_a2_lo = plan.tmap_a_lo; }
-  p.epi_stages = 0; p.epi_stage_bytes = 0; plan.epi_maps_ready = false; plan.epi_mask_ready = false;
-  if (ring) {                                               // TMA-fed epilogue: [128 rows][64 ch] boxes of the output view
-    p.epi_stages = EPI_STAGES; p.epi_stage_bytes = EPI_STAGE;
-    plan.epi_box[0] = bw; plan.epi_box[1] = bf; plan.epi_box[2] = bh; plan.epi_F = F;
-    cuuint64_t od[4] = {(cuuint64_t)p.Cout, (cuuint64_t)p.OW, (cuuint64_t)F, (cuuint64_t)p.OH};
-    cuuint64_t os[3] = {(cuuint64_t)p.out_pitch * 2, (cuuint64_t)p.OH * p.OW * p.out_pitch * 2, (cuuint64_t)p.OW * p.out_pitch * 2};
-    cuuint32_t ob[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)bw, (cuuint32_t)bf, (cuuint32_t)bh};
-    if (int rc = encode(ctx, &plan.tmap_old, 4, p.out + p.out_coff, od, os, ob)) { plan.enabled = false; return rc; }
-    plan.tmap_y = plan.tmap_old;
-    plan.epi_maps_ready = true;
-  } else {
-    plan.tmap_old = plan.tmap_a; plan.tmap_y = plan.tmap_a;  // valid descriptors, never dereferenced
-  }
-  if (pair || b_taps > 1) {                                 // pair: each CTA stages half of the weight rows; v2: b_taps taps per stage
-    cuuint64_t bd[3] = {plan.b_dims[0], plan.b_dims[1], plan.b_dims[2]};
-    cuuint64_t bs[2] = {plan.b_strides[0], plan.b_strides[1]};
-    cuuint32_t bb[3] = {(cuuint32_t)BLOCK_K, (cuuint32_t)b_rows, (cuuint32_t)b_taps};
-    if (int rc = encode(ctx, &plan.tmap_b, 3, const_cast<__half*>(plan.b_ptr), bd, bs, bb)) { plan.enabled = false; return rc; }
-    plan.tmap_b_lo = plan.tmap_b;
-    if (plan.b_lo_off)
-      if (int rc = encode(ctx, &plan.tmap_b_lo, 3, reinterpret_cast<__half*>(reinterpret_cast<char*>(const_cast<__half*>(plan.b_ptr)) + plan.b_lo_off), bd, bs, bb)) {
-        plan.enabled = false; return rc; }
-  }
-  return 0;
+  p.tc_ok = 0;
+  if (!plan.enabled || p.a_stride != 1 || p.out_stride != 1) return;
+  if (!(p.ntaps == 1 || p.ntaps == 4 || p.ntaps == 9)) return;
+  if (p.kchunks_a1 != p.kchunks && (p.ntaps != 1 || !two_sources)) return;
+  if (p.out_pitch % 16 || p.out_coff % 16 || p.out2_pitch % 16 || p.out2_coff % 16 || p.n_split % 16 || (p.bias && p.n_tiles * p.block_n > 1024)) return;
+  if (W < 7) return;
+  p.tc_ok = 1;
 }
 
 }  // namespace
@@ -549,7 +402,8 @@ int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out,
   if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, ntaps, 1, w_tap_n_k, 1, tc)) return rc;
   for (int t = 0; t < ntaps; ++t) { plan.p.tap_dy[t] = dy[t]; plan.p.tap_dx[t] = dx[t]; }
   plan.p.bias = bias; plan.p.relu = relu; plan.p.accumulate = 0;
-  return try_halo(ctx, plan, in, F);
+  mark_tc_ok(plan, in.W, false);
+  return 0;
 }
 
 int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int k, int pad,
@@ -563,7 +417,8 @@ int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, 
   for (int r = 0; r < k; ++r)
     for (int s = 0; s < k; ++s) { plan.p.tap_dy[r * k + s] = r - pad; plan.p.tap_dx[r * k + s] = s - pad; }
   plan.p.bias = bias; plan.p.relu = 1; plan.p.accumulate = 0;
-  return try_halo(ctx, plan, in, F);
+  mark_tc_ok(plan, in.W, false);
+  return 0;
 }
 
 int umma_conv_bind_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz, View dx, int F, int cin, int cout, int k, int pad,
@@ -573,7 +428,8 @@ int umma_conv_bind_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz, View dx,
   for (int r = 0; r < k; ++r)
     for (int s = 0; s < k; ++s) { plan.p.tap_dy[r * k + s] = pad - r; plan.p.tap_dx[r * k + s] = pad - s; }
   plan.p.bias = nullptr; plan.p.relu = 0; plan.p.accumulate = accumulate;
-  return try_halo(ctx, plan, dz, F);
+  mark_tc_ok(plan, dz.W, false);
+  return 0;
 }
 
 int umma_conv_bind_fused_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out1, View out2, int F, int cin, int n1, int n2,
@@ -589,7 +445,8 @@ int umma_conv_bind_fused_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View
     if (!tc->out32_2) { set_thread_error("fused fwd: the split-operand bind needs both fp32 destinations"); return 1; }
     plan.p.out32_2 = tc->out32_2; plan.p.out_hi2 = reinterpret_cast<__half*>(out2.base); plan.p.out_lo_off2 = out2.lo_off;
   }
-  return try_halo(ctx, plan, in, F);
+  mark_tc_ok(plan, in.W, false);
+  return 0;
 }
 
 int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, View dz2, View dx, int F, int cin, int k1, int k2,
@@ -613,27 +470,23 @@ int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, V
     cuuint64_t bs[2] = {(cuuint64_t)(k1p + k2) * 2, (cuuint64_t)cin * (k1p + k2) * 2};
     cuuint32_t bb[3] = {(cuuint32_t)BLOCK_K, (cuuint32_t)p.block_n, 1};
     if (int rc = encode(ctx, &plan.tmap_b, 3, const_cast<__half*>(w_n_k), bd, bs, bb)) { plan.enabled = false; return rc; }
-    plan.b_ptr = w_n_k;
     plan.tmap_b_lo = plan.tmap_b;
     if (plan.b_lo_off)
       if (int rc = encode(ctx, &plan.tmap_b_lo, 3, reinterpret_cast<__half*>(reinterpret_cast<char*>(const_cast<__half*>(w_n_k)) + plan.b_lo_off), bd, bs, bb)) {
         plan.enabled = false; return rc; }
-    for (int i = 0; i < 3; ++i) plan.b_dims[i] = bd[i];
-    for (int i = 0; i < 2; ++i) plan.b_strides[i] = bs[i];
     if (tc && !dz2.lo_off) { set_thread_error("fused dgrad: the split-operand bind needs the second source's operand planes"); plan.enabled = false; return 1; }
+    // the second source's LO plane
+    plan.tmap_a2_lo = plan.tmap_a2;
+    if (dz2.lo_off)
+      if (int rc = encode(ctx, &plan.tmap_a2_lo, 4, reinterpret_cast<__half*>(reinterpret_cast<char*>(dz2.base) + dz2.lo_off) + dz2.coff, dims, str, box)) {
+        plan.enabled = false; return rc; }
   }
-  return try_halo(ctx, plan, a, F, k1 ? &dz2 : nullptr);
+  mark_tc_ok(plan, a.W, k1 != 0);
+  return 0;
 }
 
-void umma_conv_set_mask(UmmaContext& ctx, UmmaConvPlan& plan, View y) {
+void umma_conv_set_mask(UmmaConvPlan& plan, View y) {
   plan.mask_y = reinterpret_cast<const __half*>(y.base); plan.mask_pitch = y.pitch; plan.mask_coff = y.coff;
-  plan.epi_mask_ready = false;
-  if (plan.epi_maps_ready) {                                 // TMA-fed epilogue: the activation tiles come through TMA too
-    cuuint64_t d[4] = {(cuuint64_t)plan.p.Cout, (cuuint64_t)y.W, (cuuint64_t)plan.epi_F, (cuuint64_t)y.H};
-    cuuint64_t st[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.H * y.W * y.pitch * 2, (cuuint64_t)y.W * y.pitch * 2};
-    cuuint32_t b[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)plan.epi_box[0], (cuuint32_t)plan.epi_box[1], (cuuint32_t)plan.epi_box[2]};
-    plan.epi_mask_ready = encode(ctx, &plan.tmap_y, 4, reinterpret_cast<__half*>(y.base) + y.coff, d, st, b) == 0;
-  }
 }
 
 void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag) {
@@ -642,28 +495,42 @@ void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float pla
   plan.mask_plane_scale = plane_scale; plan.mask_flag = flag;
 }
 
+namespace {
+template <int NSUB>
+int launch_nsub(const UmmaConvPlan& plan, const UmmaConvParams& p, int grid, cudaStream_t s) {
+  static bool attr_set[64] = {};          // function attributes are per device
+  auto kern = umma_conv_kernel<NSUB>;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
+      set_thread_error("umma conv: cannot raise dynamic shared memory limit"); cudaGetLastError(); return 2; }
+    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+  }
+  kern<<<grid, NUM_THREADS, SMEM_BYTES, s>>>(plan.tmap_a, plan.tmap_a2, plan.tmap_b, plan.tmap_a_lo, plan.tmap_a2_lo, plan.tmap_b_lo, p);
+  SSNB_LAUNCH_CHECK("umma_conv_kernel");
+  return 0;
+}
+}  // namespace
+
 int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask) {
   if (!plan.enabled) { set_thread_error("umma conv: plan not bound"); return 3; }
-  if (!ctx.attr_set) {
-    if (cudaFuncSetAttribute(umma_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
-      set_thread_error("umma conv: cannot raise dynamic shared memory limit"); cudaGetLastError(); return 2; }
-    ctx.attr_set = true;
-  }
   UmmaConvParams p = plan.p;
   if (mask && plan.mask_y) { p.mask_y = plan.mask_y; p.mask_pitch = plan.mask_pitch; p.mask_coff = plan.mask_coff; }
   if (mask && p.out_f32 && plan.mask32) {
     p.mask32 = plan.mask32; p.mask32_pitch = plan.mask32_pitch; p.mask32_coff = plan.mask32_coff;
     p.out_hi = plan.mask_planes; p.out_lo_off = plan.mask_planes_lo; p.plane_scale = plan.mask_plane_scale; p.flag = plan.mask_flag;
   }
-  static const int ablate = [] { const char* e = getenv("SSNB_ABLATE"); return e ? atoi(e) : 0; }();     // timing experiments only
-  p.ablate = ablate;
-  if (p.v2) return umma_conv_v2_launch(ctx, plan, p, s);
-  if (p.out_f32 && (p.mask_y || p.n_split < p.Cout || p.out_stride != 1)) { set_thread_error("umma conv: the fp32 epilogue has no mask / second destination / sampling"); return 3; }
+  if (p.out_f32 && (p.mask_y || p.out_stride != 1)) { set_thread_error("umma conv: the fp32 epilogue takes its mask through mask32 and has no sampling"); return 3; }
   const int total = p.tiles_w * p.tiles_h * p.tiles_f * p.n_tiles;
   const int grid = total < ctx.num_sms ? total : ctx.num_sms;
-  umma_conv_kernel<<<grid, NUM_THREADS, SMEM_BYTES, s>>>(plan.tmap_a, plan.tmap_a2, plan.tmap_b, plan.tmap_a_lo, plan.tmap_a2_lo, plan.tmap_b_lo, p);
-  SSNB_LAUNCH_CHECK("umma_conv_kernel");
-  return 0;
+  switch (p.block_n / MMA_N) {
+    case 1: return launch_nsub<1>(plan, p, grid, s);
+    case 2: return launch_nsub<2>(plan, p, grid, s);
+    case 3: return launch_nsub<3>(plan, p, grid, s);
+    case 4: return launch_nsub<4>(plan, p, grid, s);
+  }
+  set_thread_error("umma conv: unsupported tile width"); return 3;
 }
 
 }  // namespace ssnb

@@ -1,9 +1,10 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM convolution for SSNB_FAST_FP16 — interface.
+// wgmma (sm_90a) implicit-GEMM convolution for the tensor-core precisions -- interface.
 //
 // One kernel family computes   out[p, n] = epi( sum_taps sum_c  A[p + shift(tap), c] * B[tap][n][c] )
 // over NHWC fp16 tensors: A tiles are 4-D TMA boxes of the activation view (zero-filled outside
 // the image = free padding), B tiles are 3-D TMA boxes of the packed weights, accumulators live
-// in TMEM, the epilogue fuses folded-BN bias + ReLU (forward) or accumulation (data gradient).
+// in the registers of two consumer warpgroups, the epilogue fuses folded-BN bias + ReLU (forward)
+// or accumulation (data gradient).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -14,20 +15,18 @@
 namespace ssnb {
 
 constexpr int UMMA_MAX_TAPS = 16;
-constexpr int UMMA_V2_PIPE_BYTES = 216 * 1024;   // operand staging of the second-generation kernel
 
 struct UmmaContext {
   bool active = false;
   void* encode_tiled = nullptr;   // cuTensorMapEncodeTiled, resolved through cudaGetDriverEntryPoint
-  int num_sms = 148;
-  bool attr_set = false;
+  int num_sms = 132;
 };
 
 struct UmmaConvParams {
   int W, H, F;                    // spatial dims shared by input and output (stride-1 convolutions)
   int bw, bh, bf;                 // TMA box in pixels; bw*bh*bf <= 128 rows of the M tile
   int tiles_w, tiles_h, tiles_f;
-  int n_tiles, block_n;           // N split of Cout
+  int n_tiles, block_n;           // N split of Cout; block_n is a multiple of 64 (one m64n64 MMA per 64 columns)
   int stages, stage_bytes;        // smem pipeline depth / stride chosen from block_n
   int kchunks, ntaps, K;          // ceil(K/64), filter taps, reduction channels per tap
   int tap_dy[UMMA_MAX_TAPS], tap_dx[UMMA_MAX_TAPS];
@@ -40,25 +39,13 @@ struct UmmaConvParams {
   int kchunks_a1, K1;             // K chunks [0, kchunks_a1) come from tmap_a (K1 real channels), the rest from tmap_a2
   int n_split;                    // output columns >= n_split go to out2 (second destination), else to out
   __half* out2; int out2_pitch, out2_coff;
-  // halo mode (3x3 stride-1 layers, conv1): ONE A box per K chunk covers the tile plus its filter halo, stored
-  // [y][frame][x][64 ch]; every tap is a shifted UMMA descriptor view into it (no per-tap re-staging of A)
-  int ablate;                     // timing experiments (SSNB_ABLATE bit mask): 1 no stores, 2 no bias loads, 4 empty epilogue, 8 no MMAs
-  int halo;
-  int pair;                       // CTA-pair kernel (cta_group::2): tiles are (N tile, pair of M tiles)
-  int v2;                         // second-generation kernel (umma_conv_v2.cu): warp-uniform role loops, grouped weight stages
-  int b_taps;                     // v2: taps per weight stage
-  int tiles_q;                    // v2: frame groups (pair mode: PAIRS of frame groups) = last digit of the tile walk
-  int epi_stages, epi_stage_bytes;// v2, experimental TMA-fed epilogue: ring depth (0 = off) and stride (old + activation chunk)
-  int a_stages, b_stages, a_stage_bytes, b_stage_bytes;
-  int a_loads, a_load_bytes;      // TMA loads per A stage (1: full halo box; >1: one box per horizontal shift)
-  int halo_x0, halo_y0;           // box origin relative to the tile origin (min dx, min dy)
-  int a_load_dx[4];               // extra W shift of each load
-  int a_sbo;                      // bytes between consecutive 8-pixel row groups of a tap view
-  int tap_aoff[UMMA_MAX_TAPS];    // byte offset of each tap's view inside the A stage
+  // the split-operand (EXACT_TC) schedule runs this plan on the tensor cores: stride 1, 1 / 4 / 9 taps, images at least
+  // 7 pixels wide, 32-byte aligned output rows (the other layers of that schedule stay on the fp32 SIMT kernels)
+  int tc_ok;
   // data gradient that is the LAST writer of its output: fuse dz = dy * (y > 0), y = activation of the same value
   const __half* mask_y; int mask_pitch, mask_coff;
   // SSNB_EXACT_TC (error-compensated split operands): nseg = 3 runs every K chunk three times,
-  //   (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi), into the same TMEM accumulator; nseg = 1 is the plain fp16 product.
+  //   (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi), into the same accumulator; nseg = 1 is the plain fp16 product.
   // out_f32: the epilogue works in fp32 -- out32 = alpha * acc (+ bias, ReLU | + old out32) -- and, when out_hi is set,
   // also writes the result's fp16 hi / lo operand planes (same pitch / channel offset, lo plane out_lo_off bytes later).
   int nseg, out_f32;
@@ -82,11 +69,6 @@ struct UmmaConvPlan {
   // SSNB_EXACT_TC mask fusion, applied only when launched with mask=true (see UmmaConvParams::mask32)
   const float* mask32 = nullptr; int mask32_pitch = 0, mask32_coff = 0;
   __half* mask_planes = nullptr; long long mask_planes_lo = 0; float mask_plane_scale = 1.0f; int* mask_flag = nullptr;
-  CUtensorMap tmap_old, tmap_y;   // experimental TMA-fed epilogue: output (old gradient) and mask-activation tiles, [128 rows][64 ch] boxes
-  bool epi_maps_ready = false, epi_mask_ready = false;
-  int epi_box[3] = {0, 0, 0}, epi_F = 0;     // box {W, F, H} extents and frame count for encoding tmap_y when the mask is attached
-  // geometry of the weight map (kept so that a variant can re-encode it with another box)
-  const __half* b_ptr = nullptr; unsigned long long b_dims[3] = {0, 0, 0}, b_strides[2] = {0, 0};
   UmmaConvParams p;
 };
 
@@ -112,10 +94,7 @@ int umma_conv_bind_fused_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View
 int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, View dz2, View dx, int F, int cin, int k1, int k2,
                                const __half* w_n_k, int accumulate, const UmmaTcOpts* tc = nullptr);
 int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask = false);
-// second-generation kernel (umma_conv_v2.cu); `p` = plan.p with the per-launch fields (mask) already applied
-bool umma_conv_v2_supported(int ntaps);
-int umma_conv_v2_launch(UmmaContext& ctx, const UmmaConvPlan& plan, const UmmaConvParams& p, cudaStream_t s);
-void umma_conv_set_mask(UmmaContext& ctx, UmmaConvPlan& plan, View y);
+void umma_conv_set_mask(UmmaConvPlan& plan, View y);
 // EXACT_TC: y32 = fp32 activation of the output value, dplanes = that value's gradient operand planes (hi base + lo_off)
 void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag);
 
@@ -124,7 +103,7 @@ int umma_resolve_encode(UmmaContext& ctx);
 int umma_encode_f16(UmmaContext& ctx, CUtensorMap* m, int rank, void* addr, const cuuint64_t* dims,
                     const cuuint64_t* strides, const cuuint32_t* box, int spatial_stride = 1);
 
-// ---- weight gradient on tcgen05 (umma_wgrad.cu) -------------------------------------------------------
+// ---- weight gradient on wgmma (umma_wgrad.cu) ---------------------------------------------------------
 // partial[split][tap][co][ci] = sum over the split's pixels of dz[p, co] * x[p + (r-pad, s-pad), ci]
 // (both operands MN-major: the reduction dimension is the pixel index).
 struct UmmaWgradParams {
@@ -136,11 +115,8 @@ struct UmmaWgradParams {
   int Cout, Cin, m_tiles, n_tiles, block_n;
   int x_stride;                   // 2: stride-2 layers, the x box steps over the input with TMA element stride 2
   float* bias_partial;            // [split][Cout] column sums of dz (bias gradient) from an extra ones-operand MMA, or nullptr
-  int taps_per_cta, tap_groups, mma_n;   // taps sharing one dz tile per CTA; N of each tap's MMA
+  int taps_per_cta, tap_groups;   // taps sharing one dz tile per CTA (taps_per_cta * block_n <= 256 accumulator columns)
   int stages, stage_bytes;        // pipeline depth / stride
-  int halo;                       // x staged as one halo box per 64 channels; taps are descriptor views (tap_xoff)
-  int run_len, run_stride;        // halo: the CTA's taps are one run of equally spaced views taken by a single MMA (N = run_len*64)
-  int x_box_bytes, x_box_tx, x_sbo, halo_x0, halo_y0, tap_xoff[UMMA_MAX_TAPS];   // box stride in smem / bytes one box delivers
   float* partial;
   int nseg;                       // 3: SSNB_EXACT_TC, every pixel tile runs (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi)
 };

@@ -1,4 +1,4 @@
-// Epilogue helpers shared by the tcgen05 convolution kernels: 256-bit global accesses and the SSNB_EXACT_TC fp32 epilogue.
+// Epilogue helpers shared by the tensor-core convolution kernels: the SSNB_EXACT_TC fp32 epilogue.
 #pragma once
 #include "umma_conv.cuh"
 #include "umma_dev.cuh"
@@ -6,27 +6,19 @@
 namespace ssnb {
 namespace umma {
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one instruction per thread per 16 fp16 columns instead of two
-// 128-bit ones -- the scattered row accesses of the epilogue are bound by LSU wavefronts, not bytes
+// 32 bytes = 8 words through two 128-bit accesses
 struct U8 { uint32_t v[8]; };
 __device__ __forceinline__ U8 ldg256(const void* p) {
-  U8 r;
-  asm volatile("ld.global.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
-               : "l"(p));
-  return r;
+  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
+  return U8{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}};
 }
 __device__ __forceinline__ U8 ldg256_nc(const void* p) {
-  U8 r;
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
-               : "l"(p));
-  return r;
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
+  return U8{{a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w}};
 }
 __device__ __forceinline__ void stg256(void* p, const U8& a) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(a.v[0]), "r"(a.v[1]), "r"(a.v[2]), "r"(a.v[3]), "r"(a.v[4]),
-               "r"(a.v[5]), "r"(a.v[6]), "r"(a.v[7])
-               : "memory");
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(a.v[0], a.v[1], a.v[2], a.v[3]);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(a.v[4], a.v[5], a.v[6], a.v[7]);
 }
 
 // SSNB_EXACT_TC epilogue: one 16-column chunk of an accumulator row in fp32 -- alpha * acc (+ bias, ReLU | + old) ->
@@ -39,7 +31,7 @@ __device__ __forceinline__ void store_chunk32(const UmmaConvParams& p, float alp
   if (p.bias) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float4 b = *reinterpret_cast<const float4*>(bias + 4 * j);
+      const float4 b = __ldg(reinterpret_cast<const float4*>(bias) + j);
       v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.z; v[4 * j + 3] += b.w;
     }
   }

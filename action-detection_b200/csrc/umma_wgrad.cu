@@ -1,11 +1,11 @@
-// tcgen05 weight-gradient kernel (sm_100a).  dW[tap][co][ci] = sum_p dz[p, co] * x[p + shift(tap), ci]
+// wgmma weight-gradient kernel (sm_90a).  dW[tap][co][ci] = sum_p dz[p, co] * x[p + shift(tap), ci]
 // is a GEMM whose reduction runs over pixels, so both operands are MN-major in shared memory:
-// a TMA box is [64 pixels][64 channels] (128-byte rows, SWIZZLE_128B) and the UMMA descriptors walk
-// it with 8-pixel groups every 1024 B (SBO) and 64-channel atoms every 8 KiB (LBO).
+// a TMA box is [64 pixels][64 channels] (128-byte rows, SWIZZLE_128B) and the wgmma descriptors walk
+// it with 8-pixel groups every 1024 B (SBO).
 //
-//   CTA = (co tile of 128, ci tile of block_n <= 256, tap, pixel split); K loop over 64-pixel boxes.
-//   warp 0: TMA producer, warp 1: MMA issuer (M=128, N=block_n, fp32 TMEM accumulator),
-//   warps 2..5: epilogue -> split-K partials (reduced in fixed order by wgrad_finalize_kernel).
+//   CTA = (co tile of 128, ci tile of block_n <= 256, taps, pixel split); K loop over 64-pixel boxes.
+//   warpgroup 0: TMA producer; warpgroups 1, 2: co rows [64 * (wg - 1), +64), one m64nNk16 wgmma per 16 pixels covering
+//   every (tap, 64 input channels) block of the CTA, fp32 accumulators in registers -> split-K partials (reduced in fixed order by wgrad_finalize_kernel).
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
@@ -21,27 +21,28 @@ using namespace umma;
 constexpr int MAX_STAGES = 8;
 constexpr int BOX_BYTES = 64 * 128;                 // [64 px][64 ch] fp16
 constexpr int A_BYTES = 2 * BOX_BYTES;              // 128 output channels
-constexpr int PIPE_BYTES = 4 * (A_BYTES + 4 * BOX_BYTES);   // 192 KiB of operand staging
-constexpr int NUM_THREADS = 192;
-constexpr int ONES_OFF = PIPE_BYTES + 1024;                // [64 px][64 ch] tile of fp16 ones (bias-gradient operand), 1 KiB aligned
-constexpr int SMEM_BYTES = PIPE_BYTES + 1024 /*align slack*/ + 1024 /*barriers*/ + BOX_BYTES;
+constexpr int STAGE_BYTES = A_BYTES + 4 * BOX_BYTES;        // 2 dz boxes + up to 4 x boxes (taps x 64-channel atoms)
+constexpr int STAGES = 4;
+constexpr int PIPE_BYTES = STAGES * STAGE_BYTES;            // 192 KiB of operand staging
+constexpr int NUM_THREADS = 384;
+constexpr int ONES_OFF = PIPE_BYTES + 1024;                // [16 rows][64 px] of fp16 ones (bias-gradient operand), 1 KiB aligned
+constexpr int ONES_BYTES = 16 * 128;
+constexpr int SMEM_BYTES = PIPE_BYTES + 1024 /*align slack*/ + 1024 /*barriers*/ + ONES_BYTES;
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
+// NACC = taps_per_cta * block_n / 64 accumulator blocks of 64 columns per consumer warpgroup
+template <int NACC>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_constant__ CUtensorMap tmap_x,
                   const __grid_constant__ CUtensorMap tmap_dz_lo, const __grid_constant__ CUtensorMap tmap_x_lo,
-                  const UmmaWgradParams p) {
+                  const __grid_constant__ UmmaWgradParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int STAGES = p.stages, STAGE_BYTES = p.stage_bytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + MAX_STAGES;
-  uint64_t* tfull_bar = bars + 2 * MAX_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 1);
 
-  // warp index through a shuffle (provably warp-uniform): the role loops below run on all 32 lanes with uniform control
-  // flow, one elected lane issues the TMA / MMA instructions (see umma_conv_v2.cu for the measurements behind this)
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x / 32), 0), lane = threadIdx.x % 32;
+  const int wg = threadIdx.x / 128;
   int id = blockIdx.x;
   const int tgrp = id % p.tap_groups; id /= p.tap_groups;
   const int nt = id % p.n_tiles; id /= p.n_tiles;
@@ -56,155 +57,113 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   const int nboxes_b = p.block_n / 64;
   // CTAs of the first input tile / tap group also reduce dz over pixels: db[co] = sum_p dz[p, co] = dz^T * 1
   const bool do_bias = p.bias_partial != nullptr && nt == 0 && tgrp == 0;
-  const int bias_col = p.taps_per_cta * p.mma_n;
-  const int acc_cols = p.taps_per_cta * p.mma_n + (p.bias_partial ? 16 : 0);
-  const uint32_t tmem_cols = acc_cols <= 32 ? 32 : (acc_cols <= 64 ? 64 : (acc_cols <= 128 ? 128 : (acc_cols <= 256 ? 256 : 512)));
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_dz)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_x)) : "memory");
-    for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(tfull_bar, 1);
+    for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   if (do_bias) {
     uint32_t* ones = reinterpret_cast<uint32_t*>(smem + ONES_OFF);
-    for (int i = threadIdx.x; i < BOX_BYTES / 4; i += NUM_THREADS) ones[i] = 0x3C003C00u;     // half2(1, 1)
+    for (int i = threadIdx.x; i < ONES_BYTES / 4; i += NUM_THREADS) ones[i] = 0x3C003C00u;     // half2(1, 1)
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the tensor core
   }
   asm volatile("griddepcontrol.wait;" ::: "memory");       // programmatic dependent launch: the prologue above overlapped the previous kernel's tail
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    const bool el = elect_one_lane();
-    uint32_t stage = 0, phase = 0;
-    const uint32_t tx_bytes = p.halo ? (uint32_t)(2 * BOX_BYTES + nboxes_b * p.x_box_tx) : (uint32_t)(2 + nboxes_b * ntap) * BOX_BYTES;
-    // pixel-tile coordinates advance by carries (no divisions in the loop)
-    int tw = pt0 % p.tiles_w, th = (pt0 / p.tiles_w) % p.tiles_h, tf = pt0 / (p.tiles_w * p.tiles_h);
-    for (int pt = pt0; pt < pt1; ++pt) {
-      const int w0 = tw * p.bw, h0 = th * p.bh, f0 = tf * p.bf;
-      // SSNB_EXACT_TC (nseg = 3): the tile is staged three times, (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi)
-      for (int seg = 3 - p.nseg; seg < 3; ++seg) {
-      const CUtensorMap* mdz = seg == 0 ? &tmap_dz_lo : &tmap_dz;
-      const CUtensorMap* mx = seg == 1 ? &tmap_x_lo : &tmap_x;
-      mbar_wait(&empty_bar[stage], phase ^ 1);
-      if (el) {
-        uint8_t* sa = smem + stage * STAGE_BYTES;
-        uint8_t* sb = sa + A_BYTES;
-        mbar_expect_tx(&full_bar[stage], tx_bytes);
-        if (p.halo) {
-          // halo layout: tensor-map dims {C, W, F, H}; ONE x box per 64 input channels covers the tile plus the filter
-          // border, every tap of this CTA is a shifted descriptor view into it
-          tma_load_4d(sa, mdz, &full_bar[stage], m0, w0, f0, h0);
-          tma_load_4d(sa + BOX_BYTES, mdz, &full_bar[stage], m0 + 64, w0, f0, h0);
-          for (int b = 0; b < nboxes_b; ++b)
-            tma_load_4d(sb + b * p.x_box_bytes, mx, &full_bar[stage], n0 + b * 64, w0 + p.halo_x0, f0, h0 + p.halo_y0);
-        } else {
+  if (wg == 0) {
+    producer_regs();
+    if (threadIdx.x == 0) {
+      uint32_t stage = 0, phase = 0;
+      const uint32_t tx_bytes = (uint32_t)(2 + nboxes_b * ntap) * BOX_BYTES;
+      // pixel-tile coordinates advance by carries (no divisions in the loop)
+      int tw = pt0 % p.tiles_w, th = (pt0 / p.tiles_w) % p.tiles_h, tf = pt0 / (p.tiles_w * p.tiles_h);
+      for (int pt = pt0; pt < pt1; ++pt) {
+        const int w0 = tw * p.bw, h0 = th * p.bh, f0 = tf * p.bf;
+        // SSNB_EXACT_TC (nseg = 3): the tile is staged three times, (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi)
+        for (int seg = 3 - p.nseg; seg < 3; ++seg) {
+          const CUtensorMap* mdz = seg == 0 ? &tmap_dz_lo : &tmap_dz;
+          const CUtensorMap* mx = seg == 1 ? &tmap_x_lo : &tmap_x;
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * STAGE_BYTES;
+          uint8_t* sb = sa + A_BYTES;
+          mbar_expect_tx(&full_bar[stage], tx_bytes);
           tma_load_4d(sa, mdz, &full_bar[stage], m0, w0, h0, f0);
           tma_load_4d(sa + BOX_BYTES, mdz, &full_bar[stage], m0 + 64, w0, h0, f0);
           for (int t = 0; t < ntap; ++t)
             for (int b = 0; b < nboxes_b; ++b)
               tma_load_4d(sb + (t * nboxes_b + b) * BOX_BYTES, mx, &full_bar[stage], n0 + b * 64,
                           w0 * p.x_stride + p.tap_dx[tap0 + t], h0 * p.x_stride + p.tap_dy[tap0 + t], f0);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tf; } }
       }
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tf; } }
     }
-  } else if (warp == 1) {
-    const bool el = elect_one_lane();
-    const uint32_t idesc = make_idesc_f16_mn(p.mma_n), idesc_bias = make_idesc_f16_mn(16), idesc_run = make_idesc_f16_mn(ntap * p.mma_n);
-    // descriptors as (lo, hi) words: hi constant (SBO 1024, version, SWIZZLE_128B), lo = address >> 4 | LBO field
-    const uint32_t hi = desc_hi_sw128(1024);
-    const uint32_t lbo = (uint32_t)((BOX_BYTES >> 4) & 0x3FFF) << 16;
-    const uint32_t base_lo = ((smem_u32(smem) >> 4) & 0x3FFF) | lbo;
-    const uint32_t ones_lo = ((smem_u32(smem + ONES_OFF) >> 4) & 0x3FFF) | lbo;
-    const uint32_t kstep_lo = (UMMA_K * 128) >> 4;                    // 16 pixel rows
-    // x operand: classic = one [64 px][64 ch] box per (tap, 64 channels); halo = views into the halo box: 8-pixel row
-    // groups x_sbo bytes apart, 64-channel atoms x_box_bytes apart
-    const uint32_t hi_x = p.halo ? desc_hi_sw128(p.x_sbo) : hi;
-    const uint32_t lbo_x = p.halo ? ((uint32_t)((p.x_box_bytes >> 4) & 0x3FFF) << 16) : lbo;
-    const uint32_t kstep_x = p.halo ? (uint32_t)(2 * p.x_sbo) >> 4 : kstep_lo;
-    uint32_t stage = 0, phase = 0;
+  } else {
+    consumer_regs();
+    const int cw = wg - 1;
+    const int warp = (threadIdx.x / 32) & 3, lane = threadIdx.x & 31;
+    const int nacc = ntap * nboxes_b;                 // accumulator blocks in use (<= NACC)
+    float acc[NACC][32], accb[8];
+#pragma unroll
+    for (int j = 0; j < NACC; ++j)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) accb[i] = 0.f;
+    const uint32_t ones = smem_u32(smem + ONES_OFF);
+    uint32_t stage = 0, phase = 0, prev = 0;
+    bool first = true;
     for (int pt = pt0; pt < pt1; ++pt)
     for (int seg = 3 - p.nseg; seg < 3; ++seg) {
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      const uint32_t sa_lo = base_lo + stage * ((uint32_t)STAGE_BYTES >> 4);
-      const uint32_t sb_lo = ((sa_lo + (A_BYTES >> 4)) & 0xFFFFu) | lbo_x;
-      if (el) {
-        const uint32_t first = (pt > pt0 || seg > 3 - p.nseg) ? 1u : 0u;
-        if (p.run_len > 1) {
-          // the taps of this CTA form ONE run whose views are `run_stride` bytes apart: a single MMA takes them as
-          // consecutive 64-channel N atoms (LBO = run_stride), so the dz tile is read once per K step instead of once
-          // per tap (the kernel is bound by those shared-memory reads)
-          const uint32_t xb_lo = (sb_lo & 0xFFFFu) + ((uint32_t)p.tap_xoff[tap0] >> 4) + (((uint32_t)p.run_stride >> 4) << 16);
+      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * BOX_BYTES;
+      const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+      // the x boxes of all taps of this CTA are consecutive 64-channel N atoms BOX_BYTES apart (the LBO), so ONE m64n(64 NACC)k16
+      // MMA per 16 pixel rows takes them all and the dz rows are read from shared memory once.  A CTA of a short last tap
+      // group (nacc < NACC) multiplies stale atoms into accumulator blocks it never stores, which keeps the MMA sequence free
+      // of predication.
+      const bool bias_mma = do_bias && seg != 1;     // column sums of dz: hi and lo planes once each (seg 1 re-stages dz_hi)
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 64 / UMMA_K; ++k)
-            umma_f16_lohi(tmem_base, sa_lo + k * kstep_lo, hi, xb_lo + k * kstep_x, hi_x, idesc_run, first | (uint32_t)k);
-        } else {
-        for (int t = 0; t < ntap; ++t) {
-          const uint32_t xb_lo = sb_lo + (p.halo ? (uint32_t)p.tap_xoff[tap0 + t] >> 4 : (uint32_t)(t * nboxes_b) * (BOX_BYTES >> 4));
+      for (int k = 0; k < 64 / MMA_K; ++k)           // 16 pixel rows (2 groups of 8) per instruction
+        wgmma<NACC * MMA_N, 1, 1>(&acc[0][0], make_desc_sw128(sa + k * (MMA_K * 128), BOX_BYTES), make_desc_sw128(sb + k * (MMA_K * 128), BOX_BYTES));
+      if (bias_mma) {                                // the ones operand is K-major
 #pragma unroll
-          for (int k = 0; k < 64 / UMMA_K; ++k)      // 16 pixel rows (2 groups of 8) per instruction
-            umma_f16_lohi(tmem_base + t * p.mma_n, sa_lo + k * kstep_lo, hi, xb_lo + k * kstep_x, hi_x, idesc, first | (uint32_t)k);
-        }
-        }
-        if (do_bias && seg != 1) {          // column sums of dz: hi and lo planes once each (seg 1 re-stages dz_hi against x_lo)
-#pragma unroll
-          for (int k = 0; k < 64 / UMMA_K; ++k)
-            umma_f16_lohi(tmem_base + bias_col, sa_lo + k * kstep_lo, hi, ones_lo + k * kstep_lo, hi, idesc_bias, first | (uint32_t)k);
-        }
-        umma_commit(&empty_bar[stage]);
+        for (int k = 0; k < 64 / MMA_K; ++k)
+          wgmma<16, 1, 0>(accb, make_desc_sw128(sa + k * (MMA_K * 128), BOX_BYTES), make_desc_sw128(ones + k * MMA_K * 2));
       }
+      wgmma_commit();
+      // one group stays in flight: the previous stage's MMAs have retired, its smem slot goes back to the producer
+      wgmma_wait<1>();
+      if (!first && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      first = false;
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
-    if (el) umma_commit(tfull_bar);
-    __syncwarp();
-  } else {
-    const int quad = warp & 3;
-    const int m = m0 + quad * 32 + lane;            // output channel of this thread's accumulator row
-    mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-    for (int t = 0; t < ntap; ++t) {
-      float* orow = p.partial + (((long long)split * p.ntaps + tap0 + t) * p.Cout + m) * p.Cin + n0;
-      for (int c0 = 0; c0 < p.mma_n; c0 += 16) {
-        uint32_t r[16];
-        tmem_ld16(taddr + t * p.mma_n + c0, r);
-        tmem_ld_wait();
-        if (m < p.Cout) {
+    wgmma_wait<0>();
+    if (!first && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+    // fragments straight to the partials: register i of this thread is row 16 warp + lane/4 + 8 ((i/2)%2), column
+    // 8 (i/4) + 2 (lane%4) + i%2 of its 64 x 64 block
+    const int mrow = m0 + cw * 64 + warp * 16 + (lane >> 2);
 #pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            if (n0 + c0 + j < p.Cin)      // Cin is a multiple of 4
-              *reinterpret_cast<float4*>(orow + c0 + j) = make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                                      __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-          }
-        }
+    for (int j = 0; j < NACC; ++j) {
+      if (j >= nacc) break;
+      const int t = j / nboxes_b, b = j % nboxes_b;
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int m = mrow + 8 * ((i >> 1) & 1);
+        const int c = n0 + b * 64 + 8 * (i >> 2) + 2 * (lane & 3);
+        if (m < p.Cout && c < p.Cin)      // Cin is a multiple of 8
+          *reinterpret_cast<float2*>(p.partial + (((long long)split * p.ntaps + tap0 + t) * p.Cout + m) * p.Cin + c) = make_float2(acc[j][i], acc[j][i + 1]);
       }
     }
-    if (do_bias) {
-      uint32_t r[16];
-      tmem_ld16(taddr + bias_col, r);
-      tmem_ld_wait();
-      if (m < p.Cout) p.bias_partial[(long long)split * p.Cout + m] = __uint_as_float(r[0]);
+    if (do_bias && (lane & 3) == 0) {
+      if (mrow < p.Cout) p.bias_partial[(long long)split * p.Cout + mrow] = accb[0];
+      if (mrow + 8 < p.Cout) p.bias_partial[(long long)split * p.Cout + mrow + 8] = accb[2];
     }
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
   }
 }
 
@@ -242,75 +201,18 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   const int chunks = (cin + 63) / 64;
   p.n_tiles = (chunks + 3) / 4;
   p.block_n = ((chunks + p.n_tiles - 1) / p.n_tiles) * 64;
-  // several taps per CTA share one dz tile: stage = 2 dz boxes + taps * (block_n/64) x boxes <= 6 boxes, and
-  // the accumulators (taps * mma_n fp32 columns) must fit the 512 TMEM columns
-  p.mma_n = p.block_n;
-  if (p.n_tiles == 1 && cin < p.block_n) p.mma_n = (cin + 15) / 16 * 16;     // narrow inputs (conv1 space-to-depth: 16)
-  // halo variant (stride-1 multi-tap layers): ONE x box per 64 input channels covers the 64-pixel tile plus the filter
-  // border ([y][frame][x] pixel order, as in umma_conv_v2.cu) and every tap is a shifted descriptor view into it.
-  // Default: only where a whole ROW of taps can then be taken by a single MMA -- 64-channel layers, whose tap views are
-  // equally spaced, so they are consecutive 64-channel N atoms with LBO = the tap spacing (128 B for a 3x3 row, 1 KiB
-  // for conv1's four vertical taps).  That reads the 4 KiB dz tile once per K step instead of once per tap, which is
-  // what bounds this kernel (shared-memory bandwidth): conv2_3x3 283 -> 163 us, conv1 254 -> 148 us.  Without the
-  // fusion the halo layout is SLOWER than per-tap boxes (more taps per CTA, same dz re-reads: 3.7 vs 2.9 ms over the
-  // 69 layers), so wider layers keep the classic layout.  SSNB_WGRAD_HALO=0 off, 1 halo everywhere without fusion,
-  // 2 halo everywhere + fusion where possible.
-  int x0 = 0, x1 = 0, y0 = 0, y1 = 0;
-  for (int t = 0; t < ntaps; ++t) { x0 = std::min(x0, tdx[t]); x1 = std::max(x1, tdx[t]); y0 = std::min(y0, tdy[t]); y1 = std::max(y1, tdy[t]); }
-  const char* he = getenv("SSNB_WGRAD_HALO");
-  const int hmode = he ? atoi(he) : 3;                  // 3 = default: halo only with run fusion
-  bool halo = hmode != 0 && x_stride == 1 && ntaps > 1 && dz.W >= 7;
-  int run_len = 1, run_stride = 0;
-  if (halo && hmode >= 2 && p.block_n == 64 && p.mma_n == 64) {
-    const int pw0 = 8 + (x1 - x0);
-    int hb = 8; while (hb > 1 && dz.H % hb) hb >>= 1;
-    const int hf = 64 / (8 * hb);
-    auto off = [&](int t) { return ((tdy[t] - y0) * hf * pw0 + (tdx[t] - x0)) * 128; };
-    for (int r = 4; r >= 2; --r) {                      // longest run length (N = r*64 <= 256) that tiles the tap list evenly
-      if (ntaps % r) continue;
-      bool ok = true;
-      const int st = off(1) - off(0);
-      for (int g = 0; g < ntaps / r && ok; ++g)
-        for (int i = 1; i < r && ok; ++i) ok = off(g * r + i) - off(g * r + i - 1) == st;
-      if (ok && st > 0 && st % 16 == 0) { run_len = r; run_stride = st; break; }
-    }
-  }
-  if (hmode == 3 && run_len == 1) halo = false;
-  int hbw = 8, hbh = 8, hbf = 1, pw = 8, x_box = 0, h_taps = 1, h_stages = 0;
-  if (halo) {
-    while (hbh > 1 && dz.H % hbh) hbh >>= 1;
-    hbf = 64 / (hbw * hbh);
-    pw = hbw + (x1 - x0);
-    x_box = (pw * hbf * (hbh + (y1 - y0)) * 128 + 1023) / 1024 * 1024;
-    h_taps = run_len > 1 ? run_len : std::min(ntaps, (512 - 16) / p.mma_n);
-    h_stages = std::min(MAX_STAGES, PIPE_BYTES / (A_BYTES + (p.block_n / 64) * x_box));
-    if (h_taps < 2 || h_stages < 3) halo = false;
-  }
-  p.halo = halo ? 1 : 0;
-  p.run_len = halo ? run_len : 1; p.run_stride = run_stride;
-  if (halo) {
-    p.bw = hbw; p.bh = hbh; p.bf = hbf;
-    p.tiles_w = (dz.W + hbw - 1) / hbw; p.tiles_h = dz.H / hbh; p.tiles_f = (F + hbf - 1) / hbf;
-    p.taps_per_cta = h_taps;
-    p.x_box_bytes = x_box; p.x_box_tx = pw * hbf * (hbh + (y1 - y0)) * 128; p.x_sbo = pw * 128; p.halo_x0 = x0; p.halo_y0 = y0;
-    p.stage_bytes = A_BYTES + (p.block_n / 64) * x_box; p.stages = h_stages;
-    for (int t = 0; t < ntaps; ++t) p.tap_xoff[t] = ((tdy[t] - y0) * hbf * pw + (tdx[t] - x0)) * 128;
-  } else {
-    p.stage_bytes = A_BYTES + 4 * BOX_BYTES; p.stages = 4;
-    // several taps per CTA share one dz tile: stage = 2 dz boxes + taps * (block_n/64) x boxes <= 6 boxes, and
-    // the accumulators (taps * mma_n fp32 columns) must fit the 512 TMEM columns
-    p.taps_per_cta = 4 / (p.block_n / 64);
-    if (p.taps_per_cta < 1) p.taps_per_cta = 1;
-    while (p.taps_per_cta > 1 && p.taps_per_cta * p.mma_n > 512) --p.taps_per_cta;
-    if (p.taps_per_cta > ntaps) p.taps_per_cta = ntaps;
-  }
+  // several taps per CTA share one dz tile: stage = 2 dz boxes + taps * (block_n/64) x boxes <= 6 boxes, which also
+  // bounds the register accumulators at 256 fp32 columns
+  p.stage_bytes = STAGE_BYTES; p.stages = STAGES;
+  p.taps_per_cta = std::max(1, 4 / (p.block_n / 64));
+  if (p.taps_per_cta > ntaps) p.taps_per_cta = ntaps;
   p.tap_groups = (ntaps + p.taps_per_cta - 1) / p.taps_per_cta;
   p.taps_per_cta = (ntaps + p.tap_groups - 1) / p.tap_groups;        // balance the groups (9 taps: 3+3+3 rather than 4+4+1)
   const int ptiles = p.tiles_w * p.tiles_h * p.tiles_f;
   const int ctas = p.m_tiles * p.n_tiles * p.tap_groups;
   // one CTA per SM is resident (192 KiB pipeline), so a second wave only runs after the first: ONE wave of CTAs with
   // twice the pixels each does the same work with half the split-K partial traffic (every CTA writes its whole
-  // 128 x taps*N fp32 accumulator: 100-250 KB) and no wave tail (conv2_3x3 used to run 300 CTAs = three waves)
+  // 128 x taps*N fp32 accumulator: 100-250 KB) and no wave tail
   const char* we = getenv("SSNB_WGRAD_WAVES");
   int splits = ((we ? atoi(we) : 1) * ctx.num_sms) / ctas;
   if (splits < 1) splits = 1;
@@ -323,23 +225,6 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   p.nseg = (dz.lo_off && x.lo_off) ? 3 : 1;
   if ((dz.lo_off != 0) != (x.lo_off != 0)) { set_thread_error("umma wgrad: both operands or neither must carry LO planes"); return 1; }
   auto lo_ptr = [](const View& v) { return reinterpret_cast<__half*>(reinterpret_cast<char*>(v.base) + v.lo_off) + v.coff; };
-  if (halo) {
-    cuuint64_t dims[4] = {(cuuint64_t)cout, (cuuint64_t)dz.W, (cuuint64_t)F, (cuuint64_t)dz.H};
-    cuuint64_t str[3] = {(cuuint64_t)dz.pitch * 2, (cuuint64_t)dz.H * dz.W * dz.pitch * 2, (cuuint64_t)dz.W * dz.pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)p.bw, (cuuint32_t)p.bf, (cuuint32_t)p.bh};
-    if (int rc = umma_encode_f16(ctx, &plan.tmap_dz, 4, reinterpret_cast<__half*>(dz.base) + dz.coff, dims, str, box)) return rc;
-    cuuint64_t xd[4] = {(cuuint64_t)cin, (cuuint64_t)x.W, (cuuint64_t)F, (cuuint64_t)x.H};
-    cuuint64_t xs[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.H * x.W * x.pitch * 2, (cuuint64_t)x.W * x.pitch * 2};
-    cuuint32_t xb[4] = {64, (cuuint32_t)pw, (cuuint32_t)p.bf, (cuuint32_t)(p.bh + (y1 - y0))};
-    if (int rc = umma_encode_f16(ctx, &plan.tmap_x, 4, reinterpret_cast<__half*>(x.base) + x.coff, xd, xs, xb)) return rc;
-    plan.tmap_dz_lo = plan.tmap_dz; plan.tmap_x_lo = plan.tmap_x;
-    if (p.nseg == 3) {
-      if (int rc = umma_encode_f16(ctx, &plan.tmap_dz_lo, 4, lo_ptr(dz), dims, str, box)) return rc;
-      if (int rc = umma_encode_f16(ctx, &plan.tmap_x_lo, 4, lo_ptr(x), xd, xs, xb)) return rc;
-    }
-    plan.enabled = true;
-    return 0;
-  }
   {
     cuuint64_t dims[4] = {(cuuint64_t)cout, (cuuint64_t)dz.W, (cuuint64_t)dz.H, (cuuint64_t)F};
     cuuint64_t str[3] = {(cuuint64_t)dz.pitch * 2, (cuuint64_t)dz.W * dz.pitch * 2, (cuuint64_t)dz.H * dz.W * dz.pitch * 2};
@@ -360,18 +245,18 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   return 0;
 }
 
-int umma_wgrad_launch(UmmaContext& ctx, const UmmaWgradPlan& plan, cudaStream_t s, float* bias_partial) {
-  if (!plan.enabled) { set_thread_error("umma wgrad: plan not bound"); return 3; }
+namespace {
+template <int NACC>
+int launch_nacc(const UmmaWgradPlan& plan, const UmmaWgradParams& p, cudaStream_t s) {
   static bool attr_set[64] = {};          // function attributes are per device
+  auto kern = umma_wgrad_kernel<NACC>;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-    if (cudaFuncSetAttribute(umma_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) {
       set_thread_error("umma wgrad: cannot raise dynamic shared memory limit"); cudaGetLastError(); return 2; }
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  UmmaWgradParams p = plan.p;
-  p.bias_partial = bias_partial;
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   cfg.gridDim = dim3((unsigned)(p.m_tiles * p.n_tiles * p.tap_groups), (unsigned)p.splits);
@@ -380,10 +265,24 @@ int umma_wgrad_launch(UmmaContext& ctx, const UmmaWgradPlan& plan, cudaStream_t 
   cfg.stream = s;
   static const bool pdl = [] { const char* e = getenv("SSNB_PDL"); return !(e && e[0] == '0'); }();
   if (pdl) { attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization; attr[0].val.programmaticStreamSerializationAllowed = 1; cfg.attrs = attr; cfg.numAttrs = 1; }
-  if (cudaLaunchKernelEx(&cfg, umma_wgrad_kernel, plan.tmap_dz, plan.tmap_x, plan.tmap_dz_lo, plan.tmap_x_lo, p) != cudaSuccess) {
+  if (cudaLaunchKernelEx(&cfg, kern, plan.tmap_dz, plan.tmap_x, plan.tmap_dz_lo, plan.tmap_x_lo, p) != cudaSuccess) {
     set_thread_error(std::string("umma_wgrad_kernel launch: ") + cudaGetErrorString(cudaGetLastError())); return 2; }
   SSNB_LAUNCH_CHECK("umma_wgrad_kernel");
   return 0;
+}
+}  // namespace
+
+int umma_wgrad_launch(UmmaContext&, const UmmaWgradPlan& plan, cudaStream_t s, float* bias_partial) {
+  if (!plan.enabled) { set_thread_error("umma wgrad: plan not bound"); return 3; }
+  UmmaWgradParams p = plan.p;
+  p.bias_partial = bias_partial;
+  switch (p.taps_per_cta * (p.block_n / 64)) {
+    case 1: return launch_nacc<1>(plan, p, s);
+    case 2: return launch_nacc<2>(plan, p, s);
+    case 3: return launch_nacc<3>(plan, p, s);
+    case 4: return launch_nacc<4>(plan, p, s);
+  }
+  set_thread_error("umma wgrad: unsupported tile width"); return 3;
 }
 
 }  // namespace ssnb

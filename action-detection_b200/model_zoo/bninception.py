@@ -31,8 +31,8 @@ class BNInception(nn.Module):
 
     # ---- engine management --------------------------------------------------------------------
     def set_precision(self, precision, grad_scale=None):
-        """precision: ssn_b200.EXACT_FP32 (fp32 SIMT), ssn_b200.FAST_FP16 (tcgen05, fp16 operands) or
-        ssn_b200.EXACT_TC (tcgen05, error-compensated split fp16 operands: fp32-grade results)."""
+        """precision: ssn_b200.EXACT_FP32 (fp32 SIMT), ssn_b200.FAST_FP16 (wgmma, fp16 operands) or
+        ssn_b200.EXACT_TC (wgmma, error-compensated split fp16 operands: fp32-grade results)."""
         if precision == _lib.FAST_FP16 and grad_scale is None and self.grad_scale == 1.0:
             raise ValueError("FAST_FP16 stores gradients in fp16: pass an explicit power-of-two grad_scale (e.g. 4096) so small "
                              "gradients do not underflow, and poll engine.grad_overflow() to catch overflow")
@@ -95,7 +95,7 @@ class BNInception(nn.Module):
 
     def forward(self, input):
         if not input.is_cuda:
-            raise RuntimeError("BNInception(B200) runs on CUDA only: move the model and input to the GPU "
+            raise RuntimeError("BNInception(H100) runs on CUDA only: move the model and input to the GPU "
                                "(libssn_b200 has no CPU path)")
         bn1_train = self.bn1_training()
         cs = self._convs()

@@ -1,5 +1,5 @@
 """Drop-in for the reference's ops/ssn_ops.py: same class names, constructor arguments, call
-conventions and error behaviour; the arithmetic runs in libssn_b200.so (CUDA, sm_100a).
+conventions and error behaviour; the arithmetic runs in libssn_b200.so (CUDA, sm_90a).
 
 Reference: ops/ssn_ops.py — Identity :8-10, parse_stage_config :13-19,
 StructuredTemporalPyramidPooling :22-79, STPPReorgainzed :82-170, OHEMHingeLoss :173-213,

@@ -1,4 +1,4 @@
-"""ssn_b200 — host package of the B200-native SSN hot path (see DESIGN.md).
+"""ssn_b200 — host package of the H100-native SSN hot path (see DESIGN.md).
 
 Importing this package loads libssn_b200.so; it raises ImportError if the CUDA extension has not
 been built (there is deliberately no fallback path)."""

@@ -202,7 +202,7 @@ class BackboneFunction(torch.autograd.Function):
         eng, n = ctx.engine, ctx.n_conv
         dev = dfeat.device
         if ctx.generation != eng.generation:
-            raise RuntimeError("BNInception(B200): another forward of %d frames ran through this engine after the one being "
+            raise RuntimeError("BNInception(H100): another forward of %d frames ran through this engine after the one being "
                                "differentiated; its saved activations are gone.  Run backward before the next forward of the same "
                                "shape (or use different frame counts / a second model instance)." % eng.frames)
         bn1 = getattr(ctx, "bn1", None)

@@ -46,7 +46,7 @@ class SSN(torch.nn.Module):
         else:
             self.new_length = new_length
         if verbose:
-            print("Initializing SSN (B200) base model {} modality {} segments {}+{}+{} dropout {} stpp {} bn {}".format(
+            print("Initializing SSN (H100) base model {} modality {} segments {}+{}+{} dropout {} stpp {} bn {}".format(
                 base_model, modality, starting_segment, course_segment, ending_segment, dropout, stpp_cfg, bn_mode))
         self._prepare_base_model(base_model)
         self._prepare_ssn(num_class, stpp_cfg)
@@ -55,7 +55,7 @@ class SSN(torch.nn.Module):
     # ---- construction (ssn_models.py:69-154) ------------------------------------------------------
     def _prepare_base_model(self, base_model):
         if base_model != 'BNInception':
-            raise ValueError('Unknown base model: {} (the B200 hot path implements BNInception)'.format(base_model))
+            raise ValueError('Unknown base model: {} (the H100 hot path implements BNInception)'.format(base_model))
         if self.modality == 'RGB':
             in_ch = 3 * self.new_length
         elif self.modality == 'Flow':
@@ -267,7 +267,7 @@ class SSN(torch.nn.Module):
         from ssn_b200.engine import _stream
         assert self.with_regression, "fused_step implements the regression configuration"
         if not input.is_cuda:
-            raise RuntimeError("SSN(B200).fused_step needs CUDA tensors (libssn_b200 has no CPU path)")
+            raise RuntimeError("SSN(H100).fused_step needs CUDA tensors (libssn_b200 has no CPU path)")
         if self.base_model.bn1_training():
             raise NotImplementedError("fused_step implements bn_mode='frozen'; with bn_mode='partial' use the module path "
                                       "(model(...), criteria, loss.backward()), which runs the first BatchNorm2d in training mode")
@@ -349,7 +349,7 @@ class SSN(torch.nn.Module):
             from transforms import GroupMultiScaleCrop, GroupRandomHorizontalFlip
         except ImportError as e:
             raise NotImplementedError("get_augmentation needs the reference's transforms.py on sys.path "
-                                      "(data pipeline is out of scope for the B200 hot path)") from e
+                                      "(data pipeline is out of scope for the H100 hot path)") from e
         scales = [1, .875, .75, .66] if self.modality == 'RGB' else [1, .875, .75]
         return torchvision.transforms.Compose([GroupMultiScaleCrop(self.input_size, scales),
                                                GroupRandomHorizontalFlip(is_flow=(self.modality == 'Flow'))])

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — SSN forward/backward hot path on B200 (see DESIGN.md section 5).
+"""bench.py — SSN forward/backward hot path on H100 (see DESIGN.md section 5).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                   [--precision exact_tc|fast|exact] [--modality RGB|Flow] [--classes K] [--videos-per-gpu V]
@@ -14,7 +14,7 @@ SGD step -> weight re-pack.  The other BASELINE configs are reachable through fl
   configs[3]  --classes 200 --videos-per-gpu 8     (ActivityNet-shape heads, 64 proposals per GPU; 1 video/GPU = global 64 on 8)
   configs[4]  --mode infer                         (ssn_test.py path: 10-crop forward of a 1000-tick video + test_fc + STPP
                                                     re-organisation of 1000 proposals, forward only)
-The headline precision is exact_tc (split-operand tcgen05, meets the 1e-3 parity tolerance end to end); the fp16-operand
+The headline precision is exact_tc (split-operand wgmma, meets the 1e-3 parity tolerance end to end); the fp16-operand
 `fast` mode (parity partial: 9e-3 at the backbone output) is measured beside it in the same run and reported under
 `modes`.  Prints ONE JSON line (rank 0).
 """
@@ -47,7 +47,15 @@ def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- upper bounds, not measured rates
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "datasheet"
+
+
+def peak_label(peak_src, measured_what):
+    """what `peak` is: the measured figure, or the data-sheet bound standing in for it"""
+    if peak_src == "measured":
+        return "measured " + measured_what
+    return "H100 SXM data-sheet bf16 dense 989 TFLOP/s (an upper bound, not measured; used for both sustained and burst)"
 
 
 class ClockSampler:
@@ -158,16 +166,14 @@ def metric_name(args):
 
 # ---- reference arm: the UNMODIFIED reference on the host CPU cores ------------------------------------------
 def run_reference(args):
-    """`--impl reference`: the reference's own CPU PyTorch implementation of the same step (baseline/_ref = a copy of the
+    """`--impl reference`: the reference's own CPU PyTorch implementation of the same step (oracle/_ref = a copy of the
     reference's files made by __graft_entry__.build(); the oracle port only if that copy is missing), all host threads,
     same configuration as our arm.  Rank 0 alone works."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
     import torch
-    from oracle import synth, ssn_oracle as O
-    sys.path.insert(0, os.path.join(ROOT, "baseline"))
-    import ref_harness
+    from oracle import synth, ssn_oracle as O, ref_harness
     cores = usable_cores()
     torch.set_num_threads(cores)
     in_ch, K = IN_CH[args.modality], args.classes
@@ -246,7 +252,7 @@ def run_reference(args):
     value = units / mean
     cfg = config_dict(args, world=args.gpus)
     cfg.update({"precision": "f32 CPU", "note": "reference CPU PyTorch path (%s), rank 0 only, %d host threads" % (
-        "unmodified reference files from baseline/_ref" if kind == "reference" else "oracle restatement", cores)})
+        "unmodified reference files from oracle/_ref" if kind == "reference" else "oracle restatement", cores)})
     line = {"impl": "reference", "metric": metric_name(args), "value": value, "unit": "proposals/s", "n_gpus": args.gpus,
             "steps": len(times), "warmup": done_w, "steps_requested": args.steps, "ms_per_step": mean * 1e3,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -254,6 +260,27 @@ def run_reference(args):
             "cpu_baseline": {"value": value, "unit": "proposals/s", "cores": cores, "kind": kind, "sample": sample},
             "e2e": {"value": value, "unit": "proposals/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
+
+
+DUMP_MAX_ELEMS = 4 << 20      # per array: 16 MiB of float32; larger arrays are sampled
+
+
+def dump_outputs(dirname, arrays):
+    """--dump-outputs DIR: what the timed path computed in its last step, one DIR/<name>.npy per array (float32; float64
+    stays float64).  An array of more than DUMP_MAX_ELEMS values is replaced by a fixed sample of its flattened values:
+    DUMP_MAX_ELEMS sorted indices drawn by torch.randint from a CPU generator seeded with 0 -- the same indices in every run
+    of the same configuration, so two builds can be compared output for output."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().reshape(-1)
+        if t.numel() > DUMP_MAX_ELEMS:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.sort(torch.randint(0, t.numel(), (DUMP_MAX_ELEMS,), generator=g))[0]
+            t = t[idx.to(t.device)]
+        t = t.cpu()
+        np.save(os.path.join(dirname, name + ".npy"), t.numpy().astype(np.float64 if t.dtype == torch.float64 else np.float32))
 
 
 def config_dict(args, world):
@@ -295,6 +322,8 @@ def main():
     ap.add_argument("--no-second-mode", action="store_true", help="skip the side measurement of the other tensor-core mode")
     ap.add_argument("--grad-scale", type=float, default=4096.0)
     ap.add_argument("--no-graph", action="store_true", help="do not capture the training step in a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last timed step's outputs as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -320,8 +349,8 @@ def main():
         dist.init_process_group("nccl", device_id=dev, timeout=datetime.timedelta(seconds=int(os.environ.get("SSNB_NCCL_TIMEOUT_S", "240"))))
 
     PREC = {"fast": _lib.FAST_FP16, "exact": _lib.EXACT_FP32, "exact_tc": _lib.EXACT_TC}
-    DTYPE = {"fast": "f16 operands / f32 accumulate (tcgen05 kind::f16); parity partial",
-             "exact_tc": "f32 via split f16 operands (hi+lo, 3 tcgen05 MMAs per product) / f32 accumulate; f32 storage",
+    DTYPE = {"fast": "f16 operands / f32 accumulate (wgmma f32.f16.f16); parity partial",
+             "exact_tc": "f32 via split f16 operands (hi+lo, 3 wgmma MMAs per product) / f32 accumulate; f32 storage",
              "exact": "f32 (SIMT FMA)"}
     in_ch, K = IN_CH[args.modality], args.classes
     bb = synth.synth_backbone(in_ch, seed=0, calib_frames=2)
@@ -413,7 +442,7 @@ def main():
             return static_losses
         return graph_step
 
-    def measure_train(precision, steps, warmup, batches):
+    def measure_train(precision, steps, warmup, batches, dump=None):
         model, flat_grad, opt, eager_step = build_train(precision)
         step, used_graph = eager_step, False
         if not args.no_graph:
@@ -425,6 +454,10 @@ def main():
                 torch.cuda.synchronize()
                 step, used_graph = eager_step, False
         ms_total, clocks, losses = timed_loop(step, batches, steps, warmup)
+        if dump:
+            # the last timed step's losses, the gradient it reduced into the flat buffer and the parameters its SGD update
+            # produced (before the launch count below runs another step)
+            dump_outputs(dump, {"losses": losses, "flat_grad": flat_grad, "flat_param": opt.flat_param})
         launches = count_launches(lambda: eager_step(batches[0])) * steps     # graph replays bypass the library's counter
         props_step = args.videos_per_gpu * PROPS * world
         res = {"value": props_step * steps / (ms_total / 1e3), "ms_per_step": ms_total / steps, "clocks": clocks,
@@ -435,7 +468,8 @@ def main():
         nb = 2   # distinct device-resident batches, alternated
         batches = [tuple(t.to(dev) for t in synth.synth_batch(args.videos_per_gpu, K, in_ch, seed=100 * rank + i)) for i in range(nb)]
         host_batches = [tuple(t.pin_memory() for t in synth.synth_batch(args.videos_per_gpu, K, in_ch, seed=100 * rank + i)) for i in range(nb)]
-        main, model, flat_grad, opt, eager_step = measure_train(args.precision, args.steps, args.warmup, batches)
+        main, model, flat_grad, opt, eager_step = measure_train(args.precision, args.steps, args.warmup, batches,
+                                                                dump=args.dump_outputs if rank == 0 else None)
         props_step = args.videos_per_gpu * PROPS * world
         frames_gpu = args.videos_per_gpu * PROPS * SEG
 
@@ -559,17 +593,17 @@ def main():
 
 
 def roofline_from_rows(rows, n_steps, precision, peaks, peak_src, frames, modality):
-    """dominant kernel = the tcgen05 convolution kernel (forward + data gradient, every launch of the step); second entry =
+    """dominant kernel = the wgmma convolution kernel (forward + data gradient, every launch of the step); second entry =
     the weight-gradient kernel.  achieved = sum(algorithmic FLOPs) / sum(launch time) over ALL launches of the kernel."""
-    conv_names = ("umma_conv_v2_kernel", "umma_conv_kernel") if precision != "exact" else ("conv_kernel",)
+    conv_names = ("umma_conv_kernel",) if precision != "exact" else ("conv_kernel",)
     wg_names = ("umma_wgrad_kernel",) if precision != "exact" else ("wgrad_kernel",)
 
     def agg(names, phases):
         sel = [r for r in rows if r["kernel"] in names and r["phase"] in phases]
         return (sum(r["flop"] for r in sel) / n_steps, sum(r["ms"] for r in sel) / n_steps, sum(r["launches"] for r in sel) // n_steps)
     step_ms = sum(r["ms"] for r in rows) / n_steps
-    sustained = float(peaks.get("bf16_tflops_sustained", 1400.0))
-    burst = float(peaks.get("bf16_tflops", 1590.0))
+    sustained = float(peaks.get("bf16_tflops_sustained", 989.0))
+    burst = float(peaks.get("bf16_tflops", 989.0))
     mma_per_product = 3 if precision == "exact_tc" else 1
 
     def entry(names, phases):
@@ -585,18 +619,12 @@ def roofline_from_rows(rows, n_steps, precision, peaks, peak_src, frames, modali
         k = "%s:%s" % (r["kernel"], ("fwd", "dgrad", "wgrad", "other")[r["phase"]])
         per_kernel[k] = {"launches": r["launches"] // n_steps, "ms": r["ms"] / n_steps}
     top = dict(sorted(per_kernel.items(), key=lambda kv: -kv[1]["ms"])[:14])
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))
-        tr = traffic.get("umma_conv_v2_kernel:conv2_3x3_fwd:%s" % precision, traffic.get("umma_conv_v2_kernel:conv2_3x3_fwd", {})).get("dram_bytes")
-    except Exception:
-        tr = None
     return {"bound": "tensor", "kernel": "%s (forward + data gradient, all %d launches of a step)" % (conv_names[0], dom["launches_per_step"]),
-            "achieved": dom["achieved"], "peak": sustained, "unit": "TFLOP/s", "frac": dom["frac"], "traffic": tr,
+            "achieved": dom["achieved"], "peak": sustained, "unit": "TFLOP/s", "frac": dom["frac"], "traffic": None,
             "tensor_pipe_frac": dom["tensor_pipe_tflops"] / sustained, "mma_per_algorithmic_product": mma_per_product,
-            "traffic_unit": "bytes per launch of the largest forward launch (conv2_3x3), ncu --set full dram read+write, profiles/",
-            "peak_source": peak_src + " bf16 sustained (kernels timed inside a long step); frac_of_burst uses the burst figure",
+            "peak_source": peak_label(peak_src, "bf16 sustained (kernels timed inside a long step); frac_of_burst uses the burst figure"),
             "note": "algorithmic fp32-conv FLOPs (2*F*H*W*Cout*Cin*k*k) / summed per-launch CUDA-event time of two eager steps; "
-                    "exact_tc issues 3 tcgen05 MMAs per algorithmic product, tensor_pipe_tflops = achieved x 3",
+                    "exact_tc issues 3 wgmma MMAs per algorithmic product, tensor_pipe_tflops = achieved x 3",
             "dominant": dom, "forward": entry(conv_names, (0,)), "dgrad": entry(conv_names, (1,)), "wgrad": entry(wg_names, (2,)),
             "forward_pass_all_kernels": {"ms": fwd_all_ms, "achieved": fwd_flop / (fwd_all_ms / 1e3) / 1e12 if fwd_all_ms else None,
                                          "frac": fwd_flop / (fwd_all_ms / 1e3) / 1e12 / sustained if fwd_all_ms else None,
@@ -613,7 +641,7 @@ def stpp_bandwidth(torch, _lib, dev, l2_flush, peaks):
     try:
         import ctypes as C
         import ssn_models
-        hbm = float(peaks.get("hbm_gbs", 6650.0))
+        hbm = float(peaks.get("hbm_gbs", 3350.0))
         stpp = ssn_models.SSN(20, 2, 5, 2, "RGB", base_model="BNInception", dropout=0, stpp_cfg=STPP_CFG).stpp
         lo, hi, nm, col = stpp.part_table([2, 7, 9])
         tab = [_lib.int_array(v) for v in (lo, hi, nm, col)]
@@ -656,7 +684,7 @@ def fused_gpool_stpp_bw(torch, _lib, model, frames, precision, l2_flush, peaks):
     try:
         import ctypes as C
         dev = l2_flush.device
-        hbm = float(peaks.get("hbm_gbs", 6650.0))
+        hbm = float(peaks.get("hbm_gbs", 3350.0))
         eng = model.base_model.engine_for(frames, True, dev)
         n_prop = frames // SEG
         lo, hi, nm, col = model.stpp.part_table([2, 7, 9])
@@ -737,7 +765,9 @@ def run_infer(args, torch, dist, ssn_models, _lib, synth, dev, rank, world, loca
             return reorg.forward(out, ticks, scaling)
 
     model, reorg = build(args.precision)
-    ms_total, clocks, _ = timed_loop(lambda b: step_on(model, reorg, b), [video_dev], args.steps, args.warmup)
+    ms_total, clocks, last = timed_loop(lambda b: step_on(model, reorg, b), [video_dev], args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(zip(("activity", "completeness", "regression"), last)))
     launches = count_launches(lambda: step_on(model, reorg, video_dev)) * args.steps
     value = N * world * args.steps / (ms_total / 1e3)
     frames_s = T * crops * world * args.steps / (ms_total / 1e3)
@@ -780,7 +810,7 @@ def run_infer(args, torch, dist, ssn_models, _lib, synth, dev, rank, world, loca
     barrier()
     e2e_value = N * world * e2e_steps / (max_over_ranks(e0.elapsed_time(e1)) / 1e3)
     fwd_flop = 2.0 * MAC_FWD[args.modality] * T * crops
-    sustained = float(peaks.get("bf16_tflops_sustained", 1400.0))
+    sustained = float(peaks.get("bf16_tflops_sustained", 989.0))
     achieved = fwd_flop / (ms_total / args.steps / 1e3) / 1e12
     cpu = cpu_baseline_subprocess(args) if (rank == 0 and world == 1 and not args.no_cpu_baseline) else None
     if rank == 0:
@@ -795,7 +825,7 @@ def run_infer(args, torch, dist, ssn_models, _lib, synth, dev, rank, world, loca
                         "steps": e2e_steps, "path": "SSN.test_scores per chunk from a pinned host video (H2D double-buffered on a copy stream) + "
                                                     "STPPReorgainzed.forward + .cpu() of the three score tensors"},
                 "roofline": {"bound": "tensor", "kernel": "whole forward step (all kernels)", "achieved": achieved, "peak": sustained, "unit": "TFLOP/s",
-                             "frac": achieved / sustained, "traffic": None, "peak_source": peak_src + " bf16 sustained",
+                             "frac": achieved / sustained, "traffic": None, "peak_source": peak_label(peak_src, "bf16 sustained"),
                              "note": "algorithmic forward conv FLOPs of the step / step time; exact_tc issues 3 MMAs per product"},
                 "cpu_baseline": cpu}
         print(json.dumps(line), flush=True)

@@ -1,4 +1,4 @@
-/* ssnb.h — C ABI of libssn_b200.so: the B200-native SSN forward/backward hot path.
+/* ssnb.h — C ABI of libssn_b200.so: the H100-native SSN forward/backward hot path.
  *
  * The reference (yjxiong/action-detection) has no FFI: its hot path is Python calling stock
  * PyTorch ops.  This ABI is what a binding for that path binds instead; each entry names the
@@ -24,9 +24,9 @@ enum { SSNB_OK = 0, SSNB_EINVAL = 1, SSNB_ECUDA = 2, SSNB_ESTATE = 3, SSNB_ENOSU
 /* precision modes of the backbone */
 enum {
   SSNB_EXACT_FP32 = 0, /* fp32 storage, fp32 SIMT FMA: end-to-end parity mode */
-  SSNB_FAST_FP16 = 1,  /* fp16 storage, tcgen05 kind::f16 MMA with fp32 TMEM accumulators */
+  SSNB_FAST_FP16 = 1,  /* fp16 storage, wgmma f16 MMA with fp32 register accumulators */
   SSNB_EXACT_TC = 2    /* fp32 storage; every convolution product as error-compensated split fp16 operands
-                          (x = hi + lo, three tcgen05 MMAs a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, fp32 accumulate):
+                          (x = hi + lo, three wgmma MMAs a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, fp32 accumulate):
                           fp32-grade results (layer_factory.py:25-39 computes in fp32) on the tensor cores */
 };
 

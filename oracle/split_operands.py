@@ -1,4 +1,4 @@
-"""Test infrastructure (never imported by the product): CPU emulation of the EXACT_TC arithmetic of csrc/umma_conv_v2.cu.
+"""Test infrastructure (never imported by the product): CPU emulation of the EXACT_TC arithmetic of csrc/umma_conv.cu.
 
 A product a.b of two fp32 numbers is formed on the tensor cores from fp16 planes hi = fp16(x), lo = fp16(x - hi) as
 a_lo.b_hi + a_hi.b_lo + a_hi.b_hi (fp32 accumulate); weight planes are scaled by a power of two so that the layer's

@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI / the reference-shaped module surface) against
-the CPU oracle and the committed golden vectors.  Run on the B200 box: pytest -m gpu."""
+the CPU oracle and the committed golden vectors.  Run on an H100: pytest -m gpu."""
 import os
 
 import numpy as np
@@ -216,7 +216,7 @@ def _prec(name):
 
 @pytest.mark.parametrize("precision", ["exact", "exact_tc"])
 def test_backbone_exact_golden(golden_dir, backbone_rgb, precision):
-    """EXACT (fp32 SIMT) and EXACT_TC (split-operand tcgen05) modes, whole backbone, 18 frames: against the
+    """EXACT (fp32 SIMT) and EXACT_TC (split-operand wgmma) modes, whole backbone, 18 frames: against the
     reference's own output (golden)."""
     dev = _cuda()
     import model_zoo
@@ -232,7 +232,7 @@ def test_backbone_exact_golden(golden_dir, backbone_rgb, precision):
         out = net(frames)
     err = rel_l2(out, torch.tensor(z["rgb_base_out18"]))
     print("backbone 18 frames (%s) rel-L2 vs reference golden: %.3e" % (precision, err))
-    # tolerance: 1e-3 relative fp32 (north_star).  Measured on B200: exact ~1e-6; exact_tc 2.1e-4 (per-layer 1e-6..3e-6 --
+    # tolerance: 1e-3 relative fp32 (north_star).  Measured on H100: exact 1.0e-5; exact_tc 3.2e-5 (per-layer 1e-6..3e-6 --
     # 22-bit split operands, tensor-core accumulation -- amplified by the ReLU switching of 69 random layers)
     assert err < E2E_TOL[precision], err
 
@@ -504,7 +504,7 @@ def test_test_forward_and_prepare_test_fc(backbone_rgb):
 
 def test_fast_fused_vs_unfused_and_oracle(backbone_rgb):
     """FAST mode, whole backbone fwd+bwd on 18 frames: the fused schedule (sibling 1x1 fusion, conv1
-    space-to-depth, stride-2 sampling, tcgen05 everywhere) against the same engine with fusion and
+    space-to-depth, stride-2 sampling, wgmma everywhere) against the same engine with fusion and
     tensor cores disabled (SIMT fp16 kernels), and both against the fp32 oracle."""
     dev = _cuda()
     from ssn_b200 import _lib
@@ -558,10 +558,10 @@ def test_fast_fused_vs_unfused_and_oracle(backbone_rgb):
     print("fast fused vs unfused: feat %.2e max dW %.2e max db %.2e | vs SIMT-fp16: feat %.2e max dW %.2e | vs fp32 oracle: feat %.2e worst dW %s"
           % (u_feat, u_w, u_b, e_feat, e_w, o_feat, o_w))
     assert u_feat < 1e-4 and u_w < 1e-2 and u_b < 1e-2
-    # tcgen05 vs SIMT on the same fp16 operands: identical arithmetic up to accumulation order, but end to end a different
+    # wgmma vs SIMT on the same fp16 operands: identical arithmetic up to accumulation order, but end to end a different
     # rounding flips ReLU / arg-max decisions below; bounded per layer by the median and loosely by the worst layer
     e_ws = sorted(rel_l2(a, b) for a, b in zip(dw_fast, dw_simt))
-    print("fast tcgen05 vs SIMT-fp16 dW rel-L2: median %.2e, worst %.2e" % (e_ws[len(e_ws) // 2], e_ws[-1]))
+    print("fast wgmma vs SIMT-fp16 dW rel-L2: median %.2e, worst %.2e" % (e_ws[len(e_ws) // 2], e_ws[-1]))
     assert e_feat < 5e-3 and e_ws[len(e_ws) // 2] < 0.3 and e_ws[-1] < 0.5, (e_feat, e_ws[len(e_ws) // 2], e_ws[-1])    # measured 0.15 / 0.19
     # End-to-end gradients of FAST mode on this synthetic random-weight net are dominated by ReLU / max-pool
     # decision flips (forward differs by ~1e-2 => many flips; cf. the fp32 noise floor of ~1e-2 measured in
@@ -685,7 +685,7 @@ def test_fused_step_bench_shape(precision):
     e["backbone_grads_cos"] = _cos(lambda n_: params[n_].grad, bb_ref)
     print("fused_step F=288 (%s) vs fp32 oracle: %s" % (precision, {k: "%.3e" % v for k, v in e.items()}))
     print("fused_step F=288 (%s) losses %s oracle %s" % (precision, losses.tolist(), ref_l.tolist()))
-    # measured on B200 (round 2): exact_tc feat 3.4e-5, loss 6e-7, head grads 2.7e-5, backbone grads 1.0e-2 (cosine 0.9999; the
+    # measured on H100: exact_tc feat 3.4e-5, loss 6e-7, head grads 2.7e-5, backbone grads 1.1e-2 (cosine 0.9999; the
     # fp32 reference itself is 7.6e-3 from the float64 gradient on this random-weight net, test_ssn_train_exact_vs_oracle);
     # fast feat 9.2e-3, loss 3e-4, head grads 3.1e-3, backbone grads 0.27 (cosine 0.964): outside the 1e-3 tolerance, reported
     bars = {"exact_tc": {"feat": 2e-4, "course": 2e-4, "stpp": 2e-4, "loss": 1e-4, "head_grads": 5e-4, "backbone_grads": 5e-2},

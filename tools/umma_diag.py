@@ -1,4 +1,4 @@
-"""GPU diagnostic: tcgen05 conv kernel vs the SIMT fp16 kernel on the same engine inputs.
+"""GPU diagnostic: the wgmma conv kernels vs the SIMT kernels on the same engine inputs (python tools/umma_diag.py [frames] [tc]).
 Prints rel-L2 per layer (forward and data-gradient) and, on mismatch, where the error sits."""
 import os
 import sys
@@ -18,7 +18,7 @@ def rel(a, b):
 
 def main():
     Fn = int(sys.argv[1]) if len(sys.argv) > 1 else 18
-    # mode "tc": SSNB_EXACT_TC (split-operand tcgen05) against the fp32 SIMT kernels, bar 2e-5; default: FAST vs SIMT fp16
+    # mode "tc": SSNB_EXACT_TC (split-operand wgmma) against the fp32 SIMT kernels, bar 2e-5; default: FAST vs SIMT fp16
     tc = len(sys.argv) > 2 and sys.argv[2] == "tc"
     prec, bar = (_lib.EXACT_TC, 2e-5) if tc else (_lib.FAST_FP16, 2e-3)
     dev = torch.device("cuda:0")
