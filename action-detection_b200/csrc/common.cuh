@@ -86,16 +86,10 @@ template <typename T> int launch_avgpool3_fwd(View src, View dst, int F, int acc
 template <typename T> int launch_gpool_fwd(View src, int F, float* feat, cudaStream_t s);
 template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, View ddst, int F, const void* y, cudaStream_t s);
 template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t s);
-template <typename T> int launch_fill_zero(View v, int F, cudaStream_t s);
 
-// weight packing (pack.cu): fold BN, produce kernel layouts
-// wf [tap][ci][co], wd [tap][co][ci] in storage type T; bias' [co] fp32; scale [co] fp32
-template <typename T>
-int launch_pack_conv(const float* w, const float* b, const float* gamma, const float* beta, const float* mean,
-                     const float* var, int Cout, int Cin, int k, T* wf, T* wd, float* bias_f, float* scale,
-                     cudaStream_t s, float* absmax = nullptr);   // absmax (optional, zeroed by the caller): max |folded weight|
-
-// the same for many layers per launch (block0 = first CTA of the entry; 256 threads per CTA)
+// weight packing (simt_glue.cu), many layers per launch (block0 = first CTA of the entry; 256 threads per CTA): fold BN,
+// produce the kernel layouts wf [tap][ci][co], wd [tap][co][ci] in storage type T; bias' [co] fp32; scale [co] fp32;
+// absmax (optional, zeroed by the caller): max |folded weight|
 constexpr int PACK_MAX = 32;
 constexpr int PACK_PER_THREAD = 4;     // element-wise path of pack_all_kernel (more than PACK_TILE_TAPS taps: conv1): 256 threads x 4 elements per CTA
 constexpr int PACK_TILE = 32, PACK_TILE_TAPS = 9;   // tiled path: one CTA per 32 output x 32 input channels x taps
@@ -113,7 +107,7 @@ struct PackEntry {
 };
 struct PackTable { int n, pad_; PackEntry e[PACK_MAX]; };
 template <typename T> int launch_pack_all(const PackTable& t, int total_blocks, cudaStream_t s);
-// EXACT_TC: hi/lo planes of both fp32 weight layouts of many layers per launch (scale from each layer's absmax, see launch_split_flat)
+// EXACT_TC: hi/lo planes of both fp32 weight layouts of many layers per launch, see launch_split_all
 struct SplitEntry {
   const float *wf, *wd; __half *wf16, *wd16; long long plane_bytes, n; const float* absmax; float* inv_scale; int block0, pad_;
   // optional second copies inside a fused sibling block's operands (1x1 layers): wd rows stacked (contiguous), wf columns inside the
@@ -121,6 +115,10 @@ struct SplitEntry {
   __half *wd16_b, *wf16_b; long long b_plane_bytes; int b_pitch, cout;
 };
 struct SplitTable { int n, pad_; SplitEntry e[PACK_MAX]; };
+// every entry is split as src * 2^e with 2^e = 8192 / 2^ceil(log2(*absmax)): the largest weight lands in [4096, 8192), so
+// the LO plane stays a normal fp16 number for every weight within ~2^-13 of the largest (unscaled, a BN-folded conv1 weight
+// of ~1e-3 has a subnormal LO with 3 significant bits); thread 0 of the entry writes 2^-e to *inv_scale, the consuming
+// kernels' alpha_dev
 int launch_split_all(const SplitTable& t, int total_blocks, cudaStream_t s);
 
 // one launch finalises the weight (and bias) gradients of many layers: split-K partial reduction in fixed order,
@@ -146,9 +144,6 @@ int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stri
 //   hi = fp16(x * scale), lo = fp16(x * scale - float(hi))  =>  hi + lo carries ~22 significand bits of x * scale
 // `flag` (device int, may be null) is set to 1 when |x * scale| exceeds the fp16 range (loss-scale overflow)
 int launch_split_view(View src_f32, int F, float scale, View planes, int* flag, cudaStream_t s);
-// weights: planes of src * 2^e with 2^e = 8192 / 2^ceil(log2(*absmax)) (so that the LO plane stays a normal fp16 number for
-// every weight within ~2^-13 of the largest); thread 0 writes 2^-e to *inv_scale (the consuming kernels' alpha_dev)
-int launch_split_flat(const float* src, long long n, __half* hi, __half* lo, const float* absmax, float* inv_scale, cudaStream_t s);
 int launch_planes_to_nchw(View planes, int F, float scale, float* dst, cudaStream_t s);
 int launch_nhwc_to_s2d_split(View src_f32, int F, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);
 int launch_nchw_to_s2d_split(const float* src, int F, int Cin, int H, int W, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);

@@ -117,8 +117,6 @@ using namespace ssnb;
 struct ssnb_engine {
   ssnb_config cfg;
   int F = 0;
-  bool fp16 = false;
-  bool tc = false;                  // SSNB_EXACT_TC: fp32 storage + glue, convolutions as split-operand (hi/lo fp16) tensor-core MMAs
   size_t esz = 4;
   size_t up_plane = 0, s2d_plane = 0, s2d_w_plane = 0;
   int* tc_flag = nullptr;           // device int: set when a split pass saw |x * grad_scale| beyond the fp16 range
@@ -135,7 +133,7 @@ struct ssnb_engine {
   std::vector<PackedConv> packed;
   std::vector<FusedBlock> fused;
   size_t ws_bytes = 0, partial_off = 0, partial_bytes = 0, bpartial_off = 0;
-  size_t s2d_off = 0, s2d_w_off = 0, up_off = 0;   // FAST mode: space-to-depth input + weights, zero-upsampled dz
+  size_t s2d_off = 0, s2d_w_off = 0, up_off = 0;   // tensor-core modes: space-to-depth input + weights, zero-upsampled dz
   bool fold_pools = true;                            // SSNB_DISABLE_FUSION=1 also keeps the max-pool backward separate
   bool s2d_ready = false;                            // backbone_fwd converted the input directly
   int Cs = 0;                                        // channels of the space-to-depth input (4*Cin rounded up to 8)
@@ -149,6 +147,10 @@ struct ssnb_engine {
   UmmaContext umma_ctx;
 
   int fail(int code, const std::string& msg) { error = msg; return code; }
+  bool fast() const { return cfg.precision == SSNB_FAST_FP16; }          // fp16 storage, fp16 operands
+  bool exact_tc() const { return cfg.precision == SSNB_EXACT_TC; }       // fp32 storage, convolutions on split (hi/lo fp16) operand planes
+  bool tensor_cores() const { return cfg.precision != SSNB_EXACT_FP32; } // either of the two: the wgmma schedule
+  int nplanes() const { return exact_tc() ? 2 : 1; }                     // fp16 operand planes per tensor-core operand
   View view(int val, bool grad) const {
     const Value& v = vals[val];
     const Buffer& b = bufs[v.buf];
@@ -166,6 +168,18 @@ struct ssnb_engine {
     w.H = b.H; w.W = b.W; w.C = v.C; w.pitch = b.C; w.coff = v.coff; w.lo_off = (long long)b.plane;
     return w;
   }
+  // what the tensor-core kernels read and write for a value: the fp16 storage in FAST, the operand planes in EXACT_TC
+  View operand(int val, bool grad) const { return exact_tc() ? planes(val, grad) : view(val, grad); }
+  // tensor-core weight operands of a convolution: forward [tap][co][ci], data gradient [tap][ci][co]
+  const __half* w_fwd(const PackedConv& p) const { return (const __half*)(ws + (exact_tc() ? p.wd16 : p.wd)); }
+  const __half* w_dgrad(const PackedConv& p) const { return (const __half*)(ws + (exact_tc() ? p.wf16 : p.wf)); }
+  // EXACT_TC bind options (nullptr in FAST): LO weight plane `w_lo_off` bytes after the HI plane, fp32 result `out32`, result
+  // scale alpha times 1 / the weights' power-of-two plane scale, which the split pass writes to the second float of `wmax`
+  const UmmaTcOpts* tc_opts(UmmaTcOpts& t, size_t w_lo_off, void* out32, float alpha, size_t wmax) const {
+    if (!exact_tc()) return nullptr;
+    t.w_lo_off = (long long)w_lo_off; t.out32 = (float*)out32; t.alpha = alpha; t.alpha_dev = (const float*)(ws + wmax) + 1;
+    return &t;
+  }
 };
 
 namespace ssnb {
@@ -178,6 +192,11 @@ static bool profiled_op(const char* env, const std::string& id) {
   if (!e || !*e) return false;
   const std::string list = std::string(",") + e + ",";
   return list.find("," + id + ",") != std::string::npos;
+}
+// diagnostic switch `name` set to 1
+static bool env_on(const char* name) {
+  const char* v = getenv(name);
+  return v && v[0] == '1';
 }
 // SM count of the current device (the H100 SXM's 132 where none is visible: planning without a GPU)
 static int device_sms() {
@@ -272,7 +291,7 @@ static void plan(ssnb_engine* e) {
   for (Buffer& b : e->bufs) { b.off = off; off = align_up(off + F * b.H * b.W * b.C * e->esz, 1024); }
   if (e->cfg.training)
     for (Buffer& b : e->bufs) { b.goff = off; off = align_up(off + F * b.H * b.W * b.C * e->esz, 1024); }
-  if (e->tc) {
+  if (e->exact_tc()) {
     for (Buffer& b : e->bufs) {
       if (b.C % 8) continue;                              // the network input (3 / 10 channels) has no planes: conv1 reads its own packed copy
       b.plane = align_up(F * b.H * b.W * b.C * 2, 1024);
@@ -296,13 +315,13 @@ static void plan(ssnb_engine* e) {
     e->packed[i].wd = off; off = align_up(off + n * e->esz, 1024);
     e->packed[i].bias = off; off = align_up(off + c.cout * 4, 256);
     e->packed[i].scale = off; off = align_up(off + c.cout * 4, 256);
-    if (e->tc) {
+    if (e->exact_tc()) {
       e->packed[i].wplane = align_up(n * 2, 1024);
       e->packed[i].wf16 = off; off += 2 * e->packed[i].wplane;
       e->packed[i].wd16 = off; off += 2 * e->packed[i].wplane;
     }
   }
-  if (e->tc) {      // per layer: [0] max |folded weight| (atomicMax target, zeroed before every pack), [1] 1 / plane scale (the kernels' alpha_dev)
+  if (e->exact_tc()) {      // per layer: [0] max |folded weight| (atomicMax target, zeroed before every pack), [1] 1 / plane scale (the kernels' alpha_dev)
     e->wmax_off = off;
     for (size_t i = 0; i < e->convs.size(); ++i) e->packed[i].wmax = off + i * 8;
     off = align_up(off + (e->convs.size() + 16) * 8, 1024);     // + one shared slot per fused sibling block
@@ -337,13 +356,13 @@ static void plan(ssnb_engine* e) {
           const int ctas = ((c.cout + 127) / 128) * n_tiles * ((taps + tpc - 1) / tpc);
           o.tsplits = std::max(o.wsplits, std::min(128, std::max(1, device_sms() / ctas)));
         }
-        if (e->fp16 || e->tc) splits = std::max<long long>(splits, o.tsplits);
+        if (e->tensor_cores()) splits = std::max<long long>(splits, o.tsplits);
         const size_t need = (size_t)splits * taps * c.cout * c.cin * 4;
         if (need > pmax) pmax = need;
       }
     }
   }
-  if (e->fp16 || e->tc) {
+  if (e->tensor_cores()) {
     for (int i = 0; i < (int)e->ops.size(); ++i) {
       const Op& o = e->ops[i];
       if (o.kind != OP_CONV || o.k != 1) continue;
@@ -361,11 +380,11 @@ static void plan(ssnb_engine* e) {
       fb.c1 = fb.op1 >= 0 ? e->convs[e->ops[fb.op1].conv].cout : 0;
       const int n = fb.c1 + fb.c3r + fb.cdr, kf = (fb.c1 + 63) / 64 * 64 + fb.c3r + fb.cdr;
       fb.w_fwd_plane = align_up((size_t)n * fb.cx * 2, 1024); fb.w_dg_plane = align_up((size_t)fb.cx * kf * 2, 1024);
-      if (e->tc) fb.w_fwd_plane = fb.w_dg_plane = std::max(fb.w_fwd_plane, fb.w_dg_plane);     // one LO-plane distance for both (split_all_kernel)
-      fb.w_fwd = off; off += (e->tc ? 2 : 1) * fb.w_fwd_plane;
+      if (e->exact_tc()) fb.w_fwd_plane = fb.w_dg_plane = std::max(fb.w_fwd_plane, fb.w_dg_plane);     // one LO-plane distance for both (split_all_kernel)
+      fb.w_fwd = off; off += e->nplanes() * fb.w_fwd_plane;
       fb.bias = off; off = align_up(off + (size_t)n * 4, 256);
-      fb.w_dg = off; off += (e->tc ? 2 : 1) * fb.w_dg_plane;
-      if (e->tc) {       // the three layers share ONE power-of-two plane scale (their operands are stacked / K-concatenated in one launch)
+      fb.w_dg = off; off += e->nplanes() * fb.w_dg_plane;
+      if (e->exact_tc()) {       // the three layers share ONE power-of-two plane scale (their operands are stacked / K-concatenated in one launch)
         if (e->fused.size() >= 16) continue;
         fb.wmax = e->wmax_off + (e->convs.size() + e->fused.size()) * 8;
         for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) e->packed[e->ops[j].conv].wmax = fb.wmax;
@@ -373,33 +392,10 @@ static void plan(ssnb_engine* e) {
       e->fused.push_back(fb);
     }
   }
-  if (e->fp16) {
+  if (e->tensor_cores()) {
+    // convolutions whose only consumer is a k3/s2/pad0 max pool: that pool's backward gather is folded into their mask pass,
+    // whose vector width (8 halves in FAST, 4 floats in EXACT_TC) must divide the channel count
     for (int i = 0; i < (int)e->ops.size(); ++i) {
-      Op& po = e->ops[i];
-      if (po.kind != OP_MAXPOOL || po.k != 3 || po.stride != 2) continue;
-      int producer = -1, consumers = 0;
-      for (int j = 0; j < (int)e->ops.size(); ++j) {
-        if (e->ops[j].out_val == po.in_val && e->ops[j].kind == OP_CONV) producer = j;
-        if (e->ops[j].in_val == po.in_val) ++consumers;
-      }
-      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % 8 == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
-    }
-    e->Cs = (4 * e->cfg.in_channels + 7) / 8 * 8;
-    e->s2d_off = off; off = align_up(off + F * 112 * 112 * 4 * e->Cs * 2, 1024);   // packed: 4 horizontal neighbours per pixel
-    e->s2d_w_off = off; off = align_up(off + (size_t)16 * 64 * e->Cs * 2, 1024);
-    if (e->cfg.training) {
-      size_t up = 0;
-      for (const Op& o : e->ops)
-        if (o.kind == OP_CONV && o.stride == 2 && o.conv != 0) {
-          const Buffer& ib = e->bufs[e->vals[o.in_val].buf];
-          up = std::max(up, F * ib.H * ib.W * (size_t)e->convs[o.conv].cout * 2);
-        }
-      e->up_off = off; off = align_up(off + up, 1024);
-      pmax = std::max(pmax, (size_t)128 * 16 * 64 * e->Cs * 4);
-    }
-  }
-  if (e->tc) {
-    for (int i = 0; i < (int)e->ops.size(); ++i) {      // convolutions whose only consumer is a k3/s2/pad0 max pool: backward gather folded in
       Op& po = e->ops[i];
       if (po.kind != OP_MAXPOOL || po.k != 3 || po.stride != 2 || po.pad != 0) continue;
       int producer = -1, consumers = 0;
@@ -407,13 +403,19 @@ static void plan(ssnb_engine* e) {
         if (e->ops[j].out_val == po.in_val && e->ops[j].kind == OP_CONV) producer = j;
         if (e->ops[j].in_val == po.in_val) ++consumers;
       }
-      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % 4 == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
+      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % (e->fast() ? 8 : 4) == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
     }
+    // fp16 operand regions: one plane in FAST (the next region starts 1024-aligned behind it), hi + lo planes `plane`
+    // bytes apart in EXACT_TC
+    auto operand_region = [&](size_t bytes, size_t& plane) {
+      const size_t at = off;
+      if (e->exact_tc()) { plane = align_up(bytes, 1024); off += 2 * plane; }
+      else off = align_up(off + bytes, 1024);
+      return at;
+    };
     e->Cs = (4 * e->cfg.in_channels + 7) / 8 * 8;
-    e->s2d_plane = align_up(F * 112 * 112 * 4 * e->Cs * 2, 1024);
-    e->s2d_off = off; off += 2 * e->s2d_plane;
-    e->s2d_w_plane = align_up((size_t)16 * 64 * e->Cs * 2, 1024);
-    e->s2d_w_off = off; off += 2 * e->s2d_w_plane;
+    e->s2d_off = operand_region(F * 112 * 112 * 4 * e->Cs * 2, e->s2d_plane);      // packed: 4 horizontal neighbours per pixel
+    e->s2d_w_off = operand_region((size_t)16 * 64 * e->Cs * 2, e->s2d_w_plane);
     if (e->cfg.training) {
       size_t up = 0;
       for (const Op& o : e->ops)
@@ -421,8 +423,7 @@ static void plan(ssnb_engine* e) {
           const Buffer& ib = e->bufs[e->vals[o.in_val].buf];
           up = std::max(up, F * ib.H * ib.W * (size_t)e->convs[o.conv].cout * 2);
         }
-      e->up_plane = align_up(up, 1024);
-      e->up_off = off; off += 2 * e->up_plane;
+      e->up_off = operand_region(up, e->up_plane);
       pmax = std::max(pmax, (size_t)128 * 16 * 64 * e->Cs * 4);
     }
   }
@@ -431,9 +432,9 @@ static void plan(ssnb_engine* e) {
     for (Op& o : e->ops)
       if (o.kind == OP_CONV) {
         const ConvSpec& c = e->convs[o.conv];
-        const int nsplit = (e->fp16 || e->tc) ? std::max(o.wsplits, o.tsplits) : o.wsplits;
+        const int nsplit = e->tensor_cores() ? std::max(o.wsplits, o.tsplits) : o.wsplits;
         size_t need = (size_t)nsplit * c.k * c.k * c.cout * c.cin * 4;
-        if (o.conv == 0 && (e->fp16 || e->tc)) need = std::max(need, (size_t)128 * 16 * 64 * e->Cs * 4);
+        if (o.conv == 0 && e->tensor_cores()) need = std::max(need, (size_t)128 * 16 * 64 * e->Cs * 4);
         o.partial_off = off; off = align_up(off + need, 1024);
         o.bias_partial_off = off; off = align_up(off + (size_t)std::max(nsplit, 128) * c.cout * 4, 256);
       }
@@ -442,7 +443,7 @@ static void plan(ssnb_engine* e) {
 }
 
 // ---- op execution --------------------------------------------------------------------------------
-#define DISPATCH(e, call_f, call_h) ((e)->fp16 ? (call_h) : (call_f))
+#define DISPATCH(e, call_f, call_h) ((e)->fast() ? (call_h) : (call_f))
 
 // timing tags (common.cuh): the next launch is the convolution `o` in pass `phase`
 static double conv_flops(const ssnb_engine* e, const Op& o) {
@@ -454,34 +455,39 @@ static inline void tag_next(int phase, double flop) { t_tag.phase = phase; t_tag
 
 // EXACT_TC: operand planes of a value produced by a kernel that only wrote fp32 (pools, SIMT convolutions, value_write)
 static int tc_split_value(ssnb_engine* e, int val, bool grad, float scale, cudaStream_t s) {
-  if (!e->tc || !e->bufs[e->vals[val].buf].plane) return 0;
+  if (!e->exact_tc() || !e->bufs[e->vals[val].buf].plane) return 0;
   return launch_split_view(e->view(val, grad), e->F, scale, e->planes(val, grad), grad ? e->tc_flag : nullptr, s);
 }
 
 static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s);
 static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s) {
-  if (e->tc && o.kind == OP_CONV && o.umma.enabled) {
-    // split-operand tensor-core convolution: reads the input's hi/lo planes, writes fp32 + the output's planes
-    if (o.conv == 0 && !e->s2d_ready)
-      if (int rc = launch_nhwc_to_s2d_split(e->view(o.in_val, false), e->F, (__half*)(e->ws + e->s2d_off), (long long)e->s2d_plane, e->Cs, s)) return rc;
+  tag_next(0, 0.0);
+  if (o.kind == OP_CONV && o.umma.enabled) {
+    // tensor-core convolution (EXACT_TC: reads the input's hi/lo planes, writes fp32 + the output's planes); conv1 runs as a
+    // 4x4 stride-1 convolution over the space-to-depth input
+    if (o.conv == 0 && !e->s2d_ready) {
+      const View in = e->view(o.in_val, false);
+      __half* s2d = (__half*)(e->ws + e->s2d_off);
+      if (int rc = e->exact_tc() ? launch_nhwc_to_s2d_split(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s) : launch_nhwc_to_s2d(in, e->F, s2d, e->Cs, s))
+        return rc;
+    }
     tag_next(0, conv_flops(e, o));
     return umma_conv_launch(e->umma_ctx, o.umma, s);
   }
-  tag_next(0, 0.0);
   if (o.kind == OP_BN1) {
     if (!e->bn1_gamma || !e->bn1_beta) { set_thread_error("bn1_train engine: call ssnb_set_bn1 first"); return SSNB_ESTATE; }
-    return launch_bn_train_fwd(e->view(o.in_val, false), e->view(o.out_val, false), e->tc ? e->planes(o.out_val, false) : View(), e->F, e->bn1_gamma,
+    return launch_bn_train_fwd(e->view(o.in_val, false), e->view(o.out_val, false), e->exact_tc() ? e->planes(o.out_val, false) : View(), e->F, e->bn1_gamma,
                                e->bn1_beta, e->bn1_eps, e->bn1_momentum, e->bn1_rmean, e->bn1_rvar, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, s);
   }
-  if (e->tc && (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) && e->bufs[e->vals[o.out_val].buf].plane) {
+  if (e->exact_tc() && (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) && e->bufs[e->vals[o.out_val].buf].plane) {
     // vectorised fp32 pooling that also emits the output's operand planes (glue_fp32.cu)
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false), pl = e->planes(o.out_val, false);
     if (o.kind == OP_MAXPOOL) return launch_maxpool_fwd_f4(in, out, pl, e->F, o.k, o.stride, o.pad, (uint8_t*)(e->ws + o.argmax_off), s);
     return launch_avgpool3_f4(in, out, pl, e->F, 0, s);
   }
   if (int rc = run_fwd_impl(e, o, input_nchw, feat, s)) return rc;
-  return (e->tc && o.out_val >= 0) ? tc_split_value(e, o.out_val, false, 1.0f, s) : 0;
+  return o.out_val >= 0 ? tc_split_value(e, o.out_val, false, 1.0f, s) : 0;
 }
 
 static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s) {
@@ -489,12 +495,6 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
   if (o.kind == OP_CONV) {
     const ConvSpec& c = e->convs[o.conv];
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    if (e->fp16 && o.umma.enabled) {
-      if (o.conv == 0 && !e->s2d_ready)   // conv1 runs as a 4x4 stride-1 convolution over the space-to-depth input
-        if (int rc = launch_nhwc_to_s2d(in, F, (__half*)(e->ws + e->s2d_off), e->Cs, s)) return rc;
-      tag_next(0, conv_flops(e, o));
-      return umma_conv_launch(e->umma_ctx, o.umma, s);
-    }
     ConvArgs a;
     a.src = in.base; a.SH = in.H; a.SW = in.W; a.Csrc = in.C; a.src_pitch = in.pitch; a.src_coff = in.coff;
     a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
@@ -506,13 +506,13 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
   if (o.kind == OP_MAXPOOL) {
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
     uint8_t* am = (uint8_t*)(e->ws + o.argmax_off);
-    if (e->fp16 && in.C % 8 == 0) return launch_maxpool_fwd_h8(in, out, F, o.k, o.stride, o.pad, am, s);
+    if (e->fast() && in.C % 8 == 0) return launch_maxpool_fwd_h8(in, out, F, o.k, o.stride, o.pad, am, s);
     return DISPATCH(e, launch_maxpool_fwd<float>(in, out, F, o.k, o.stride, o.pad, am, s),
                     launch_maxpool_fwd<__half>(in, out, F, o.k, o.stride, o.pad, am, s));
   }
   if (o.kind == OP_AVGPOOL) {
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    if (e->fp16 && in.C % 8 == 0) return launch_avgpool3_h8(in, out, F, 0, s);
+    if (e->fast() && in.C % 8 == 0) return launch_avgpool3_h8(in, out, F, 0, s);
     return DISPATCH(e, launch_avgpool3_fwd<float>(in, out, F, 0, s), launch_avgpool3_fwd<__half>(in, out, F, 0, s));
   }
   if (o.kind == OP_GPOOL) {
@@ -523,9 +523,38 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
   return SSNB_EINVAL;
 }
 
+// SIMT convolution backward (EXACT_FP32, and layers or passes without a tensor-core plan), reading the masked fp32 / fp16
+// dz = d(out): weight gradient into the layer's split-K partials + finalize; data gradient into d(in)
+static int simt_wgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
+  const ConvSpec& c = e->convs[o.conv];
+  const View x = e->view(o.in_val, false), dz = e->view(o.out_val, true);
+  float* partial = (float*)(e->ws + o.partial_off);
+  WgradArgs w;
+  w.dz = dz.base; w.OH = dz.H; w.OW = dz.W; w.Cout = dz.C; w.dz_pitch = dz.pitch; w.dz_coff = dz.coff;
+  w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
+  w.partial = partial; w.F = e->F; w.k = c.k; w.stride = c.stride; w.pad = c.pad;
+  w.rows_per_split = o.wrows; w.splits = o.wsplits;
+  tag_next(2, conv_flops(e, o));
+  if (int rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s))) return rc;
+  const float out_scale = e->fast() ? 1.0f / e->cfg.grad_scale : 1.0f;      // FAST stores gradients times the loss scale
+  return launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
+                               e->dw[o.conv], e->grad_accumulate, s);
+}
+static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
+  const ConvSpec& c = e->convs[o.conv];
+  const View dz = e->view(o.out_val, true), dx = e->view(o.in_val, true);
+  ConvArgs a;
+  a.src = dz.base; a.SH = dz.H; a.SW = dz.W; a.Csrc = dz.C; a.src_pitch = dz.pitch; a.src_coff = dz.coff;
+  a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
+  a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
+  a.F = e->F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
+  tag_next(1, conv_flops(e, o));
+  return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
+}
+
 static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t s, bool skip_dgrad = false, bool full = false) {
   const int F = e->F;
-  const float gs = e->fp16 ? e->cfg.grad_scale : 1.0f;
+  const float gs = e->fast() ? e->cfg.grad_scale : 1.0f;
   int rc = 0;
   tag_next(3, 0.0);
   if (o.kind == OP_GPOOL) {
@@ -536,156 +565,104 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   }
   if (o.kind == OP_BN1) {
     return launch_bn_train_bwd(e->view(o.in_val, false), e->view(o.out_val, true), e->view(o.out_val, false), e->view(o.in_val, true),
-                               e->tc ? e->planes(o.in_val, true) : View(), e->cfg.grad_scale, e->tc_flag, F, e->bn1_gamma, (float*)(e->ws + e->bn_stat_off),
+                               e->exact_tc() ? e->planes(o.in_val, true) : View(), e->cfg.grad_scale, e->tc_flag, F, e->bn1_gamma, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, e->bn1_dgamma, e->bn1_dbeta, e->grad_accumulate, s);
   }
   if (o.kind == OP_MAXPOOL) {
-    if (full && (e->fp16 || e->tc) && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass
+    if (full && e->tensor_cores() && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
     const uint8_t* am = (const uint8_t*)(e->ws + o.argmax_off);
-    if (e->tc && din.C % 4 == 0) return launch_maxpool_bwd_f4(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
-    if (e->fp16 && din.C % 8 == 0) return launch_maxpool_bwd_h8(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
+    if (e->exact_tc() && din.C % 4 == 0) return launch_maxpool_bwd_f4(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
+    if (e->fast() && din.C % 8 == 0) return launch_maxpool_bwd_h8(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
     return DISPATCH(e, launch_maxpool_bwd<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s),
                     launch_maxpool_bwd<__half>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s));
   }
   if (o.kind == OP_AVGPOOL) {
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
-    if (e->tc && din.C % 4 == 0) return launch_avgpool3_f4(dout, din, View(), F, o.grad_accumulate, s);
-    if (e->fp16 && din.C % 8 == 0) return launch_avgpool3_h8(dout, din, F, o.grad_accumulate, s);
+    if (e->exact_tc() && din.C % 4 == 0) return launch_avgpool3_f4(dout, din, View(), F, o.grad_accumulate, s);
+    if (e->fast() && din.C % 8 == 0) return launch_avgpool3_h8(dout, din, F, o.grad_accumulate, s);
     return DISPATCH(e, launch_avgpool3_fwd<float>(dout, din, F, o.grad_accumulate, s),
                     launch_avgpool3_fwd<__half>(dout, din, F, o.grad_accumulate, s));
   }
   // convolution: dz = dy * (y > 0); db, dW from dz; dx = dgrad(dz)
   const ConvSpec& c = e->convs[o.conv];
-  const View x = e->view(o.in_val, false), y = e->view(o.out_val, false);
-  const View dx = e->view(o.in_val, true), dy = e->view(o.out_val, true);
+  const View x = e->view(o.in_val, false), y = e->view(o.out_val, false), dy = e->view(o.out_val, true);
   const float* scale = (const float*)(e->ws + e->packed[o.conv].scale);
-  float* partial = (float*)(e->ws + o.partial_off);
   float* bpartial = (float*)(e->ws + e->bpartial_off);
-  const long long M = (long long)F * y.H * y.W;
   float* dbp = (e->db.size() && e->db[o.conv]) ? e->db[o.conv] : nullptr;
-  if (e->tc) {
-    // EXACT_TC: fp32 mask + bias gradient (as EXACT), then dz * grad_scale as hi/lo planes for the tensor-core products
-    const float gst = e->cfg.grad_scale;
-    const bool want_w = e->dw.size() && e->dw[o.conv];
-    const bool want_x = e->vals[o.in_val].name != "data" && !skip_dgrad;
-    const bool tc_w = want_w && o.umma_wgrad.enabled, tc_x = want_x && o.umma_dgrad.enabled;
-    const bool pre = full && e->fold_pools && o.dy_premasked;      // the last writer of dy masked it and wrote its operand planes
-    const bool bias_w = pre && o.bias_in_wgrad && dbp && tc_w;     // ... and the column sums ride on the weight-gradient MMAs
-    if (o.raw) {
-      // the training-mode BatchNorm behind this convolution produced dz and its planes: only the bias-gradient column sums are left
-      if (dbp)
-        if ((rc = launch_mask_bias_split_f4(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, (1024 * 512 - 64) / y.C, dbp, e->grad_accumulate, s))) return rc;
-    } else if (pre) {
-      if (!bias_w && dbp)       // bias gradient only: column sums of the (already masked) fp32 dz, no planes, nothing written back
-        if ((rc = launch_mask_bias_split_f4(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, (1024 * 512 - 64) / y.C, dbp, e->grad_accumulate, s))) return rc;
-    } else if (full && e->fold_pools && o.pool_consumer >= 0) {
-      // the consuming max pool's backward gather + ReLU mask + bias sums + planes in one pass (the fp32 dy is never materialised)
-      const Op& po = e->ops[o.pool_consumer];
-      const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
-      View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
-      if ((rc = launch_pool_mask_bias_split_f4(dy, y, e->view(po.out_val, true), pl, gst, need_f32 ? 1 : 0, e->tc_flag, F,
-                                               (const uint8_t*)(e->ws + po.argmax_off), scale, 1.0f, bpartial, (1024 * 512 - 64) / y.C, dbp,
-                                               e->grad_accumulate, s))) return rc;
-    } else {
-      // one pass over dy: ReLU mask, bias-gradient column sums and the hi/lo planes of dz * grad_scale; the masked fp32 dz is
-      // written back only when a SIMT kernel will read it
-      const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x) || !full;
-      View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
-      if ((rc = launch_mask_bias_split_f4(dy, y, pl, gst, need_f32 ? 1 : 0, e->tc_flag, F, scale, 1.0f, bpartial, (1024 * 512 - 64) / y.C, dbp,
-                                          e->grad_accumulate, s))) return rc;
-    }
-    if (tc_x && c.stride == 2 && o.conv != 0) {              // dz at input resolution (zero-upsampled), both planes
-      const View dzp = e->planes(o.out_val, true);
-      View lo = dzp; lo.base = (char*)dzp.base + dzp.lo_off;
-      if ((rc = launch_upsample2_zero(dzp, (__half*)(e->ws + e->up_off), x.H, x.W, F, s))) return rc;
-      if ((rc = launch_upsample2_zero(lo, (__half*)(e->ws + e->up_off + e->up_plane), x.H, x.W, F, s))) return rc;
-    }
-    if (tc_w) {
-      tag_next(2, conv_flops(e, o));
-      if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bias_w ? (float*)(e->ws + o.bias_partial_off) : nullptr))) return rc;
-      if (full && o.conv != 0) { e->pending_finalize.push_back((int)(&o - e->ops.data())); rc = 0; }     // batched at the end of the backward
-      else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s);
-      else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s);
-      if (rc) return rc;
-    } else if (want_w) {
-      WgradArgs w;
-      w.dz = dy.base; w.OH = y.H; w.OW = y.W; w.Cout = y.C; w.dz_pitch = dy.pitch; w.dz_coff = dy.coff;
-      w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
-      w.partial = partial; w.F = F; w.k = c.k; w.stride = c.stride; w.pad = c.pad;
-      w.rows_per_split = o.wrows; w.splits = o.wsplits;
-      tag_next(2, conv_flops(e, o));
-      if ((rc = launch_wgrad<float>(w, s))) return rc;
-      if ((rc = launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, scale, 1.0f, e->dw[o.conv], e->grad_accumulate, s))) return rc;
-    }
-    tag_next(1, conv_flops(e, o));
-    if (tc_x) return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
-    if (want_x) {
-      ConvArgs a;
-      a.src = dy.base; a.SH = dy.H; a.SW = dy.W; a.Csrc = dy.C; a.src_pitch = dy.pitch; a.src_coff = dy.coff;
-      a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
-      a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
-      a.F = F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
-      rc = launch_conv<float>(a, s);
-    }
-    return rc;
-  }
-  if (e->fp16 && full && e->fold_pools && o.pool_consumer >= 0) {
-    // max-pool backward gather + ReLU mask + bias-gradient column sums in one pass (dy is never materialised)
-    const Op& po = e->ops[o.pool_consumer];
-    if ((rc = launch_pool_mask_bias_h8(dy, y, e->view(po.out_val, true), F, po.k, po.stride, po.pad, (const uint8_t*)(e->ws + po.argmax_off),
-                                       scale, 1.0f / gs, bpartial, (1024 * 512 - 64) / y.C, dbp, e->grad_accumulate, s))) return rc;
-  } else if (e->fp16) {
-    // one pass: ReLU gradient mask in place + bias-gradient column sums (mask skipped when the producer of dy applied it)
-    const bool pre = full && e->fold_pools && o.dy_premasked;
-    const bool bias_w = pre && o.bias_in_wgrad && dbp && e->dw.size() && e->dw[o.conv] && o.umma_wgrad.enabled;
-    if (bias_w) { /* no pass at all: dy is already masked and the column sums ride on the weight-gradient MMAs */ }
-    else if ((rc = launch_mask_bias_h8(dy, pre ? View() : y, F, scale, 1.0f / gs, bpartial, (1024 * 512 - 64) / y.C, dbp, e->grad_accumulate, s))) return rc;
-  } else {
+  const bool want_w = e->dw.size() && e->dw[o.conv];
+  const bool want_x = e->vals[o.in_val].name != "data" && !skip_dgrad;
+  if (!e->tensor_cores()) {
     if (!o.raw && (rc = launch_relu_mask<float>(dy, y, F, s))) return rc;
     if (dbp) {
+      const long long M = (long long)F * y.H * y.W;
       int bs = (int)((M + 4095) / 4096); if (bs > 64) bs = 64; if (bs < 1) bs = 1;
-      if ((rc = launch_bias_grad<float>(dy.base, (int)M, y.C, dy.pitch, dy.coff, scale, 1.0f / gs, bpartial, bs, dbp, e->grad_accumulate, s))) return rc;
+      if ((rc = launch_bias_grad<float>(dy.base, (int)M, y.C, dy.pitch, dy.coff, scale, 1.0f, bpartial, bs, dbp, e->grad_accumulate, s))) return rc;
+    }
+    if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
+    return want_x ? simt_dgrad(e, o, s) : 0;
+  }
+
+  // tensor-core modes; the tensor-core products read dz times the loss scale (FAST: the fp16 storage, EXACT_TC: the planes)
+  const float gst = e->cfg.grad_scale;
+  const bool tc_w = want_w && o.umma_wgrad.enabled, tc_x = want_x && o.umma_dgrad.enabled;
+  const bool pre = full && e->fold_pools && o.dy_premasked;      // the last writer of dy masked it (EXACT_TC: and wrote its planes)
+  const bool bias_w = pre && o.bias_in_wgrad && dbp && tc_w;     // ... and the bias column sums ride on the weight-gradient MMAs
+  // the only consumer is a max pool whose backward gather is folded into this mask pass (the pooled input's dy is never materialised)
+  const Op* pool = (full && e->fold_pools && o.pool_consumer >= 0) ? &e->ops[o.pool_consumer] : nullptr;
+  const int max_ctas = (1024 * 512 - 64) / y.C;
+  // 1. one pass over dy: ReLU mask + bias-gradient column sums.  FAST masks the fp16 dy in place.  EXACT_TC reads the fp32 dy,
+  //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it.
+  if (e->fast()) {
+    if (pool) rc = launch_pool_mask_bias_h8(dy, y, e->view(pool->out_val, true), F, pool->k, pool->stride, pool->pad, (const uint8_t*)(e->ws + pool->argmax_off),
+                                            scale, 1.0f / gst, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    else if (!bias_w) rc = launch_mask_bias_h8(dy, pre ? View() : y, F, scale, 1.0f / gst, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+  } else {
+    const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
+    const View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
+    if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz and its planes: only the bias sums are left
+      if (dbp) rc = launch_mask_bias_split_f4(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    } else if (pre) {    // bias sums of the already masked fp32 dz only: no planes, nothing written back
+      if (!bias_w && dbp) rc = launch_mask_bias_split_f4(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    } else if (pool) {
+      rc = launch_pool_mask_bias_split_f4(dy, y, e->view(pool->out_val, true), pl, gst, need_f32 ? 1 : 0, e->tc_flag, F, (const uint8_t*)(e->ws + pool->argmax_off),
+                                          scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    } else {
+      rc = launch_mask_bias_split_f4(dy, y, pl, gst, (need_f32 || !full) ? 1 : 0, e->tc_flag, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     }
   }
-  if (e->fp16 && c.stride == 2 && o.conv != 0 && o.umma_dgrad.enabled && !skip_dgrad)
-    if ((rc = launch_upsample2_zero(dy, (__half*)(e->ws + e->up_off), x.H, x.W, F, s))) return rc;   // dz at input resolution
-  if (e->dw.size() && e->dw[o.conv] && e->fp16 && o.umma_wgrad.enabled) {
-    const bool bias_w = full && e->fold_pools && o.dy_premasked && o.bias_in_wgrad && dbp;
+  if (rc) return rc;
+  // 2. a stride-2 data gradient reads dz zero-upsampled to the input resolution, every operand plane
+  if (tc_x && c.stride == 2 && o.conv != 0) {
+    View dz = e->operand(o.out_val, true);
+    for (int p = 0; p < e->nplanes(); ++p, dz.base = (char*)dz.base + dz.lo_off)
+      if ((rc = launch_upsample2_zero(dz, (__half*)(e->ws + e->up_off + p * e->up_plane), x.H, x.W, F, s))) return rc;
+  }
+  // 3. weight gradient.  The wgmma partials of a whole backward are finalised in one batch at its end; conv1's space-to-depth
+  //    partials and those of a single op (ssnb_run_op) right away.
+  if (tc_w) {
+    float* partial = (float*)(e->ws + o.partial_off);
     float* bp = bias_w ? (float*)(e->ws + o.bias_partial_off) : nullptr;
     tag_next(2, conv_flops(e, o));
     if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bp))) return rc;
-    if (full && e->fold_pools && o.conv != 0) { e->pending_finalize.push_back((int)(&o - e->ops.data())); rc = 0; }   // batched at the end of the backward
-    else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gs, e->dw[o.conv], e->grad_accumulate, s);
-    else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gs, e->dw[o.conv], e->grad_accumulate, s, bp, dbp, e->tc_flag);
+    if (full && o.conv != 0) e->pending_finalize.push_back((int)(&o - e->ops.data()));
+    else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s);
+    else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s,
+                                    nullptr, nullptr, e->tc_flag);
     if (rc) return rc;
-  } else if (e->dw.size() && e->dw[o.conv]) {
-    WgradArgs w;
-    w.dz = dy.base; w.OH = y.H; w.OW = y.W; w.Cout = y.C; w.dz_pitch = dy.pitch; w.dz_coff = dy.coff;
-    w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
-    w.partial = partial; w.F = F; w.k = c.k; w.stride = c.stride; w.pad = c.pad;
-    w.rows_per_split = o.wrows; w.splits = o.wsplits;
-    tag_next(2, conv_flops(e, o));
-    if ((rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s)))) return rc;
-    if ((rc = launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gs, e->dw[o.conv], e->grad_accumulate, s))) return rc;
-  }
-  if (e->vals[o.in_val].name != "data" && !skip_dgrad) {
+  } else if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
+  // 4. data gradient; as the last writer of d(in) the wgmma epilogue applies in's ReLU mask
+  if (tc_x) {
     tag_next(1, conv_flops(e, o));
-    if (e->fp16 && o.umma_dgrad.enabled) return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
-    ConvArgs a;
-    a.src = dy.base; a.SH = dy.H; a.SW = dy.W; a.Csrc = dy.C; a.src_pitch = dy.pitch; a.src_coff = dy.coff;
-    a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
-    a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
-    a.F = F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
-    rc = DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
+    return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
   }
-  return rc;
+  return want_x ? simt_dgrad(e, o, s) : 0;
 }
 
 int engine_tail_view(ssnb_handle h, View* v, int* F, int* fp16) {
   if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
   *v = h->view(h->ops.back().in_val, false);
-  *F = h->F; *fp16 = h->fp16 ? 1 : 0;
+  *F = h->F; *fp16 = h->fast() ? 1 : 0;
   return 0;
 }
 
@@ -717,14 +694,12 @@ int ssnb_create(const ssnb_config* cfg, ssnb_handle* out) {
   e->cfg = *cfg;
   if (!(e->cfg.grad_scale > 0.f)) e->cfg.grad_scale = 1.0f;
   e->F = cfg->frames;
-  e->fp16 = cfg->precision == SSNB_FAST_FP16;
-  e->tc = cfg->precision == SSNB_EXACT_TC;
   e->bn1_train = cfg->bn1_train != 0;
-  if (e->bn1_train && e->fp16) { delete e; set_thread_error("ssnb_create: bn1_train (bn_mode='partial') needs EXACT_FP32 or EXACT_TC"); return SSNB_ENOSUPPORT; }
-  e->esz = e->fp16 ? 2 : 4;
+  if (e->bn1_train && e->fast()) { delete e; set_thread_error("ssnb_create: bn1_train (bn_mode='partial') needs EXACT_FP32 or EXACT_TC"); return SSNB_ENOSUPPORT; }
+  e->esz = e->fast() ? 2 : 4;
   build_graph(e);
   if ((int)e->convs.size() != 69) { delete e; set_thread_error("internal: conv table size"); return SSNB_ESTATE; }
-  umma_context_init(e->umma_ctx, e->fp16 || e->tc);
+  umma_context_init(e->umma_ctx);
   plan(e);
   e->launches0 = g_launches.load();
   *out = e;
@@ -746,244 +721,145 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
   if (((uintptr_t)dev_ptr) % 1024) return h->fail(SSNB_EINVAL, "workspace must be 1024-byte aligned");
   h->ws = (char*)dev_ptr;
   h->weights_ready = false;
-  if ((h->fp16 || h->tc) && cudaMemset(h->ws + h->bpartial_off, 0, 256) != cudaSuccess) { cudaGetLastError(); /* no device (CPU-only planning) */ }
+  if (h->tensor_cores() && cudaMemset(h->ws + h->bpartial_off, 0, 256) != cudaSuccess) { cudaGetLastError(); /* no device (CPU-only planning) */ }
   h->tc_flag = (int*)(h->ws + h->tc_flag_off);
   if (cudaMemset(h->tc_flag, 0, 256) != cudaSuccess) cudaGetLastError();
-  if (h->tc) {
-    // SSNB_EXACT_TC: split-operand plans over the hi/lo planes.  SSNB_DISABLE_UMMA=1 leaves every convolution on the fp32
-    // SIMT kernels (= SSNB_EXACT_FP32 arithmetic; what the tensor-core launches are diffed against).
-    const char* dis_tc = getenv("SSNB_DISABLE_UMMA");
-    const bool use_tc = !(dis_tc && dis_tc[0] == '1');
-    const char* disw_tc = getenv("SSNB_DISABLE_UMMA_WGRAD");
-    const bool use_wgrad_tc = h->cfg.training && !(disw_tc && disw_tc[0] == '1');
-    const float gs = h->cfg.grad_scale;
-    for (Op& o : h->ops) {
-      o.umma.enabled = false; o.umma_dgrad.enabled = false; o.umma_wgrad.enabled = false;
-      o.fuse_role = 0; o.fuse_block = -1; o.dgrad_masks = false; o.dy_premasked = false; o.bias_in_wgrad = false;
-      if (o.kind != OP_CONV || !use_tc) continue;
-      const ConvSpec& c = h->convs[o.conv];
-      const PackedConv& pk = h->packed[o.conv];
-      const View out32 = h->view(o.out_val, false);
-      int rc = 0;
-      if (o.conv == 0) {
-        // conv1 7x7/2: four vertical taps over the packed space-to-depth input planes (see the FAST binding below)
-        const int Ck = 4 * h->Cs;
-        View xs; xs.base = h->ws + h->s2d_off; xs.H = 112; xs.W = 112; xs.C = Ck; xs.pitch = Ck; xs.coff = 0; xs.lo_off = (long long)h->s2d_plane;
-        int dy[4], dx[4];
-        for (int t = 0; t < 4; ++t) { dy[t] = t - 2; dx[t] = 0; }
-        UmmaTcOpts t; t.w_lo_off = (long long)h->s2d_w_plane; t.out32 = (float*)out32.base; t.alpha = 1.0f; t.alpha_dev = (const float*)(h->ws + pk.wmax) + 1;
-        rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, h->planes(o.out_val, false), h->F, Ck, c.cout, 4, dy, dx,
-                                 (const __half*)(h->ws + h->s2d_w_off), (const float*)(h->ws + pk.bias), o.raw ? 0 : 1, &t);
-        if (rc) return h->fail(rc, "tc conv1 bind: " + ssnb::thread_error());
-        if (!o.umma.p.tc_ok) o.umma.enabled = false;
-        if (use_wgrad_tc) {
-          rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->planes(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
-                                    (float*)(h->ws + o.partial_off), 128);
-          if (rc) return h->fail(rc, "tc conv1 wgrad bind: " + ssnb::thread_error());
-        }
-        continue;
-      }
-      if (c.cin % 8 != 0 || c.k * c.k > UMMA_MAX_TAPS) continue;
-      UmmaTcOpts t; t.w_lo_off = (long long)pk.wplane; t.out32 = (float*)out32.base; t.alpha = 1.0f; t.alpha_dev = (const float*)(h->ws + pk.wmax) + 1;
-      rc = umma_conv_bind_fwd(h->umma_ctx, o.umma, h->planes(o.in_val, false), h->planes(o.out_val, false), h->F, c.cin, c.cout, c.k, c.pad,
-                              c.stride, (const __half*)(h->ws + pk.wd16), (const float*)(h->ws + pk.bias), &t);
-      if (rc) return h->fail(rc, "tc bind_fwd(" + c.id + "): " + ssnb::thread_error());
-      if (!h->cfg.training) continue;
-      View dz = h->planes(o.out_val, true);
-      const View in = h->view(o.in_val, false);
-      if (c.stride == 2) { dz.base = h->ws + h->up_off; dz.H = in.H; dz.W = in.W; dz.C = c.cout; dz.pitch = c.cout; dz.coff = 0; dz.lo_off = (long long)h->up_plane; }
-      View dxp = h->planes(o.in_val, true); dxp.base = nullptr; dxp.lo_off = 0;          // data gradients: fp32 only (masked and split by their consumer)
-      UmmaTcOpts tg; tg.w_lo_off = (long long)pk.wplane; tg.out32 = (float*)h->view(o.in_val, true).base; tg.alpha = 1.0f / gs; tg.alpha_dev = (const float*)(h->ws + pk.wmax) + 1;
-      rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, dxp, h->F, c.cin, c.cout, c.k, c.pad, (const __half*)(h->ws + pk.wf16),
-                                o.grad_accumulate, &tg);
-      if (rc) return h->fail(rc, "tc bind_dgrad(" + c.id + "): " + ssnb::thread_error());
-      if (!o.umma_dgrad.p.tc_ok) o.umma_dgrad.enabled = false;
-      if (use_wgrad_tc) {
-        rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->planes(o.out_val, true), h->planes(o.in_val, false), h->F, c.cin, c.cout, c.k, c.pad,
-                             (float*)(h->ws + o.partial_off), o.tsplits, c.stride);
-        if (rc) return h->fail(rc, "tc wgrad_bind(" + c.id + "): " + ssnb::thread_error());
-      }
-    }
-    h->fold_pools = false;
-    for (FusedBlock& fb : h->fused) fb.enabled = false;
-    const char* disf_sib = getenv("SSNB_DISABLE_FUSION");
-    if (use_tc && !(disf_sib && disf_sib[0] == '1')) {
-      // horizontal fusion of the sibling 1x1 convolutions of each inception block: ONE forward launch (stacked weights; the first
-      // c1 columns land in the concat buffer, the rest in the shared reduce buffer) and ONE data-gradient launch (K-concatenated
-      // dz planes from two sources) instead of three read-modify-write passes over the block input's gradient
-      for (size_t bi = 0; bi < h->fused.size(); ++bi) {
-        FusedBlock& fb = h->fused[bi];
-        Op& o3 = h->ops[fb.op_r3]; Op& od = h->ops[fb.op_rd];
-        if (!o3.umma.enabled || !od.umma.enabled) continue;
-        const View xp = h->planes(o3.in_val, false);
-        View redp = h->planes(o3.out_val, false); redp.C = fb.c3r + fb.cdr;
-        const View red32 = h->view(o3.out_val, false);
-        const float* alpha_dev = (const float*)(h->ws + fb.wmax) + 1;
-        int rc;
-        UmmaTcOpts t; t.w_lo_off = (long long)fb.w_fwd_plane; t.alpha = 1.0f; t.alpha_dev = alpha_dev;
-        if (fb.op1 >= 0) {
-          t.out32 = (float*)h->view(h->ops[fb.op1].out_val, false).base; t.out32_2 = (float*)red32.base;
-          rc = umma_conv_bind_fused_fwd(h->umma_ctx, fb.fwd, xp, h->planes(h->ops[fb.op1].out_val, false), redp, h->F, fb.cx, fb.c1, fb.c3r + fb.cdr,
-                                        (const __half*)(h->ws + fb.w_fwd), (const float*)(h->ws + fb.bias), &t);
-        } else {
-          t.out32 = (float*)red32.base;
-          rc = umma_conv_bind_fwd(h->umma_ctx, fb.fwd, xp, redp, h->F, fb.cx, fb.c3r + fb.cdr, 1, 0, 1, (const __half*)(h->ws + fb.w_fwd),
-                                  (const float*)(h->ws + fb.bias), &t);
-        }
-        if (rc) return h->fail(rc, "tc fused fwd bind(" + o3.id + "): " + ssnb::thread_error());
-        if (!fb.fwd.p.tc_ok) continue;
-        if (h->cfg.training) {
-          View dredp = h->planes(o3.out_val, true); dredp.C = fb.c3r + fb.cdr;
-          View d1p = fb.op1 >= 0 ? h->planes(h->ops[fb.op1].out_val, true) : dredp;
-          View dxp = h->planes(o3.in_val, true); dxp.base = nullptr; dxp.lo_off = 0;
-          UmmaTcOpts tg; tg.w_lo_off = (long long)fb.w_dg_plane; tg.out32 = (float*)h->view(o3.in_val, true).base; tg.alpha = 1.0f / gs; tg.alpha_dev = alpha_dev;
-          rc = umma_conv_bind_fused_dgrad(h->umma_ctx, fb.dgrad, d1p, dredp, dxp, h->F, fb.cx, fb.c1, fb.c3r + fb.cdr, (const __half*)(h->ws + fb.w_dg),
-                                          od.grad_accumulate, &tg);
-          if (rc) return h->fail(rc, "tc fused dgrad bind(" + o3.id + "): " + ssnb::thread_error());
-          if (!fb.dgrad.p.tc_ok) continue;
-          // zero the K padding of the concatenated data-gradient weights once (both planes); split_all_kernel never writes it
-          if (cudaMemset(h->ws + fb.w_dg, 0, 2 * fb.w_dg_plane) != cudaSuccess) cudaGetLastError();
-        }
-        fb.enabled = true;
-        const int leader = fb.op1 >= 0 ? fb.op1 : fb.op_r3;
-        for (int j : {fb.op1, fb.op_r3, fb.op_rd})
-          if (j >= 0) { h->ops[j].fuse_block = (int)bi; h->ops[j].fuse_role = (j == leader) ? 1 : 2; }
-      }
-    }
-    // ReLU-mask fusion (same rule as the FAST schedule below): the consumer with the smallest forward index is the LAST writer
-    // of a value's gradient in the reverse schedule; when that is a tensor-core data gradient its fp32 epilogue applies
-    // dz = dy * (y > 0) and emits the value's gradient operand planes (dz * grad_scale), so the producing convolutions run
-    // neither a mask pass nor a split pass: their bias gradients ride on the weight-gradient MMAs (ones operand).
-    // SSNB_DISABLE_FUSION=1 keeps one mask + bias + split pass per convolution.
-    const char* disf_tc = getenv("SSNB_DISABLE_FUSION");
-    if (use_tc && h->cfg.training && !(disf_tc && disf_tc[0] == '1')) {
-      h->fold_pools = true;
-      std::vector<int> first_consumer(h->vals.size(), -1);
-      for (int i = 0; i < (int)h->ops.size(); ++i)
-        if (first_consumer[h->ops[i].in_val] < 0) first_consumer[h->ops[i].in_val] = i;
-      for (size_t v = 0; v < h->vals.size(); ++v) {
-        const int fc = first_consumer[v];
-        if (fc < 0 || h->vals[v].name == "data" || !h->bufs[h->vals[v].buf].plane) continue;
-        bool conv_made = false;                    // only buffers that hold convolution outputs have a ReLU to differentiate
-        for (const Op& q : h->ops) conv_made = conv_made || (q.kind == OP_CONV && h->vals[q.out_val].buf == h->vals[v].buf);
-        if (!conv_made) continue;
-        Op& c = h->ops[fc];
-        if (c.kind == OP_CONV && c.fuse_role == 1 && h->fused[c.fuse_block].enabled) {
-          c.dgrad_masks = true;
-          umma_conv_set_mask_tc(h->fused[c.fuse_block].dgrad, h->view((int)v, false), h->planes((int)v, true), gs, h->tc_flag);
-        } else if (c.kind == OP_CONV && c.fuse_role == 0 && c.umma_dgrad.enabled) {
-          c.dgrad_masks = true;
-          umma_conv_set_mask_tc(c.umma_dgrad, h->view((int)v, false), h->planes((int)v, true), gs, h->tc_flag);
-        }
-      }
-      for (Op& o : h->ops) {
-        if (o.kind != OP_CONV) continue;
-        int w = o.out_val;
-        if (first_consumer[w] < 0) {               // a slice of a concat buffer: gradients are written through the whole-buffer value
-          const Value& ov = h->vals[o.out_val];
-          for (size_t v = 0; v < h->vals.size(); ++v)
-            if (h->vals[v].buf == ov.buf && h->vals[v].coff == 0 && h->vals[v].C == h->bufs[ov.buf].C && first_consumer[v] >= 0) { w = (int)v; break; }
-        }
-        if (first_consumer[w] >= 0 && h->ops[first_consumer[w]].dgrad_masks) o.dy_premasked = true;
-        o.bias_in_wgrad = o.dy_premasked && o.conv != 0 && o.umma_wgrad.enabled;
-      }
-    }
-    return SSNB_OK;
-  }
-  // bind tensor-core plans (tensor maps need final addresses); SSNB_DISABLE_UMMA=1 keeps FAST mode on the SIMT kernels
-  const char* dis = getenv("SSNB_DISABLE_UMMA");
-  const bool use_umma = h->fp16 && !(dis && dis[0] == '1');
+  // Bind the tensor-core plans (tensor maps need final addresses).  The diagnostic switches are read here, once per engine:
+  // SSNB_DISABLE_UMMA=1 keeps every convolution on the SIMT kernels (FAST: fp16; EXACT_TC: fp32, the EXACT_FP32 arithmetic
+  // that tools/umma_diag.py diffs the tensor-core launches against), SSNB_DISABLE_UMMA_WGRAD=1 only the weight gradients, and
+  // SSNB_DISABLE_FUSION=1 turns off sibling fusion, last-writer masking and the max-pool backward folding.
+  const bool training = h->cfg.training != 0;
+  const bool use_tc = h->tensor_cores() && !env_on("SSNB_DISABLE_UMMA");
+  const bool use_wgrad = use_tc && training && !env_on("SSNB_DISABLE_UMMA_WGRAD");
+  const bool fuse = !env_on("SSNB_DISABLE_FUSION");
+  const float gs = h->cfg.grad_scale;
   for (Op& o : h->ops) {
-    o.umma.enabled = false; o.umma_dgrad.enabled = false; o.umma_wgrad.enabled = false;
-    if (o.kind != OP_CONV || !use_umma) continue;
+    o.umma.enabled = o.umma_dgrad.enabled = o.umma_wgrad.enabled = false;
+    o.fuse_role = 0; o.fuse_block = -1; o.dgrad_masks = o.dy_premasked = o.bias_in_wgrad = false;
+  }
+  for (FusedBlock& fb : h->fused) fb.enabled = false;
+  // FAST folds the max-pool backward into its producer on the SIMT kernels as well; EXACT_TC only in the tensor-core training schedule
+  h->fold_pools = fuse && (h->fast() || (use_tc && training));
+  // Where EXACT_TC runs a convolution.  umma_conv_kernel's split-operand epilogue covers the plans with UmmaConvParams::tc_ok:
+  // stride-1 tiles of 1, 4 or 9 taps over images at least 7 pixels wide with 32-byte aligned outputs.  conv1's forward, the
+  // per-layer data gradients and both fused sibling launches run on the tensor cores only when tc_ok holds, and otherwise on
+  // the fp32 SIMT kernels.  The per-layer forward is not gated: the stride-2 3x3 forwards (tc_ok = 0, element-stride A
+  // boxes) run on umma_conv_kernel as well.  Stride-2 data gradients are stride-1 convolutions of the zero-upsampled dz and
+  // pass tc_ok.  In the default schedule every gated plan passes, so no convolution of EXACT_TC runs on the SIMT kernels.
+  // FAST runs every plan it binds.
+  auto tc_gate = [&](UmmaConvPlan& p) {
+    if (h->exact_tc() && !p.p.tc_ok) p.enabled = false;
+    return p.enabled;
+  };
+  for (Op& o : h->ops) {
+    if (o.kind != OP_CONV || !use_tc) continue;
     const ConvSpec& c = h->convs[o.conv];
-    const char* disw = getenv("SSNB_DISABLE_UMMA_WGRAD");
-    const bool use_wgrad = h->cfg.training && !(disw && disw[0] == '1');
-    const View in = h->view(o.in_val, false), out = h->view(o.out_val, false);
+    const PackedConv& pk = h->packed[o.conv];
+    UmmaTcOpts tf, tg;
     int rc = 0;
     if (o.conv == 0) {
       // conv1 7x7/2: four vertical taps over the packed space-to-depth input (r = 2*dr + a - 1, s = 2*ds + b - 1)
       const int Ck = 4 * h->Cs;
-      View xs; xs.base = h->ws + h->s2d_off; xs.H = 112; xs.W = 112; xs.C = Ck; xs.pitch = Ck; xs.coff = 0;
+      View xs; xs.base = h->ws + h->s2d_off; xs.H = 112; xs.W = 112; xs.C = Ck; xs.pitch = Ck; xs.coff = 0; xs.lo_off = (long long)h->s2d_plane;
       int dy[4], dx[4];
       for (int t = 0; t < 4; ++t) { dy[t] = t - 2; dx[t] = 0; }
-      rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, out, h->F, Ck, c.cout, 4, dy, dx, (const __half*)(h->ws + h->s2d_w_off),
-                               (const float*)(h->ws + h->packed[0].bias), 1);
-      if (rc) return h->fail(rc, "umma conv1 bind: " + ssnb::thread_error());
-      if (use_wgrad) {
-        rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->view(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
-                                  (float*)(h->ws + o.partial_off), 128);
-        if (rc) return h->fail(rc, "umma conv1 wgrad bind: " + ssnb::thread_error());
-      }
+      rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, h->operand(o.out_val, false), h->F, Ck, c.cout, 4, dy, dx, (const __half*)(h->ws + h->s2d_w_off),
+                               (const float*)(h->ws + pk.bias), o.raw ? 0 : 1, h->tc_opts(tf, h->s2d_w_plane, h->view(o.out_val, false).base, 1.0f, pk.wmax));
+      if (rc) return h->fail(rc, "conv1 bind: " + ssnb::thread_error());
+      tc_gate(o.umma);
+      if (use_wgrad && (rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->operand(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
+                                                  (float*)(h->ws + o.partial_off), 128)))
+        return h->fail(rc, "conv1 wgrad bind: " + ssnb::thread_error());
       continue;
     }
     if (c.cin % 8 != 0 || c.k * c.k > UMMA_MAX_TAPS) continue;
-    rc = umma_conv_bind_fwd(h->umma_ctx, o.umma, in, out, h->F, c.cin, c.cout, c.k, c.pad, c.stride,
-                            (const __half*)(h->ws + h->packed[o.conv].wd), (const float*)(h->ws + h->packed[o.conv].bias));
-    if (rc) return h->fail(rc, "umma_conv_bind_fwd(" + c.id + "): " + ssnb::thread_error());
-    if (!h->cfg.training) continue;
-    // backward operands: the output gradient (stride-2 layers: its zero-upsampled copy at input resolution)
-    View dz = h->view(o.out_val, true);
-    if (c.stride == 2) { dz.base = h->ws + h->up_off; dz.H = in.H; dz.W = in.W; dz.C = c.cout; dz.pitch = c.cout; dz.coff = 0; }
-    rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, h->view(o.in_val, true), h->F, c.cin, c.cout, c.k, c.pad,
-                              (const __half*)(h->ws + h->packed[o.conv].wf), o.grad_accumulate);
-    if (rc) return h->fail(rc, "umma_conv_bind_dgrad(" + c.id + "): " + ssnb::thread_error());
-    if (use_wgrad) {
-      // stride-2 layers: dz at its own (output) resolution, the x boxes step over the input with element stride 2
-      rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->view(o.out_val, true), in, h->F, c.cin, c.cout, c.k, c.pad,
-                           (float*)(h->ws + o.partial_off), o.tsplits, c.stride);
-      if (rc) return h->fail(rc, "umma_wgrad_bind(" + c.id + "): " + ssnb::thread_error());
-    }
+    rc = umma_conv_bind_fwd(h->umma_ctx, o.umma, h->operand(o.in_val, false), h->operand(o.out_val, false), h->F, c.cin, c.cout, c.k, c.pad,
+                            c.stride, h->w_fwd(pk), (const float*)(h->ws + pk.bias), h->tc_opts(tf, pk.wplane, h->view(o.out_val, false).base, 1.0f, pk.wmax));
+    if (rc) return h->fail(rc, "bind_fwd(" + c.id + "): " + ssnb::thread_error());
+    if (!training) continue;
+    // data gradient: stride-2 layers read the zero-upsampled dz at input resolution.  EXACT_TC writes the fp32 d(in) only:
+    // its consumer masks and splits it.
+    const View in = h->view(o.in_val, false);
+    View dz = h->operand(o.out_val, true);
+    if (c.stride == 2) { dz.base = h->ws + h->up_off; dz.H = in.H; dz.W = in.W; dz.C = c.cout; dz.pitch = c.cout; dz.coff = 0; dz.lo_off = (long long)h->up_plane; }
+    View dx = h->view(o.in_val, true);
+    const UmmaTcOpts* og = h->tc_opts(tg, pk.wplane, dx.base, 1.0f / gs, pk.wmax);
+    if (og) dx.base = nullptr;
+    rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, dx, h->F, c.cin, c.cout, c.k, c.pad, h->w_dgrad(pk), o.grad_accumulate, og);
+    if (rc) return h->fail(rc, "bind_dgrad(" + c.id + "): " + ssnb::thread_error());
+    tc_gate(o.umma_dgrad);
+    // weight gradient: stride-2 layers read dz at its own (output) resolution, the x boxes step over the input with element stride 2
+    if (use_wgrad && (rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->operand(o.out_val, true), h->operand(o.in_val, false), h->F, c.cin, c.cout,
+                                           c.k, c.pad, (float*)(h->ws + o.partial_off), o.tsplits, c.stride)))
+      return h->fail(rc, "wgrad_bind(" + c.id + "): " + ssnb::thread_error());
   }
-  // horizontal fusion of the sibling 1x1 convolutions of each inception block (SSNB_DISABLE_FUSION=1 turns it off)
-  const char* disf = getenv("SSNB_DISABLE_FUSION");
-  h->fold_pools = !(disf && disf[0] == '1');
-  for (Op& o : h->ops) { o.fuse_role = 0; o.fuse_block = -1; }
-  for (size_t bi = 0; bi < h->fused.size(); ++bi) {
+  // horizontal fusion of the sibling 1x1 convolutions of each inception block: ONE forward launch (stacked weights; the first
+  // c1 columns land in the concat buffer, the rest in the shared reduce buffer) and ONE data-gradient launch (K-concatenated
+  // dz from two sources) instead of three read-modify-write passes over the block input's gradient
+  for (size_t bi = 0; bi < h->fused.size() && use_tc && fuse; ++bi) {
     FusedBlock& fb = h->fused[bi];
-    fb.enabled = false;
-    if (!use_umma || (disf && disf[0] == '1')) continue;
-    Op& o3 = h->ops[fb.op_r3]; Op& od = h->ops[fb.op_rd];
-    const View x = h->view(o3.in_val, false);
-    View red = h->view(o3.out_val, false); red.C = fb.c3r + fb.cdr;          // both reduce outputs: adjacent slices of one buffer
+    const Op& o3 = h->ops[fb.op_r3]; const Op& od = h->ops[fb.op_rd];
+    if (!o3.umma.enabled || !od.umma.enabled) continue;
+    const int nr = fb.c3r + fb.cdr;                  // both reduce outputs: adjacent slices of one buffer
+    const View x = h->operand(o3.in_val, false);
+    View red = h->operand(o3.out_val, false); red.C = nr;
+    UmmaTcOpts tf, tg;
     int rc;
-    if (fb.op1 >= 0) rc = umma_conv_bind_fused_fwd(h->umma_ctx, fb.fwd, x, h->view(h->ops[fb.op1].out_val, false), red, h->F, fb.cx, fb.c1,
-                                                  fb.c3r + fb.cdr, (const __half*)(h->ws + fb.w_fwd), (const float*)(h->ws + fb.bias));
-    else rc = umma_conv_bind_fwd(h->umma_ctx, fb.fwd, x, red, h->F, fb.cx, fb.c3r + fb.cdr, 1, 0, 1, (const __half*)(h->ws + fb.w_fwd),
-                                 (const float*)(h->ws + fb.bias));
+    if (fb.op1 >= 0) {
+      const int v1 = h->ops[fb.op1].out_val;
+      const UmmaTcOpts* of = h->tc_opts(tf, fb.w_fwd_plane, h->view(v1, false).base, 1.0f, fb.wmax);
+      tf.out32_2 = (float*)h->view(o3.out_val, false).base;
+      rc = umma_conv_bind_fused_fwd(h->umma_ctx, fb.fwd, x, h->operand(v1, false), red, h->F, fb.cx, fb.c1, nr, (const __half*)(h->ws + fb.w_fwd),
+                                    (const float*)(h->ws + fb.bias), of);
+    } else {
+      rc = umma_conv_bind_fwd(h->umma_ctx, fb.fwd, x, red, h->F, fb.cx, nr, 1, 0, 1, (const __half*)(h->ws + fb.w_fwd), (const float*)(h->ws + fb.bias),
+                              h->tc_opts(tf, fb.w_fwd_plane, h->view(o3.out_val, false).base, 1.0f, fb.wmax));
+    }
     if (rc) return h->fail(rc, "fused fwd bind(" + o3.id + "): " + ssnb::thread_error());
-    if (h->cfg.training) {
-      View dred = h->view(o3.out_val, true); dred.C = fb.c3r + fb.cdr;
-      View d1 = fb.op1 >= 0 ? h->view(h->ops[fb.op1].out_val, true) : dred;
-      rc = umma_conv_bind_fused_dgrad(h->umma_ctx, fb.dgrad, d1, dred, h->view(o3.in_val, true), h->F, fb.cx, fb.c1, fb.c3r + fb.cdr,
-                                      (const __half*)(h->ws + fb.w_dg), od.grad_accumulate);
+    if (!tc_gate(fb.fwd)) continue;
+    if (training) {
+      View dred = h->operand(o3.out_val, true); dred.C = nr;
+      const View d1 = fb.op1 >= 0 ? h->operand(h->ops[fb.op1].out_val, true) : dred;
+      View dx = h->view(o3.in_val, true);
+      const UmmaTcOpts* og = h->tc_opts(tg, fb.w_dg_plane, dx.base, 1.0f / gs, fb.wmax);
+      if (og) dx.base = nullptr;
+      rc = umma_conv_bind_fused_dgrad(h->umma_ctx, fb.dgrad, d1, dred, dx, h->F, fb.cx, fb.c1, nr, (const __half*)(h->ws + fb.w_dg), od.grad_accumulate, og);
       if (rc) return h->fail(rc, "fused dgrad bind(" + o3.id + "): " + ssnb::thread_error());
+      if (!tc_gate(fb.dgrad)) continue;
+      // EXACT_TC: zero the K padding of the concatenated data-gradient weights once (both planes); split_all_kernel never
+      // writes it.  FAST assembles these weights by copies and zeroes them on every pack.
+      if (h->exact_tc() && cudaMemset(h->ws + fb.w_dg, 0, 2 * fb.w_dg_plane) != cudaSuccess) cudaGetLastError();
     }
     fb.enabled = true;
     const int leader = fb.op1 >= 0 ? fb.op1 : fb.op_r3;
     for (int j : {fb.op1, fb.op_r3, fb.op_rd})
       if (j >= 0) { h->ops[j].fuse_block = (int)bi; h->ops[j].fuse_role = (j == leader) ? 1 : 2; }
   }
-  // ReLU-mask fusion: the consumer with the smallest forward index is the last writer of a value's gradient in the
-  // reverse schedule (sibling followers are folded into their leader); if that writer is a tensor-core data gradient or the
-  // global pool, it applies dz = dy * (y > 0) in its epilogue and the producing conv skips its own mask pass.
-  for (Op& o : h->ops) { o.dgrad_masks = false; o.dy_premasked = false; }
-  if (use_umma && h->cfg.training) {
+  // ReLU-mask fusion: the consumer with the smallest forward index is the LAST writer of a value's gradient in the reverse
+  // schedule (sibling followers are folded into their leader).  When that writer is a tensor-core data gradient, its epilogue
+  // applies dz = dy * (y > 0) (EXACT_TC: and emits the gradient's operand planes dz * grad_scale), so the producing
+  // convolutions run neither a mask pass nor a split pass, and their bias gradients ride on the weight-gradient MMAs (ones operand).
+  if (use_tc && training && fuse) {
     std::vector<int> first_consumer(h->vals.size(), -1);
     for (int i = 0; i < (int)h->ops.size(); ++i)
       if (first_consumer[h->ops[i].in_val] < 0) first_consumer[h->ops[i].in_val] = i;
     for (size_t v = 0; v < h->vals.size(); ++v) {
       const int fc = first_consumer[v];
       if (fc < 0 || h->vals[v].name == "data") continue;
+      if (h->exact_tc() && !h->bufs[h->vals[v].buf].plane) continue;      // no operand planes to emit
       bool conv_made = false;                    // only buffers that hold convolution outputs have a ReLU to differentiate
       for (const Op& q : h->ops) conv_made = conv_made || (q.kind == OP_CONV && h->vals[q.out_val].buf == h->vals[v].buf);
       if (!conv_made) continue;
       Op& c = h->ops[fc];
-      if (c.kind == OP_GPOOL) c.dgrad_masks = true;
-      else if (c.kind == OP_CONV && (c.fuse_role == 1 ? h->fused[c.fuse_block].enabled : (c.fuse_role == 0 && c.umma_dgrad.enabled))) {
+      UmmaConvPlan* dg = nullptr;
+      if (c.kind == OP_CONV && c.fuse_role == 1 && h->fused[c.fuse_block].enabled) dg = &h->fused[c.fuse_block].dgrad;
+      else if (c.kind == OP_CONV && c.fuse_role == 0 && c.umma_dgrad.enabled) dg = &c.umma_dgrad;
+      if (dg) {
         c.dgrad_masks = true;
-        const View yv = h->view((int)v, false);
-        if (c.fuse_role == 1) umma_conv_set_mask(h->fused[c.fuse_block].dgrad, yv); else umma_conv_set_mask(c.umma_dgrad, yv);
+        if (h->exact_tc()) umma_conv_set_mask_tc(*dg, h->view((int)v, false), h->planes((int)v, true), gs, h->tc_flag);
+        else umma_conv_set_mask(*dg, h->view((int)v, false));
+      } else if (c.kind == OP_GPOOL && h->fast()) {
+        c.dgrad_masks = true;       // FAST only: gpool_bwd<float> writes no operand planes, so EXACT_TC keeps the producers' split pass
       }
     }
     for (Op& o : h->ops) {
@@ -1005,7 +881,7 @@ int ssnb_pack_weights(ssnb_handle h, const float* const* w, const float* const* 
                       const float* const* beta, const float* const* mean, const float* const* var, void* stream) {
   if (!h || !h->ws) return h ? h->fail(SSNB_ESTATE, "set_workspace first") : SSNB_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  if (h->tc && cudaMemsetAsync(h->ws + h->wmax_off, 0, (h->convs.size() + 16) * 8, s) != cudaSuccess) return h->fail(SSNB_ECUDA, "pack_weights: memset");
+  if (h->exact_tc() && cudaMemsetAsync(h->ws + h->wmax_off, 0, (h->convs.size() + 16) * 8, s) != cudaSuccess) return h->fail(SSNB_ECUDA, "pack_weights: memset");
   {
     // fold + re-layout of all 69 layers in a few launches (PACK_MAX entries per launch); EXACT_TC: every fold launch first (the
     // layers of a fused sibling block share one absmax slot), then the hi/lo splits
@@ -1038,12 +914,12 @@ int ssnb_pack_weights(ssnb_handle h, const float* const* w, const float* const* 
       PackEntry& q = pt.back().e[pt.back().n++];
       q.w = w[i]; q.b = b[i]; q.gamma = gamma[i]; q.beta = beta[i]; q.mean = mean[i]; q.var = var[i];
       q.wf = h->ws + p.wf; q.wd = h->ws + p.wd; q.bias = (float*)(h->ws + p.bias); q.scale = (float*)(h->ws + p.scale);
-      q.absmax = h->tc ? (float*)(h->ws + p.wmax) : nullptr;
+      q.absmax = h->exact_tc() ? (float*)(h->ws + p.wmax) : nullptr;
       q.cout = c.cout; q.cin = c.cin; q.k = c.k; q.block0 = pblocks.back();
       q.nofold = (h->bn1_train && i == 0) ? 1 : 0; q.pad_[0] = q.pad_[1] = q.pad_[2] = 0;
-      q.bias_b = (h->tc && fb) ? (float*)(h->ws + fb->bias) + mb.row : nullptr;
+      q.bias_b = (h->exact_tc() && fb) ? (float*)(h->ws + fb->bias) + mb.row : nullptr;
       pblocks.back() += pack_ctas(c.cout, c.cin, c.k);
-      if (h->tc) {
+      if (h->exact_tc()) {
         SplitEntry& e = stt.back().e[stt.back().n++];
         e.wf = (const float*)(h->ws + p.wf); e.wd = (const float*)(h->ws + p.wd);
         e.wf16 = (__half*)(h->ws + p.wf16); e.wd16 = (__half*)(h->ws + p.wd16); e.plane_bytes = (long long)p.wplane; e.n = n;
@@ -1062,27 +938,23 @@ int ssnb_pack_weights(ssnb_handle h, const float* const* w, const float* const* 
       }
     }
     for (size_t k = 0; k < pt.size(); ++k) {
-      int rc = h->fp16 ? launch_pack_all<__half>(pt[k], pblocks[k], s) : launch_pack_all<float>(pt[k], pblocks[k], s);
+      int rc = h->fast() ? launch_pack_all<__half>(pt[k], pblocks[k], s) : launch_pack_all<float>(pt[k], pblocks[k], s);
       if (rc) return h->fail(rc, "pack_weights: " + ssnb::thread_error());
     }
-    if (h->tc)
+    if (h->exact_tc())
       for (size_t k = 0; k < stt.size(); ++k)
         if (int rc = launch_split_all(stt[k], sblocks[k], s)) return h->fail(rc, "pack_weights split: " + ssnb::thread_error());
   }
-  if (h->tc && h->ops.size() && h->ops[0].umma.enabled) {
-    for (int pl = 0; pl < 2; ++pl) {
-      int rc = launch_pack_conv1_s2d((const __half*)(h->ws + h->packed[0].wd16 + pl * h->packed[0].wplane), h->convs[0].cout, h->convs[0].cin, h->Cs,
+  if (h->ops.size() && h->ops[0].umma.enabled) {      // conv1's space-to-depth weights, every operand plane
+    const PackedConv& p = h->packed[0];
+    for (int pl = 0; pl < h->nplanes(); ++pl) {
+      int rc = launch_pack_conv1_s2d((const __half*)((const char*)h->w_fwd(p) + pl * p.wplane), h->convs[0].cout, h->convs[0].cin, h->Cs,
                                      (__half*)(h->ws + h->s2d_w_off + pl * h->s2d_w_plane), s);
-      if (rc) return h->fail(rc, "pack conv1 s2d (tc): " + ssnb::thread_error());
+      if (rc) return h->fail(rc, "pack conv1 s2d: " + ssnb::thread_error());
     }
   }
-  if (h->fp16 && h->ops.size() && h->ops[0].umma.enabled) {
-    int rc = launch_pack_conv1_s2d((const __half*)(h->ws + h->packed[0].wd), h->convs[0].cout, h->convs[0].cin, h->Cs,
-                                   (__half*)(h->ws + h->s2d_w_off), s);
-    if (rc) return h->fail(rc, "pack conv1 s2d: " + ssnb::thread_error());
-  }
   for (FusedBlock& fb : h->fused) {
-    if (!fb.enabled || !h->fp16) continue;          // EXACT_TC: split_all_kernel wrote the fused operands directly
+    if (!fb.enabled || !h->fast()) continue;          // EXACT_TC: split_all_kernel wrote the fused operands directly
     // forward: rows of wd ([co][ci]) stacked; bias stacked.  data gradient: wf ([ci][co]) concatenated along K,
     // the 1x1 part padded to a multiple of 64 so each K chunk has a single activation source.
     const int k1p = (fb.c1 + 63) / 64 * 64, kf = k1p + fb.c3r + fb.cdr;
@@ -1121,10 +993,10 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
   cudaStream_t s = (cudaStream_t)stream;
   const View d = h->view(h->val_by_name["data"], false);
   int rc;
-  h->s2d_ready = (h->fp16 || h->tc) && h->ops[0].umma.enabled;
-  if (h->s2d_ready && h->tc) rc = launch_nchw_to_s2d_split(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
+  h->s2d_ready = h->tensor_cores() && h->ops[0].umma.enabled;
+  if (h->s2d_ready && h->exact_tc()) rc = launch_nchw_to_s2d_split(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
   else if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), h->Cs, s);
-  else rc = h->fp16 ? launch_nchw_to_nhwc<__half>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s)
+  else rc = h->fast() ? launch_nchw_to_nhwc<__half>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s)
                     : launch_nchw_to_nhwc<float>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s);
   if (rc) { h->s2d_ready = false; return h->fail(rc, "input layout: " + ssnb::thread_error()); }
   for (size_t i = 0; i < h->ops.size(); ++i) {
@@ -1185,7 +1057,7 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
     return 0;
   };
   auto finalize = [&]() -> int {
-    const float gs = (h->fp16 || h->tc) ? h->cfg.grad_scale : 1.0f;
+    const float gs = h->tensor_cores() ? h->cfg.grad_scale : 1.0f;
     FinalizeTable t; t.n = 0; t.total_blocks = 0; t.flag = h->tc_flag;
     auto flush = [&]() -> int { int rc = launch_wgrad_finalize_all(t, 1.0f / gs, h->grad_accumulate, s); t.n = 0; t.total_blocks = 0; return rc; };
     for (int oi : h->pending_finalize) {
@@ -1243,10 +1115,10 @@ int ssnb_value_write(ssnb_handle h, const char* name, int grad, const float* src
   if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
   if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
   const View v = h->view(it->second, grad != 0);
-  const float sc = (grad && h->fp16) ? h->cfg.grad_scale : 1.0f;
-  int rc = h->fp16 ? launch_nchw_to_nhwc<__half>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream)
+  const float sc = (grad && h->fast()) ? h->cfg.grad_scale : 1.0f;
+  int rc = h->fast() ? launch_nchw_to_nhwc<__half>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream)
                    : launch_nchw_to_nhwc<float>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream);
-  if (!rc && h->tc && !grad) rc = tc_split_value(h, it->second, false, 1.0f, (cudaStream_t)stream);   // activation planes follow the fp32 value
+  if (!rc && h->exact_tc() && !grad) rc = tc_split_value(h, it->second, false, 1.0f, (cudaStream_t)stream);   // activation planes follow the fp32 value
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
 }
 
@@ -1256,13 +1128,13 @@ int ssnb_value_read(ssnb_handle h, const char* name, int grad, float* dst_nchw, 
   if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
   if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
   if (grad & 2) {       // diagnostic: read hi + lo of the value's EXACT_TC operand planes (bit 0: gradient planes, un-scaled)
-    if (!h->tc || !h->bufs[h->vals[it->second].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
+    if (!h->exact_tc() || !h->bufs[h->vals[it->second].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
     int rc = launch_planes_to_nchw(h->planes(it->second, (grad & 1) != 0), h->F, (grad & 1) ? 1.0f / h->cfg.grad_scale : 1.0f, dst_nchw, (cudaStream_t)stream);
     return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
   }
   const View v = h->view(it->second, grad != 0);
-  const float sc = (grad && h->fp16) ? 1.0f / h->cfg.grad_scale : 1.0f;
-  int rc = h->fp16 ? launch_nhwc_to_nchw<__half>(v, h->F, sc, dst_nchw, (cudaStream_t)stream)
+  const float sc = (grad && h->fast()) ? 1.0f / h->cfg.grad_scale : 1.0f;
+  int rc = h->fast() ? launch_nhwc_to_nchw<__half>(v, h->F, sc, dst_nchw, (cudaStream_t)stream)
                    : launch_nhwc_to_nchw<float>(v, h->F, sc, dst_nchw, (cudaStream_t)stream);
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
 }

@@ -157,47 +157,6 @@ __global__ void relu_mask_kernel(T* __restrict__ dy, int dpitch, int dcoff, cons
   if (!(to_f<T>(y[p * ypitch + ycoff + c]) > 0.f)) dy[p * dpitch + dcoff + c] = from_f<T>(0.f);
 }
 
-template <typename T>
-__global__ void fill_zero_kernel(T* __restrict__ v, int pitch, int coff, long long pixels, int C) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= pixels * C) return;
-  v[(i / C) * pitch + coff + (int)(i % C)] = from_f<T>(0.f);
-}
-
-// fold BN: s = gamma / sqrt(var + eps); W' = W*s ; b' = (b - mean)*s + beta
-template <typename T>
-__global__ void pack_conv_kernel(const float* __restrict__ w, const float* __restrict__ b,
-                                 const float* __restrict__ gamma, const float* __restrict__ beta,
-                                 const float* __restrict__ mean, const float* __restrict__ var, int Cout, int Cin, int k,
-                                 T* __restrict__ wf, T* __restrict__ wd, float* __restrict__ bias_f,
-                                 float* __restrict__ scale, float* __restrict__ absmax) {
-  const int taps = k * k;
-  const long long total = (long long)Cout * Cin * taps;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < Cout) {
-    const float s = gamma[i] / sqrtf(var[i] + 1e-5f);
-    scale[i] = s;
-    bias_f[i] = (b[i] - mean[i]) * s + beta[i];
-  }
-  float av = 0.f;
-  if (i < total) {
-    const int tap = (int)(i % taps);
-    const int ci = (int)((i / taps) % Cin);
-    const int co = (int)(i / ((long long)taps * Cin));
-    const float s = gamma[co] / sqrtf(var[co] + 1e-5f);
-    const float fv = w[i] * s;
-    const T v = from_f<T>(fv);
-    wf[((long long)tap * Cin + ci) * Cout + co] = v;
-    wd[((long long)tap * Cout + co) * Cin + ci] = v;
-    av = fabsf(fv);
-  }
-  if (absmax) {          // SSNB_EXACT_TC: largest folded weight of the layer (non-negative floats order like their bit patterns)
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) av = fmaxf(av, __shfl_xor_sync(0xffffffffu, av, o));
-    if (threadIdx.x % 32 == 0 && av > 0.f) atomicMax(reinterpret_cast<int*>(absmax), __float_as_int(av));
-  }
-}
-
 // all layers of the network in a few launches (69 per-layer launches would be mostly launch latency: the weights are
 // re-packed after every optimizer step)
 template <typename T>
@@ -295,9 +254,6 @@ template <typename T> int launch_pack_all(const PackTable& t, int total_blocks, 
 template int launch_pack_all<float>(const PackTable&, int, cudaStream_t);
 template int launch_pack_all<__half>(const PackTable&, int, cudaStream_t);
 
-namespace {
-}  // namespace
-
 #define V(T, v) reinterpret_cast<T*>((v).base)
 
 template <typename T> int launch_nchw_to_nhwc(const float* src, int F, int C, int H, int W, View dst, float scale, cudaStream_t s) {
@@ -355,22 +311,6 @@ template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t 
   SSNB_LAUNCH_CHECK("relu_mask_kernel");
   return 0;
 }
-template <typename T> int launch_fill_zero(View v, int F, cudaStream_t s) {
-  const long long px = (long long)F * v.H * v.W;
-  fill_zero_kernel<T><<<blocks_for(px * v.C), TPB, 0, s>>>(V(T, v), v.pitch, v.coff, px, v.C);
-  SSNB_LAUNCH_CHECK("fill_zero_kernel");
-  return 0;
-}
-template <typename T>
-int launch_pack_conv(const float* w, const float* b, const float* gamma, const float* beta, const float* mean,
-                     const float* var, int Cout, int Cin, int k, T* wf, T* wd, float* bias_f, float* scale,
-                     cudaStream_t s, float* absmax) {
-  const long long n = (long long)Cout * Cin * k * k;
-  pack_conv_kernel<T><<<blocks_for(n > Cout ? n : Cout), TPB, 0, s>>>(w, b, gamma, beta, mean, var, Cout, Cin, k, wf, wd, bias_f, scale, absmax);
-  SSNB_LAUNCH_CHECK("pack_conv_kernel");
-  return 0;
-}
-
 #define INST(T)                                                                                              \
   template int launch_nchw_to_nhwc<T>(const float*, int, int, int, int, View, float, cudaStream_t);                 \
   template int launch_nhwc_to_nchw<T>(View, int, float, float*, cudaStream_t);                               \
@@ -379,10 +319,7 @@ int launch_pack_conv(const float* w, const float* b, const float* gamma, const f
   template int launch_avgpool3_fwd<T>(View, View, int, int, cudaStream_t);                                   \
   template int launch_gpool_fwd<T>(View, int, float*, cudaStream_t);                                         \
   template int launch_gpool_bwd<T>(const float*, float, View, int, const void*, cudaStream_t);                            \
-  template int launch_relu_mask<T>(View, View, int, cudaStream_t);                                           \
-  template int launch_fill_zero<T>(View, int, cudaStream_t);                                                 \
-  template int launch_pack_conv<T>(const float*, const float*, const float*, const float*, const float*,     \
-                                   const float*, int, int, int, T*, T*, float*, float*, cudaStream_t, float*);
+  template int launch_relu_mask<T>(View, View, int, cudaStream_t);
 INST(float)
 INST(__half)
 

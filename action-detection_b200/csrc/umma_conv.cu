@@ -372,9 +372,9 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   return 0;
 }
 
-// Which plans the split-operand (EXACT_TC) schedule runs on the tensor cores (UmmaConvParams::tc_ok): stride-1 layers of
-// 1, 4 or 9 taps on images at least 7 pixels wide whose outputs are 32-byte aligned NHWC slices; a fused sibling data
-// gradient (two K sources) only as a 1x1 layer.
+// UmmaConvParams::tc_ok: stride-1 layers of 1, 4 or 9 taps on images at least 7 pixels wide whose outputs are 32-byte
+// aligned NHWC slices; a fused sibling data gradient (two K sources) only as a 1x1 layer.  Which EXACT_TC launches require
+// it: ssnb_set_workspace (engine.cu).
 void mark_tc_ok(UmmaConvPlan& plan, int W, bool two_sources) {
   UmmaConvParams& p = plan.p;
   p.tc_ok = 0;
@@ -394,7 +394,7 @@ int umma_encode_f16(UmmaContext& ctx, CUtensorMap* m, int rank, void* addr, cons
   return encode(ctx, m, rank, addr, dims, strides, box, spatial_stride);
 }
 
-void umma_context_init(UmmaContext& ctx, bool fp16) { ctx.active = fp16; }
+void umma_context_init(UmmaContext&) {}
 void umma_context_destroy(UmmaContext&) {}
 
 int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int ntaps,

@@ -17,7 +17,6 @@ namespace ssnb {
 constexpr int UMMA_MAX_TAPS = 16;
 
 struct UmmaContext {
-  bool active = false;
   void* encode_tiled = nullptr;   // cuTensorMapEncodeTiled, resolved through cudaGetDriverEntryPoint
   int num_sms = 132;
 };
@@ -39,8 +38,8 @@ struct UmmaConvParams {
   int kchunks_a1, K1;             // K chunks [0, kchunks_a1) come from tmap_a (K1 real channels), the rest from tmap_a2
   int n_split;                    // output columns >= n_split go to out2 (second destination), else to out
   __half* out2; int out2_pitch, out2_coff;
-  // the split-operand (EXACT_TC) schedule runs this plan on the tensor cores: stride 1, 1 / 4 / 9 taps, images at least
-  // 7 pixels wide, 32-byte aligned output rows (the other layers of that schedule stay on the fp32 SIMT kernels)
+  // stride 1, 1 / 4 / 9 taps, images at least 7 pixels wide, 32-byte aligned output rows: the plans whose tensor-core launch
+  // the split-operand (EXACT_TC) schedule requires for conv1's forward, data gradients and fused launches (ssnb_set_workspace)
   int tc_ok;
   // data gradient that is the LAST writer of its output: fuse dz = dy * (y > 0), y = activation of the same value
   const __half* mask_y; int mask_pitch, mask_coff;
@@ -76,7 +75,7 @@ struct UmmaConvPlan {
 // (the bind call's own out/dx view then names the fp16 HI plane of the result, lo_off its LO plane; base == nullptr: no
 // planes are written), accumulator scale alpha
 struct UmmaTcOpts { long long w_lo_off = 0; float* out32 = nullptr; float alpha = 1.0f; const float* alpha_dev = nullptr; float* out32_2 = nullptr; };
-void umma_context_init(UmmaContext& ctx, bool fp16);
+void umma_context_init(UmmaContext& ctx);
 void umma_context_destroy(UmmaContext& ctx);
 // forward convolution plan (stride 1): in/out views, weights wd = [tap][cout][cin] fp16
 int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int k, int pad,

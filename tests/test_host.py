@@ -28,6 +28,19 @@ def test_conv_table_matches_oracle():
         assert conv_table(cin) == [tuple(r) for r in O.conv_layers(cin)]
 
 
+# ssnb_workspace_bytes at 288 frames, keyed by (precision, training, in_channels) -> (bn1_train 0, bn1_train 1); None: the
+# engine rejects the combination.  The split-K partials of the tensor-core weight gradients are sized from the SM count:
+# these sizes are for 132 SMs (H100 SXM, and the planner's default without a visible GPU).
+WORKSPACE_BYTES_288 = {
+    (0, 0, 3): (6264953856, 7190413312), (0, 0, 10): (6669749248, 7595208704),
+    (0, 1, 3): (12904324096, 14754627584), (0, 1, 10): (13718204416, 15568507904),
+    (1, 0, 3): (3678438400, None), (1, 0, 10): (4574518272, None),
+    (1, 1, 3): (7519796224, None), (1, 1, 10): (8634438656, None),
+    (2, 0, 3): (13159997440, 15010300928), (2, 0, 10): (14952333312, 16802636800),
+    (2, 1, 3): (25958072320, 29658063872), (2, 1, 10): (28171280384, 31871271936),
+}
+
+
 def test_engine_plan_without_gpu():
     from ssn_b200 import _lib
     cfg = _lib.Config(3, 18, _lib.EXACT_FP32, 1, 1.0)
@@ -46,6 +59,27 @@ def test_engine_plan_without_gpu():
     _lib.lib.ssnb_destroy(h)
     bad = _lib.Config(3, 0, 0, 0, 1.0)
     assert _lib.lib.ssnb_create(C.byref(bad), C.byref(h)) != 0
+    # every precision x training x in_channels x bn1_train plans, to the exact workspace size; FAST refuses bn1_train
+    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else 132
+    assert sorted({k[0] for k in WORKSPACE_BYTES_288}) == [_lib.EXACT_FP32, _lib.FAST_FP16, _lib.EXACT_TC]
+    for (prec, training, cin), sizes in WORKSPACE_BYTES_288.items():
+        for bn1, want in zip((0, 1), sizes):
+            cfg = _lib.Config(cin, 288, prec, training, 4096.0, bn1)
+            h = C.c_void_p()
+            rc = _lib.lib.ssnb_create(C.byref(cfg), C.byref(h))
+            if want is None:
+                assert rc == 4, (prec, training, cin, bn1, rc)        # SSNB_ENOSUPPORT
+                assert b"bn1_train" in _lib.lib.ssnb_last_error(None)
+                continue
+            _lib.check(rc)
+            try:
+                assert _lib.lib.ssnb_num_ops(h) == 69 + 13 + bn1
+                got = _lib.lib.ssnb_workspace_bytes(h)
+                assert got > 0 and got % 1024 == 0
+                if sms == 132:
+                    assert got == want, (prec, training, cin, bn1, got, want)
+            finally:
+                _lib.lib.ssnb_destroy(h)
 
 
 def test_module_surface_matches_reference(golden_dir):
