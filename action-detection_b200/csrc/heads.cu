@@ -106,7 +106,7 @@ __global__ void stpp_fwd_v4_kernel(const float* __restrict__ ft, const float* __
 #pragma unroll
   for (int t = 0; t < SMAX; ++t)
     if (t < S) v[t] = __ldg(reinterpret_cast<const float4*>(row + (long long)t * D));
-  const float s0 = scaling[p * 2], s1 = scaling[p * 2 + 1];
+  const float s0 = pt.n ? scaling[p * 2] : 0.f, s1 = pt.n ? scaling[p * 2 + 1] : 0.f;     // no parts: scaling may be NULL
   auto part = [&](int lo, int hi) {
     float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
@@ -134,7 +134,7 @@ __global__ void stpp_bwd_v4_kernel(const float* __restrict__ dcourse, const floa
   if (i >= (long long)n * D4) return;
   const int d = (int)(i % D4) * 4;
   const long long p = i / D4;
-  const float s0 = scaling[p * 2], s1 = scaling[p * 2 + 1];
+  const float s0 = pt.n ? scaling[p * 2] : 0.f, s1 = pt.n ? scaling[p * 2 + 1] : 0.f;     // no parts: scaling may be NULL
   float4 g[PMAX];
 #pragma unroll
   for (int q = 0; q < PMAX; ++q)
@@ -792,8 +792,9 @@ __global__ void sgd_groups_kernel(float* __restrict__ p, const float* __restrict
   p[i] = w - s_lr[lo] * b;
 }
 
+// n_parts == 0: the course mean alone (BinaryClassifier's segment mean, binary_model.py:229-230); no part array is read
 int fill_parts(PartTable& pt, int n_parts, const int* lo, const int* hi, const int* norm, const int* col, int clo, int chi, int S) {
-  if (n_parts < 1 || n_parts > MAX_PARTS) { set_thread_error("stpp: 1..32 parts supported"); return SSNB_EINVAL; }
+  if (n_parts < 0 || n_parts > MAX_PARTS) { set_thread_error("stpp: 0..32 parts supported"); return SSNB_EINVAL; }
   pt.n = n_parts;
   for (int i = 0; i < n_parts; ++i) {
     if (lo[i] < 0 || hi[i] > S || hi[i] < lo[i] || norm[i] <= 0 || col[i] > 1) { set_thread_error("stpp: bad part table"); return SSNB_EINVAL; }
@@ -816,7 +817,7 @@ int ssnb_stpp_fwd(const float* ft, const float* scaling, int n, int n_seg, int D
                   const int* part_hi, const int* part_norm, const int* part_scale_col, int course_lo, int course_hi,
                   float* course_ft, float* stpp_ft, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
-  if (!ft || !scaling || !course_ft || !stpp_ft || n < 0 || D <= 0) { set_thread_error("stpp_fwd: bad argument"); return SSNB_EINVAL; }
+  if (!ft || !course_ft || n < 0 || D <= 0 || (n_parts != 0 && (!scaling || !stpp_ft))) { set_thread_error("stpp_fwd: bad argument"); return SSNB_EINVAL; }
   PartTable pt;
   if (int rc = fill_parts(pt, n_parts, part_lo, part_hi, part_norm, part_scale_col, course_lo, course_hi, n_seg)) return rc;
   if (n == 0) return SSNB_OK;
@@ -839,7 +840,8 @@ int ssnb_stpp_bwd(const float* d_course, const float* d_stpp, const float* scali
                   const int* part_lo, const int* part_hi, const int* part_norm, const int* part_scale_col, int course_lo,
                   int course_hi, float* d_ft, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
-  if (!d_stpp || !scaling || !d_ft || n < 0 || D <= 0) { set_thread_error("stpp_bwd: bad argument"); return SSNB_EINVAL; }
+  if (!d_ft || n < 0 || D <= 0 || (n_parts != 0 && (!d_stpp || !scaling)) || (n_parts == 0 && !d_course)) {
+    set_thread_error("stpp_bwd: bad argument"); return SSNB_EINVAL; }
   PartTable pt;
   if (int rc = fill_parts(pt, n_parts, part_lo, part_hi, part_norm, part_scale_col, course_lo, course_hi, n_seg)) return rc;
   if (n == 0) return SSNB_OK;
@@ -864,7 +866,7 @@ int ssnb_gpool_stpp_fwd(ssnb_handle h, const float* drop_mask, const float* scal
                         int course_lo, int course_hi, float* feat, float* course_ft, float* stpp_ft, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   View v; int F = 0, fp16 = 0;
-  if (!h || !scaling || !feat || !course_ft || !stpp_ft) { set_thread_error("gpool_stpp: null argument"); return SSNB_EINVAL; }
+  if (!h || !feat || !course_ft || (n_parts != 0 && (!scaling || !stpp_ft))) { set_thread_error("gpool_stpp: null argument"); return SSNB_EINVAL; }
   if (int rc = engine_tail_view(h, &v, &F, &fp16)) return rc;
   if (n_seg <= 0 || n_seg > 32 || F % n_seg) { set_thread_error("gpool_stpp: frames must be a multiple of n_seg (<= 32)"); return SSNB_EINVAL; }
   PartTable pt;

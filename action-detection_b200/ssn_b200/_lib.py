@@ -76,6 +76,8 @@ SIGNATURES = {
     "ssnb_classwise_reg_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _vp]),
     "ssnb_heads_loss_workspace_bytes": (_sz, [C.POINTER(HeadsCfg)]),
     "ssnb_heads_loss_fwd_bwd": (_i, [C.POINTER(HeadsCfg)] + [_vp] * 25),
+    "ssnb_classifier_ce_workspace_bytes": (_sz, [_i, _i]),
+    "ssnb_classifier_ce_fwd_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "ssnb_grad_overflow": (_i, [_vp, _i]),
     "ssnb_timing_begin": (_i, [_vp]),
     "ssnb_timing_report": (C.c_char_p, []),

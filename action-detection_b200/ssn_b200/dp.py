@@ -6,8 +6,8 @@ fixed row counts, so rank means average to the global mean; the completeness los
 ohem_ratio) of the GLOBAL batch (ops/ssn_ops.py:236-239), which is NOT world * the per-rank value in general (B=64:
 int(65.28)=65 vs 8*int(8.16)=64).
 
-GradSync exchanges the flat gradient buffer in BUCKETS (heads -> inception_5b..4e -> 4d..4a -> 3c..conv1) on a
-communication stream while the backward of the layers below is still running (ssnb_backbone_bwd_range finalises a
+GradSync exchanges the flat gradient buffer in BUCKETS (heads -> inception_5b..4e -> 4d..4a -> 3c..conv1; "heads" is every
+parameter outside base_model) on a communication stream while the backward of the layers below is still running (ssnb_backbone_bwd_range finalises a
 bucket's weight gradients before returning); the whole pattern is capturable in a CUDA graph.
 """
 import torch
@@ -88,8 +88,9 @@ class GradSync:
         bm = model.base_model
         convs = bm._convs()
         self.conv_offsets = [self.offset_of[id(c.weight)] for c in convs]
-        head_params = [p for fc in (model.activity_fc, model.completeness_fc, model.regressor_fc) if fc is not None for p in fc.parameters()]
-        self.heads_lo = min(self.offset_of[id(p)] for p in head_params)
+        # the head bucket: every parameter of the flat buffer outside base_model (SSN's three heads, BinaryClassifier's classifier_fc)
+        in_backbone = {id(p) for p in bm.parameters()}
+        self.heads_lo = min(self.offset_of[id(p)] for p in params if id(p) not in in_backbone)
         assert self.heads_lo >= max(self.conv_offsets), "flat buffer must hold the backbone parameters before the heads"
         self._ranges = {}
         self.launched = []

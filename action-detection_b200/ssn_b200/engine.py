@@ -250,20 +250,24 @@ def stpp_part_table(parts, norm_num, seg_split):
 
 
 class STPPFunction(torch.autograd.Function):
+    """(course_ft, stpp_ft) = STPP(ft).  An empty part table means the course mean alone (BinaryClassifier's segment mean);
+    scaling may then be None and stpp_ft is [n, 0]."""
+
     @staticmethod
     def forward(ctx, ft, scaling, table, n_seg, course):
         _need_cuda(ft, "ft")
         lo, hi, nm, col = table
         ft = ft.contiguous().float()
-        scaling = scaling.contiguous().float().view(-1, 2)
+        if scaling is not None:
+            scaling = scaling.contiguous().float().view(-1, 2)
         D = ft.shape[1]
         n = ft.shape[0] // n_seg
         act = torch.empty(n, D, dtype=torch.float32, device=ft.device)
         comp = torch.empty(n, len(lo) * D, dtype=torch.float32, device=ft.device)
         with torch.cuda.device(ft.device):
-            check(lib.ssnb_stpp_fwd(ft.data_ptr(), scaling.data_ptr(), n, n_seg, D, len(lo), _lib.int_array(lo),
-                                    _lib.int_array(hi), _lib.int_array(nm), _lib.int_array(col), course[0], course[1],
-                                    act.data_ptr(), comp.data_ptr(), _stream()), None, "stpp_fwd")
+            check(lib.ssnb_stpp_fwd(ft.data_ptr(), None if scaling is None else scaling.data_ptr(), n, n_seg, D, len(lo),
+                                    _lib.int_array(lo), _lib.int_array(hi), _lib.int_array(nm), _lib.int_array(col), course[0],
+                                    course[1], act.data_ptr(), comp.data_ptr() if lo else None, _stream()), None, "stpp_fwd")
         ctx.save_for_backward(scaling)
         ctx.meta = (table, n_seg, course, n, D)
         return act, comp
@@ -276,7 +280,8 @@ class STPPFunction(torch.autograd.Function):
         d_comp = d_comp.contiguous().float()
         dft = torch.empty(n * n_seg, D, dtype=torch.float32, device=d_comp.device)
         with torch.cuda.device(d_comp.device):
-            check(lib.ssnb_stpp_bwd(d_act.data_ptr(), d_comp.data_ptr(), scaling.data_ptr(), n, n_seg, D, len(lo),
+            check(lib.ssnb_stpp_bwd(d_act.data_ptr(), d_comp.data_ptr() if lo else None, None if scaling is None else scaling.data_ptr(),
+                                    n, n_seg, D, len(lo),
                                     _lib.int_array(lo), _lib.int_array(hi), _lib.int_array(nm), _lib.int_array(col),
                                     course[0], course[1], dft.data_ptr(), _stream()), None, "stpp_bwd")
         return dft, None, None, None, None

@@ -21,36 +21,11 @@ class _HeadLinear(nn.Linear):
         return LinearFunction.apply(input, self.weight, self.bias)
 
 
-class SSN(torch.nn.Module):
-    def __init__(self, num_class,
-                 starting_segment, course_segment, ending_segment, modality,
-                 base_model='resnet101', new_length=None,
-                 dropout=0.8,
-                 crop_num=1, no_regression=False, test_mode=False,
-                 stpp_cfg=(1, (1, 2), 1), bn_mode='frozen', verbose=False):
-        super(SSN, self).__init__()
-        self.modality = modality
-        self.num_segments = starting_segment + course_segment + ending_segment
-        self.starting_segment = starting_segment
-        self.course_segment = course_segment
-        self.ending_segment = ending_segment
-        self.reshape = True
-        self.dropout = dropout
-        self.crop_num = crop_num
-        self.with_regression = not no_regression
-        self.test_mode = test_mode
-        self.bn_mode = bn_mode
-        self.num_class = num_class
-        if new_length is None:
-            self.new_length = 1 if modality == "RGB" else 5
-        else:
-            self.new_length = new_length
-        if verbose:
-            print("Initializing SSN (H100) base model {} modality {} segments {}+{}+{} dropout {} stpp {} bn {}".format(
-                base_model, modality, starting_segment, course_segment, ending_segment, dropout, stpp_cfg, bn_mode))
-        self._prepare_base_model(base_model)
-        self._prepare_ssn(num_class, stpp_cfg)
-        self.prepare_bn()
+class _BNInceptionModel(torch.nn.Module):
+    """What SSN and BinaryClassifier share (ssn_models.py:69-174,203-251,318-343 and binary_model.py:55-80,117-145,
+    165-215,260-307 of the reference are the same code): the BNInception backbone for RGB or Flow input with its last
+    layer replaced by Dropout / Identity, bn_mode handling, optimiser policies and the data-side attributes.  Subclasses
+    set modality, new_length and dropout before calling _prepare_base_model."""
 
     # ---- construction (ssn_models.py:69-154) ------------------------------------------------------
     def _prepare_base_model(self, base_model):
@@ -95,26 +70,13 @@ class SSN(torch.nn.Module):
         base_model._engines = {}               # engines are planned per input-channel count
         return base_model
 
-    def _prepare_ssn(self, num_class, stpp_cfg):
+    def _replace_last_layer(self):
+        """fc -> Dropout(p=dropout), or Identity for dropout 0 (ssn_models.py:71-75); returns the feature dimension"""
         feature_dim = getattr(self.base_model, self.base_model.last_layer_name).in_features
         if self.dropout == 0:
             setattr(self.base_model, self.base_model.last_layer_name, Identity())
         else:
             setattr(self.base_model, self.base_model.last_layer_name, nn.Dropout(p=self.dropout))
-        self.stpp = StructuredTemporalPyramidPooling(feature_dim, True, configs=stpp_cfg)
-        self.activity_fc = _HeadLinear(self.stpp.activity_feat_dim(), num_class + 1)
-        self.completeness_fc = _HeadLinear(self.stpp.completeness_feat_dim(), num_class)
-        nn.init.normal_(self.activity_fc.weight.data, 0, 0.001)
-        nn.init.constant_(self.activity_fc.bias.data, 0)
-        nn.init.normal_(self.completeness_fc.weight.data, 0, 0.001)
-        nn.init.constant_(self.completeness_fc.bias.data, 0)
-        self.test_fc = None
-        if self.with_regression:
-            self.regressor_fc = _HeadLinear(self.stpp.completeness_feat_dim(), 2 * num_class)
-            nn.init.normal_(self.regressor_fc.weight.data, 0, 0.001)
-            nn.init.constant_(self.regressor_fc.bias.data, 0)
-        else:
-            self.regressor_fc = None
         return feature_dim
 
     # bn_mode -> 1-based index of the first BatchNorm2d that stays in eval mode with frozen affine parameters
@@ -141,6 +103,137 @@ class SSN(torch.nn.Module):
     def set_precision(self, precision, grad_scale=None):
         self.base_model.set_precision(precision, grad_scale)
 
+    # ---- optimiser groups (ssn_models.py:203-251) ---------------------------------------------------
+    def get_optim_policies(self):
+        first_conv_weight, first_conv_bias, normal_weight, normal_bias, bn = [], [], [], [], []
+        conv_cnt = 0
+        for m in self.modules():
+            if isinstance(m, (torch.nn.Conv2d, torch.nn.Conv1d)):
+                ps = list(m.parameters())
+                conv_cnt += 1
+                (first_conv_weight if conv_cnt == 1 else normal_weight).append(ps[0])
+                if len(ps) == 2:
+                    (first_conv_bias if conv_cnt == 1 else normal_bias).append(ps[1])
+            elif isinstance(m, torch.nn.Linear):
+                ps = list(m.parameters())
+                normal_weight.append(ps[0])
+                if len(ps) == 2:
+                    normal_bias.append(ps[1])
+            elif isinstance(m, torch.nn.BatchNorm1d):
+                bn.extend(list(m.parameters()))
+            elif isinstance(m, torch.nn.BatchNorm2d):
+                pass  # frozen (train())
+            elif len(m._modules) == 0:
+                if len(list(m.parameters())) > 0:
+                    raise ValueError("New atomic module type: {}. Need to give it a learning policy".format(type(m)))
+        return [
+            {'params': first_conv_weight, 'lr_mult': 1, 'decay_mult': 1, 'name': "first_conv_weight"},
+            {'params': first_conv_bias, 'lr_mult': 2, 'decay_mult': 0, 'name': "first_conv_bias"},
+            {'params': normal_weight, 'lr_mult': 1, 'decay_mult': 1, 'name': "normal_weight"},
+            {'params': normal_bias, 'lr_mult': 2, 'decay_mult': 0, 'name': "normal_bias"},
+            {'params': bn, 'lr_mult': 1, 'decay_mult': 0, 'name': "BN scale/shift"},
+        ]
+
+    def _frames(self, input):
+        sample_len = (3 if self.modality == "RGB" else 2) * self.new_length
+        return input.view((-1, sample_len) + input.size()[-2:])
+
+    @staticmethod
+    def _accumulate_grad(p, g):
+        if p.grad is None:
+            p.grad = g
+        else:
+            p.grad.add_(g)
+
+    def _fused_backbone_backward(self, eng, dft, grad_sync):
+        """the tail of fused_step once the head gradients are in .grad: start the head bucket's exchange, then the engine
+        backward from dfeat straight into the convolutions' .grad, bucket by bucket when grad_sync is given"""
+        if grad_sync is not None:
+            grad_sync.begin()
+            grad_sync.heads_done()
+        cs = self.base_model._convs()
+        params = [c.weight for c in cs] + [c.bias for c in cs]
+        for p in params:
+            if p.requires_grad and p.grad is None:
+                p.grad = torch.zeros_like(p)
+        # straight into .grad; parameters with requires_grad=False get no gradient (None -> the kernels skip them)
+        buckets = grad_sync.engine_buckets(eng)[0] if grad_sync is not None else None
+        eng.backward(dft, [c.weight.grad if c.weight.requires_grad else None for c in cs],
+                     [c.bias.grad if c.bias.requires_grad else None for c in cs], accumulate=True, buckets=buckets,
+                     on_bucket=(lambda i: grad_sync.bucket_done(eng, i)) if grad_sync is not None else None)
+
+    # ---- data-side attributes the drivers read (ssn_train.py:60-65, ssn_test.py:109-142) -------------
+    @property
+    def crop_size(self):
+        return self.input_size
+
+    @property
+    def scale_size(self):
+        return self.input_size * 256 // 224
+
+    def get_augmentation(self):
+        # PIL group transforms are CPU data-pipeline code outside this hot path (SURVEY.md §2.1);
+        # if the reference's transforms.py is importable, use it.
+        try:
+            import torchvision
+            from transforms import GroupMultiScaleCrop, GroupRandomHorizontalFlip
+        except ImportError as e:
+            raise NotImplementedError("get_augmentation needs the reference's transforms.py on sys.path "
+                                      "(data pipeline is out of scope for the H100 hot path)") from e
+        scales = [1, .875, .75, .66] if self.modality == 'RGB' else [1, .875, .75]
+        return torchvision.transforms.Compose([GroupMultiScaleCrop(self.input_size, scales),
+                                               GroupRandomHorizontalFlip(is_flow=(self.modality == 'Flow'))])
+
+
+class SSN(_BNInceptionModel):
+    def __init__(self, num_class,
+                 starting_segment, course_segment, ending_segment, modality,
+                 base_model='resnet101', new_length=None,
+                 dropout=0.8,
+                 crop_num=1, no_regression=False, test_mode=False,
+                 stpp_cfg=(1, (1, 2), 1), bn_mode='frozen', verbose=False):
+        super(SSN, self).__init__()
+        self.modality = modality
+        self.num_segments = starting_segment + course_segment + ending_segment
+        self.starting_segment = starting_segment
+        self.course_segment = course_segment
+        self.ending_segment = ending_segment
+        self.reshape = True
+        self.dropout = dropout
+        self.crop_num = crop_num
+        self.with_regression = not no_regression
+        self.test_mode = test_mode
+        self.bn_mode = bn_mode
+        self.num_class = num_class
+        if new_length is None:
+            self.new_length = 1 if modality == "RGB" else 5
+        else:
+            self.new_length = new_length
+        if verbose:
+            print("Initializing SSN (H100) base model {} modality {} segments {}+{}+{} dropout {} stpp {} bn {}".format(
+                base_model, modality, starting_segment, course_segment, ending_segment, dropout, stpp_cfg, bn_mode))
+        self._prepare_base_model(base_model)
+        self._prepare_ssn(num_class, stpp_cfg)
+        self.prepare_bn()
+
+    def _prepare_ssn(self, num_class, stpp_cfg):
+        feature_dim = self._replace_last_layer()
+        self.stpp = StructuredTemporalPyramidPooling(feature_dim, True, configs=stpp_cfg)
+        self.activity_fc = _HeadLinear(self.stpp.activity_feat_dim(), num_class + 1)
+        self.completeness_fc = _HeadLinear(self.stpp.completeness_feat_dim(), num_class)
+        nn.init.normal_(self.activity_fc.weight.data, 0, 0.001)
+        nn.init.constant_(self.activity_fc.bias.data, 0)
+        nn.init.normal_(self.completeness_fc.weight.data, 0, 0.001)
+        nn.init.constant_(self.completeness_fc.bias.data, 0)
+        self.test_fc = None
+        if self.with_regression:
+            self.regressor_fc = _HeadLinear(self.stpp.completeness_feat_dim(), 2 * num_class)
+            nn.init.normal_(self.regressor_fc.weight.data, 0, 0.001)
+            nn.init.constant_(self.regressor_fc.bias.data, 0)
+        else:
+            self.regressor_fc = None
+        return feature_dim
+
     # ---- test-time FC folding (ssn_models.py:176-201) ----------------------------------------------
     def prepare_test_fc(self):
         M = self.stpp.feat_multiplier
@@ -164,46 +257,11 @@ class SSN(torch.nn.Module):
         self.test_fc.weight.data = weight
         self.test_fc.bias.data = bias
 
-    # ---- optimiser groups (ssn_models.py:203-251) ---------------------------------------------------
-    def get_optim_policies(self):
-        first_conv_weight, first_conv_bias, normal_weight, normal_bias, bn = [], [], [], [], []
-        conv_cnt = 0
-        for m in self.modules():
-            if isinstance(m, (torch.nn.Conv2d, torch.nn.Conv1d)):
-                ps = list(m.parameters())
-                conv_cnt += 1
-                (first_conv_weight if conv_cnt == 1 else normal_weight).append(ps[0])
-                if len(ps) == 2:
-                    (first_conv_bias if conv_cnt == 1 else normal_bias).append(ps[1])
-            elif isinstance(m, torch.nn.Linear):
-                ps = list(m.parameters())
-                normal_weight.append(ps[0])
-                if len(ps) == 2:
-                    normal_bias.append(ps[1])
-            elif isinstance(m, torch.nn.BatchNorm1d):
-                bn.extend(list(m.parameters()))
-            elif isinstance(m, torch.nn.BatchNorm2d):
-                pass  # frozen in SSN
-            elif len(m._modules) == 0:
-                if len(list(m.parameters())) > 0:
-                    raise ValueError("New atomic module type: {}. Need to give it a learning policy".format(type(m)))
-        return [
-            {'params': first_conv_weight, 'lr_mult': 1, 'decay_mult': 1, 'name': "first_conv_weight"},
-            {'params': first_conv_bias, 'lr_mult': 2, 'decay_mult': 0, 'name': "first_conv_bias"},
-            {'params': normal_weight, 'lr_mult': 1, 'decay_mult': 1, 'name': "normal_weight"},
-            {'params': normal_bias, 'lr_mult': 2, 'decay_mult': 0, 'name': "normal_bias"},
-            {'params': bn, 'lr_mult': 1, 'decay_mult': 0, 'name': "BN scale/shift"},
-        ]
-
     # ---- forward (ssn_models.py:253-300) -------------------------------------------------------------
     def forward(self, input, aug_scaling, target, reg_target, prop_type):
         if not self.test_mode:
             return self.train_forward(input, aug_scaling, target, reg_target, prop_type)
         return self.test_forward(input)
-
-    def _frames(self, input):
-        sample_len = (3 if self.modality == "RGB" else 2) * self.new_length
-        return input.view((-1, sample_len) + input.size()[-2:])
 
     def _seg_split(self):
         return [self.starting_segment, self.starting_segment + self.course_segment, self.num_segments]
@@ -306,50 +364,11 @@ class SSN(torch.nn.Module):
                                     self.starting_segment + self.course_segment, dft.data_ptr(), _stream()), None, "stpp_bwd")
         if mask is not None:
             dft = dft * mask
-        def acc(p, g):
-            if p.grad is None:
-                p.grad = g
-            else:
-                p.grad.add_(g)
         for fc, k in ((self.activity_fc, "act"), (self.completeness_fc, "comp"), (self.regressor_fc, "reg")):
             if fc.weight.requires_grad:
-                acc(fc.weight, out["d_%s_w" % k])
+                self._accumulate_grad(fc.weight, out["d_%s_w" % k])
             if fc.bias.requires_grad:
-                acc(fc.bias, out["d_%s_b" % k])
-        if grad_sync is not None:
-            grad_sync.begin()
-            grad_sync.heads_done()
-        cs = bm._convs()
-        params = [c.weight for c in cs] + [c.bias for c in cs]
-        for p in params:
-            if p.requires_grad and p.grad is None:
-                p.grad = torch.zeros_like(p)
-        # straight into .grad; parameters with requires_grad=False get no gradient (None -> the kernels skip them)
-        buckets = grad_sync.engine_buckets(eng)[0] if grad_sync is not None else None
-        eng.backward(dft, [c.weight.grad if c.weight.requires_grad else None for c in cs],
-                     [c.bias.grad if c.bias.requires_grad else None for c in cs], accumulate=True, buckets=buckets,
-                     on_bucket=(lambda i: grad_sync.bucket_done(eng, i)) if grad_sync is not None else None)
+                self._accumulate_grad(fc.bias, out["d_%s_b" % k])
+        self._fused_backbone_backward(eng, dft, grad_sync)
         self.last_fused = dict(out, feat=feat, course=course, stpp=stpp)
         return out["losses"]
-
-    # ---- data-side attributes the drivers read (ssn_train.py:60-65, ssn_test.py:109-142) -------------
-    @property
-    def crop_size(self):
-        return self.input_size
-
-    @property
-    def scale_size(self):
-        return self.input_size * 256 // 224
-
-    def get_augmentation(self):
-        # PIL group transforms are CPU data-pipeline code outside this hot path (SURVEY.md §2.1);
-        # if the reference's transforms.py is importable, use it.
-        try:
-            import torchvision
-            from transforms import GroupMultiScaleCrop, GroupRandomHorizontalFlip
-        except ImportError as e:
-            raise NotImplementedError("get_augmentation needs the reference's transforms.py on sys.path "
-                                      "(data pipeline is out of scope for the H100 hot path)") from e
-        scales = [1, .875, .75, .66] if self.modality == 'RGB' else [1, .875, .75]
-        return torchvision.transforms.Compose([GroupMultiScaleCrop(self.input_size, scales),
-                                               GroupRandomHorizontalFlip(is_flow=(self.modality == 'Flow'))])

@@ -112,7 +112,9 @@ int64_t ssnb_global_launch_count(void);
 /* ---- STPP: replaces StructuredTemporalPyramidPooling.forward (ops/ssn_ops.py:39-70) ----------
  * ft [n*n_seg, D]; scaling [n,2]; parts: n_parts entries (lo, hi, norm, scale_col) over segment
  * indices (host mirrors the tick arithmetic of :49-53); course = mean over [course_lo, course_hi).
- * out: course_ft [n,D], stpp_ft [n, n_parts*D]. */
+ * out: course_ft [n,D], stpp_ft [n, n_parts*D].
+ * n_parts == 0 (0..32 parts): the course mean only (BinaryClassifier, binary_model.py:229-230); the part arrays, scaling,
+ * stpp_ft / d_stpp are not read or written and may be NULL (ssnb_stpp_bwd then needs d_course). */
 int ssnb_stpp_fwd(const float* ft, const float* scaling, int n, int n_seg, int D, int n_parts, const int* part_lo,
                   const int* part_hi, const int* part_norm, const int* part_scale_col, int course_lo, int course_hi,
                   float* course_ft, float* stpp_ft, void* stream);
@@ -194,6 +196,20 @@ int ssnb_heads_loss_fwd_bwd(const ssnb_heads_cfg* cfg, const float* course_ft, c
                             const float* reg_target, float* raw_act, float* raw_comp, float* raw_reg, float* losses,
                             float* d_course_ft, float* d_stpp_ft, float* d_act_w, float* d_act_b, float* d_comp_w,
                             float* d_comp_b, float* d_reg_w, float* d_reg_b, void* workspace, void* stream);
+
+/* ---- BinaryClassifier (TAG actionness) head + loss: classifier_fc (binary_model.py:231) + torch.nn.CrossEntropyLoss()
+ *      (mean over rows, binary_train.py:135,162) + loss.backward() down to the segment-mean features ------------------------
+ * x [n, in_dim] (the course features), w [K, in_dim], b [K], target int64 [n] -> logits [n,K], loss[1] = mean_i
+ * (logsumexp(logits_i) - logits_i[target_i]), dx [n, in_dim], dw [K, in_dim], db [K] (overwritten).  Every gradient is
+ * multiplied by loss_scale (1/world_size for data parallel; a power of two scales them exactly); the loss is not.
+ * Two launches, no host synchronisation and no allocation (graph-capturable); deterministic: fixed-order reductions, no
+ * floating-point atomics, so repeated calls are bitwise equal.  workspace: ssnb_classifier_ce_workspace_bytes(n, K) bytes.
+ * 1 <= K <= 4096.  A target outside [0, K) is never used as an index: that row's loss is NaN, so the returned mean loss is
+ * NaN, and the row contributes no gradient (torch raises instead; its ignore_index = -100 is not honoured here). */
+size_t ssnb_classifier_ce_workspace_bytes(int n, int num_class);
+int ssnb_classifier_ce_fwd_bwd(const float* x, const float* w, const float* b, const int64_t* target, int n, int in_dim,
+                               int num_class, float loss_scale, float* logits, float* loss, float* dx, float* dw, float* db,
+                               void* workspace, void* stream);
 
 /* ---- detection post-processing of one video (eval_detection_results.py:91-183, ops/utils.py:38-40,56-82) --------------
  * rel_props [N,2] (start, end in [0,1]), act_scores [N,K+1], comp_scores [N,K], reg_scores [N,K,2] (already de-normalised,
