@@ -32,6 +32,12 @@ class HeadsCfg(C.Structure):
                 ("loss_scale", C.c_float)]
 
 
+class TagProposalsCfg(C.Structure):
+    _fields_ = [("cls", C.c_int32), ("n_thresholds", C.c_int32), ("n_tolerances", C.c_int32), ("reserved", C.c_int32),
+                ("sigma", C.c_double), ("nms_thresh", C.c_double), ("minimum_len", C.c_double),
+                ("thresholds", C.POINTER(C.c_double)), ("tolerances", C.POINTER(C.c_double))]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 _pp = C.POINTER(C.c_void_p)
@@ -83,6 +89,9 @@ SIGNATURES = {
     "ssnb_timing_report": (C.c_char_p, []),
     "ssnb_detect_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_detect_postprocess": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp]),
+    "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
+    "ssnb_tag_proposals": (_i, [C.POINTER(TagProposalsCfg), _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp] + [_vp] * 10
+                           + [_sz, _vp]),
     "ssnb_sgd_step": (_i, [_vp, _vp, _vp, _sz, _f, _f, _f, _f, _vp]),
     "ssnb_sgd_step_groups": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp]),
 }

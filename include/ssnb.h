@@ -223,6 +223,42 @@ int ssnb_detect_postprocess(const float* rel_props, const float* act_scores, con
                             int n_props, int num_class, double nms_thresh, int regress, float* detections, int* counts,
                             float* combined_ws, void* stream);
 
+/* ---- TAG bottom-up proposals of many videos (gen_bottom_up_proposals.py:116-142, ops/sequence_funcs.py:11-34,71-136) ----
+ * Per video v with T_v = offsets[v+1] - offsets[v] ticks of the merged crop-mean score f_score [T_v, num_cols] (rows
+ * offsets[v] .. offsets[v+1]-1 of one packed fp32 [offsets[V], num_cols] array): softmax (ops/metrics.py:8-11), column
+ * cls + 1, scipy.ndimage.gaussian_filter(col, sigma) (truncate 4, 'reflect', double, rounded to fp32), labels col > fp32(thr)
+ * per threshold, build_box_by_search per (threshold, tolerance) with box scores summed left to right in fp32 over the raw
+ * column f_score[:, cls+1], temporal_nms_fallback(boxes, nms_thresh) with tied scores kept in search order, then seconds
+ * (start / T * duration, end / T * duration, double) and the filter t1 - t0 > minimum_len.
+ * Box slots: a video has at most n_thresholds * n_tolerances * (T_v + 1) boxes; its outputs start at slot
+ * n_thresholds * n_tolerances * (offsets[v] + v), so every per-slot array below holds
+ * n_thresholds * n_tolerances * (offsets[V] + V) entries (<= INT_MAX; split larger batches).
+ *   frames [slots, 2] int32 (start, end frame), scores [slots] fp32, seconds [slots, 2] double: the kept boxes of video v in
+ *   NMS order, counts[v] of them.  Optional (NULL: not written): smoothed [offsets[V]] fp32 (the softmax column when sigma is
+ *   0), labels [offsets[V]] uint32 (bit k: threshold k), raw_frames [slots, 2] / raw_scores [slots] the boxes before NMS in the
+ *   reference's order, raw_counts [V].
+ * offsets (int64 [V+1], offsets[0] = 0, strictly increasing) and the config's threshold / tolerance arrays are HOST memory:
+ * they are validated and size the call.  offsets_dev (the same V+1 values) and durations_dev (double [V], seconds) are device
+ * memory, as is everything else.  The call enqueues kernels only: no host synchronisation, no allocation, no copy from host
+ * memory, so it can be captured in a CUDA graph. */
+typedef struct {
+  int32_t cls;               /* foreground column cls + 1 (gen_prop: 0) */
+  int32_t n_thresholds;      /* 1..32 */
+  int32_t n_tolerances;      /* 1..32 */
+  int32_t reserved;
+  double sigma;              /* Gaussian bandwidth (gen_prop: 3); 0 = no smoothing (bw=None); radius int(4 sigma + 0.5) <= 63 */
+  double nms_thresh;         /* [0, 1) (gen_prop: 0.9) */
+  double minimum_len;        /* seconds (--minimum_len, default 0) */
+  const double* thresholds;  /* host [n_thresholds] */
+  const double* tolerances;  /* host [n_tolerances] */
+} ssnb_tag_proposals_cfg;
+/* 0 for arguments ssnb_tag_proposals would reject */
+size_t ssnb_tag_proposals_workspace_bytes(int n_videos, int64_t total_ticks, int n_thresholds, int n_tolerances);
+int ssnb_tag_proposals(const ssnb_tag_proposals_cfg* cfg, const float* f_score, int num_cols, const int64_t* offsets,
+                       const int64_t* offsets_dev, int n_videos, const double* durations_dev, int32_t* frames, float* scores, double* seconds, int32_t* counts, float* smoothed,
+                       uint32_t* labels, int32_t* raw_frames, float* raw_scores, int32_t* raw_counts, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
 /* fused SGD-momentum step over flat fp32 buffers (ssn_train.py:141-144 torch.optim.SGD semantics):
  * g = grad*grad_mult + wd*p; buf = mom*buf + g; p -= lr*buf */
 int ssnb_sgd_step(float* param, const float* grad, float* momentum_buf, size_t n, float lr, float momentum,
