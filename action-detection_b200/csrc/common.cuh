@@ -24,8 +24,14 @@ void set_thread_error(const std::string& s);
 // Per-launch device timing (ssnb_timing_begin / ssnb_timing_report, bench.py's roofline): while a timing session is open
 // on this thread, every launch records a CUDA event behind itself on its stream; a launch's time is the distance to the
 // previous event (launches are back to back on one stream).  The engine tags the launches it is about to make with the
-// pass they belong to and the algorithmic FLOPs of the convolution they compute.
-struct LaunchTag { int phase = 3; double flop = 0.0; };      // phase: 0 forward, 1 data gradient, 2 weight gradient, 3 other
+// pass they belong to, the algorithmic FLOPs of the convolution they compute and its op name; umma_conv_launch adds its
+// tile count and tile width.
+struct LaunchTag {
+  int phase = 3;                  // 0 forward, 1 data gradient, 2 weight gradient, 3 other
+  double flop = 0.0;
+  const char* op = nullptr;       // copied when the launch is recorded
+  int tiles = 0, block_n = 0;
+};
 extern thread_local bool t_timing;
 extern thread_local LaunchTag t_tag;
 void timing_mark(const char* what, cudaStream_t s);

@@ -26,7 +26,7 @@ const std::string& thread_error() { return t_error; }
 // ---- per-launch timing session (see common.cuh) ---------------------------------------------------
 thread_local bool t_timing = false;
 thread_local LaunchTag t_tag;
-struct TimingMark { const char* what; LaunchTag tag; cudaEvent_t ev; };
+struct TimingMark { const char* what; LaunchTag tag; std::string op; cudaEvent_t ev; };
 static thread_local std::vector<TimingMark> t_marks;
 static thread_local std::vector<cudaEvent_t> t_event_pool;
 static thread_local std::string t_report;
@@ -37,10 +37,20 @@ static cudaEvent_t timing_event() {
   return e;
 }
 void timing_mark(const char* what, cudaStream_t s) {
-  TimingMark m{what, t_tag, timing_event()};
+  TimingMark m{what, t_tag, t_tag.op ? t_tag.op : "", timing_event()};
+  m.tag.op = nullptr;
   if (m.ev && cudaEventRecord(m.ev, s) == cudaSuccess) t_marks.push_back(m);
   else cudaGetLastError();
-  t_tag.flop = 0.0;                 // FLOPs belong to the one launch they were set for
+  // FLOPs, name and tiles belong to the one launch they were set for
+  t_tag.flop = 0.0; t_tag.op = nullptr; t_tag.tiles = 0; t_tag.block_n = 0;
+}
+
+// closes the session and waits for its last launch; false if the events cannot be read
+static bool timing_close() {
+  t_timing = false;
+  if (t_marks.empty()) return false;
+  if (cudaEventSynchronize(t_marks.back().ev) != cudaSuccess) { cudaGetLastError(); return false; }
+  return true;
 }
 
 // ---- graph table ---------------------------------------------------------------------------------
@@ -451,7 +461,16 @@ static double conv_flops(const ssnb_engine* e, const Op& o) {
   const Buffer& ob = e->bufs[e->vals[o.out_val].buf];
   return 2.0 * e->F * ob.H * ob.W * (double)c.cout * c.cin * c.k * c.k;
 }
-static inline void tag_next(int phase, double flop) { t_tag.phase = phase; t_tag.flop = flop; }
+static inline void tag_next(int phase, double flop, const char* op = nullptr) { t_tag.phase = phase; t_tag.flop = flop; t_tag.op = op; }
+// a fused sibling launch is named after its convolutions, "a+b+c"
+static thread_local std::string t_fused_name;
+static const char* fused_name(const ssnb_engine* e, const FusedBlock& fb) {
+  if (!t_timing) return nullptr;
+  t_fused_name.clear();
+  for (int j : {fb.op1, fb.op_r3, fb.op_rd})
+    if (j >= 0) t_fused_name += (t_fused_name.empty() ? "" : "+") + e->ops[j].id;
+  return t_fused_name.c_str();
+}
 
 // EXACT_TC: operand planes of a value produced by a kernel that only wrote fp32 (pools, SIMT convolutions, value_write)
 static int tc_split_value(ssnb_engine* e, int val, bool grad, float scale, cudaStream_t s) {
@@ -471,7 +490,7 @@ static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* 
       if (int rc = e->exact_tc() ? launch_nhwc_to_s2d_split(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s) : launch_nhwc_to_s2d(in, e->F, s2d, e->Cs, s))
         return rc;
     }
-    tag_next(0, conv_flops(e, o));
+    tag_next(0, conv_flops(e, o), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma, s);
   }
   if (o.kind == OP_BN1) {
@@ -500,7 +519,7 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
     a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
     a.wgt = e->ws + e->packed[o.conv].wf; a.bias = (const float*)(e->ws + e->packed[o.conv].bias);
     a.F = F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = o.raw ? 0 : 1; a.accumulate = 0; a.dgrad = 0;
-    tag_next(0, conv_flops(e, o));
+    tag_next(0, conv_flops(e, o), o.id.c_str());
     return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
   }
   if (o.kind == OP_MAXPOOL) {
@@ -534,7 +553,7 @@ static int simt_wgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
   w.partial = partial; w.F = e->F; w.k = c.k; w.stride = c.stride; w.pad = c.pad;
   w.rows_per_split = o.wrows; w.splits = o.wsplits;
-  tag_next(2, conv_flops(e, o));
+  tag_next(2, conv_flops(e, o), o.id.c_str());
   if (int rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s))) return rc;
   const float out_scale = e->fast() ? 1.0f / e->cfg.grad_scale : 1.0f;      // FAST stores gradients times the loss scale
   return launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
@@ -548,7 +567,7 @@ static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
   a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
   a.F = e->F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
-  tag_next(1, conv_flops(e, o));
+  tag_next(1, conv_flops(e, o), o.id.c_str());
   return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
 }
 
@@ -643,7 +662,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   if (tc_w) {
     float* partial = (float*)(e->ws + o.partial_off);
     float* bp = bias_w ? (float*)(e->ws + o.bias_partial_off) : nullptr;
-    tag_next(2, conv_flops(e, o));
+    tag_next(2, conv_flops(e, o), o.id.c_str());
     if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bp))) return rc;
     if (full && o.conv != 0) e->pending_finalize.push_back((int)(&o - e->ops.data()));
     else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s);
@@ -653,7 +672,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   } else if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
   // 4. data gradient; as the last writer of d(in) the wgmma epilogue applies in's ReLU mask
   if (tc_x) {
-    tag_next(1, conv_flops(e, o));
+    tag_next(1, conv_flops(e, o), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
   }
   return want_x ? simt_dgrad(e, o, s) : 0;
@@ -1009,7 +1028,7 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
       const FusedBlock& fb = h->fused[o.fuse_block];
       double fl = 0.0;
       for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += conv_flops(h, h->ops[j]);
-      tag_next(0, fl);
+      tag_next(0, fl, fused_name(h, fb));
       r = umma_conv_launch(h->umma_ctx, fb.fwd, s);
     } else r = run_fwd(h, o, input_nchw, feat, s);
     if (prof) cudaProfilerStop();
@@ -1048,7 +1067,7 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
         const FusedBlock& fb = h->fused[o.fuse_block];
         double fl = 0.0;
         for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += conv_flops(h, h->ops[j]);
-        tag_next(1, fl);
+        tag_next(1, fl, fused_name(h, fb));
         rc = umma_conv_launch(h->umma_ctx, fb.dgrad, s, h->fold_pools && o.dgrad_masks);
       }
       if (prof) cudaProfilerStop();
@@ -1171,10 +1190,8 @@ int ssnb_timing_begin(void* stream) {
 
 const char* ssnb_timing_report(void) {
   // closes the session, waits for the last launch and aggregates by (kernel, phase): "kernel\tphase\tlaunches\tms\tflop\n"
-  ssnb::t_timing = false;
   ssnb::t_report.clear();
-  if (ssnb::t_marks.empty()) return ssnb::t_report.c_str();
-  if (cudaEventSynchronize(ssnb::t_marks.back().ev) != cudaSuccess) { cudaGetLastError(); return ssnb::t_report.c_str(); }
+  if (!ssnb::timing_close()) return ssnb::t_report.c_str();
   struct Agg { int n = 0; double ms = 0, flop = 0; };
   std::map<std::pair<std::string, int>, Agg> agg;
   for (size_t i = 1; i < ssnb::t_marks.size(); ++i) {
@@ -1186,6 +1203,22 @@ const char* ssnb_timing_report(void) {
   char line[256];
   for (const auto& kv : agg) {
     snprintf(line, sizeof line, "%s\t%d\t%d\t%.6f\t%.0f\n", kv.first.first.c_str(), kv.first.second, kv.second.n, kv.second.ms, kv.second.flop);
+    ssnb::t_report += line;
+  }
+  return ssnb::t_report.c_str();
+}
+
+const char* ssnb_timing_launches(void) {
+  // closes the session (if still open) and lists its launches in order: "kernel\tphase\top\tms\tflop\ttiles\tblock_n\n"
+  ssnb::t_report.clear();
+  if (!ssnb::timing_close()) return ssnb::t_report.c_str();
+  char line[512];
+  for (size_t i = 1; i < ssnb::t_marks.size(); ++i) {
+    const ssnb::TimingMark& m = ssnb::t_marks[i];
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, ssnb::t_marks[i - 1].ev, m.ev) != cudaSuccess) { cudaGetLastError(); continue; }
+    snprintf(line, sizeof line, "%s\t%d\t%s\t%.6f\t%.0f\t%d\t%d\n", m.what, m.tag.phase, m.op.empty() ? "-" : m.op.c_str(), ms, m.tag.flop,
+             m.tag.tiles, m.tag.block_n);
     ssnb::t_report += line;
   }
   return ssnb::t_report.c_str();

@@ -1,15 +1,17 @@
 // wgmma implicit-GEMM convolution (sm_90a): host-side planning and the kernel that runs every tensor-core convolution
 // (forward, data gradient, fused sibling 1x1 forward / data gradient, stride-2 forward through TMA element strides).
 //
-//   warpgroup 0     : TMA producer (one thread; A: 4-D activation box, B: 3-D weight box, SWIZZLE_128B)
-//   warpgroups 1, 2 : consumers -- rows [64 * (wg - 1), +64) of the 128-row tile, one m64nNk16 wgmma (N = block_n) per 16 channels,
-//                     fp32 accumulators in registers; then the epilogue: each 64-column slice of the accumulator goes
-//                     through shared memory so that every thread owns one output row (bias/ReLU or accumulate/mask ->
-//                     fp16 NHWC stores, or the SSNB_EXACT_TC fp32 epilogue of umma_epi32.cuh)
+//   warpgroup 0     : TMA producer (one thread; A: 4-D activation box, B: 3-D weight box, SWIZZLE_128B), stages in tile order
+//   warpgroups 1, 2 : ping-pong consumers -- each owns every other tile of the CTA's persistent sequence, all 128 rows: two
+//                     m64nNk16 wgmmas (N = block_n <= 128) per 16 channels, fp32 accumulators in registers; then the
+//                     epilogue: each 32-column slice of the accumulator goes through the warpgroup's own shared-memory
+//                     staging so that every thread owns one output row (bias/ReLU or accumulate/mask -> fp16 NHWC stores,
+//                     or the SSNB_EXACT_TC fp32 epilogue of umma_epi32.cuh).  An order barrier hands the tensor pipe from
+//                     one warpgroup to the other once a tile's MMAs are issued, so one tile's epilogue runs under the
+//                     next tile's MMAs.
 //
 // Rows of the M tile are the pixels of one TMA box (bw x bh x bf); taps shift the box origin and
-// rely on TMA's out-of-bounds zero fill for the convolution padding.  The producer runs ahead into the next tile
-// while the consumers drain the current one.
+// rely on TMA's out-of-bounds zero fill for the convolution padding.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -25,13 +27,20 @@ namespace {
 
 using namespace umma;
 constexpr int MAX_STAGES = 8;
-constexpr int PIPE_BYTES = 180 * 1024;             // operand staging
+constexpr int PIPE_BYTES = 192 * 1024;             // operand staging: 3 four-plane EXACT_TC stages at block_n 128
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;     // 16 KiB
 constexpr int NUM_THREADS = 384;
-constexpr int EPI_PITCH = 68;                      // floats per staged accumulator row (64 + 4: 16-byte aligned, banks rotate)
-constexpr int EPI_BYTES = BLOCK_M * EPI_PITCH * 4;
+constexpr int N_STEP = 16;                         // block_n granularity (wgmma N is any multiple of 8; the epilogue works in 16-column chunks)
+constexpr int MAX_BLOCK_N = 128;                   // 128 accumulators per consumer thread
+constexpr int EPI_COLS = 16;                       // accumulator columns per staged epilogue slice
+constexpr int EPI_PITCH = EPI_COLS + 4;            // floats per staged row (16-byte aligned, banks rotate)
+constexpr int EPI_BYTES = BLOCK_M * EPI_PITCH * 4; // per consumer warpgroup: 10 KiB
 constexpr int BAR_BYTES = 256;
-constexpr int SMEM_BYTES = PIPE_BYTES + EPI_BYTES + BAR_BYTES + 1024 /*align slack*/;
+constexpr int SMEM_BYTES = PIPE_BYTES + 2 * EPI_BYTES + BAR_BYTES + 1024 /*align slack*/;
+// named barriers: 1 + cw orders the consumers' mainloops (256 threads: one warpgroup arrives, the other waits),
+// 3 + cw guards warpgroup cw's epilogue staging (128 threads)
+constexpr int ORDER_BAR = 1;
+constexpr int EPI_BAR = 3;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
 struct TileCoord { int w0, h0, f0, n0; };
@@ -126,15 +135,38 @@ __device__ __forceinline__ void epilogue_row_chunk(const UmmaConvParams& p, cons
   epilogue_chunk(p, r, col, dst, o0, o1, y0, y1);
 }
 
-// the first NK 16-channel steps of a staged K chunk: A rows [sa, +64 rows) x B rows [sb, +64 NSUB rows), both K-major
-template <int NSUB, int NK>
-__device__ __forceinline__ void mma_k(float* d, uint32_t sa, uint32_t sb) {
+// the first NK 16-channel steps of a staged K chunk: A rows [sa, +128 rows) x B rows [sb, +BN rows), both K-major; one
+// m64nBNk16 MMA per 64-row block, both on the same B slice
+template <int BN, int NK>
+__device__ __forceinline__ void mma_k(float* d0, float* d1, uint32_t sa, uint32_t sb) {
 #pragma unroll
-  for (int k = 0; k < NK; ++k) wgmma<NSUB * MMA_N, 0, 0>(d, make_desc_sw128(sa + k * MMA_K * 2), make_desc_sw128(sb + k * MMA_K * 2));
+  for (int k = 0; k < NK; ++k) {
+    const uint64_t bdesc = make_desc_sw128(sb + k * MMA_K * 2);
+    wgmma<BN, 0, 0>(d0, make_desc_sw128(sa + k * MMA_K * 2), bdesc);
+    wgmma<BN, 0, 0>(d1, make_desc_sw128(sa + 64 * 128 + k * MMA_K * 2), bdesc);
+  }
 }
 
-// NSUB = block_n / 64 accumulator slices per consumer warpgroup
-template <int NSUB>
+// one stage's MMAs: EXACT_TC (split) issues the three products of the hi / lo planes, small terms first, into the same
+// accumulators; otherwise the one fp16 product
+template <int BN, int NK>
+__device__ __forceinline__ void mma_stage(float* d0, float* d1, uint32_t sa, uint32_t sb, uint32_t b_bytes, bool split) {
+  if (split) {
+    mma_k<BN, NK>(d0, d1, sa + A_BYTES, sb);               // A_lo . B_hi
+    mma_k<BN, NK>(d0, d1, sa, sb + b_bytes);               // A_hi . B_lo
+  }
+  mma_k<BN, NK>(d0, d1, sa, sb);                           // A_hi . B_hi
+}
+
+// move a ring position n stages ahead
+__device__ __forceinline__ void ring_advance(uint32_t& stage, uint32_t& phase, int n, int stages) {
+  const uint32_t s = stage + (uint32_t)n;
+  phase ^= (s / (uint32_t)stages) & 1u;
+  stage = s % (uint32_t)stages;
+}
+
+// BN = block_n: a multiple of 16, at most 128 (BN accumulators per consumer thread)
+template <int BN>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                  const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a_lo,
@@ -145,111 +177,131 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   // pipeline depth adapts to the tile: narrow-N layers get more stages in the same staging area
   const int STAGES = p.stages, STAGE_BYTES = p.stage_bytes;
-  float* epi = reinterpret_cast<float*>(smem + PIPE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES + EPI_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES + 2 * EPI_BYTES);
   uint64_t* full_bar = bars;                     // [MAX_STAGES]
   uint64_t* empty_bar = bars + MAX_STAGES;       // [MAX_STAGES]
 
-  const int wg = threadIdx.x / 128;
+  // warp-uniform by construction (a shuffle from lane 0): the consumers' tile loop branches on it, and ptxas serialises
+  // wgmmas it cannot prove warpgroup-convergent
+  const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);
   const int total_tiles = p.tiles_w * p.tiles_h * p.tiles_f * p.n_tiles;
-  const int nseg = p.nseg > 1 ? p.nseg : 1;          // SSNB_EXACT_TC: (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi) per (tap, K chunk)
-  const int ksteps = p.ntaps * p.kchunks * nseg;
+  // SSNB_EXACT_TC: a stage holds the hi and lo planes of both operands of one (tap, K chunk): [A_hi | A_lo | B_hi | B_lo]
+  const bool split = p.nseg > 1;
+  const int nplanes = split ? 2 : 1;
+  const uint32_t b_bytes = (uint32_t)p.block_n * BLOCK_K * 2;
+  const int ksteps = p.ntaps * p.kchunks;
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a2)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }   // one release per consumer warpgroup
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }   // released by the consumer that owns the tile
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
   if (wg == 0) {
-    // ===== TMA producer =====
+    // ===== TMA producer: stages in tile order, whichever consumer owns the tile =====
     producer_regs();
     if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
       // bytes the two TMA boxes deliver (zero-filled out-of-bounds elements count; a 7x1x18 box has 126 rows)
       const uint32_t a_bytes = (uint32_t)(p.bw * p.bh * p.bf) * BLOCK_K * 2;
-      const uint32_t tx_bytes = a_bytes + (uint32_t)p.block_n * BLOCK_K * 2;
+      const uint32_t tx_bytes = (a_bytes + b_bytes) * nplanes;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const TileCoord t = decode_tile(p, tile);
-        for (int seg = 3 - nseg; seg < 3; ++seg)
         for (int tap = 0; tap < p.ntaps; ++tap) {
           for (int kc = 0; kc < p.kchunks; ++kc) {
-            const CUtensorMap* ma = seg == 0 ? &tmap_a_lo : &tmap_a;
-            const CUtensorMap* ma2 = seg == 0 ? &tmap_a2_lo : &tmap_a2;
-            const CUtensorMap* mb = seg == 1 ? &tmap_b_lo : &tmap_b;
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sa = smem + stage * STAGE_BYTES;
-            uint8_t* sb = sa + A_BYTES;
+            uint8_t* sb = sa + nplanes * A_BYTES;
             mbar_expect_tx(&full_bar[stage], tx_bytes);
-            if (kc < p.kchunks_a1) tma_load_4d(sa, ma, &full_bar[stage], kc * BLOCK_K, t.w0 * p.a_stride + p.tap_dx[tap], t.h0 * p.a_stride + p.tap_dy[tap], t.f0);
-            else tma_load_4d(sa, ma2, &full_bar[stage], (kc - p.kchunks_a1) * BLOCK_K, t.w0 + p.tap_dx[tap], t.h0 + p.tap_dy[tap], t.f0);
-            tma_load_3d(sb, mb, &full_bar[stage], kc * BLOCK_K, t.n0, tap);
+            for (int pl = 0; pl < nplanes; ++pl) {     // 0: hi (or the single fp16 plane), 1: lo
+              if (kc < p.kchunks_a1)
+                tma_load_4d(sa + pl * A_BYTES, pl ? &tmap_a_lo : &tmap_a, &full_bar[stage], kc * BLOCK_K, t.w0 * p.a_stride + p.tap_dx[tap],
+                            t.h0 * p.a_stride + p.tap_dy[tap], t.f0);
+              else
+                tma_load_4d(sa + pl * A_BYTES, pl ? &tmap_a2_lo : &tmap_a2, &full_bar[stage], (kc - p.kchunks_a1) * BLOCK_K, t.w0 + p.tap_dx[tap],
+                            t.h0 + p.tap_dy[tap], t.f0);
+              tma_load_3d(sb + pl * b_bytes, pl ? &tmap_b_lo : &tmap_b, &full_bar[stage], kc * BLOCK_K, t.n0, tap);
+            }
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
   } else {
-    // ===== consumers: warpgroup cw owns tile rows [64 cw, 64 cw + 64) =====
+    // ===== consumers (ping-pong): warpgroup cw owns the CTA's tiles cw, cw + 2, ... of its sequence, all 128 rows =====
     consumer_regs();
-    const int cw = wg - 1, ct = threadIdx.x - 128;
-    const int warp = (threadIdx.x / 32) & 3, lane = threadIdx.x & 31;
-    uint32_t stage = 0, phase = 0, prev = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const TileCoord t = decode_tile(p, tile);
-      float acc[NSUB][32];
+    const int cw = wg - 1, row = threadIdx.x & 127;
+    const int warp = row / 32, lane = row & 31;
+    float* epi = reinterpret_cast<float*>(smem + PIPE_BYTES + cw * EPI_BYTES);
+    // grid <= total_tiles, so every CTA has at least one tile
+    const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    uint32_t stage = 0, phase = 0;
+    if (cw) ring_advance(stage, phase, ksteps, STAGES);
+    for (int j = cw; j < my_tiles; j += 2) {
+      const TileCoord t = decode_tile(p, (int)blockIdx.x + j * (int)gridDim.x);
+      float acc[2][BN / 2];
 #pragma unroll
-      for (int j = 0; j < NSUB; ++j)
+      for (int b = 0; b < 2; ++b)
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[j][i] = 0.f;
+        for (int i = 0; i < BN / 2; ++i) acc[b][i] = 0.f;
+      // order barrier: the MMAs of tile j start once the other warpgroup has issued all of tile j - 1's, so the tensor
+      // pipe runs one tile at a time while the other warpgroup is in its epilogue.  Invariant: every sync at j > 0 pairs
+      // with exactly one arrive by the other warpgroup at j - 1 (guarded by j + 1 < my_tiles below).  It also keeps the
+      // two consumers' full_bar parity waits from aliasing a ring phase two fills ahead.  bar.sync has no timeout, so
+      // an edit that breaks the pairing hangs rather than traps: keep both guards in step.
+      if (j > 0) named_bar_sync(ORDER_BAR + cw, 256);
+      uint32_t prev = 0;
       int kc = 0;
       for (int ks = 0; ks < ksteps; ++ks) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * (64 * 128);
-        const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
+        const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES);
+        const uint32_t sb = sa + nplanes * A_BYTES;
         // K chunks whose tail is TMA zero fill (Cin % 64 != 0) skip the all-zero MMAs
         const int kvalid = kc < p.kchunks_a1 ? p.K1 - kc * BLOCK_K : p.K - p.K1 - (kc - p.kchunks_a1) * BLOCK_K;
         const int nk = kvalid >= BLOCK_K ? BLOCK_K / MMA_K : (kvalid + MMA_K - 1) / MMA_K;
-        // one m64n(64 NSUB)k16 MMA per 16 channels: the A rows are read from shared memory once for all columns of the
-        // tile.  Every path issues a compile-time number of MMAs (no predicated wgmma inside a sequence).
+        // per 16 channels one m64nBNk16 MMA per row block: the B slice is read from shared memory for both.  Every path
+        // issues a compile-time number of MMAs (no predicated wgmma inside a sequence).
         wgmma_fence();
-        float* d = &acc[0][0];
         switch (nk) {
-          case 1: mma_k<NSUB, 1>(d, sa, sb); break;
-          case 2: mma_k<NSUB, 2>(d, sa, sb); break;
-          case 3: mma_k<NSUB, 3>(d, sa, sb); break;
-          default: mma_k<NSUB, BLOCK_K / MMA_K>(d, sa, sb); break;
+          case 1: mma_stage<BN, 1>(acc[0], acc[1], sa, sb, b_bytes, split); break;
+          case 2: mma_stage<BN, 2>(acc[0], acc[1], sa, sb, b_bytes, split); break;
+          case 3: mma_stage<BN, 3>(acc[0], acc[1], sa, sb, b_bytes, split); break;
+          default: mma_stage<BN, BLOCK_K / MMA_K>(acc[0], acc[1], sa, sb, b_bytes, split); break;
         }
         wgmma_commit();
         // one group stays in flight: the previous stage's MMAs have retired, its smem slot goes back to the producer
         wgmma_wait<1>();
-        if (ks > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        if (ks > 0 && row == 0) mbar_arrive(&empty_bar[prev]);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
         if (++kc == p.kchunks) kc = 0;
       }
+      if (j + 1 < my_tiles) named_bar_arrive(ORDER_BAR + (cw ^ 1), 256);
       wgmma_wait<0>();
-      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-      // epilogue, one 64-column slice at a time: fragments -> shared memory -> one row per thread, 32 columns per thread
-      const int row = ct & 127, half = ct >> 7;
+      if (row == 0) mbar_arrive(&empty_bar[prev]);
+      ring_advance(stage, phase, ksteps, STAGES);      // the other warpgroup's tile j + 1
+      // epilogue, one EPI_COLS-column slice at a time: fragments -> this warpgroup's staging -> one row per thread
 #pragma unroll
-      for (int j = 0; j < NSUB; ++j) {
-        consumer_sync();                             // the previous slice has been read
+      for (int sl = 0; sl < (BN + EPI_COLS - 1) / EPI_COLS; ++sl) {
+        named_bar_sync(EPI_BAR + cw, 128);               // the previous slice (or tile) has been read
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          const int r = cw * 64 + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-          const int c = 8 * (i >> 2) + 2 * (lane & 3);
-          *reinterpret_cast<float2*>(epi + r * EPI_PITCH + c) = make_float2(acc[j][i], acc[j][i + 1]);
-        }
-        consumer_sync();
+        for (int b = 0; b < 2; ++b)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int c = half * 32 + h * 16;
-          epilogue_row_chunk(p, t, row, t.n0 + j * MMA_N + c, epi + row * EPI_PITCH + c);
-        }
+          for (int i = 0; i < EPI_COLS / 2; i += 2) {
+            const int ai = sl * (EPI_COLS / 2) + i;      // accumulator registers [16 sl, 16 sl + 16) are slice sl's columns
+            if (ai < BN / 2) {
+              const int r = b * 64 + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+              const int c = 8 * (i >> 2) + 2 * (lane & 3);
+              *reinterpret_cast<float2*>(epi + r * EPI_PITCH + c) = make_float2(acc[b][ai], acc[b][ai + 1]);
+            }
+          }
+        named_bar_sync(EPI_BAR + cw, 128);
+#pragma unroll
+        for (int c = 0; c < EPI_COLS; c += 16)
+          if (sl * EPI_COLS + c < BN) epilogue_row_chunk(p, t, row, t.n0 + sl * EPI_COLS + c, epi + row * EPI_PITCH + c);
       }
     }
   }
@@ -330,14 +382,12 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   p.W = a.W; p.H = a.H; p.F = F;
   pick_box(a.W, p.bw, p.bh, p.bf);
   p.tiles_w = (a.W + p.bw - 1) / p.bw; p.tiles_h = (a.H + p.bh - 1) / p.bh; p.tiles_f = (F + p.bf - 1) / p.bf;
-  // N split: equal tiles of block_n <= 256 (multiple of 64); the last tile may overhang N (TMA zero-fills the
+  // N split: equal tiles of block_n <= 128 (multiple of 16); the last tile may overhang N (TMA zero-fills the
   // missing weight rows, the epilogue masks the columns)
-  p.n_tiles = (N + 255) / 256;
-  p.block_n = (((N + p.n_tiles - 1) / p.n_tiles) + MMA_N - 1) / MMA_N * MMA_N;
+  p.n_tiles = (N + MAX_BLOCK_N - 1) / MAX_BLOCK_N;
+  p.block_n = (((N + p.n_tiles - 1) / p.n_tiles) + N_STEP - 1) / N_STEP * N_STEP;
   p.kchunks = (K + BLOCK_K - 1) / BLOCK_K;
   p.K = K;
-  p.stage_bytes = (A_BYTES + p.block_n * BLOCK_K * 2 + 1023) / 1024 * 1024;
-  p.stages = PIPE_BYTES / p.stage_bytes; if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
   p.ntaps = ntaps;
   p.out = reinterpret_cast<__half*>(o.base); p.out_pitch = o.pitch; p.out_coff = o.coff; p.Cout = N;
   p.out_stride = out_stride; p.OH = o.H; p.OW = o.W; p.a_stride = 1; p.mask_y = nullptr; p.mask_pitch = 0; p.mask_coff = 0;
@@ -362,8 +412,12 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
       if (int rc = encode(ctx, &plan.tmap_b_lo, 3, reinterpret_cast<__half*>(reinterpret_cast<char*>(const_cast<__half*>(w)) + plan.b_lo_off), dims, str, box)) return rc;
   }
   plan.tmap_a2 = plan.tmap_a; plan.tmap_a2_lo = plan.tmap_a_lo;
-  // SSNB_EXACT_TC: three operand segments per K chunk, fp32 epilogue (+ fp16 operand planes of the result)
-  p.nseg = tc ? 3 : 1; p.out_f32 = tc ? 1 : 0; p.alpha = tc ? tc->alpha : 1.0f; p.alpha_dev = tc ? tc->alpha_dev : nullptr;
+  // SSNB_EXACT_TC: three products per (tap, K chunk) from a four-plane stage, fp32 epilogue (+ fp16 operand planes of the result)
+  p.nseg = tc ? 3 : 1; p.out_f32 = tc ? 1 : 0;
+  // a stage holds one (tap, K chunk) of A and B; EXACT_TC: of both planes of each
+  p.stage_bytes = ((A_BYTES + p.block_n * BLOCK_K * 2) * (tc ? 2 : 1) + 1023) / 1024 * 1024;
+  p.stages = PIPE_BYTES / p.stage_bytes; if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
+  p.alpha = tc ? tc->alpha : 1.0f; p.alpha_dev = tc ? tc->alpha_dev : nullptr;
   p.mask32 = nullptr; p.mask32_pitch = 0; p.mask32_coff = 0; p.plane_scale = 1.0f; p.flag = nullptr;
   p.out32 = tc ? tc->out32 : nullptr; p.out_hi = tc ? reinterpret_cast<__half*>(o.base) : nullptr; p.out_lo_off = tc ? o.lo_off : 0;
   p.out32_2 = p.out32; p.out_hi2 = p.out_hi; p.out_lo_off2 = p.out_lo_off;       // second destination = the first unless a fused bind redirects it
@@ -496,10 +550,10 @@ void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float pla
 }
 
 namespace {
-template <int NSUB>
-int launch_nsub(const UmmaConvPlan& plan, const UmmaConvParams& p, int grid, cudaStream_t s) {
+template <int BN>
+int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, int grid, cudaStream_t s) {
   static bool attr_set[64] = {};          // function attributes are per device
-  auto kern = umma_conv_kernel<NSUB>;
+  auto kern = umma_conv_kernel<BN>;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
@@ -524,11 +578,16 @@ int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s,
   if (p.out_f32 && (p.mask_y || p.out_stride != 1)) { set_thread_error("umma conv: the fp32 epilogue takes its mask through mask32 and has no sampling"); return 3; }
   const int total = p.tiles_w * p.tiles_h * p.tiles_f * p.n_tiles;
   const int grid = total < ctx.num_sms ? total : ctx.num_sms;
-  switch (p.block_n / MMA_N) {
-    case 1: return launch_nsub<1>(plan, p, grid, s);
-    case 2: return launch_nsub<2>(plan, p, grid, s);
-    case 3: return launch_nsub<3>(plan, p, grid, s);
-    case 4: return launch_nsub<4>(plan, p, grid, s);
+  t_tag.tiles = total; t_tag.block_n = p.block_n;
+  switch (p.block_n) {
+    case 16: return launch_bn<16>(plan, p, grid, s);
+    case 32: return launch_bn<32>(plan, p, grid, s);
+    case 48: return launch_bn<48>(plan, p, grid, s);
+    case 64: return launch_bn<64>(plan, p, grid, s);
+    case 80: return launch_bn<80>(plan, p, grid, s);
+    case 96: return launch_bn<96>(plan, p, grid, s);
+    case 112: return launch_bn<112>(plan, p, grid, s);
+    case 128: return launch_bn<128>(plan, p, grid, s);
   }
   set_thread_error("umma conv: unsupported tile width"); return 3;
 }

@@ -3,7 +3,7 @@
 // One kernel family computes   out[p, n] = epi( sum_taps sum_c  A[p + shift(tap), c] * B[tap][n][c] )
 // over NHWC fp16 tensors: A tiles are 4-D TMA boxes of the activation view (zero-filled outside
 // the image = free padding), B tiles are 3-D TMA boxes of the packed weights, accumulators live
-// in the registers of two consumer warpgroups, the epilogue fuses folded-BN bias + ReLU (forward)
+// in the registers of two ping-pong consumer warpgroups, the epilogue fuses folded-BN bias + ReLU (forward)
 // or accumulation (data gradient).
 #pragma once
 #include <cuda.h>
@@ -25,7 +25,7 @@ struct UmmaConvParams {
   int W, H, F;                    // spatial dims shared by input and output (stride-1 convolutions)
   int bw, bh, bf;                 // TMA box in pixels; bw*bh*bf <= 128 rows of the M tile
   int tiles_w, tiles_h, tiles_f;
-  int n_tiles, block_n;           // N split of Cout; block_n is a multiple of 64 (one m64n64 MMA per 64 columns)
+  int n_tiles, block_n;           // N split of Cout into ceil(N/128) tiles; block_n is a multiple of 16, at most 128
   int stages, stage_bytes;        // smem pipeline depth / stride chosen from block_n
   int kchunks, ntaps, K;          // ceil(K/64), filter taps, reduction channels per tap
   int tap_dy[UMMA_MAX_TAPS], tap_dx[UMMA_MAX_TAPS];
@@ -43,8 +43,8 @@ struct UmmaConvParams {
   int tc_ok;
   // data gradient that is the LAST writer of its output: fuse dz = dy * (y > 0), y = activation of the same value
   const __half* mask_y; int mask_pitch, mask_coff;
-  // SSNB_EXACT_TC (error-compensated split operands): nseg = 3 runs every K chunk three times,
-  //   (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi), into the same accumulator; nseg = 1 is the plain fp16 product.
+  // SSNB_EXACT_TC (error-compensated split operands): nseg = 3 stages the hi and lo planes of A and B of each (tap, K chunk)
+  //   together and issues (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi) into the same accumulator; nseg = 1 is the plain fp16 product.
   // out_f32: the epilogue works in fp32 -- out32 = alpha * acc (+ bias, ReLU | + old out32) -- and, when out_hi is set,
   // also writes the result's fp16 hi / lo operand planes (same pitch / channel offset, lo plane out_lo_off bytes later).
   int nseg, out_f32;

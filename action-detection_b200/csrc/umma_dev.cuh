@@ -8,10 +8,10 @@
 namespace ssnb {
 namespace umma {
 
-constexpr int BLOCK_M = 128;            // rows of a tile: two consumer warpgroups x wgmma M = 64
+constexpr int BLOCK_M = 128;            // rows of a tile: two wgmma row blocks of M = 64
 constexpr int BLOCK_K = 64;             // fp16 elements = 128 B = one SWIZZLE_128B row
 constexpr int MMA_K = 16;
-constexpr int MMA_N = 64;               // N granularity of the accumulator slices (MMAs are m64nNk16, N = 64 x slices)
+constexpr int MMA_N = 64;               // umma_wgrad.cu: N granularity of its accumulator slices (the conv kernel uses block_n directly)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -127,11 +127,61 @@ __device__ __forceinline__ void wgmma_n256(float* d, uint64_t adesc, uint64_t bd
       : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
       : "memory");
 }
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n48(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1, %26, %27;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n80(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, %42, %43;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n96(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1, %50, %51;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
+      : "memory");
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n112(float* d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n112k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1, %58, %59;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+      : "l"(adesc), "l"(bdesc), "n"(TA), "n"(TB)
+      : "memory");
+}
 template <int N, int TA, int TB>
 __device__ __forceinline__ void wgmma(float* d, uint64_t adesc, uint64_t bdesc) {
-  static_assert(N == 16 || N == 64 || N == 128 || N == 192 || N == 256, "wgmma N");
+  static_assert((N % 16 == 0 && N <= 128) || N == 192 || N == 256, "wgmma N");
   if constexpr (N == 16) wgmma_n16<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 32) wgmma_n32<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 48) wgmma_n48<TA, TB>(d, adesc, bdesc);
   else if constexpr (N == 64) wgmma_n64<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 80) wgmma_n80<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 96) wgmma_n96<TA, TB>(d, adesc, bdesc);
+  else if constexpr (N == 112) wgmma_n112<TA, TB>(d, adesc, bdesc);
   else if constexpr (N == 128) wgmma_n128<TA, TB>(d, adesc, bdesc);
   else if constexpr (N == 192) wgmma_n192<TA, TB>(d, adesc, bdesc);
   else wgmma_n256<TA, TB>(d, adesc, bdesc);
@@ -140,8 +190,9 @@ __device__ __forceinline__ void wgmma(float* d, uint64_t adesc, uint64_t bdesc) 
 // register budget of the warp-specialised kernels: 1 producer + 2 consumer warpgroups on 64K registers
 __device__ __forceinline__ void producer_regs() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void consumer_regs() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
-// barrier among the 256 consumer threads only (the producer warpgroup runs ahead)
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// named barriers (id 0 is __syncthreads): `threads` counts every thread of the barrier's phase, arriving or waiting
+__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 }  // namespace umma
 }  // namespace ssnb

@@ -87,6 +87,7 @@ SIGNATURES = {
     "ssnb_grad_overflow": (_i, [_vp, _i]),
     "ssnb_timing_begin": (_i, [_vp]),
     "ssnb_timing_report": (C.c_char_p, []),
+    "ssnb_timing_launches": (C.c_char_p, []),
     "ssnb_detect_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_detect_postprocess": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp]),
     "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
