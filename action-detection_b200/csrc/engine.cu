@@ -1145,7 +1145,7 @@ int ssnb_value_read(ssnb_handle h, const char* name, int grad, float* dst_nchw, 
   if (!h || !name || !dst_nchw || !h->ws) return SSNB_EINVAL;
   auto it = h->val_by_name.find(name);
   if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
-  if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
+  if ((grad & 1) && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");     // grad = 2: an activation's planes
   if (grad & 2) {       // diagnostic: read hi + lo of the value's EXACT_TC operand planes (bit 0: gradient planes, un-scaled)
     if (!h->exact_tc() || !h->bufs[h->vals[it->second].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
     int rc = launch_planes_to_nchw(h->planes(it->second, (grad & 1) != 0), h->F, (grad & 1) ? 1.0f / h->cfg.grad_scale : 1.0f, dst_nchw, (cudaStream_t)stream);

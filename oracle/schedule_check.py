@@ -16,13 +16,21 @@ Consumed representation, per precision:
 Checks (one `Record` each):
   fwd     conv: relu(conv64(X, W', b')); max pool: bitwise; avg pool: to the rounding of the stored result;
           global pool: the 7x7 mean of the last block's output;
+          bn_mode='partial' (bn1): conv1 is conv64(X, W, b) without fold and ReLU, and its training-mode BatchNorm + ReLU
+          is relu(gamma * xhat + beta) with float64 batch statistics of the consumed z;
   planes  exact_tc: the activation planes of every conv / pool output against its fp32 value;
   dZ      a conv output V: (Y > 0) * G_V against the dZ its backward consumed, where G_V is the sum over V's consumers of
           the vjp of each applied to ITS consumed output gradient (a branch of a concat takes its slice of the block
           output's G; the global pool contributes dfeat / 49);
   G       any other value: G_V against the stored gradient (a max-pool branch of a concat under its own ReLU mask, which
           the last writer of the block output's gradient may apply);
-  dW, db  s * wgrad64(X, dZ) and s * sum(dZ) against what the engine returned in reference layout, s = gamma / sqrt(var + eps).
+  dW, db  s * wgrad64(X, dZ) and s * sum(dZ) against what the engine returned in reference layout, s = gamma / sqrt(var + eps)
+          (s = 1 for the raw conv1 of bn1, whose db, a sum that vanishes, is measured against sum |dZ|);
+  bn1     conv1's dZ is the BatchNorm vjp of the consumed dy masked by the engine's own y > 0 (no further ReLU mask), with
+          sum g and sum g * xhat taken over all frames first; dgamma / dbeta; running_mean / running_var: one momentum step
+          from the statistics held before the forward (unbiased variance).
+
+Forward-only (dfeat None, e.g. an engine created with training=0): the fwd and planes records only; no gradient is read.
 
 Besides the tensor-wide rel-L2, every record keeps rel-L2 per frame and per 64-output-channel slice; the worst frame and
 the worst slice are held to SLICE_FACTOR x the tensor bar, so an error confined to one tile is not averaged away.
@@ -45,8 +53,15 @@ BARS = {"exact": (5e-6, 2e-6), "exact_tc": (1.5e-5, 2e-4), "fast": (3e-3, 2e-4)}
 ROUND = {"exact": 1e-6, "exact_tc": 1e-6, "fast": 1e-3}     # avg pool: rounding of the stored result (fp32 / fp16)
 FEAT_BAR = 1e-6                                               # global pool: fp32 mean of 49 stored values
 PLANES_BAR = 2e-6                                             # exact_tc: hi + lo against the fp32 value (22-bit split)
+# bn1 (bn_mode='partial'): bars of the training-mode BatchNorm's own records, (its fwd and conv1's dZ through its vjp,
+# dgamma / dbeta), and of the running statistics after one momentum step.  Worst measured on an H100 80GB HBM3 (400 W) at
+# F = 288, 37 and 1 (tests/test_gpu_schedule_modes.py): exact_tc 1.8e-7 (conv1 dZ) / 2.0e-7 (dgamma at F = 288), exact 6.2e-8 / 1.2e-7,
+# running statistics 4.7e-8 (two momentum steps 6.8e-8).  The bars are about 4x those.
+BN1_BARS = {"exact": (2.5e-7, 5e-7), "exact_tc": (7e-7, 8e-7)}
+RUNSTAT_BAR = 2e-7
 SLICE_FACTOR = 4.0
 EPS = 1e-5
+BN1_CONV, BN1_RAW, BN1_OUT = "conv1_7x7_s2", "conv1_7x7_s2_raw", "conv1_7x7_s2_bn"
 
 
 class Record:
@@ -92,11 +107,12 @@ class _Acc:
         self.num = torch.zeros(frames, self.ns, dtype=torch.float64, device=device)
         self.den = torch.zeros_like(self.num)
 
-    def add(self, f0, got, ref):
+    def add(self, f0, got, ref, scale=None):
+        """scale: what the error is relative to, in place of ref"""
         n, c = got.shape[:2]
         d = (got.double() - ref).reshape(n, c, -1)
         e = d.pow(2).sum(2)
-        r = ref.reshape(n, c, -1).pow(2).sum(2)
+        r = (ref if scale is None else scale).reshape(n, c, -1).pow(2).sum(2)
         pad = self.ns * 64 - c
         self.num[f0:f0 + n] += F.pad(e, (0, pad)).view(n, self.ns, 64).sum(2)
         self.den[f0:f0 + n] += F.pad(r, (0, pad)).view(n, self.ns, 64).sum(2)
@@ -121,11 +137,13 @@ def _pool_out(h, k, s, p):       # ceil_mode (layer_factory.py:46-50)
 
 
 class Graph:
-    """BNInception from O.bninception_ops: the engine's op list, every value's shape, consumers and concat slices."""
+    """BNInception from O.bninception_ops: the engine's op list, every value's shape, consumers and concat slices.
+    bn1_train: bn_mode='partial', as the engine plans it: conv1 writes conv1_7x7_s2_raw (no fold, no ReLU) and an op of kind
+    "bn" (training-mode BatchNorm + ReLU) turns it into conv1_7x7_s2_bn."""
 
-    def __init__(self, in_channels=3):
-        self.in_channels = in_channels
-        self.ops = []            # dicts: kind (conv / maxpool / avgpool / gpool), id, inp, out, attrs
+    def __init__(self, in_channels=3, bn1_train=False):
+        self.in_channels, self.bn1_train = in_channels, bn1_train
+        self.ops = []            # dicts: kind (conv / bn / maxpool / avgpool / gpool), id, inp, out, attrs; raw convs: raw=True
         self.shape = {"data": (in_channels, 224, 224)}
         self.branch = {}         # branch value -> (block output, channel offset)
         self.members = {}        # block output -> [branch values]
@@ -133,6 +151,12 @@ class Graph:
             c, h, w = self.shape.get(ins[0], (0, 0, 0))
             if kind == "conv":
                 ho = (h + 2 * a["pad"] - a["k"]) // a["stride"] + 1
+                if bn1_train and id_ == BN1_CONV:
+                    self.shape[BN1_RAW] = (a["cout"], ho, ho)
+                    self.ops.append(dict(kind="conv", id=id_, inp=ins[0], out=BN1_RAW, a=a, raw=True))
+                    self.shape[out] = (a["cout"], ho, ho)
+                    self.ops.append(dict(kind="bn", id=out, inp=BN1_RAW, out=out, a={}))
+                    continue
                 self.shape[out] = (a["cout"], ho, ho)
                 self.ops.append(dict(kind="conv", id=id_, inp=ins[0], out=out, a=a))
             elif kind == "pool" and id_ == "global_pool":
@@ -218,21 +242,35 @@ class _Reader:
         self.cache.clear()
 
 
-def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3, chunk=16, device=None, bars=None):
-    """Check one forward + backward of `eng` (see the module docstring).  params: the reference state dict (CPU or device);
-    x: the forward's input; feat: what it returned; dfeat: the backward's input; dw / db: the 69 gradient tensors the backward
-    filled (reference layout); bars: (fwd / dZ / G, dW / db) in place of BARS[precision].  Returns [Record] in schedule order."""
-    G = Graph(in_channels)
+def check_schedule(eng, params, x, feat, dfeat=None, dw=None, db=None, precision=None, in_channels=3, chunk=16, device=None,
+                   bars=None, bn1=None):
+    """Check one forward (+ backward) of `eng` (see the module docstring).  params: the reference state dict (CPU or device);
+    x: the forward's input; feat: what it returned; dfeat: the backward's input, None for a forward-only check; dw / db: the
+    69 gradient tensors the backward filled (reference layout); bars: (fwd / dZ / G, dW / db) in place of BARS[precision]
+    (and of BN1_BARS[precision]).
+    bn1: for an engine created with bn1_train (bn_mode='partial'), a dict of the first BatchNorm's gamma, beta, momentum, eps,
+    running_mean0 / running_var0 (held before the forward), running_mean / running_var (after it) and the dgamma / dbeta the
+    backward filled.  Returns [Record] in schedule order."""
+    if precision not in BARS:
+        raise ValueError("precision must be one of %s" % sorted(BARS))
+    backward = dfeat is not None
+    G = Graph(in_channels, bn1_train=bn1 is not None)
     dev = torch.device(device) if device is not None else feat.device
     act_bar, par_bar = bars or BARS[precision]
+    bn_act_bar, bn_par_bar = bars or BN1_BARS.get(precision, BARS[precision])
     frames = feat.shape[0]
     R = _Reader(eng, precision, x.to(dev))
     folded = {}
+    bnstat = {}              # bn1: float64 batch statistics of the consumed z (mu, invstd, rows per channel)
     recs = []
 
     def W(cid):
         if cid not in folded:
-            folded[cid] = fold(params, cid, dev)
+            if bn1 is not None and cid == BN1_CONV:      # raw conv1: its BatchNorm runs in training mode, nothing folds, s = 1
+                w, b = (params[cid + k].detach().to(device=dev, dtype=torch.float64) for k in (".weight", ".bias"))
+                folded[cid] = (w, b, torch.ones_like(b))
+            else:
+                folded[cid] = fold(params, cid, dev)
         return folded[cid]
 
     def chunks():
@@ -240,6 +278,13 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
             yield f0, slice(f0, min(frames, f0 + chunk))
 
     d64 = lambda t: t.to(device=dev, dtype=torch.float64)
+    col = lambda t: d64(t).view(1, -1, 1, 1)
+
+    def vector(op, quantity, got, ref, bar, scale=None):        # one record over a per-channel (or per-output-channel) tensor
+        acc = _Acc(1, ref.shape[0], dev)
+        shape = (1, ref.shape[0], -1)
+        acc.add(0, d64(got).reshape(shape), ref.reshape(shape), None if scale is None else scale.reshape(shape))
+        return acc.record(op, quantity, bar, frames=False)
 
     # ---- forward ----
     for o in G.ops:
@@ -260,9 +305,20 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
             w, b, _s = W(o["id"])
             xin = R.operand(o["inp"])
             for f0, sl in chunks():
-                ref = F.relu(F.conv2d(d64(xin[sl]), w, b, a["stride"], a["pad"]))
-                acc.add(f0, d64(y[sl]), ref)
+                ref = F.conv2d(d64(xin[sl]), w, b, a["stride"], a["pad"])
+                acc.add(f0, d64(y[sl]), ref if o.get("raw") else F.relu(ref))
             bar = act_bar
+        elif o["kind"] == "bn":
+            z = R.get(o["inp"])                          # the fp32 z the statistics pass read
+            n = frames * z.shape[2] * z.shape[3]
+            mu = sum(d64(z[sl]).sum((0, 2, 3)) for _f0, sl in chunks()) / n
+            var = sum((d64(z[sl]) - mu.view(1, -1, 1, 1)).pow(2).sum((0, 2, 3)) for _f0, sl in chunks()) / n
+            invstd = 1.0 / torch.sqrt(var + bn1["eps"])
+            bnstat.update(mu=mu, invstd=invstd, n=n)
+            for f0, sl in chunks():
+                xh = (d64(z[sl]) - mu.view(1, -1, 1, 1)) * invstd.view(1, -1, 1, 1)
+                acc.add(f0, d64(y[sl]), F.relu(xh * col(bn1["gamma"]) + col(bn1["beta"])))
+            bar = bn_act_bar
         else:
             xin = R.get(o["inp"])
             for f0, sl in chunks():
@@ -276,7 +332,15 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
             for f0, sl in chunks():
                 acc.add(f0, d64(pl[sl]), d64(y[sl]))
             recs.append(acc.record(o["id"], "planes", PLANES_BAR))
+        if o["kind"] == "bn" and backward:
+            m, n = float(bn1["momentum"]), bnstat["n"]
+            rm = (1 - m) * d64(bn1["running_mean0"]) + m * mu
+            rv = (1 - m) * d64(bn1["running_var0"]) + m * var * (n / max(n - 1, 1))
+            recs.append(vector(o["id"], "running_mean", bn1["running_mean"], rm, RUNSTAT_BAR))
+            recs.append(vector(o["id"], "running_var", bn1["running_var"], rv, RUNSTAT_BAR))
         R.clear()
+    if not backward:
+        return recs
 
     # ---- data gradients: one group per value whose gradient is accumulated (a block output covers its branches) ----
     producer = {o["out"]: o for o in G.ops}
@@ -286,6 +350,16 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
         cons = G.consumers[v]
         members = G.members.get(v, [v])
         accs = {m: _Acc(frames, G.shape[m][0], dev) for m in members}
+        bn_sums = {}
+        for c in cons:
+            if c["kind"] == "bn":       # the BatchNorm vjp couples all frames: sum g and sum g * xhat first
+                mu, invstd = bnstat["mu"].view(1, -1, 1, 1), bnstat["invstd"].view(1, -1, 1, 1)
+                sb = sg = 0.0
+                for _f0, sl in chunks():
+                    g = (d64(R.get(c["out"])[sl]) > 0) * d64(R.get(c["out"], grad=True)[sl])
+                    sb = sb + g.sum((0, 2, 3))
+                    sg = sg + (g * (d64(R.get(v)[sl]) - mu) * invstd).sum((0, 2, 3))
+                bn_sums[c["id"]] = (sb, sg)
         for f0, sl in chunks():
             n = sl.stop - sl.start
             g = torch.zeros((n,) + G.shape[v], dtype=torch.float64, device=dev)
@@ -294,6 +368,12 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
                 if c["kind"] == "conv":
                     w, _b, _s = W(c["id"])
                     g += torch.nn.grad.conv2d_input(g.shape, w, d64(R.dz(c["out"])[sl]), a["stride"], a["pad"])
+                elif c["kind"] == "bn":
+                    sb, sg = bn_sums[c["id"]]
+                    mu, invstd, m = bnstat["mu"].view(1, -1, 1, 1), bnstat["invstd"].view(1, -1, 1, 1), bnstat["n"]
+                    gy = (d64(R.get(c["out"])[sl]) > 0) * d64(R.get(c["out"], grad=True)[sl])
+                    xh = (d64(R.get(v)[sl]) - mu) * invstd
+                    g += col(bn1["gamma"]) * invstd * (gy - sb.view(1, -1, 1, 1) / m - xh * sg.view(1, -1, 1, 1) / m)
                 elif c["kind"] == "maxpool":
                     g += maxpool_route(d64(R.get(v)[sl]), d64(R.get(c["out"], grad=True)[sl]), a["k"], a["stride"], a["pad"])
                 elif c["kind"] == "avgpool":
@@ -304,7 +384,7 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
                 off = G.branch[m][1] if m in G.branch else 0
                 gm = g[:, off:off + G.shape[m][0]]
                 if producer[m]["kind"] == "conv":
-                    accs[m].add(f0, d64(R.dz(m)[sl]), (d64(R.get(m)[sl]) > 0) * gm)
+                    accs[m].add(f0, d64(R.dz(m)[sl]), gm if producer[m].get("raw") else (d64(R.get(m)[sl]) > 0) * gm)
                 elif m in G.branch:     # max-pool branch: its gradient may be masked by the block output's last writer
                     mask = d64(R.get(m)[sl]) > 0
                     accs[m].add(f0, mask * d64(R.get(m, grad=True)[sl]), mask * gm)
@@ -313,7 +393,10 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
         names = tuple(c["id"] for c in cons)
         for m in members:
             q = "dZ" if producer[m]["kind"] == "conv" else "G"
-            recs.append(accs[m].record(producer[m]["id"], q, act_bar, names))
+            recs.append(accs[m].record(producer[m]["id"], q, bn_act_bar if bn_sums else act_bar, names))
+        for op_id, (sb, sg) in bn_sums.items():
+            recs.append(vector(op_id, "dgamma", bn1["dgamma"], sg, bn_par_bar))
+            recs.append(vector(op_id, "dbeta", bn1["dbeta"], sb, bn_par_bar))
         R.clear()
 
     # ---- weight and bias gradients ----
@@ -323,18 +406,18 @@ def check_schedule(eng, params, x, feat, dfeat, dw, db, precision, in_channels=3
         xin, dz = R.operand(o["inp"]), R.dz(o["out"])
         rw = torch.zeros_like(w)
         rb = torch.zeros_like(s)
+        l1 = torch.zeros_like(s)
         for _f0, sl in chunks():
             z = d64(dz[sl])
             rw += torch.nn.grad.conv2d_weight(d64(xin[sl]), w.shape, z, a["stride"], a["pad"])
             rb += z.sum((0, 2, 3))
+            l1 += z.abs().sum((0, 2, 3))
         rw *= s.view(-1, 1, 1, 1)
         rb *= s
-        acc = _Acc(1, w.shape[0], dev)
-        acc.add(0, d64(dw[ci]).reshape(1, w.shape[0], -1), rw.reshape(1, w.shape[0], -1))     # slices of output channels
-        recs.append(acc.record(o["id"], "dW", par_bar, frames=False))
-        acc = _Acc(1, w.shape[0], dev)
-        acc.add(0, d64(db[ci]).view(1, -1, 1, 1), rb.view(1, -1, 1, 1))
-        recs.append(acc.record(o["id"], "db", par_bar, frames=False))
+        recs.append(vector(o["id"], "dW", dw[ci], rw, par_bar))       # slices of output channels
+        # in front of a training-mode BatchNorm sum(dZ) vanishes (sum xhat = 0), so the raw conv1's db is a cancellation of
+        # large partial sums: its error is taken relative to sum |dZ|, the scale of the rounding of any summation order
+        recs.append(vector(o["id"], "db", db[ci], rb, par_bar, l1 * s if o.get("raw") else None))
         R.clear()
     return recs
 
