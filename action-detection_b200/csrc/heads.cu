@@ -601,10 +601,12 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
     a.dlogit[e] = 0.f;
   }
   grid_barrier(a.barrier, gridDim.x * 2);
-  // phase 2b: block 0 computes the three losses and d(loss)/d(logits)
+  // phase 2b: block 0 computes the three losses and d(loss)/d(logits).  Each thread sums its own rows / groups (ascending),
+  // then thread 0 adds the per-thread partials in thread order: the losses are the same bits on every call
   if (blockIdx.x == 0) {
     __shared__ int cnt[3];
-    __shared__ float lsum[3];
+    __shared__ float lpart[3][HL_THREADS];
+    float lsum[3] = {0.f, 0.f, 0.f};
     if (threadIdx.x == 0) {
       int ca = 0, cc = 0, cr = 0;
       for (int i = 0; i < n; ++i) {      // ascending flat order == nonzero() (ssn_models.py:276-282)
@@ -613,7 +615,7 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
         if (t == 0 || t == 1) a.rowlist[n + cc++] = i;
         if (t == 0) a.rowlist[2 * n + cr++] = i;
       }
-      cnt[0] = ca; cnt[1] = cc; cnt[2] = cr; lsum[0] = lsum[1] = lsum[2] = 0.f;
+      cnt[0] = ca; cnt[1] = cc; cnt[2] = cr;
     }
     __syncthreads();
     const float gscale = c.loss_scale;
@@ -627,7 +629,7 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
       for (int j = 0; j < na; ++j) se += expf(z[j] - mx);
       const int t = (int)a.target[i];
       const float lse = mx + logf(se);
-      atomicAdd(&lsum[0], lse - z[t]);
+      lsum[0] += lse - z[t];
       for (int j = 0; j < na; ++j)
         a.dlogit[(long long)i * ncols + j] = (expf(z[j] - lse) - (j == t ? 1.f : 0.f)) / (float)cnt[0] * gscale;
     }
@@ -659,7 +661,7 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
           if (nl[q] != 0.f) a.dlogit[(long long)i * ncols + na + wrap_label(a.target[i], K)] = 1.f / denom * c.comp_w * gscale;
         }
       }
-      atomicAdd(&lsum[1], ls);
+      lsum[1] += ls;
     }
     // regression: class-wise smooth L1 (mean over 2*n_fg) * 2
     for (int q = threadIdx.x; q < cnt[2]; q += HL_THREADS) {
@@ -671,10 +673,17 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
         ls += smooth_l1(d);
         a.dlogit[(long long)i * ncols + na + K + col * 2 + t] = smooth_l1_grad(d) / (float)(2 * cnt[2]) * 2.f * c.reg_w * gscale;
       }
-      atomicAdd(&lsum[2], ls);
+      lsum[2] += ls;
     }
+    for (int k = 0; k < 3; ++k) lpart[k][threadIdx.x] = lsum[k];
     __syncthreads();
     if (threadIdx.x == 0) {
+      const int busy[3] = {min(cnt[0], HL_THREADS), min(ngroups, HL_THREADS), min(cnt[2], HL_THREADS)};   // the rest hold 0
+      for (int k = 0; k < 3; ++k) {
+        float v = 0.f;
+        for (int t = 0; t < busy[k]; ++t) v += lpart[k][t];
+        lsum[k] = v;
+      }
       const float la = cnt[0] ? lsum[0] / (float)cnt[0] : 0.f;
       // the completeness rows must come in whole groups of comp_group per video (the reference's pred.view(-1, group, K) raises
       // otherwise, ops/ssn_ops.py:225): signalled as a NaN completeness / total loss instead of silently dropping the tail rows

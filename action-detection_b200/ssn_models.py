@@ -370,5 +370,5 @@ class SSN(_BNInceptionModel):
             if fc.bias.requires_grad:
                 self._accumulate_grad(fc.bias, out["d_%s_b" % k])
         self._fused_backbone_backward(eng, dft, grad_sync)
-        self.last_fused = dict(out, feat=feat, course=course, stpp=stpp)
+        self.last_fused = dict(out, feat=feat, course=course, stpp=stpp, mask=mask)
         return out["losses"]
