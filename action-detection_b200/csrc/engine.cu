@@ -875,8 +875,12 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       else if (c.kind == OP_CONV && c.fuse_role == 0 && c.umma_dgrad.enabled) dg = &c.umma_dgrad;
       if (dg) {
         c.dgrad_masks = true;
-        if (h->exact_tc()) umma_conv_set_mask_tc(*dg, h->view((int)v, false), h->planes((int)v, true), gs, h->tc_flag);
-        else umma_conv_set_mask(*dg, h->view((int)v, false));
+        if (h->exact_tc()) {
+          if (int rc = umma_conv_set_mask_tc(h->umma_ctx, *dg, h->view((int)v, false), h->planes((int)v, true), gs, h->tc_flag))
+            return h->fail(rc, "mask bind(" + h->vals[v].name + "): " + ssnb::thread_error());
+        } else {
+          umma_conv_set_mask(*dg, h->view((int)v, false));
+        }
       } else if (c.kind == OP_GPOOL && h->fast()) {
         c.dgrad_masks = true;       // FAST only: gpool_bwd<float> writes no operand planes, so EXACT_TC keeps the producers' split pass
       }

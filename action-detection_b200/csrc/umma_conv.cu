@@ -4,11 +4,12 @@
 //   warpgroup 0     : TMA producer (one thread; A: 4-D activation box, B: 3-D weight box, SWIZZLE_128B), stages in tile order
 //   warpgroups 1, 2 : ping-pong consumers -- each owns every other tile of the CTA's persistent sequence, all 128 rows: two
 //                     m64nNk16 wgmmas (N = block_n <= 128) per 16 channels, fp32 accumulators in registers; then the
-//                     epilogue: each 32-column slice of the accumulator goes through the warpgroup's own shared-memory
-//                     staging so that every thread owns one output row (bias/ReLU or accumulate/mask -> fp16 NHWC stores,
-//                     or the SSNB_EXACT_TC fp32 epilogue of umma_epi32.cuh).  An order barrier hands the tensor pipe from
-//                     one warpgroup to the other once a tile's MMAs are issued, so one tile's epilogue runs under the
-//                     next tile's MMAs.
+//                     epilogue, one 16-column slice at a time: bias/ReLU or accumulate/mask on the accumulator fragments
+//                     (fp16 result in FAST; fp32 result and its fp16 hi / lo operand planes in SSNB_EXACT_TC), written to
+//                     the warpgroup's own swizzled shared-memory staging in the output box layout and stored by TMA
+//                     (clipped at the image and at the destination's channel count).  An order barrier hands the tensor
+//                     pipe from one warpgroup to the other once a tile's MMAs are issued, so one tile's epilogue runs
+//                     under the next tile's MMAs.
 //
 // Rows of the M tile are the pixels of one TMA box (bw x bh x bf); taps shift the box origin and
 // rely on TMA's out-of-bounds zero fill for the convolution padding.
@@ -19,7 +20,6 @@
 
 #include "umma_conv.cuh"
 #include "umma_dev.cuh"
-#include "umma_epi32.cuh"
 
 namespace ssnb {
 
@@ -30,11 +30,12 @@ constexpr int MAX_STAGES = 8;
 constexpr int PIPE_BYTES = 192 * 1024;             // operand staging: 3 four-plane EXACT_TC stages at block_n 128
 constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;     // 16 KiB
 constexpr int NUM_THREADS = 384;
-constexpr int N_STEP = 16;                         // block_n granularity (wgmma N is any multiple of 8; the epilogue works in 16-column chunks)
+constexpr int N_STEP = 16;                         // block_n granularity (wgmma N is any multiple of 8; the epilogue works in 16-column slices)
 constexpr int MAX_BLOCK_N = 128;                   // 128 accumulators per consumer thread
-constexpr int EPI_COLS = 16;                       // accumulator columns per staged epilogue slice
-constexpr int EPI_PITCH = EPI_COLS + 4;            // floats per staged row (16-byte aligned, banks rotate)
-constexpr int EPI_BYTES = BLOCK_M * EPI_PITCH * 4; // per consumer warpgroup: 10 KiB
+constexpr int EPI_COLS = 16;                       // accumulator columns per epilogue slice = the width of one output store box
+constexpr int EPI_F32_BYTES = BLOCK_M * EPI_COLS * 4;          // a slice of fp32 results: 128 rows of 64 bytes
+constexpr int EPI_F16_BYTES = BLOCK_M * EPI_COLS * 2;          // a slice of fp16 values: 128 rows of 32 bytes
+constexpr int EPI_BYTES = EPI_F32_BYTES + 2 * EPI_F16_BYTES;   // per consumer warpgroup: fp32 | hi | lo = 16 KiB (FAST: fp16 only)
 constexpr int BAR_BYTES = 256;
 constexpr int SMEM_BYTES = PIPE_BYTES + 2 * EPI_BYTES + BAR_BYTES + 1024 /*align slack*/;
 // named barriers: 1 + cw orders the consumers' mainloops (256 threads: one warpgroup arrives, the other waits),
@@ -55,85 +56,14 @@ __device__ __forceinline__ TileCoord decode_tile(const UmmaConvParams& p, int ti
   return t;
 }
 
-// bias / accumulate / ReLU / ReLU-gradient mask on one 16-column chunk of an accumulator row, then fp16 store
-__device__ __forceinline__ void epilogue_chunk(const UmmaConvParams& p, const uint32_t* r, int col, uint4* dst, const uint4& o0,
-                                               const uint4& o1, const uint4& y0, const uint4& y1) {
-  float v[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
-  if (p.bias) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] += __ldg(p.bias + col + j);
-  }
-  if (p.accumulate) {
-    const __half2* h0 = reinterpret_cast<const __half2*>(&o0);
-    const __half2* h1 = reinterpret_cast<const __half2*>(&o1);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float2 a = __half22float2(h0[j]), b = __half22float2(h1[j]);
-      v[2 * j] += a.x; v[2 * j + 1] += a.y; v[8 + 2 * j] += b.x; v[8 + 2 * j + 1] += b.y;
-    }
-  }
-  if (p.relu) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-  }
-  if (p.mask_y) {
-    const __half2* a0 = reinterpret_cast<const __half2*>(&y0);
-    const __half2* a1 = reinterpret_cast<const __half2*>(&y1);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 ya = __half22float2(a0[j]), yb = __half22float2(a1[j]);
-      if (!(ya.x > 0.f)) v[2 * j] = 0.f;
-      if (!(ya.y > 0.f)) v[2 * j + 1] = 0.f;
-      if (!(yb.x > 0.f)) v[8 + 2 * j] = 0.f;
-      if (!(yb.y > 0.f)) v[8 + 2 * j + 1] = 0.f;
-    }
-  }
-  uint4 q0, q1;
-  __half2* g0 = reinterpret_cast<__half2*>(&q0);
-  __half2* g1 = reinterpret_cast<__half2*>(&q1);
-#pragma unroll
-  for (int j = 0; j < 4; ++j) { g0[j] = __floats2half2_rn(v[2 * j], v[2 * j + 1]); g1[j] = __floats2half2_rn(v[8 + 2 * j], v[8 + 2 * j + 1]); }
-  dst[0] = q0; dst[1] = q1;
-}
+// Byte offset of (row r, column c) of a staged slice in the layout a TMA box of 16 columns reads it from: rows in
+// decode_tile's numbering ([bf][bh][bw]), 16-byte chunks of each row XORed with address bits 7-8 (SWIZZLE_64B, 64-byte fp32
+// rows) or bit 7 (SWIZZLE_32B, 32-byte fp16 rows).  The staging is 1024-byte aligned, so these are the absolute address bits
+// the TMA unit swizzles with.
+__device__ __forceinline__ uint32_t sw64_off(int r, int c) { return r * 64 + ((((c >> 2) ^ (r >> 1)) & 3) << 4) + (c & 3) * 4; }
+__device__ __forceinline__ uint32_t sw32_off(int r, int c) { return r * 32 + ((((c >> 3) ^ (r >> 2)) & 1) << 4) + (c & 7) * 2; }
 
-// One 16-column chunk (tile columns [c, c + 16)) of accumulator row `row`, read from the staged slice `st`.
-// Row r of the tile is pixel (x, y, f) = (r % bw, (r / bw) % bh, r / (bw*bh)).
-__device__ __forceinline__ void epilogue_row_chunk(const UmmaConvParams& p, const TileCoord& t, int row, int col, const float* st) {
-  const int rw = row % p.bw, rh = (row / p.bw) % p.bh, rf = row / (p.bw * p.bh);
-  const int w = t.w0 + rw, h = t.h0 + rh, f = t.f0 + rf;
-  const int os = p.out_stride;
-  const bool valid = (rf < p.bf) && (w < p.W) && (h < p.H) && (f < p.F) && (w % os == 0) && (h % os == 0);
-  if (!valid || col >= p.Cout) return;
-  const long long opix = (long long)(f * p.OH + h / os) * p.OW + w / os;
-  uint32_t r[16];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float4 q = reinterpret_cast<const float4*>(st)[j];
-    r[4 * j] = __float_as_uint(q.x); r[4 * j + 1] = __float_as_uint(q.y); r[4 * j + 2] = __float_as_uint(q.z); r[4 * j + 3] = __float_as_uint(q.w);
-  }
-  const bool d1 = col < p.n_split;
-  if (p.out_f32) {
-    // SSNB_EXACT_TC: fp32 epilogue + the result's fp16 hi / lo operand planes (umma_epi32.cuh); a fused sibling forward sends
-    // columns >= n_split to the second destination (its own pitch / channel offset)
-    const float alpha = p.alpha * (p.alpha_dev ? __ldg(p.alpha_dev) : 1.0f);
-    float* o32 = d1 ? p.out32 + opix * p.out_pitch + p.out_coff + col : p.out32_2 + opix * p.out2_pitch + p.out2_coff - p.n_split + col;
-    __half* hi = d1 ? p.out_hi : p.out_hi2;
-    if (hi) hi += d1 ? opix * p.out_pitch + p.out_coff + col : opix * p.out2_pitch + p.out2_coff - p.n_split + col;
-    const float* m32 = p.mask32 ? p.mask32 + opix * p.mask32_pitch + p.mask32_coff + col : nullptr;
-    store_chunk32(p, alpha, r, p.bias + col, o32, hi, m32, d1 ? p.out_lo_off : p.out_lo_off2);
-    return;
-  }
-  uint4* dst = reinterpret_cast<uint4*>(d1 ? p.out + opix * p.out_pitch + p.out_coff + col : p.out2 + opix * p.out2_pitch + p.out2_coff - p.n_split + col);
-  uint4 o0 = {}, o1 = {}, y0 = {}, y1 = {};
-  if (p.accumulate) { o0 = dst[0]; o1 = dst[1]; }
-  if (p.mask_y) {
-    const uint4* my = reinterpret_cast<const uint4*>(p.mask_y + opix * p.mask_pitch + p.mask_coff + col);
-    y0 = __ldg(my); y1 = __ldg(my + 1);
-  }
-  epilogue_chunk(p, r, col, dst, o0, o1, y0, y1);
-}
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
 
 // the first NK 16-channel steps of a staged K chunk: A rows [sa, +128 rows) x B rows [sb, +BN rows), both K-major; one
 // m64nBNk16 MMA per 64-row block, both on the same B slice
@@ -171,6 +101,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
                  const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a_lo,
                  const __grid_constant__ CUtensorMap tmap_a2_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
+                 const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o_hi,
+                 const __grid_constant__ CUtensorMap tmap_o_lo, const __grid_constant__ CUtensorMap tmap_o2,
+                 const __grid_constant__ CUtensorMap tmap_o2_hi, const __grid_constant__ CUtensorMap tmap_o2_lo,
                  const __grid_constant__ UmmaConvParams p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operand tiles need 1024-byte alignment
@@ -195,6 +128,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_a2)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_b)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmap_o)) : "memory");
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }   // released by the consumer that owns the tile
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -235,7 +169,8 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     consumer_regs();
     const int cw = wg - 1, row = threadIdx.x & 127;
     const int warp = row / 32, lane = row & 31;
-    float* epi = reinterpret_cast<float*>(smem + PIPE_BYTES + cw * EPI_BYTES);
+    uint8_t* epi = smem + PIPE_BYTES + cw * EPI_BYTES;
+    const float alpha = p.out_f32 ? p.alpha * (p.alpha_dev ? __ldg(p.alpha_dev) : 1.0f) : 1.0f;
     // grid <= total_tiles, so every CTA has at least one tile
     const int my_tiles = (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     uint32_t stage = 0, phase = 0;
@@ -283,27 +218,194 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       wgmma_wait<0>();
       if (row == 0) mbar_arrive(&empty_bar[prev]);
       ring_advance(stage, phase, ksteps, STAGES);      // the other warpgroup's tile j + 1
-      // epilogue, one EPI_COLS-column slice at a time: fragments -> this warpgroup's staging -> one row per thread
+      // epilogue, one 16-column slice at a time, in the accumulators' fragment layout: thread (warp, lane) holds rows
+      // 64 b + 16 warp + lane / 4 + 8 h and columns 8 k + 2 (lane % 4) + {0, 1} of the slice (b, h, k in {0, 1}).  The
+      // results go to this warpgroup's staging in the output box layout, from which one thread stores them by TMA.
+      bool rv[2][2];                                   // the row is a pixel of the image (TMA clips the others)
+      int rpix[2][2];                                  // its pixel index (f * H + h) * W + w
 #pragma unroll
-      for (int sl = 0; sl < (BN + EPI_COLS - 1) / EPI_COLS; ++sl) {
-        named_bar_sync(EPI_BAR + cw, 128);               // the previous slice (or tile) has been read
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = b * 64 + warp * 16 + (lane >> 2) + 8 * h;
+          const int rw = r % p.bw, rh = (r / p.bw) % p.bh, rf = r / (p.bw * p.bh);
+          const int w = t.w0 + rw, y = t.h0 + rh, f = t.f0 + rf;
+          rv[b][h] = rf < p.bf && w < p.W && y < p.H && f < p.F;
+          rpix[b][h] = (f * p.H + y) * p.W + w;
+        }
+      const int q2 = 2 * (lane & 3);
+#pragma unroll
+      for (int sl = 0; sl < BN / EPI_COLS; ++sl) {
+        const int col = t.n0 + sl * EPI_COLS;          // N % 16 == 0: a slice is all inside N or all past it
+        if (col >= p.Cout) break;
+        const bool d1 = col < p.n_split;               // n_split % 16 == 0: a slice has one destination
+        const int cd = d1 ? col : col - p.n_split;     // its first column in that destination
+        const int opitch = d1 ? p.out_pitch : p.out2_pitch, ocoff = d1 ? p.out_coff : p.out2_coff;
+        float v[2][2][4];                              // [b][h][2 k + e]
 #pragma unroll
         for (int b = 0; b < 2; ++b)
 #pragma unroll
-          for (int i = 0; i < EPI_COLS / 2; i += 2) {
-            const int ai = sl * (EPI_COLS / 2) + i;      // accumulator registers [16 sl, 16 sl + 16) are slice sl's columns
-            if (ai < BN / 2) {
-              const int r = b * 64 + warp * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
-              const int c = 8 * (i >> 2) + 2 * (lane & 3);
-              *reinterpret_cast<float2*>(epi + r * EPI_PITCH + c) = make_float2(acc[b][ai], acc[b][ai + 1]);
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const int i = sl * (EPI_COLS / 2) + 4 * k + 2 * h;   // accumulator registers [8 sl, 8 sl + 8) are slice sl's columns
+              v[b][h][2 * k] = acc[b][i]; v[b][h][2 * k + 1] = acc[b][i + 1];
+            }
+        // the per-element operations and their order are those of the row-per-thread epilogue this replaced; explicit
+        // rounding keeps the compiler from contracting alpha * acc + bias / old into an FMA
+        const bool planes = p.out_f32 && (d1 ? p.planes : p.planes2);   // EXACT_TC: write the hi / lo operand planes as well
+        if (p.out_f32) {
+#pragma unroll
+          for (int b = 0; b < 2; ++b)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int j = 0; j < 4; ++j) v[b][h][j] = __fmul_rn(v[b][h][j], alpha);
+          if (p.bias) {
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col + 8 * k + q2));
+#pragma unroll
+              for (int b = 0; b < 2; ++b)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) { v[b][h][2 * k] = __fadd_rn(v[b][h][2 * k], bb.x); v[b][h][2 * k + 1] = __fadd_rn(v[b][h][2 * k + 1], bb.y); }
             }
           }
-        named_bar_sync(EPI_BAR + cw, 128);
+          if (p.accumulate) {
+            const float* o32 = (d1 ? p.out32 : p.out32_2) + ocoff + cd + q2;
 #pragma unroll
-        for (int c = 0; c < EPI_COLS; c += 16)
-          if (sl * EPI_COLS + c < BN) epilogue_row_chunk(p, t, row, t.n0 + sl * EPI_COLS + c, epi + row * EPI_PITCH + c);
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                if (rv[b][h])
+#pragma unroll
+                  for (int k = 0; k < 2; ++k) {
+                    const float2 o = *reinterpret_cast<const float2*>(o32 + (long long)rpix[b][h] * opitch + 8 * k);
+                    v[b][h][2 * k] = __fadd_rn(v[b][h][2 * k], o.x); v[b][h][2 * k + 1] = __fadd_rn(v[b][h][2 * k + 1], o.y);
+                  }
+          }
+          if (p.relu) {
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) v[b][h][j] = fmaxf(v[b][h][j], 0.f);
+          }
+          if (p.mask32) {                              // ReLU gradient of the value this data gradient completes: keep where y > 0 (NaN -> 0)
+            const float* m32 = p.mask32 + p.mask32_coff + col + q2;
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                  const float2 y = rv[b][h] ? __ldg(reinterpret_cast<const float2*>(m32 + (long long)rpix[b][h] * p.mask32_pitch + 8 * k)) : make_float2(0.f, 0.f);
+                  if (!(y.x > 0.f)) v[b][h][2 * k] = 0.f;
+                  if (!(y.y > 0.f)) v[b][h][2 * k + 1] = 0.f;
+                }
+          }
+        } else {
+          if (p.bias) {
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(p.bias + col + 8 * k + q2));
+#pragma unroll
+              for (int b = 0; b < 2; ++b)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) { v[b][h][2 * k] += bb.x; v[b][h][2 * k + 1] += bb.y; }
+            }
+          }
+          if (p.accumulate) {
+            const __half* o16 = (d1 ? p.out : p.out2) + ocoff + cd + q2;
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                if (rv[b][h])
+#pragma unroll
+                  for (int k = 0; k < 2; ++k) {
+                    const float2 o = __half22float2(*reinterpret_cast<const __half2*>(o16 + (long long)rpix[b][h] * opitch + 8 * k));
+                    v[b][h][2 * k] += o.x; v[b][h][2 * k + 1] += o.y;
+                  }
+          }
+          if (p.relu) {
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) v[b][h][j] = fmaxf(v[b][h][j], 0.f);
+          }
+          if (p.mask_y) {
+            const __half* my = p.mask_y + p.mask_coff + col + q2;
+#pragma unroll
+            for (int b = 0; b < 2; ++b)
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                  const float2 y = rv[b][h] ? __half22float2(__ldg(reinterpret_cast<const __half2*>(my + (long long)rpix[b][h] * p.mask_pitch + 8 * k)))
+                                            : make_float2(0.f, 0.f);
+                  if (!(y.x > 0.f)) v[b][h][2 * k] = 0.f;
+                  if (!(y.y > 0.f)) v[b][h][2 * k + 1] = 0.f;
+                }
+          }
+        }
+        // the staging is free once the TMA has read the previous slice out of it
+        if (row == 0) bulk_wait_read0();
+        named_bar_sync(EPI_BAR + cw, 128);
+        const bool scaled = p.flag || p.plane_scale != 1.0f;   // gradient planes: scaled by the loss scale, guarded against the fp16 range
+        float m = 0.f;
+#pragma unroll
+        for (int b = 0; b < 2; ++b)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = b * 64 + warp * 16 + (lane >> 2) + 8 * h;
+            if (p.out_f32) {
+              // a half-warp writes rows r0..r0+3: rows with (r >> 1) & 1 write their columns 8..15 first, so that the four
+              // rows' 32-byte pieces of one store fall in four different bank quarters
+              const bool s = (lane >> 3) & 1;
+              const float2 x0 = make_float2(v[b][h][0], v[b][h][1]), x1 = make_float2(v[b][h][2], v[b][h][3]);
+              *reinterpret_cast<float2*>(epi + sw64_off(r, q2 + (s ? 8 : 0))) = s ? x1 : x0;
+              *reinterpret_cast<float2*>(epi + sw64_off(r, q2 + (s ? 0 : 8))) = s ? x0 : x1;
+              if (planes)
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                  float x0 = v[b][h][2 * k], x1 = v[b][h][2 * k + 1];
+                  if (scaled) {
+                    x0 = __fmul_rn(x0, p.plane_scale); x1 = __fmul_rn(x1, p.plane_scale);
+                    if (rv[b][h]) {
+                      m = fmaxf(m, fabsf(x0)); if (x0 != x0) m = INFINITY;
+                      m = fmaxf(m, fabsf(x1)); if (x1 != x1) m = INFINITY;
+                    }
+                  }
+                  const __half2 hh = __floats2half2_rn(x0, x1);
+                  const float2 hf = __half22float2(hh);
+                  *reinterpret_cast<uint32_t*>(epi + EPI_F32_BYTES + sw32_off(r, 8 * k + q2)) = h2_bits(hh);
+                  *reinterpret_cast<uint32_t*>(epi + EPI_F32_BYTES + EPI_F16_BYTES + sw32_off(r, 8 * k + q2)) =
+                      h2_bits(__floats2half2_rn(__fsub_rn(x0, hf.x), __fsub_rn(x1, hf.y)));
+                }
+            } else {
+#pragma unroll
+              for (int k = 0; k < 2; ++k)
+                *reinterpret_cast<uint32_t*>(epi + sw32_off(r, 8 * k + q2)) = h2_bits(__floats2half2_rn(v[b][h][2 * k], v[b][h][2 * k + 1]));
+            }
+          }
+        if (planes && p.flag && !(m <= 65504.f)) *p.flag = 1;
+        fence_proxy_async_smem();
+        named_bar_sync(EPI_BAR + cw, 128);
+        if (row == 0) {
+          tma_store_4d(d1 ? &tmap_o : &tmap_o2, epi, cd, t.w0, t.h0, t.f0);
+          if (planes) {
+            tma_store_4d(d1 ? &tmap_o_hi : &tmap_o2_hi, epi + EPI_F32_BYTES, cd, t.w0, t.h0, t.f0);
+            tma_store_4d(d1 ? &tmap_o_lo : &tmap_o2_lo, epi + EPI_F32_BYTES + EPI_F16_BYTES, cd, t.w0, t.h0, t.f0);
+          }
+          bulk_commit();
+        }
       }
     }
+    if (row == 0) bulk_wait0();                        // the stores are complete before the CTA retires
   }
 }
 
@@ -329,11 +431,12 @@ int resolve_encode(UmmaContext& ctx) {
 }
 
 int encode(UmmaContext& ctx, CUtensorMap* m, int rank, void* addr, const cuuint64_t* dims, const cuuint64_t* strides,
-           const cuuint32_t* box, int spatial_stride = 1) {
+           const cuuint32_t* box, int spatial_stride = 1, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+           CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   // spatial_stride 2: the box traverses W and H with step 2 (box extents are given in un-strided elements)
   cuuint32_t es[5] = {1, (cuuint32_t)spatial_stride, (cuuint32_t)spatial_stride, 1, 1};
-  CUresult r = reinterpret_cast<EncodeTiledFn>(ctx.encode_tiled)(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, addr, dims, strides,
-                                                                box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  CUresult r = reinterpret_cast<EncodeTiledFn>(ctx.encode_tiled)(m, dtype, (cuuint32_t)rank, addr, dims, strides,
+                                                                box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                                                                 CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     char buf[128];
@@ -352,14 +455,51 @@ void pick_box(int W, int& bw, int& bh, int& bf) {
   else { bw = 1; bh = 1; bf = 128; }
 }
 
-int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int K, int N, int ntaps, int out_stride, const __half* w,
+// the epilogue's store box over one destination: channels [0, n) of the NHWC tensor at `base` (already offset to the
+// destination's first channel, `pitch` channels per pixel) at the plan's output geometry; fp32 results in 64-byte
+// SWIZZLE_64B rows, fp16 values in 32-byte SWIZZLE_32B rows (the layouts of sw64_off / sw32_off)
+int encode_out(UmmaContext& ctx, CUtensorMap* m, const UmmaConvParams& p, const void* base, int pitch, int n, bool f32) {
+  const cuuint64_t es = f32 ? 4 : 2;
+  cuuint64_t dims[4] = {(cuuint64_t)n, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.F};
+  cuuint64_t str[3] = {(cuuint64_t)pitch * es, (cuuint64_t)p.W * pitch * es, (cuuint64_t)p.H * p.W * pitch * es};
+  cuuint32_t box[4] = {(cuuint32_t)EPI_COLS, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)p.bf};
+  return encode(ctx, m, 4, const_cast<void*>(base), dims, str, box, 1, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                f32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
+// fp16 hi / lo operand planes of one destination: hi at `hi` (offset to the first channel), lo `lo_off` bytes later
+int encode_planes(UmmaContext& ctx, CUtensorMap* mhi, CUtensorMap* mlo, const UmmaConvParams& p, const __half* hi, long long lo_off, int pitch, int n) {
+  if (int rc = encode_out(ctx, mhi, p, hi, pitch, n, false)) return rc;
+  return encode_out(ctx, mlo, p, reinterpret_cast<const char*>(hi) + lo_off, pitch, n, false);
+}
+
+// the output maps of one destination (second: the columns >= n_split of a fused sibling forward): view o names the fp16
+// result (FAST) or the result's operand planes (EXACT_TC, o.base == nullptr: none), out32 the EXACT_TC fp32 result with
+// o's pitch and channel offset
+int bind_out(UmmaContext& ctx, UmmaConvPlan& plan, View o, float* out32, int n, bool second) {
+  UmmaConvParams& p = plan.p;
+  CUtensorMap* m = second ? &plan.tmap_o2 : &plan.tmap_o;
+  CUtensorMap* mhi = second ? &plan.tmap_o2_hi : &plan.tmap_o_hi;
+  CUtensorMap* mlo = second ? &plan.tmap_o2_lo : &plan.tmap_o_lo;
+  const bool f32 = p.out_f32 != 0;
+  if (int rc = encode_out(ctx, m, p, f32 ? (const void*)(out32 + o.coff) : (const void*)(reinterpret_cast<__half*>(o.base) + o.coff), o.pitch, n, f32))
+    return rc;
+  *mhi = *m; *mlo = *m;
+  const int planes = f32 && o.base;
+  if (planes)
+    if (int rc = encode_planes(ctx, mhi, mlo, p, reinterpret_cast<__half*>(o.base) + o.coff, o.lo_off, o.pitch, n)) return rc;
+  (second ? p.planes2 : p.planes) = planes;
+  return 0;
+}
+
+int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int K, int N, int ntaps, const __half* w,
                 int a_stride = 1, const UmmaTcOpts* tc = nullptr) {
   plan.enabled = false;
   if (int rc = resolve_encode(ctx)) return rc;
   if (a_stride == 2) {
     // strided TMA: tiles enumerate OUTPUT pixels, the A box steps over the input with stride 2
     View ao = a; ao.H = o.H; ao.W = o.W;
-    if (int rc = bind_common(ctx, plan, ao, o, F, K, N, ntaps, 1, w, 1, tc)) return rc;
+    if (int rc = bind_common(ctx, plan, ao, o, F, K, N, ntaps, w, 1, tc)) return rc;
     plan.enabled = false;
     UmmaConvParams& q = plan.p;
     q.a_stride = 2;
@@ -374,7 +514,7 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
     plan.enabled = true;
     return 0;
   }
-  if ((a.H + out_stride - 1) / out_stride != o.H || (a.W + out_stride - 1) / out_stride != o.W) { set_thread_error("umma conv: geometry mismatch"); return 1; }
+  if (a.H != o.H || a.W != o.W) { set_thread_error("umma conv: geometry mismatch"); return 1; }
   if (K % 8 || N % 16 || a.pitch % 8 || a.coff % 8 || o.pitch % 8 || o.coff % 8 || ntaps > UMMA_MAX_TAPS) {
     set_thread_error("umma conv: unsupported channel alignment"); return 1; }
   UmmaConvParams& p = plan.p;
@@ -390,7 +530,7 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   p.K = K;
   p.ntaps = ntaps;
   p.out = reinterpret_cast<__half*>(o.base); p.out_pitch = o.pitch; p.out_coff = o.coff; p.Cout = N;
-  p.out_stride = out_stride; p.OH = o.H; p.OW = o.W; p.a_stride = 1; p.mask_y = nullptr; p.mask_pitch = 0; p.mask_coff = 0;
+  p.a_stride = 1; p.mask_y = nullptr; p.mask_pitch = 0; p.mask_coff = 0;
   p.kchunks_a1 = (K + BLOCK_K - 1) / BLOCK_K; p.K1 = K; p.n_split = 1 << 30; p.out2 = p.out; p.out2_pitch = o.pitch; p.out2_coff = o.coff;
   {
     cuuint64_t dims[4] = {(cuuint64_t)K, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)F};
@@ -419,9 +559,12 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   p.stages = PIPE_BYTES / p.stage_bytes; if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
   p.alpha = tc ? tc->alpha : 1.0f; p.alpha_dev = tc ? tc->alpha_dev : nullptr;
   p.mask32 = nullptr; p.mask32_pitch = 0; p.mask32_coff = 0; p.plane_scale = 1.0f; p.flag = nullptr;
-  p.out32 = tc ? tc->out32 : nullptr; p.out_hi = tc ? reinterpret_cast<__half*>(o.base) : nullptr; p.out_lo_off = tc ? o.lo_off : 0;
-  p.out32_2 = p.out32; p.out_hi2 = p.out_hi; p.out_lo_off2 = p.out_lo_off;       // second destination = the first unless a fused bind redirects it
+  p.out32 = tc ? tc->out32 : nullptr;
   if (tc && (!tc->out32 || !a.lo_off || !tc->w_lo_off)) { set_thread_error("umma conv: split-operand bind needs operand planes and an fp32 output"); return 1; }
+  if (int rc = bind_out(ctx, plan, o, p.out32, N, false)) return rc;
+  // second destination = the first unless a fused bind redirects it
+  p.out32_2 = p.out32; p.planes2 = p.planes;
+  plan.tmap_o2 = plan.tmap_o; plan.tmap_o2_hi = plan.tmap_o_hi; plan.tmap_o2_lo = plan.tmap_o_lo;
   plan.enabled = true;
   return 0;
 }
@@ -432,7 +575,7 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
 void mark_tc_ok(UmmaConvPlan& plan, int W, bool two_sources) {
   UmmaConvParams& p = plan.p;
   p.tc_ok = 0;
-  if (!plan.enabled || p.a_stride != 1 || p.out_stride != 1) return;
+  if (!plan.enabled || p.a_stride != 1) return;
   if (!(p.ntaps == 1 || p.ntaps == 4 || p.ntaps == 9)) return;
   if (p.kchunks_a1 != p.kchunks && (p.ntaps != 1 || !two_sources)) return;
   if (p.out_pitch % 16 || p.out_coff % 16 || p.out2_pitch % 16 || p.out2_coff % 16 || p.n_split % 16 || (p.bias && p.n_tiles * p.block_n > 1024)) return;
@@ -453,7 +596,7 @@ void umma_context_destroy(UmmaContext&) {}
 
 int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int ntaps,
                         const int* dy, const int* dx, const __half* w_tap_n_k, const float* bias, int relu, const UmmaTcOpts* tc) {
-  if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, ntaps, 1, w_tap_n_k, 1, tc)) return rc;
+  if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, ntaps, w_tap_n_k, 1, tc)) return rc;
   for (int t = 0; t < ntaps; ++t) { plan.p.tap_dy[t] = dy[t]; plan.p.tap_dx[t] = dx[t]; }
   plan.p.bias = bias; plan.p.relu = relu; plan.p.accumulate = 0;
   mark_tc_ok(plan, in.W, false);
@@ -462,12 +605,9 @@ int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out,
 
 int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int k, int pad,
                        int stride, const __half* w_tap_n_k, const float* bias, const UmmaTcOpts* tc) {
-  // a stride-2 layer (k=3, pad=1): tiles over OUTPUT pixels whose A boxes step over the input with TMA element
-  // stride 2 (default), or the stride-1 convolution sampled at even pixels (4x redundant MMAs, SSNB_TMA_STRIDED=0)
-  const char* st = getenv("SSNB_TMA_STRIDED");           // default on; "0" falls back to the sampled-epilogue variant
-  const bool strided = stride == 2 && !(st && st[0] == '0');
-  if (int rc = strided ? bind_common(ctx, plan, in, out, F, cin, cout, k * k, 1, w_tap_n_k, 2, tc)
-                       : bind_common(ctx, plan, in, out, F, cin, cout, k * k, stride, w_tap_n_k, 1, tc)) return rc;
+  // a stride-2 layer (k=3, pad=1): tiles over OUTPUT pixels whose A boxes step over the input with TMA element stride 2
+  if (stride != 1 && stride != 2) { set_thread_error("umma conv: stride must be 1 or 2"); return 1; }
+  if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, k * k, w_tap_n_k, stride, tc)) return rc;
   for (int r = 0; r < k; ++r)
     for (int s = 0; s < k; ++s) { plan.p.tap_dy[r * k + s] = r - pad; plan.p.tap_dx[r * k + s] = s - pad; }
   plan.p.bias = bias; plan.p.relu = 1; plan.p.accumulate = 0;
@@ -478,7 +618,7 @@ int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, 
 int umma_conv_bind_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz, View dx, int F, int cin, int cout, int k, int pad,
                          const __half* w_tap_k_n, int accumulate, const UmmaTcOpts* tc) {
   // dx[p, ci] = sum_{r,s,co} dz[p + (pad-r, pad-s), co] * W[co][ci][r][s] : K = cout, N = cin
-  if (int rc = bind_common(ctx, plan, dz, dx, F, cout, cin, k * k, 1, w_tap_k_n, 1, tc)) return rc;
+  if (int rc = bind_common(ctx, plan, dz, dx, F, cout, cin, k * k, w_tap_k_n, 1, tc)) return rc;
   for (int r = 0; r < k; ++r)
     for (int s = 0; s < k; ++s) { plan.p.tap_dy[r * k + s] = pad - r; plan.p.tap_dx[r * k + s] = pad - s; }
   plan.p.bias = nullptr; plan.p.relu = 0; plan.p.accumulate = accumulate;
@@ -491,14 +631,16 @@ int umma_conv_bind_fused_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View
   // bind as one convolution with N = n1 + n2 writing to out1's geometry, then redirect columns >= n1
   View o = out1; o.C = n1 + n2;
   if (out1.H != out2.H || out1.W != out2.W || n1 % 16 || n2 % 16 || out2.pitch % 8 || out2.coff % 8) { set_thread_error("fused fwd: bad views"); return 1; }
-  if (int rc = bind_common(ctx, plan, in, o, F, cin, n1 + n2, 1, 1, w_n_k, 1, tc)) return rc;
+  if (tc && !tc->out32_2) { set_thread_error("fused fwd: the split-operand bind needs both fp32 destinations"); return 1; }
+  if (int rc = bind_common(ctx, plan, in, o, F, cin, n1 + n2, 1, w_n_k, 1, tc)) return rc;
   plan.p.tap_dy[0] = 0; plan.p.tap_dx[0] = 0;
   plan.p.bias = bias; plan.p.relu = 1; plan.p.accumulate = 0;
   plan.p.n_split = n1; plan.p.out2 = reinterpret_cast<__half*>(out2.base); plan.p.out2_pitch = out2.pitch; plan.p.out2_coff = out2.coff;
-  if (tc) {        // EXACT_TC: out1 / out2 are the operand-plane views of the two destinations, tc->out32 / out32_2 their fp32 buffers
-    if (!tc->out32_2) { set_thread_error("fused fwd: the split-operand bind needs both fp32 destinations"); return 1; }
-    plan.p.out32_2 = tc->out32_2; plan.p.out_hi2 = reinterpret_cast<__half*>(out2.base); plan.p.out_lo_off2 = out2.lo_off;
-  }
+  // EXACT_TC: out1 / out2 are the operand-plane views of the two destinations, tc->out32 / out32_2 their fp32 buffers.  Each
+  // destination's maps end at its own channel count, so TMA clips there.
+  if (tc) plan.p.out32_2 = tc->out32_2;
+  if (int rc = bind_out(ctx, plan, out1, plan.p.out32, n1, false)) { plan.enabled = false; return rc; }
+  if (int rc = bind_out(ctx, plan, out2, plan.p.out32_2, n2, true)) { plan.enabled = false; return rc; }
   mark_tc_ok(plan, in.W, false);
   return 0;
 }
@@ -508,7 +650,7 @@ int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, V
   const int k1p = (k1 + BLOCK_K - 1) / BLOCK_K * BLOCK_K;
   // bind with the first source as the A view and the full fused K; then attach the second source
   View a = k1 ? dz1 : dz2;
-  if (int rc = bind_common(ctx, plan, a, dx, F, k1 ? k1 : k2, cin, 1, 1, w_n_k, 1, tc)) return rc;
+  if (int rc = bind_common(ctx, plan, a, dx, F, k1 ? k1 : k2, cin, 1, w_n_k, 1, tc)) return rc;
   UmmaConvParams& p = plan.p;
   p.tap_dy[0] = 0; p.tap_dx[0] = 0; p.bias = nullptr; p.relu = 0; p.accumulate = accumulate;
   if (k1) {
@@ -543,15 +685,18 @@ void umma_conv_set_mask(UmmaConvPlan& plan, View y) {
   plan.mask_y = reinterpret_cast<const __half*>(y.base); plan.mask_pitch = y.pitch; plan.mask_coff = y.coff;
 }
 
-void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag) {
+int umma_conv_set_mask_tc(UmmaContext& ctx, UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag) {
+  // a data gradient has one destination: the planes replace the first destination's
+  if (int rc = encode_planes(ctx, &plan.tmap_mask_hi, &plan.tmap_mask_lo, plan.p, reinterpret_cast<__half*>(dplanes.base) + dplanes.coff, dplanes.lo_off,
+                             dplanes.pitch, plan.p.Cout)) return rc;
   plan.mask32 = reinterpret_cast<const float*>(y32.base); plan.mask32_pitch = y32.pitch; plan.mask32_coff = y32.coff;
-  plan.mask_planes = reinterpret_cast<__half*>(dplanes.base); plan.mask_planes_lo = dplanes.lo_off;
-  plan.mask_plane_scale = plane_scale; plan.mask_flag = flag;
+  plan.mask_planes = true; plan.mask_plane_scale = plane_scale; plan.mask_flag = flag;
+  return 0;
 }
 
 namespace {
 template <int BN>
-int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, int grid, cudaStream_t s) {
+int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, const CUtensorMap& o_hi, const CUtensorMap& o_lo, int grid, cudaStream_t s) {
   static bool attr_set[64] = {};          // function attributes are per device
   auto kern = umma_conv_kernel<BN>;
   int dev = 0;
@@ -561,7 +706,8 @@ int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, int grid, cudaS
       set_thread_error("umma conv: cannot raise dynamic shared memory limit"); cudaGetLastError(); return 2; }
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  kern<<<grid, NUM_THREADS, SMEM_BYTES, s>>>(plan.tmap_a, plan.tmap_a2, plan.tmap_b, plan.tmap_a_lo, plan.tmap_a2_lo, plan.tmap_b_lo, p);
+  kern<<<grid, NUM_THREADS, SMEM_BYTES, s>>>(plan.tmap_a, plan.tmap_a2, plan.tmap_b, plan.tmap_a_lo, plan.tmap_a2_lo, plan.tmap_b_lo, plan.tmap_o, o_hi, o_lo,
+                                             plan.tmap_o2, plan.tmap_o2_hi, plan.tmap_o2_lo, p);
   SSNB_LAUNCH_CHECK("umma_conv_kernel");
   return 0;
 }
@@ -571,23 +717,26 @@ int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s,
   if (!plan.enabled) { set_thread_error("umma conv: plan not bound"); return 3; }
   UmmaConvParams p = plan.p;
   if (mask && plan.mask_y) { p.mask_y = plan.mask_y; p.mask_pitch = plan.mask_pitch; p.mask_coff = plan.mask_coff; }
-  if (mask && p.out_f32 && plan.mask32) {
+  const bool mplanes = mask && p.out_f32 && plan.mask32 && plan.mask_planes;
+  if (mplanes) {
     p.mask32 = plan.mask32; p.mask32_pitch = plan.mask32_pitch; p.mask32_coff = plan.mask32_coff;
-    p.out_hi = plan.mask_planes; p.out_lo_off = plan.mask_planes_lo; p.plane_scale = plan.mask_plane_scale; p.flag = plan.mask_flag;
+    p.planes = 1; p.plane_scale = plan.mask_plane_scale; p.flag = plan.mask_flag;
   }
-  if (p.out_f32 && (p.mask_y || p.out_stride != 1)) { set_thread_error("umma conv: the fp32 epilogue takes its mask through mask32 and has no sampling"); return 3; }
+  if (p.out_f32 && p.mask_y) { set_thread_error("umma conv: the fp32 epilogue takes its mask through mask32"); return 3; }
+  const CUtensorMap& o_hi = mplanes ? plan.tmap_mask_hi : plan.tmap_o_hi;
+  const CUtensorMap& o_lo = mplanes ? plan.tmap_mask_lo : plan.tmap_o_lo;
   const int total = p.tiles_w * p.tiles_h * p.tiles_f * p.n_tiles;
   const int grid = total < ctx.num_sms ? total : ctx.num_sms;
   t_tag.tiles = total; t_tag.block_n = p.block_n;
   switch (p.block_n) {
-    case 16: return launch_bn<16>(plan, p, grid, s);
-    case 32: return launch_bn<32>(plan, p, grid, s);
-    case 48: return launch_bn<48>(plan, p, grid, s);
-    case 64: return launch_bn<64>(plan, p, grid, s);
-    case 80: return launch_bn<80>(plan, p, grid, s);
-    case 96: return launch_bn<96>(plan, p, grid, s);
-    case 112: return launch_bn<112>(plan, p, grid, s);
-    case 128: return launch_bn<128>(plan, p, grid, s);
+    case 16: return launch_bn<16>(plan, p, o_hi, o_lo, grid, s);
+    case 32: return launch_bn<32>(plan, p, o_hi, o_lo, grid, s);
+    case 48: return launch_bn<48>(plan, p, o_hi, o_lo, grid, s);
+    case 64: return launch_bn<64>(plan, p, o_hi, o_lo, grid, s);
+    case 80: return launch_bn<80>(plan, p, o_hi, o_lo, grid, s);
+    case 96: return launch_bn<96>(plan, p, o_hi, o_lo, grid, s);
+    case 112: return launch_bn<112>(plan, p, o_hi, o_lo, grid, s);
+    case 128: return launch_bn<128>(plan, p, o_hi, o_lo, grid, s);
   }
   set_thread_error("umma conv: unsupported tile width"); return 3;
 }

@@ -30,7 +30,6 @@ struct UmmaConvParams {
   int kchunks, ntaps, K;          // ceil(K/64), filter taps, reduction channels per tap
   int tap_dy[UMMA_MAX_TAPS], tap_dx[UMMA_MAX_TAPS];
   __half* out; int out_pitch, out_coff, Cout;
-  int out_stride, OH, OW;         // stride-2 layers: tiles run at input resolution, only even pixels are stored
   int a_stride;                   // 2: tiles run at OUTPUT resolution and the A box uses TMA element stride 2
   const float* bias;              // [Cout] or nullptr
   int relu, accumulate;
@@ -45,16 +44,18 @@ struct UmmaConvParams {
   const __half* mask_y; int mask_pitch, mask_coff;
   // SSNB_EXACT_TC (error-compensated split operands): nseg = 3 stages the hi and lo planes of A and B of each (tap, K chunk)
   //   together and issues (A_lo, B_hi), (A_hi, B_lo), (A_hi, B_hi) into the same accumulator; nseg = 1 is the plain fp16 product.
-  // out_f32: the epilogue works in fp32 -- out32 = alpha * acc (+ bias, ReLU | + old out32) -- and, when out_hi is set,
-  // also writes the result's fp16 hi / lo operand planes (same pitch / channel offset, lo plane out_lo_off bytes later).
+  // out_f32: the epilogue works in fp32 -- out32 = alpha * acc (+ bias, ReLU | + old out32) -- and, when `planes` is set,
+  // also writes the result's fp16 hi / lo operand planes (same pitch / channel offset; UmmaConvPlan::tmap_o_hi / _lo).
   int nseg, out_f32;
   float alpha;
   const float* alpha_dev;         // optional device scalar multiplied into alpha (1 / the power-of-two scale of the weight planes)
-  float* out32; __half* out_hi; long long out_lo_off;
-  float* out32_2; __half* out_hi2; long long out_lo_off2;   // fused sibling forward: columns >= n_split go here (pitch / offset: out2_pitch / out2_coff)
+  float* out32; int planes;
+  float* out32_2; int planes2;    // fused sibling forward: columns >= n_split go here (pitch / offset: out2_pitch / out2_coff)
   // out_f32 data gradient that is the LAST writer of its output value v: dz = (alpha * acc + old) * (y > 0) with y = the fp32
-  // activation of v; the planes written through out_hi then hold dz * plane_scale (the loss scale) for v's producers'
+  // activation of v; the planes written through UmmaConvPlan::tmap_mask_hi / _lo then hold dz * plane_scale (the loss scale) for v's producers'
   // weight / data gradients, and *flag is raised when that leaves the fp16 range
+  // (the global reads of the epilogue -- bias, old value, mask -- go through the pointers above; its stores through the
+  // output tensor maps of UmmaConvPlan)
   const float* mask32; int mask32_pitch, mask32_coff;
   float plane_scale; int* flag;
 };
@@ -65,9 +66,15 @@ struct UmmaConvPlan {
   CUtensorMap tmap_a, tmap_a2, tmap_b;
   CUtensorMap tmap_a_lo, tmap_a2_lo, tmap_b_lo;   // SSNB_EXACT_TC: LO planes of the three operands (copies of the HI maps otherwise)
   long long b_lo_off = 0;                        // byte offset of the LO weight plane (0: single plane)
-  // SSNB_EXACT_TC mask fusion, applied only when launched with mask=true (see UmmaConvParams::mask32)
+  // epilogue stores, 4-D boxes [bf][bh][bw][16 columns] of the output: the fp32 result (EXACT_TC, SWIZZLE_64B) or the fp16
+  // result (FAST, SWIZZLE_32B), then the fp16 hi / lo operand planes (EXACT_TC, SWIZZLE_32B).  The *2 maps serve columns
+  // >= n_split of a fused sibling forward.  dims[0] of each map is its destination's channel count, so TMA clips a tile
+  // overhanging N or the image instead of writing past it.  Maps a plan does not use are copies of tmap_o.
+  CUtensorMap tmap_o, tmap_o_hi, tmap_o_lo, tmap_o2, tmap_o2_hi, tmap_o2_lo;
+  // SSNB_EXACT_TC mask fusion, applied only when launched with mask=true (see UmmaConvParams::mask32); the gradient planes
+  // it writes replace tmap_o_hi / tmap_o_lo
   const float* mask32 = nullptr; int mask32_pitch = 0, mask32_coff = 0;
-  __half* mask_planes = nullptr; long long mask_planes_lo = 0; float mask_plane_scale = 1.0f; int* mask_flag = nullptr;
+  CUtensorMap tmap_mask_hi, tmap_mask_lo; bool mask_planes = false; float mask_plane_scale = 1.0f; int* mask_flag = nullptr;
   UmmaConvParams p;
 };
 
@@ -95,7 +102,7 @@ int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, V
 int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask = false);
 void umma_conv_set_mask(UmmaConvPlan& plan, View y);
 // EXACT_TC: y32 = fp32 activation of the output value, dplanes = that value's gradient operand planes (hi base + lo_off)
-void umma_conv_set_mask_tc(UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag);
+int umma_conv_set_mask_tc(UmmaContext& ctx, UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag);
 
 // host helpers shared by the tensor-core kernels
 int umma_resolve_encode(UmmaContext& ctx);

@@ -59,6 +59,21 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, u
       : "memory");
 }
 
+// TMA store of a 4-D box from shared memory, tracked by the issuing thread's bulk async-group.  The box's elements outside
+// the tensor map's dims are not written (clipping).
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(reinterpret_cast<uint64_t>(map)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's bulk stores have finished reading their shared-memory source (it may be overwritten)
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// the issuing thread's bulk stores have completed
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy shared-memory writes become visible to the async proxy (TMA) of this CTA
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 // SWIZZLE_128B shared-memory matrix descriptor (sm_90 GMMA layout):
 // start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout_type=1 (128-byte swizzle) [62,64)
 // K-major: SBO = 1024 (8 rows x 128 B), LBO unused.  MN-major: SBO = 1024 between 8-row K groups, LBO = distance between
