@@ -24,8 +24,17 @@ __global__ void combined_scores_kernel(const float* __restrict__ act, const floa
   for (int c = 0; c < K; ++c) combined[(long long)i * K + c] = (expf(a[c + 1] - m) / sum) * expf(comp[(long long)i * K + c]);
 }
 
-// one CTA per class: bitonic sort of (score, index) descending (ties: larger index first = a stable ascending argsort
-// reversed), greedy NMS over the sorted list, regression of the survivors, written in kept order
+// (score, index) a precedes b in the sorted list: NaN first (numpy's argsort()[::-1] puts NaN first), then larger score, ties
+// and NaN against NaN: larger index first (a stable ascending argsort reversed); the padding (index < 0) after everything
+__device__ __forceinline__ bool nms_precedes(float ka, int ia, float kb, int ib) {
+  if (ia < 0 || ib < 0) return ib < 0 && ia >= 0;
+  const bool na = ka != ka, nb = kb != kb;
+  if (na || nb) return na && (!nb || ia > ib);
+  return ka > kb || (ka == kb && ia > ib);
+}
+
+// one CTA per class: bitonic sort of (score, index) in nms_precedes order, greedy NMS over the sorted list, regression of the
+// survivors, written in kept order
 __global__ void __launch_bounds__(256) nms_regress_kernel(const float* __restrict__ props, const float* __restrict__ combined,
                                                           const float* __restrict__ reg, int N, int K, int P, double thresh, int regress,
                                                           float* __restrict__ out, int* __restrict__ count) {
@@ -50,17 +59,16 @@ __global__ void __launch_bounds__(256) nms_regress_kernel(const float* __restric
           const bool desc = (i & k) == 0;                   // this run sorted descending
           const float ka = key[i], kb = key[l];
           const int ia = idx[i], ib = idx[l];
-          // a precedes b in descending order: larger score first (NaN last), ties: larger index first
-          const bool a_first = (ka > kb) || (ka == kb && ia > ib) || (kb != kb && ka == ka);
+          const bool a_first = nms_precedes(ka, ia, kb, ib);
           if (a_first != desc) { key[i] = kb; key[l] = ka; idx[i] = ib; idx[l] = ia; }
         }
       }
       __syncthreads();
     }
-  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {       // the padding sorts after the N proposals: s >= 0 here
     const int s = idx[i];
-    t1[i] = props[2 * s]; t2[i] = props[2 * s + 1];
-    alive[i] = 1;
+    t1[i] = s >= 0 ? props[2 * s] : 0.f; t2[i] = s >= 0 ? props[2 * s + 1] : 0.f;
+    alive[i] = s >= 0;
   }
   if (threadIdx.x == 0) n_kept = 0;
   __syncthreads();

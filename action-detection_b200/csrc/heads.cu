@@ -255,6 +255,17 @@ __device__ __forceinline__ void py_slice(int pl, int pr, int T, int& a, int& b) 
   if (b < a) b = a;
 }
 
+// int(np.arange(left, right + 1e-5, step)[q]) (ops/ssn_ops.py:144-147): numpy stores p[0] = left and p[1] = left + step, then
+// fills p[q] = left + q * (p[1] - p[0]) for q >= 2, each operation rounded on its own (no DFMA), which is not left + q * step
+// when the part count is not a power of two
+__device__ __forceinline__ int reorg_tick(int left, double step, int q) {
+  const double l = (double)left;
+  if (q == 0) return left;
+  const double t1 = __dadd_rn(l, step);
+  if (q == 1) return (int)t1;
+  return (int)__dadd_rn(l, __dmul_rn((double)q, __dsub_rn(t1, l)));
+}
+
 __device__ void pspool_dev(const float* __restrict__ scores, int T, int D, int col0, int score_len, const int* tk,
                            float s0, float s1, const ReorgCfg& cfg, float* __restrict__ out) {
   // threads stride over the score_len output columns
@@ -270,8 +281,8 @@ __device__ void pspool_dev(const float* __restrict__ scores, int T, int D, int c
         const int np_ = cfg.lev[si][l];
         const double step = (double)(right - left) / (double)np_;
         for (int q = 0; q < np_; ++q) {
-          const int pl = (int)((double)left + (double)q * step);
-          const int pr = (int)((double)left + (double)(q + 1) * step);
+          const int pl = reorg_tick(left, step, q);
+          const int pr = reorg_tick(left, step, q + 1);
           if (pr - pl >= 1) {
             int a, b;
             py_slice(pl, pr, T, a, b);
@@ -316,8 +327,8 @@ __device__ void pspool_prefix_dev(const double* __restrict__ P, int T, int D, in
         const int np_ = cfg.lev[si][l];
         const double step = (double)(right - left) / (double)np_;
         for (int q = 0; q < np_; ++q) {
-          const int pl = (int)((double)left + (double)q * step);
-          const int pr = (int)((double)left + (double)(q + 1) * step);
+          const int pl = reorg_tick(left, step, q);
+          const int pr = reorg_tick(left, step, q + 1);
           if (pr - pl >= 1) {
             int a, b;
             py_slice(pl, pr, T, a, b);
