@@ -11,7 +11,8 @@
 //                           signal[down]; every forward / backward search is one O(log U) tree walk instead of the
 //                           reference's O(U) scan, and writes its box to the slot the reference's loop order gives it
 //   score_kernel            per box: sum(frm_scores[a:b]) left to right in fp32, as Python's sum over np.float32 does
-//   cub segmented radix sort by descending score (stable: ties keep the search order)
+//   cub segmented radix sort by descending score (stable: ties keep the search order; every NaN score ranks ahead of
+//                           +inf, NaN-scored boxes in search order, as the reference's argsort()[::-1] puts NaN first)
 //   nms_kernel              one CTA per video: drops identical copies (same start, end and score bits, adjacent after the
 //                           sort), greedy NMS, seconds and the minimum-length filter
 #include <cub/cub.cuh>
@@ -224,8 +225,11 @@ __global__ void __launch_bounds__(kSearchThreads) search_kernel(const VideoDesc*
   }
 }
 
-// descending score as an ascending radix key; -0 and +0 share a key, as they compare equal
+// descending score as an ascending radix key; -0 and +0 share a key, as they compare equal.  Every NaN, whatever its
+// sign or payload, gets key 0, ahead of +inf (key 0x007fffff): NaN-scored boxes rank first, as in the reference's
+// argsort()[::-1], and among themselves keep the search order.  key_score(0) is the NaN 0x7fffffff.
 __device__ __forceinline__ uint32_t score_key(float s) {
+  if (s != s) return 0u;
   uint32_t u = __float_as_uint(s == 0.f ? 0.f : s);
   u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
   return ~u;

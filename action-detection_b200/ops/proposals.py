@@ -7,6 +7,9 @@ Deliberate differences from the reference:
   - gen_prop returns the scores of all NMS survivors next to the boxes that pass the minimum-length filter, so the two lists
     disagree once minimum_len > 0; here every returned box comes with its own score.
   - numpy's argsort leaves the order of tied scores open; here tied boxes stay in the order the search emitted them.
+  - a box whose score is NaN (a NaN or +inf and -inf inside its window) ranks first, as the reference's
+    argsort()[::-1] puts NaN first; among themselves NaN-scored boxes keep the search order too, whatever the NaN's sign
+    (numpy's order among several NaNs is not a rule).
   - the regression branch (:130-132, which calls the undefined regress_box) is not provided.
 """
 import collections

@@ -1,4 +1,5 @@
-"""tests/golden/proposals.npz from the REAL reference (build container only: python -m oracle.gen_golden_proposals).
+"""tests/golden/proposals.npz from the REAL reference (build container only: python -m oracle.gen_golden_proposals), and
+tests/golden/proposals_nms.npz, the reference's NMS on random box lists (python -m oracle.gen_golden_proposals nms).
 
 ops/sequence_funcs.py imports cleanly once the reference root is on sys.path (ops/metrics.py pulls in sklearn; the
 optional GPU `nms.nms_wrapper` is absent, so temporal_nms runs temporal_nms_fallback).  gen_bottom_up_proposals.py is a
@@ -197,5 +198,23 @@ def main():
     print("wrote proposals.npz:", len(out), "arrays")
 
 
+def main_nms():
+    """tests/golden/proposals_nms.npz: the reference's temporal_nms_fallback on proposal_check.nms_cases(7) -- distinct
+    scores with one NaN, +inf and -inf, IoU exactly at the threshold -- as kept indices, for machines without oracle/_ref
+    (python -m oracle.gen_golden_proposals nms)"""
+    sys.path.insert(0, REF)
+    import ops.sequence_funcs as SF
+    from oracle.proposal_check import nms_cases
+    assert SF.nms is None, "the reference's optional GPU nms is importable; temporal_nms would not be the fallback"
+    out = {}
+    for c, (s, e, sc, thresh) in enumerate(nms_cases(7)):
+        kept = SF.temporal_nms([(a, b, i, x) for i, (a, b, x) in enumerate(zip(s.tolist(), e.tolist(), sc))], thresh)
+        out.update({"c%d_start" % c: s, "c%d_end" % c: e, "c%d_score" % c: sc, "c%d_thresh" % c: np.float64(thresh),
+                    "c%d_kept" % c: np.array([k[2] for k in kept], np.int64)})
+    out["n_cases"] = np.int64(len(out) // 5)
+    np.savez_compressed(os.path.join(GOLD, "proposals_nms.npz"), **out)
+    print("wrote proposals_nms.npz:", int(out["n_cases"]), "cases")
+
+
 if __name__ == "__main__":
-    main()
+    main_nms() if sys.argv[1:] == ["nms"] else main()

@@ -14,6 +14,9 @@ Pinned by tests/golden/proposals.npz, produced by oracle/gen_golden_proposals.py
 Two choices the reference leaves open are fixed here, as in csrc/proposals.cu:
   - tied scores: numpy's argsort()[::-1] does not order them; here they keep the order the search emitted them in
     (a stable sort by descending score);
+  - NaN scores: argsort()[::-1] puts them first but, once there are several, in an order numpy does not promise (with
+    numpy 2.3 it already differs from a stable reversed argsort at 17 elements); here every NaN-scored box comes first,
+    in search order, whatever the NaN's sign, then the rest by stable descending score;
   - gen_prop returns the score of every NMS survivor next to the length-filtered boxes (the two lists disagree once
     minimum_len > 0); here every surviving box keeps its own score.
 """
@@ -144,11 +147,15 @@ def build_boxes(labels, frm_scores, tolerances=TOLERANCES):
 
 def temporal_nms(t1, t2, scores, thresh):
     """temporal_nms_fallback: frame-inclusive durations t2 - t1 + 1, intersection min - max + 1 (negative for disjoint
-    boxes, which are never suppressed), IoU divided in double, a box survives while IoU <= thresh.  Ties in score keep
-    their input order.  -> indices of the survivors, in the order they were kept"""
+    boxes, which are never suppressed), IoU divided in double, a box survives while IoU <= thresh.  NaN-scored boxes
+    come first in input order, then the rest by descending score; ties in score keep their input order.  -> indices of
+    the survivors, in the order they were kept"""
     t1, t2 = np.asarray(t1, np.int64), np.asarray(t2, np.int64)
     durations = t2 - t1 + 1
-    order = np.argsort(-np.asarray(scores, np.float32), kind="stable")
+    scores = np.asarray(scores, np.float32)
+    nan = np.isnan(scores)
+    rest = np.nonzero(~nan)[0]
+    order = np.concatenate([np.nonzero(nan)[0], rest[np.argsort(-scores[rest], kind="stable")]]).astype(np.int64)
     keep = []
     while order.size > 0:
         i = order[0]
