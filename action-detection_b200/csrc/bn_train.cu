@@ -102,15 +102,16 @@ __global__ void bn_stat_finish_kernel(const float* __restrict__ partial, int npa
 
 // backward stage 2: dbeta = sum g, dgamma = sum g * xhat; also kept in stat[2C..4C) for the apply pass
 __global__ void bn_grad_finish_kernel(const float* __restrict__ partial, int nparts, int C, float* __restrict__ stat, float* __restrict__ dgamma,
-                                      float* __restrict__ dbeta, int accumulate) {
+                                      float* __restrict__ dbeta, const float* __restrict__ unscale, int accumulate) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
   double sb = 0.0, sg = 0.0;
   for (int i = 0; i < nparts; ++i) { sb += (double)partial[(long long)i * 2 * C + c]; sg += (double)partial[(long long)i * 2 * C + C + c]; }
-  stat[2 * C + c] = (float)sb;
+  stat[2 * C + c] = (float)sb;          // the apply pass works on the scaled gradient, like every kernel between entry and exit
   stat[3 * C + c] = (float)sg;
-  if (dbeta) dbeta[c] = (accumulate ? dbeta[c] : 0.f) + (float)sb;
-  if (dgamma) dgamma[c] = (accumulate ? dgamma[c] : 0.f) + (float)sg;
+  const double u = unscale ? (double)__ldg(unscale) : 1.0;
+  if (dbeta) dbeta[c] = (accumulate ? dbeta[c] : 0.f) + (float)(sb * u);
+  if (dgamma) dgamma[c] = (accumulate ? dgamma[c] : 0.f) + (float)(sg * u);
 }
 
 // y = relu(gamma * xhat + beta)  (+ the value's fp16 hi / lo operand planes in EXACT_TC)
@@ -198,7 +199,7 @@ int launch_bn_train_fwd(View z, View y, View y_planes, int F, const float* gamma
 }
 
 int launch_bn_train_bwd(View z, View dy, View y, View dz, View dz_planes, float plane_scale, int* flag, int F, const float* gamma, float* stat,
-                        float* partial, int max_ctas, float* dgamma, float* dbeta, int accumulate, cudaStream_t s) {
+                        float* partial, int max_ctas, float* dgamma, float* dbeta, const float* unscale, int accumulate, cudaStream_t s) {
   const int C = z.C;
   if (C % 4 || C / 4 > BN_THREADS || dy.pitch % 4 || dy.coff % 4 || dz.pitch % 4 || dz.coff % 4) { set_thread_error("bn_train_bwd: unsupported view"); return 1; }
   const long long rows = (long long)F * z.H * z.W;
@@ -208,7 +209,7 @@ int launch_bn_train_bwd(View z, View dy, View y, View dz, View dz_planes, float 
   bn_colreduce_kernel<2><<<ctas, BN_THREADS, (size_t)lanes * 2 * C * 4, s>>>((const float*)z.base, z.pitch, z.coff, (const float*)dy.base, dy.pitch, dy.coff,
                                                                            (const float*)y.base, y.pitch, y.coff, stat, rows, C, rpc, partial);
   SSNB_LAUNCH_CHECK("bn_colreduce_kernel<grad>");
-  bn_grad_finish_kernel<<<(C + 127) / 128, 128, 0, s>>>(partial, ctas, C, stat, dgamma, dbeta, accumulate);
+  bn_grad_finish_kernel<<<(C + 127) / 128, 128, 0, s>>>(partial, ctas, C, stat, dgamma, dbeta, unscale, accumulate);
   SSNB_LAUNCH_CHECK("bn_grad_finish_kernel");
   const long long n = rows * (C / 4);
   bn_bwd_apply_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const float*)z.base, z.pitch, z.coff, (const float*)dy.base, dy.pitch, dy.coff,

@@ -73,9 +73,12 @@ struct WgradArgs {
 template <typename T> int launch_conv(const ConvArgs& a, cudaStream_t s);
 template <typename T> int launch_wgrad(const WgradArgs& a, cudaStream_t s);
 // dW_ref[co][ci][r][s] = mult[co] * sum_splits partial ; mult = bn_scale * 1/loss_scale
+// unscale (optional device scalar, here and in every launcher below that takes one): multiplied into out_scale on the
+// device -- the 2^-k of the backward's gradient exponent (launch_grad_exponent)
 int launch_wgrad_finalize(const float* partial, int splits, int taps, int Cout, int Cin, const float* mult,
                           float out_scale, float* dw_ref, int accumulate, cudaStream_t s, const float* bias_partial = nullptr,
-                          float* db = nullptr, int* flag = nullptr);    // flag: set to 1 when a summed partial is inf / NaN
+                          float* db = nullptr, int* flag = nullptr,     // flag: set to 1 when a summed partial is inf / NaN
+                          const float* unscale = nullptr);
 template <typename T>
 int launch_bias_grad(const void* dz, int rows, int C, int pitch, int coff, const float* mult, float out_scale,
                      float* partial, int splits, float* db, int accumulate, cudaStream_t s);
@@ -90,7 +93,15 @@ int launch_maxpool_bwd(View dsrc, View ddst, int F, int k, int stride, int pad, 
                        cudaStream_t s);
 template <typename T> int launch_avgpool3_fwd(View src, View dst, int F, int accumulate, cudaStream_t s);
 template <typename T> int launch_gpool_fwd(View src, int F, float* feat, cudaStream_t s);
-template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, View ddst, int F, const void* y, cudaStream_t s);
+// d(in) = dfeat / HW * scale * (scale_dev ? *scale_dev : 1)
+template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, const float* scale_dev, View ddst, int F, const void* y,
+                                           cudaStream_t s);
+// the backward's gradient exponent, one CTA: k such that max|dfeat| * grad_scale * 2^k / HW lies in [2^(GRAD_EXP_TOP-1),
+// 2^GRAD_EXP_TOP) (k = 0 when dfeat is all zero; k = 0 and *flag = 1 when it holds an inf or NaN), |k| <= GRAD_EXP_MAX;
+// writes gscale[0] = 2^k, gscale[1] = 2^-k.  [2^7, 2^8): the largest gradient plane of the SSN step is at most 43x the
+// entry value on the H100 (tests/test_gpu_grad_range.py), so the planes stay 6x below the fp16 range
+constexpr int GRAD_EXP_TOP = 8, GRAD_EXP_MAX = 100;
+int launch_grad_exponent(const float* dfeat, long long n, float grad_scale, int HW, float* gscale, int* flag, cudaStream_t s);
 template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t s);
 
 // weight packing (simt_glue.cu), many layers per launch (block0 = first CTA of the entry; 256 threads per CTA): fold BN,
@@ -134,7 +145,7 @@ struct FinalizeEntry {
   const float* partial; const float* mult; float* dw; const float* bias_partial; float* db;
   int splits, taps, Cout, Cin, block0, pad_;
 };
-struct FinalizeTable { int n, total_blocks; int* flag; FinalizeEntry e[FIN_MAX]; };
+struct FinalizeTable { int n, total_blocks; int* flag; const float* unscale; FinalizeEntry e[FIN_MAX]; };
 int launch_wgrad_finalize_all(const FinalizeTable& t, float out_scale, int accumulate, cudaStream_t s);
 
 // FAST-mode vectorised glue (glue_fp16.cu)
@@ -142,10 +153,11 @@ int launch_maxpool_fwd_h8(View src, View dst, int F, int k, int stride, int pad,
 int launch_maxpool_bwd_h8(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate,
                           cudaStream_t s);
 int launch_avgpool3_h8(View src, View dst, int F, int accumulate, cudaStream_t s);
-int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_scale, float* partial, int max_ctas, float* db,
-                        int accumulate, cudaStream_t s);
+int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas,
+                        float* db, int accumulate, cudaStream_t s);
 int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stride, int pad, const uint8_t* argmax,
-                             const float* mult, float out_scale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
+                             const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
+                             cudaStream_t s);
 // SSNB_EXACT_TC glue (tc_glue.cu): error-compensated fp16 operand planes of fp32 tensors.
 //   hi = fp16(x * scale), lo = fp16(x * scale - float(hi))  =>  hi + lo carries ~22 significand bits of x * scale
 // `flag` (device int, may be null) is set to 1 when |x * scale| exceeds the fp16 range (loss-scale overflow)
@@ -158,20 +170,21 @@ int launch_maxpool_fwd_f4(View src, View dst, View dst_planes, int F, int k, int
 int launch_maxpool_bwd_f4(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate, cudaStream_t s);
 int launch_avgpool3_f4(View src, View dst, View dst_planes, int F, int accumulate, cudaStream_t s);
 int launch_mask_bias_split_f4(View dy, View y, View planes, float scale, int write_f32, int* flag, int F, const float* mult, float out_scale,
-                              float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
+                              const float* unscale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
 int launch_pool_mask_bias_split_f4(View dz, View y, View dpool, View planes, float scale, int write_f32, int* flag, int F, const uint8_t* argmax,
-                                   const float* mult, float out_scale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
+                                   const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
+                                   cudaStream_t s);
 // training-mode BatchNorm + ReLU of the first layer (bn_train.cu); stat: 4*C floats, partial: max_ctas * 2 * C floats
 int launch_bn_train_fwd(View z, View y, View y_planes, int F, const float* gamma, const float* beta, float eps, float momentum, float* running_mean,
                         float* running_var, float* stat, float* partial, int max_ctas, cudaStream_t s);
 int launch_bn_train_bwd(View z, View dy, View y, View dz, View dz_planes, float plane_scale, int* flag, int F, const float* gamma, float* stat,
-                        float* partial, int max_ctas, float* dgamma, float* dbeta, int accumulate, cudaStream_t s);
+                        float* partial, int max_ctas, float* dgamma, float* dbeta, const float* unscale, int accumulate, cudaStream_t s);
 // FAST-mode layout helpers (s2d_glue.cu)
 int launch_nhwc_to_s2d(View src, int F, __half* dst, int Cs, cudaStream_t s);
 int launch_nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, int Cs, cudaStream_t s);
 int launch_pack_conv1_s2d(const __half* wd, int Cout, int Cin, int Cs, __half* ws, cudaStream_t s);
 int launch_wgrad_finalize_s2d(const float* partial, int splits, int Cout, int Cin, int Cs, const float* mult, float out_scale,
-                              float* dw_ref, int accumulate, cudaStream_t s);
+                              const float* unscale, float* dw_ref, int accumulate, cudaStream_t s);
 int launch_upsample2_zero(View src, __half* dst, int H, int W, int F, cudaStream_t s);
 
 }  // namespace ssnb

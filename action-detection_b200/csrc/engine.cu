@@ -131,6 +131,10 @@ struct ssnb_engine {
   size_t up_plane = 0, s2d_plane = 0, s2d_w_plane = 0;
   int* tc_flag = nullptr;           // device int: set when a split pass saw |x * grad_scale| beyond the fp16 range
   size_t tc_flag_off = 0, wmax_off = 0;
+  // tensor-core modes: the backward's gradient exponent, [0] = 2^k, [1] = 2^-k (launch_grad_exponent, at the start of every
+  // backward).  Every gradient buffer holds dz * 2^k (FAST: times grad_scale as well); the global pool's backward multiplies
+  // by 2^k and every kernel that writes a gradient the caller sees (dW, db, dgamma, dbeta) by 2^-k
+  float* gscale = nullptr;           // in the flag's 256-byte slot, 16 bytes after the flag
   bool bn1_train = false;           // bn_mode='partial': the first BatchNorm2d in training mode (bn_train.cu)
   const float *bn1_gamma = nullptr, *bn1_beta = nullptr; float *bn1_rmean = nullptr, *bn1_rvar = nullptr, *bn1_dgamma = nullptr, *bn1_dbeta = nullptr;
   float bn1_momentum = 0.1f, bn1_eps = 1e-5f;
@@ -160,6 +164,8 @@ struct ssnb_engine {
   bool fast() const { return cfg.precision == SSNB_FAST_FP16; }          // fp16 storage, fp16 operands
   bool exact_tc() const { return cfg.precision == SSNB_EXACT_TC; }       // fp32 storage, convolutions on split (hi/lo fp16) operand planes
   bool tensor_cores() const { return cfg.precision != SSNB_EXACT_FP32; } // either of the two: the wgmma schedule
+  const float* grad_scale_dev() const { return tensor_cores() ? gscale : nullptr; }      // 2^k (nullptr: 1)
+  const float* grad_unscale_dev() const { return tensor_cores() ? gscale + 1 : nullptr; }  // 2^-k
   int nplanes() const { return exact_tc() ? 2 : 1; }                     // fp16 operand planes per tensor-core operand
   View view(int val, bool grad) const {
     const Value& v = vals[val];
@@ -309,7 +315,7 @@ static void plan(ssnb_engine* e) {
       if (e->cfg.training) { b.ghoff = off; off += 2 * b.plane; }
     }
   }
-  e->tc_flag_off = off; off = align_up(off + 256, 1024);      // gradient overflow flag (every mode)
+  e->tc_flag_off = off; off = align_up(off + 256, 1024);      // gradient overflow flag (every mode), gradient exponent
   if (e->bn1_train) { e->bn_stat_off = off; off = align_up(off + 4 * 64 * 4, 1024); e->bn_partial_off = off; off = align_up(off + (size_t)1200 * 2 * 64 * 4, 1024); }
   for (Op& o : e->ops)
     if (o.kind == OP_MAXPOOL) {
@@ -557,7 +563,7 @@ static int simt_wgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   if (int rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s))) return rc;
   const float out_scale = e->fast() ? 1.0f / e->cfg.grad_scale : 1.0f;      // FAST stores gradients times the loss scale
   return launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
-                               e->dw[o.conv], e->grad_accumulate, s);
+                               e->dw[o.conv], e->grad_accumulate, s, nullptr, nullptr, nullptr, e->grad_unscale_dev());
 }
 static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   const ConvSpec& c = e->convs[o.conv];
@@ -580,12 +586,13 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
     if (!dfeat) return e->fail(SSNB_EINVAL, "global_pool backward needs dfeat");
     const View din = e->view(o.in_val, true);
     const void* ym = (full && e->fold_pools && o.dgrad_masks) ? e->view(o.in_val, false).base : nullptr;
-    return DISPATCH(e, launch_gpool_bwd<float>(dfeat, gs, din, F, ym, s), launch_gpool_bwd<__half>(dfeat, gs, din, F, ym, s));
+    const float* gsd = e->grad_scale_dev();
+    return DISPATCH(e, launch_gpool_bwd<float>(dfeat, gs, gsd, din, F, ym, s), launch_gpool_bwd<__half>(dfeat, gs, gsd, din, F, ym, s));
   }
   if (o.kind == OP_BN1) {
     return launch_bn_train_bwd(e->view(o.in_val, false), e->view(o.out_val, true), e->view(o.out_val, false), e->view(o.in_val, true),
                                e->exact_tc() ? e->planes(o.in_val, true) : View(), e->cfg.grad_scale, e->tc_flag, F, e->bn1_gamma, (float*)(e->ws + e->bn_stat_off),
-                               (float*)(e->ws + e->bn_partial_off), 1200, e->bn1_dgamma, e->bn1_dbeta, e->grad_accumulate, s);
+                               (float*)(e->ws + e->bn_partial_off), 1200, e->bn1_dgamma, e->bn1_dbeta, e->grad_unscale_dev(), e->grad_accumulate, s);
   }
   if (o.kind == OP_MAXPOOL) {
     if (full && e->tensor_cores() && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass
@@ -624,6 +631,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
 
   // tensor-core modes; the tensor-core products read dz times the loss scale (FAST: the fp16 storage, EXACT_TC: the planes)
   const float gst = e->cfg.grad_scale;
+  const float* us = e->grad_unscale_dev();
   const bool tc_w = want_w && o.umma_wgrad.enabled, tc_x = want_x && o.umma_dgrad.enabled;
   const bool pre = full && e->fold_pools && o.dy_premasked;      // the last writer of dy masked it (EXACT_TC: and wrote its planes)
   const bool bias_w = pre && o.bias_in_wgrad && dbp && tc_w;     // ... and the bias column sums ride on the weight-gradient MMAs
@@ -634,20 +642,20 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it.
   if (e->fast()) {
     if (pool) rc = launch_pool_mask_bias_h8(dy, y, e->view(pool->out_val, true), F, pool->k, pool->stride, pool->pad, (const uint8_t*)(e->ws + pool->argmax_off),
-                                            scale, 1.0f / gst, bpartial, max_ctas, dbp, e->grad_accumulate, s);
-    else if (!bias_w) rc = launch_mask_bias_h8(dy, pre ? View() : y, F, scale, 1.0f / gst, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+                                            scale, 1.0f / gst, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    else if (!bias_w) rc = launch_mask_bias_h8(dy, pre ? View() : y, F, scale, 1.0f / gst, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
   } else {
     const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
     const View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
     if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz and its planes: only the bias sums are left
-      if (dbp) rc = launch_mask_bias_split_f4(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      if (dbp) rc = launch_mask_bias_split_f4(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pre) {    // bias sums of the already masked fp32 dz only: no planes, nothing written back
-      if (!bias_w && dbp) rc = launch_mask_bias_split_f4(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      if (!bias_w && dbp) rc = launch_mask_bias_split_f4(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pool) {
       rc = launch_pool_mask_bias_split_f4(dy, y, e->view(pool->out_val, true), pl, gst, need_f32 ? 1 : 0, e->tc_flag, F, (const uint8_t*)(e->ws + pool->argmax_off),
-                                          scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+                                          scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else {
-      rc = launch_mask_bias_split_f4(dy, y, pl, gst, (need_f32 || !full) ? 1 : 0, e->tc_flag, F, scale, 1.0f, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      rc = launch_mask_bias_split_f4(dy, y, pl, gst, (need_f32 || !full) ? 1 : 0, e->tc_flag, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     }
   }
   if (rc) return rc;
@@ -665,9 +673,10 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
     tag_next(2, conv_flops(e, o), o.id.c_str());
     if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bp))) return rc;
     if (full && o.conv != 0) e->pending_finalize.push_back((int)(&o - e->ops.data()));
-    else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s);
+    else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, us, e->dw[o.conv],
+                                                         e->grad_accumulate, s);
     else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s,
-                                    nullptr, nullptr, e->tc_flag);
+                                    nullptr, nullptr, e->tc_flag, us);
     if (rc) return rc;
   } else if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
   // 4. data gradient; as the last writer of d(in) the wgmma epilogue applies in's ReLU mask
@@ -743,6 +752,9 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
   if (h->tensor_cores() && cudaMemset(h->ws + h->bpartial_off, 0, 256) != cudaSuccess) { cudaGetLastError(); /* no device (CPU-only planning) */ }
   h->tc_flag = (int*)(h->ws + h->tc_flag_off);
   if (cudaMemset(h->tc_flag, 0, 256) != cudaSuccess) cudaGetLastError();
+  h->gscale = (float*)(h->ws + h->tc_flag_off + 16);
+  const float one[2] = {1.0f, 1.0f};          // k = 0 until the first backward (ssnb_run_op / ssnb_value_write before any)
+  if (cudaMemcpy(h->gscale, one, sizeof one, cudaMemcpyHostToDevice) != cudaSuccess) cudaGetLastError();
   // Bind the tensor-core plans (tensor maps need final addresses).  The diagnostic switches are read here, once per engine:
   // SSNB_DISABLE_UMMA=1 keeps every convolution on the SIMT kernels (FAST: fp16; EXACT_TC: fp32, the EXACT_FP32 arithmetic
   // that tools/umma_diag.py diffs the tensor-core launches against), SSNB_DISABLE_UMMA_WGRAD=1 only the weight gradients, and
@@ -1081,7 +1093,7 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
   };
   auto finalize = [&]() -> int {
     const float gs = h->tensor_cores() ? h->cfg.grad_scale : 1.0f;
-    FinalizeTable t; t.n = 0; t.total_blocks = 0; t.flag = h->tc_flag;
+    FinalizeTable t; t.n = 0; t.total_blocks = 0; t.flag = h->tc_flag; t.unscale = h->grad_unscale_dev();
     auto flush = [&]() -> int { int rc = launch_wgrad_finalize_all(t, 1.0f / gs, h->grad_accumulate, s); t.n = 0; t.total_blocks = 0; return rc; };
     for (int oi : h->pending_finalize) {
       const Op& o = h->ops[oi];
@@ -1101,6 +1113,12 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
   const int last = (int)h->ops.size() - 1;
   if (op_hi < 0 || op_hi > last) op_hi = last;
   if (op_lo < 0 || op_lo > op_hi) return h->fail(SSNB_EINVAL, "backbone_bwd_range: bad op range");
+  // the range that starts at the global pool reads dfeat: choose the gradient exponent of this backward from it first
+  if (op_hi == last && h->tensor_cores()) {
+    if (int rc = launch_grad_exponent(dfeat, (long long)h->F * h->vals[h->ops[last].in_val].C, h->cfg.grad_scale,
+                                      h->bufs[h->vals[h->ops[last].in_val].buf].H * h->bufs[h->vals[h->ops[last].in_val].buf].W, h->gscale, h->tc_flag, s))
+      return h->fail(rc, "gradient exponent: " + ssnb::thread_error());
+  }
   if (int rc = run_range(op_hi, op_lo)) return rc;
   return finalize();
 }
@@ -1132,13 +1150,22 @@ int ssnb_value_shape(ssnb_handle h, const char* name, int* c, int* hh, int* ww) 
   return SSNB_OK;
 }
 
+// the gradient exponent's 2^k (which = 0) or 2^-k (which = 1) on the host, after the work queued on `stream` (1 in EXACT_FP32)
+static float host_gscale(ssnb_handle h, int which, cudaStream_t s) {
+  float v = 1.0f;
+  if (!h->tensor_cores() || cudaMemcpyAsync(&v, h->gscale + which, sizeof v, cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+      cudaStreamSynchronize(s) != cudaSuccess) { cudaGetLastError(); return 1.0f; }
+  return v;
+}
+
 int ssnb_value_write(ssnb_handle h, const char* name, int grad, const float* src_nchw, void* stream) {
   if (!h || !name || !src_nchw || !h->ws) return SSNB_EINVAL;
   auto it = h->val_by_name.find(name);
   if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
   if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
   const View v = h->view(it->second, grad != 0);
-  const float sc = (grad && h->fast()) ? h->cfg.grad_scale : 1.0f;
+  // a gradient is stored in the units of the last backward: times 2^k (FAST: and grad_scale)
+  const float sc = grad ? (h->fast() ? h->cfg.grad_scale : 1.0f) * host_gscale(h, 0, (cudaStream_t)stream) : 1.0f;
   int rc = h->fast() ? launch_nchw_to_nhwc<__half>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream)
                    : launch_nchw_to_nhwc<float>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream);
   if (!rc && h->exact_tc() && !grad) rc = tc_split_value(h, it->second, false, 1.0f, (cudaStream_t)stream);   // activation planes follow the fp32 value
@@ -1152,11 +1179,12 @@ int ssnb_value_read(ssnb_handle h, const char* name, int grad, float* dst_nchw, 
   if ((grad & 1) && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");     // grad = 2: an activation's planes
   if (grad & 2) {       // diagnostic: read hi + lo of the value's EXACT_TC operand planes (bit 0: gradient planes, un-scaled)
     if (!h->exact_tc() || !h->bufs[h->vals[it->second].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
-    int rc = launch_planes_to_nchw(h->planes(it->second, (grad & 1) != 0), h->F, (grad & 1) ? 1.0f / h->cfg.grad_scale : 1.0f, dst_nchw, (cudaStream_t)stream);
+    const float sc = (grad & 1) ? host_gscale(h, 1, (cudaStream_t)stream) / h->cfg.grad_scale : 1.0f;
+    int rc = launch_planes_to_nchw(h->planes(it->second, (grad & 1) != 0), h->F, sc, dst_nchw, (cudaStream_t)stream);
     return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
   }
   const View v = h->view(it->second, grad != 0);
-  const float sc = (grad && h->fast()) ? 1.0f / h->cfg.grad_scale : 1.0f;
+  const float sc = grad ? host_gscale(h, 1, (cudaStream_t)stream) / (h->fast() ? h->cfg.grad_scale : 1.0f) : 1.0f;
   int rc = h->fast() ? launch_nhwc_to_nchw<__half>(v, h->F, sc, dst_nchw, (cudaStream_t)stream)
                    : launch_nhwc_to_nchw<float>(v, h->F, sc, dst_nchw, (cudaStream_t)stream);
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;

@@ -231,8 +231,8 @@ __global__ void avgpool3_pair_h8(const __half* __restrict__ src, int H, int W, i
 constexpr int MB_THREADS = 256;
 // the last CTA to finish reduces the per-CTA partials in CTA order (deterministic) into db
 __device__ __forceinline__ void colsum_tail(float* __restrict__ partial, unsigned* __restrict__ counter, int C,
-                                            const float* __restrict__ mult, float out_scale, float* __restrict__ db,
-                                            bool* is_last, int accumulate) {
+                                            const float* __restrict__ mult, float out_scale, const float* __restrict__ unscale,
+                                            float* __restrict__ db, bool* is_last, int accumulate) {
   if (!db) return;
   __threadfence();
   __syncthreads();
@@ -241,6 +241,7 @@ __device__ __forceinline__ void colsum_tail(float* __restrict__ partial, unsigne
   if (!*is_last) return;
   __threadfence();
   const int n = (int)gridDim.x;
+  if (unscale) out_scale *= __ldg(unscale);
   for (int c = threadIdx.x; c < C; c += MB_THREADS) {      // coalesced across threads, 4 independent chains per thread
     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
     int i = 0;
@@ -258,7 +259,7 @@ __global__ void __launch_bounds__(MB_THREADS) mask_bias_h8(__half* __restrict__ 
                                                            long long rows, int C, long long rows_per_cta,
                                                            float* __restrict__ partial, unsigned* __restrict__ counter,
                                                            const float* __restrict__ mult, float out_scale,
-                                                           float* __restrict__ db, int accumulate) {
+                                                           const float* __restrict__ unscale, float* __restrict__ db, int accumulate) {
   extern __shared__ float red[];                 // [lanes][C]
   __shared__ bool is_last;
   const int G = C / 8;
@@ -306,7 +307,7 @@ __global__ void __launch_bounds__(MB_THREADS) mask_bias_h8(__half* __restrict__ 
     for (int l = 0; l < lanes; ++l) s += red[l * C + c];
     partial[(long long)blockIdx.x * C + c] = s;
   }
-  colsum_tail(partial, counter, C, mult, out_scale, db, &is_last, accumulate);
+  colsum_tail(partial, counter, C, mult, out_scale, unscale, db, &is_last, accumulate);
 }
 
 // Same pass for a convolution whose only consumer is a stride-2 max pool (conv1 -> pool1, conv2_3x3 -> pool2):
@@ -319,7 +320,8 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias_h8(__half* __restri
                                                                 int k, int stride, int pad, long long rows, int C,
                                                                 long long rows_per_cta, float* __restrict__ partial,
                                                                 unsigned* __restrict__ counter, const float* __restrict__ mult,
-                                                                float out_scale, float* __restrict__ db, int accumulate) {
+                                                                float out_scale, const float* __restrict__ unscale, float* __restrict__ db,
+                                                                int accumulate) {
   extern __shared__ float red[];
   __shared__ bool is_last;
   const int G = C / 8;
@@ -378,7 +380,7 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias_h8(__half* __restri
     for (int l = 0; l < lanes; ++l) s += red[l * C + c];
     partial[(long long)blockIdx.x * C + c] = s;
   }
-  colsum_tail(partial, counter, C, mult, out_scale, db, &is_last, accumulate);
+  colsum_tail(partial, counter, C, mult, out_scale, unscale, db, &is_last, accumulate);
 }
 
 
@@ -391,7 +393,8 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias2x2_h8(__half* __res
                                                                    const uint8_t* __restrict__ argmax, long long blocks, int C,
                                                                    long long blocks_per_cta, float* __restrict__ partial,
                                                                    unsigned* __restrict__ counter, const float* __restrict__ mult,
-                                                                   float out_scale, float* __restrict__ db, int accumulate) {
+                                                                   float out_scale, const float* __restrict__ unscale, float* __restrict__ db,
+                                                                   int accumulate) {
   extern __shared__ float red[];
   __shared__ bool is_last;
   const int G = C / 8;
@@ -473,7 +476,7 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias2x2_h8(__half* __res
     for (int l = 0; l < lanes; ++l) s += red[l * C + c];
     partial[(long long)blockIdx.x * C + c] = s;
   }
-  colsum_tail(partial, counter, C, mult, out_scale, db, &is_last, accumulate);
+  colsum_tail(partial, counter, C, mult, out_scale, unscale, db, &is_last, accumulate);
 }
 
 }  // namespace
@@ -507,8 +510,8 @@ int launch_avgpool3_h8(View src, View dst, int F, int accumulate, cudaStream_t s
   return 0;
 }
 // partial must hold max_ctas * C floats; db may be nullptr (mask only)
-int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_scale, float* partial, int max_ctas, float* db,
-                        int accumulate, cudaStream_t s) {
+int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas,
+                        float* db, int accumulate, cudaStream_t s) {
   const long long rows = (long long)F * dy.H * dy.W;
   const int C = dy.C;
   if (C % 8 || C / 8 > 64) { set_thread_error("mask_bias: C must be a multiple of 8 and <= 512"); return 1; }
@@ -522,7 +525,7 @@ int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_sca
   unsigned* counter = reinterpret_cast<unsigned*>(partial);          // first 256 bytes of the scratch: completion counter
   float* part = partial + 64;
   mask_bias_h8<<<ctas, MB_THREADS, (size_t)lanes * C * 4, s>>>(HP(dy), dy.pitch, dy.coff, HP(y), y.pitch, y.coff, rows, C, rpc, part,
-                                                              counter, mult, out_scale, db, accumulate);
+                                                              counter, mult, out_scale, unscale, db, accumulate);
   SSNB_LAUNCH_CHECK("mask_bias_h8");
   return 0;
 }
@@ -530,7 +533,8 @@ int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_sca
 
 // conv output y/dz views at full resolution; dpool = gradient of the max pool's output, argmax from its forward
 int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stride, int pad, const uint8_t* argmax,
-                             const float* mult, float out_scale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s) {
+                             const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
+                             cudaStream_t s) {
   const long long rows = (long long)F * dz.H * dz.W;
   const int C = dz.C;
   if (C % 8 || C / 8 > 64 || stride != 2 || k != 3) { set_thread_error("pool_mask_bias: k3/s2 pools, C multiple of 8 and <= 512"); return 1; }
@@ -547,7 +551,7 @@ int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stri
     ctas = (int)((blocks + bpc - 1) / bpc);
     pool_mask_bias2x2_h8<<<ctas, MB_THREADS, (size_t)lanes * C * 4, s>>>(HP(dz), dz.pitch, dz.coff, HP(y), y.pitch, y.coff, dz.H, dz.W, HP(dpool),
                                                                         dpool.H, dpool.W, dpool.pitch, dpool.coff, argmax, blocks, C, bpc, part,
-                                                                        counter, mult, out_scale, db, accumulate);
+                                                                        counter, mult, out_scale, unscale, db, accumulate);
     SSNB_LAUNCH_CHECK("pool_mask_bias2x2_h8");
     return 0;
   }
@@ -559,7 +563,7 @@ int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stri
   ctas = (int)((rows + rpc - 1) / rpc);
   pool_mask_bias_h8<<<ctas, MB_THREADS, (size_t)lanes * C * 4, s>>>(HP(dz), dz.pitch, dz.coff, HP(y), y.pitch, y.coff, dz.H, dz.W, HP(dpool),
                                                                    dpool.H, dpool.W, dpool.pitch, dpool.coff, argmax, k, stride, pad, rows, C,
-                                                                   rpc, part, counter, mult, out_scale, db, accumulate);
+                                                                   rpc, part, counter, mult, out_scale, unscale, db, accumulate);
   SSNB_LAUNCH_CHECK("pool_mask_bias_h8");
   return 0;
 }

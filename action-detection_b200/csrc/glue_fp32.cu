@@ -224,7 +224,8 @@ __global__ void avgpool3_pair_f4(const float* __restrict__ src, int H, int W, in
 constexpr int MB_THREADS = 256;
 // the last CTA to finish reduces the per-CTA partials in CTA order (deterministic) into db
 __device__ __forceinline__ void colsum_tail(float* __restrict__ partial, unsigned* __restrict__ counter, int C, const float* __restrict__ mult,
-                                            float out_scale, float* __restrict__ db, bool* is_last, int accumulate) {
+                                            float out_scale, const float* __restrict__ unscale, float* __restrict__ db, bool* is_last,
+                                            int accumulate) {
   if (!db) return;
   __threadfence();
   __syncthreads();
@@ -233,6 +234,7 @@ __device__ __forceinline__ void colsum_tail(float* __restrict__ partial, unsigne
   if (!*is_last) return;
   __threadfence();
   const int n = (int)gridDim.x;
+  if (unscale) out_scale *= __ldg(unscale);
   for (int c = threadIdx.x; c < C; c += MB_THREADS) {
     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
     int i = 0;
@@ -251,7 +253,8 @@ __global__ void __launch_bounds__(MB_THREADS) mask_bias_split_f4(float* __restri
                                                                  long long lo_off, float scale, int write_f32, int* __restrict__ flag,
                                                                  long long rows, int C, long long rows_per_cta, float* __restrict__ partial,
                                                                  unsigned* __restrict__ counter, const float* __restrict__ mult,
-                                                                 float out_scale, float* __restrict__ db, int accumulate) {
+                                                                 float out_scale, const float* __restrict__ unscale, float* __restrict__ db,
+                                                                 int accumulate) {
   extern __shared__ float red[];                 // [lanes][C]
   __shared__ bool is_last;
   const int G = C / 4;
@@ -306,7 +309,7 @@ __global__ void __launch_bounds__(MB_THREADS) mask_bias_split_f4(float* __restri
     for (int l = 0; l < lanes; ++l) s += red[l * C + c];
     partial[(long long)blockIdx.x * C + c] = s;
   }
-  colsum_tail(partial, counter, C, mult, out_scale, db, &is_last, accumulate);
+  colsum_tail(partial, counter, C, mult, out_scale, unscale, db, &is_last, accumulate);
 }
 
 // Same pass for a convolution whose only consumer is a k3/s2/pad0 max pool (conv1 -> pool1, conv2_3x3 -> pool2): the pool's
@@ -321,7 +324,8 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias_split2x2_f4(float* 
                                                                          int write_f32, int* __restrict__ flag, long long blocks, int C,
                                                                          long long blocks_per_cta, float* __restrict__ partial,
                                                                          unsigned* __restrict__ counter, const float* __restrict__ mult,
-                                                                         float out_scale, float* __restrict__ db, int accumulate) {
+                                                                         float out_scale, const float* __restrict__ unscale, float* __restrict__ db,
+                                                                         int accumulate) {
   extern __shared__ float red[];
   __shared__ bool is_last;
   const int G = C / 4;
@@ -397,7 +401,7 @@ __global__ void __launch_bounds__(MB_THREADS) pool_mask_bias_split2x2_f4(float* 
     for (int l = 0; l < lanes; ++l) s += red[l * C + c];
     partial[(long long)blockIdx.x * C + c] = s;
   }
-  colsum_tail(partial, counter, C, mult, out_scale, db, &is_last, accumulate);
+  colsum_tail(partial, counter, C, mult, out_scale, unscale, db, &is_last, accumulate);
 }
 
 }  // namespace
@@ -440,7 +444,7 @@ int launch_avgpool3_f4(View src, View dst, View dst_planes, int F, int accumulat
 }
 // partial must hold 64 + max_ctas * C floats (first 256 bytes: completion counter); db may be nullptr (mask / planes only)
 int launch_mask_bias_split_f4(View dy, View y, View planes, float scale, int write_f32, int* flag, int F, const float* mult, float out_scale,
-                              float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s) {
+                              const float* unscale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s) {
   const long long rows = (long long)F * dy.H * dy.W;
   const int C = dy.C;
   if (C % 4 || C / 4 > MB_THREADS || dy.pitch % 4 || dy.coff % 4 || (y.base && (y.pitch % 4 || y.coff % 4)) || (planes.base && (!planes.lo_off || planes.pitch % 4 || planes.coff % 4))) {
@@ -456,14 +460,15 @@ int launch_mask_bias_split_f4(View dy, View y, View planes, float scale, int wri
   float* part = partial + 64;
   mask_bias_split_f4<<<ctas, MB_THREADS, (size_t)lanes * C * 4, s>>>(FP(dy), dy.pitch, dy.coff, FP(y), y.pitch, y.coff, (__half*)planes.base,
                                                                     planes.pitch, planes.coff, planes.lo_off, scale, write_f32, flag, rows, C, rpc,
-                                                                    part, counter, mult, out_scale, db, accumulate);
+                                                                    part, counter, mult, out_scale, unscale, db, accumulate);
   SSNB_LAUNCH_CHECK("mask_bias_split_f4");
   return 0;
 }
 
 // conv output y / dz views at full resolution; dpool = fp32 gradient of the k3/s2/pad0 max pool's output, argmax from its forward
 int launch_pool_mask_bias_split_f4(View dz, View y, View dpool, View planes, float scale, int write_f32, int* flag, int F, const uint8_t* argmax,
-                                   const float* mult, float out_scale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s) {
+                                   const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
+                                   cudaStream_t s) {
   const int C = dz.C;
   if (C % 4 || C / 4 > MB_THREADS || dz.pitch % 4 || dz.coff % 4 || y.pitch % 4 || y.coff % 4 || dpool.pitch % 4 || dpool.coff % 4 ||
       (planes.base && (!planes.lo_off || planes.pitch % 4 || planes.coff % 4))) { set_thread_error("pool_mask_bias_split_f4: unsupported view"); return 1; }
@@ -480,7 +485,7 @@ int launch_pool_mask_bias_split_f4(View dz, View y, View dpool, View planes, flo
   pool_mask_bias_split2x2_f4<<<ctas, MB_THREADS, (size_t)lanes * C * 4, s>>>(FP(dz), dz.pitch, dz.coff, FP(y), y.pitch, y.coff, dz.H, dz.W, FP(dpool),
                                                                             dpool.H, dpool.W, dpool.pitch, dpool.coff, argmax, (__half*)planes.base,
                                                                             planes.pitch, planes.coff, planes.lo_off, scale, write_f32, flag, blocks, C,
-                                                                            bpc, part, counter, mult, out_scale, db, accumulate);
+                                                                            bpc, part, counter, mult, out_scale, unscale, db, accumulate);
   SSNB_LAUNCH_CHECK("pool_mask_bias_split2x2_f4");
   return 0;
 }

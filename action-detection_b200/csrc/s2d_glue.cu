@@ -52,7 +52,8 @@ __global__ void pack_conv1_s2d_kernel(const __half* __restrict__ wd, int Cout, i
 
 // dw_ref[co][c][r][s] = mult[co]*out_scale * sum_splits partial[sp][dr][co][ds*Cs + (a*2+b)*Cin + c]
 __global__ void wgrad_finalize_s2d_kernel(const float* __restrict__ partial, int splits, int Cout, int Cin, int Cs,
-                                          const float* __restrict__ mult, float out_scale, float* __restrict__ dw, int accumulate) {
+                                          const float* __restrict__ mult, float out_scale, const float* __restrict__ unscale,
+                                          float* __restrict__ dw, int accumulate) {
   const int Ck = 4 * Cs;
   const long long total = (long long)Cout * Cin * 49;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -63,6 +64,7 @@ __global__ void wgrad_finalize_s2d_kernel(const float* __restrict__ partial, int
   const int ch = ds * Cs + (a * 2 + b) * Cin + c;
   float acc = 0.f;
   for (int sp = 0; sp < splits; ++sp) acc += partial[(((long long)sp * 4 + dr) * Cout + co) * Ck + ch];
+  if (unscale) out_scale *= __ldg(unscale);
   dw[i] = (accumulate ? dw[i] : 0.f) + acc * mult[co] * out_scale;
 }
 
@@ -146,9 +148,9 @@ int launch_pack_conv1_s2d(const __half* wd, int Cout, int Cin, int Cs, __half* w
   return 0;
 }
 int launch_wgrad_finalize_s2d(const float* partial, int splits, int Cout, int Cin, int Cs, const float* mult, float out_scale,
-                              float* dw_ref, int accumulate, cudaStream_t s) {
+                              const float* unscale, float* dw_ref, int accumulate, cudaStream_t s) {
   const long long n = (long long)Cout * Cin * 49;
-  wgrad_finalize_s2d_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(partial, splits, Cout, Cin, Cs, mult, out_scale, dw_ref, accumulate);
+  wgrad_finalize_s2d_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(partial, splits, Cout, Cin, Cs, mult, out_scale, unscale, dw_ref, accumulate);
   SSNB_LAUNCH_CHECK("wgrad_finalize_s2d_kernel");
   return 0;
 }

@@ -266,9 +266,11 @@ __global__ void __launch_bounds__(NT) wgrad_kernel(WgradArgs a) {
 // layout [co][ci][tap]
 __global__ void wgrad_finalize_kernel(const float* __restrict__ partial, int splits, int taps, int Cout, int Cin,
                                       const float* __restrict__ mult, float out_scale, float* __restrict__ dw, int accumulate,
-                                      const float* __restrict__ bias_partial, float* __restrict__ db, int* __restrict__ flag) {
+                                      const float* __restrict__ bias_partial, float* __restrict__ db, int* __restrict__ flag,
+                                      const float* __restrict__ unscale) {
   const long long total = (long long)taps * Cout * Cin;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (unscale) out_scale *= __ldg(unscale);
   if (bias_partial && db && i < Cout) {          // bias gradient from the weight-gradient kernel's ones-operand accumulator
     float sb = 0.f;
     for (int sp = 0; sp < splits; ++sp) sb += bias_partial[(long long)sp * Cout + i];
@@ -291,6 +293,7 @@ __global__ void wgrad_finalize_all_kernel(const __grid_constant__ FinalizeTable 
   const FinalizeEntry& q = t.e[ei];
   const long long total = (long long)q.taps * q.Cout * q.Cin;
   const long long i = (long long)(blockIdx.x - q.block0) * blockDim.x + threadIdx.x;
+  if (t.unscale) out_scale *= __ldg(t.unscale);
   if (q.bias_partial && q.db && i < q.Cout) {
     float sb = 0.f;
     for (int sp = 0; sp < q.splits; ++sp) sb += q.bias_partial[(long long)sp * q.Cout + i];
@@ -368,10 +371,11 @@ template int launch_wgrad<float>(const WgradArgs&, cudaStream_t);
 template int launch_wgrad<__half>(const WgradArgs&, cudaStream_t);
 
 int launch_wgrad_finalize(const float* partial, int splits, int taps, int Cout, int Cin, const float* mult,
-                          float out_scale, float* dw_ref, int accumulate, cudaStream_t s, const float* bias_partial, float* db, int* flag) {
+                          float out_scale, float* dw_ref, int accumulate, cudaStream_t s, const float* bias_partial, float* db, int* flag,
+                          const float* unscale) {
   const long long total = (long long)taps * Cout * Cin;
   wgrad_finalize_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(partial, splits, taps, Cout, Cin, mult,
-                                                                       out_scale, dw_ref, accumulate, bias_partial, db, flag);
+                                                                       out_scale, dw_ref, accumulate, bias_partial, db, flag, unscale);
   SSNB_LAUNCH_CHECK("wgrad_finalize_kernel");
   return 0;
 }

@@ -2,6 +2,8 @@
 // pooling (Caffe ceil-mode semantics, model_zoo/bninception/layer_factory.py:41-53), 7x7 global
 // pooling (bn_inception.yaml:552), ReLU gradient masks, and BN-folding weight packing
 // (frozen BatchNorm2d, ssn_models.py:156-174).
+#include <cfloat>
+
 #include "common.cuh"
 
 namespace ssnb {
@@ -135,16 +137,52 @@ __global__ void gpool_fwd_kernel(const T* __restrict__ src, int HW, int C, int p
 }
 
 template <typename T>
-__global__ void gpool_bwd_kernel(const float* __restrict__ dfeat, float scale, int HW, int C, int pitch, int coff, int F,
-                                 T* __restrict__ ddst, const T* __restrict__ y) {
+__global__ void gpool_bwd_kernel(const float* __restrict__ dfeat, float scale, const float* __restrict__ scale_dev, int HW, int C, int pitch,
+                                 int coff, int F, T* __restrict__ ddst, const T* __restrict__ y) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)F * HW * C) return;
+  if (scale_dev) scale *= __ldg(scale_dev);
   const int c = (int)(i % C);
   const long long p = i / C;
   const long long f = p / HW;
   float g = dfeat[f * C + c] / (float)HW * scale;
   if (y && !(to_f<T>(y[p * pitch + coff + c]) > 0.f)) g = 0.f;     // fused ReLU gradient mask (same view geometry)
   ddst[p * pitch + coff + c] = from_f<T>(g);
+}
+
+// one CTA: max |dfeat| (any inf / NaN noted separately: fmaxf drops NaN) -> the gradient exponent k (see launch_grad_exponent).
+// The entry gradient max|dfeat| * grad_scale / HW = m * 2^e with m in [0.5, 1) is formed from the three operands' exponents, so no
+// intermediate overflows: frexp(max|dfeat|) * frexp(grad_scale) / HW in fp32, whose frexp exponent is added to theirs.
+constexpr int GE_THREADS = 1024;
+__global__ void __launch_bounds__(GE_THREADS) grad_exponent_kernel(const float* __restrict__ dfeat, long long n, float grad_scale, int HW,
+                                                                   float* __restrict__ gscale, int* __restrict__ flag) {
+  __shared__ float wmax[GE_THREADS / 32];
+  __shared__ int wbad[GE_THREADS / 32];
+  float m = 0.f;
+  int bad = 0;
+  for (long long i = threadIdx.x; i < n; i += GE_THREADS) {
+    const float a = fabsf(__ldg(dfeat + i));
+    if (!(a <= FLT_MAX)) bad = 1;
+    m = fmaxf(m, a);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) { m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o)); bad |= __shfl_xor_sync(0xffffffffu, bad, o); }
+  if (threadIdx.x % 32 == 0) { wmax[threadIdx.x / 32] = m; wbad[threadIdx.x / 32] = bad; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < GE_THREADS / 32; ++w) { m = fmaxf(m, wmax[w]); bad |= wbad[w]; }
+  int k = 0;
+  if (bad) {
+    if (flag) *flag = 1;
+  } else if (m > 0.f) {
+    int ea, eg, e;
+    const float fa = frexpf(m, &ea), fg = frexpf(grad_scale, &eg);
+    frexpf(fa * fg / (float)HW, &e);
+    k = GRAD_EXP_TOP - (ea + eg + e);
+    k = k < -GRAD_EXP_MAX ? -GRAD_EXP_MAX : (k > GRAD_EXP_MAX ? GRAD_EXP_MAX : k);
+  }
+  gscale[0] = ldexpf(1.0f, k);
+  gscale[1] = ldexpf(1.0f, -k);
 }
 
 template <typename T>
@@ -299,10 +337,17 @@ template <typename T> int launch_gpool_fwd(View src, int F, float* feat, cudaStr
   SSNB_LAUNCH_CHECK("gpool_fwd_kernel");
   return 0;
 }
-template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, View ddst, int F, const void* y, cudaStream_t s) {
+template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, const float* scale_dev, View ddst, int F, const void* y,
+                                           cudaStream_t s) {
   const long long n = (long long)F * ddst.H * ddst.W * ddst.C;
-  gpool_bwd_kernel<T><<<blocks_for(n), TPB, 0, s>>>(dfeat, scale, ddst.H * ddst.W, ddst.C, ddst.pitch, ddst.coff, F, V(T, ddst), reinterpret_cast<const T*>(y));
+  gpool_bwd_kernel<T><<<blocks_for(n), TPB, 0, s>>>(dfeat, scale, scale_dev, ddst.H * ddst.W, ddst.C, ddst.pitch, ddst.coff, F, V(T, ddst),
+                                                    reinterpret_cast<const T*>(y));
   SSNB_LAUNCH_CHECK("gpool_bwd_kernel");
+  return 0;
+}
+int launch_grad_exponent(const float* dfeat, long long n, float grad_scale, int HW, float* gscale, int* flag, cudaStream_t s) {
+  grad_exponent_kernel<<<1, GE_THREADS, 0, s>>>(dfeat, n, grad_scale, HW, gscale, flag);
+  SSNB_LAUNCH_CHECK("grad_exponent_kernel");
   return 0;
 }
 template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t s) {
@@ -318,7 +363,7 @@ template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t 
   template int launch_maxpool_bwd<T>(View, View, int, int, int, int, const uint8_t*, int, cudaStream_t);     \
   template int launch_avgpool3_fwd<T>(View, View, int, int, cudaStream_t);                                   \
   template int launch_gpool_fwd<T>(View, int, float*, cudaStream_t);                                         \
-  template int launch_gpool_bwd<T>(const float*, float, View, int, const void*, cudaStream_t);                            \
+  template int launch_gpool_bwd<T>(const float*, float, const float*, View, int, const void*, cudaStream_t);              \
   template int launch_relu_mask<T>(View, View, int, cudaStream_t);
 INST(float)
 INST(__half)

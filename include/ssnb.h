@@ -35,8 +35,9 @@ typedef struct {
   int32_t frames;      /* F = proposals * segments processed per call */
   int32_t precision;   /* SSNB_EXACT_FP32 | SSNB_FAST_FP16 | SSNB_EXACT_TC */
   int32_t training;    /* 1: keep activations + allocate gradient buffers */
-  float grad_scale;    /* power-of-two loss scale: FAST scales dfeat (fp16 gradient storage); EXACT_TC scales the
-                          fp16 operand planes of the output gradients (fp32 gradients themselves are unscaled) */
+  float grad_scale;    /* loss scale (FAST: fp16 gradient storage; EXACT_TC: the fp16 operand planes of the output gradients).
+                          Not needed for range: every backward of the tensor-core modes also multiplies the gradient by 2^k,
+                          k chosen on the device from max |dfeat|, and divides dW / db / dgamma / dbeta by it again */
   int32_t bn1_train;   /* 1: the FIRST BatchNorm2d (conv1's) runs in training mode -- batch statistics, running-stat update, gradients for
                           its weight / bias: bn_mode='partial' (ssn_models.py:95-105,156-174).  EXACT_FP32 / EXACT_TC only. */
   int32_t reserved[2];
@@ -94,8 +95,8 @@ int ssnb_value_shape(ssnb_handle h, const char* name, int* c, int* hh, int* ww);
 int ssnb_value_write(ssnb_handle h, const char* name, int grad, const float* src_nchw, void* stream);
 int ssnb_value_read(ssnb_handle h, const char* name, int grad, float* dst_nchw, void* stream);
 int ssnb_run_op(ssnb_handle h, int op, int backward, void* stream);
-/* Loss-scale guard: 1 when a gradient left the fp16 range under grad_scale since the last clear (EXACT_TC: an operand plane
- * saw |dz * grad_scale| > 65504 or NaN; FAST: a weight-gradient sum came out inf / NaN), 0 otherwise, -1 on error.
+/* Loss-scale guard: 1 when a gradient left the fp16 range since the last clear (dfeat held an inf / NaN; EXACT_TC: an operand
+ * plane saw |dz * grad_scale * 2^k| > 65504 or NaN; FAST: a weight-gradient sum came out inf / NaN), 0 otherwise, -1 on error.
  * Synchronises the device: poll it every N steps and skip / rescale like a dynamic loss scaler would. */
 int ssnb_grad_overflow(ssnb_handle h, int clear);
 

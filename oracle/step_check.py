@@ -12,12 +12,16 @@ stpp).  Device-agnostic torch, float64.
 `Checker` compares a kernel's outputs with these: the error of a quantity is max |got - ref| over the tensor, divided by
 max |ref| of the tensor or, for per-row quantities (one row per proposal or frame), of the row; a record holds the worst
 value and where it sits.  A NaN in got is an error unless ref has a NaN in the same place.
+
+`ssn_step_dfeat` is the gradient such a step hands the backbone's backward, at the magnitude training produces.
 """
 import math
 
 import torch
+import torch.nn.functional as F
 
 from . import ssn_oracle as O
+from . import synth
 
 HEAD_KEYS = ("activity_fc.weight", "activity_fc.bias", "completeness_fc.weight", "completeness_fc.bias",
              "regressor_fc.weight", "regressor_fc.bias")
@@ -310,3 +314,33 @@ def check_sgd(chk, op, seg_end, param, mom, ref_param, ref_mom, bar=SGD_BAR):
                 worst[q] = Record(op, q, r.err, bar, "segment %d, %s" % (i, r.where))
         lo = hi
     chk.records.extend(worst.values())
+
+
+# bench.py's training step: 4 videos x 8 proposals x 9 segments (F = 288), K = 20
+STEP_VIDEOS, STEP_PROPS, STEP_SEG, STEP_K = 4, 8, 9, 20
+
+
+def ssn_step_dfeat(feat, seed=0):
+    """dL/dfeat of one SSN training step in float64, rounded to fp32: bench-shaped proposals (4 videos x 8 proposals x 9
+    segments, K = 20), heads as ssn_models initialises them (N(0, 0.001), zero bias), a seeded dropout 0.8 mask on feat
+    (ssn_models.fused_step), STPP (1, (1, 2), 1) and SSN's loss (oracle total_loss).  feat: [F, 1024]; F below 288 frames
+    is tiled up to 288 and the first F rows of the gradient are returned."""
+    F_ = feat.shape[0]
+    n = STEP_VIDEOS * STEP_PROPS * STEP_SEG
+    f64 = feat.detach().double().cpu().repeat((n + F_ - 1) // F_, 1)[:n].clone().requires_grad_(True)
+    _x, scaling, target, reg_target, prop_type = synth.synth_batch(STEP_VIDEOS, STEP_K, 3, seed=seed, size=8)
+    heads = {k: v.double() for k, v in synth.synth_heads(STEP_K, 5, std=0.001).items()}
+    g = torch.Generator().manual_seed(500 + seed)
+    keep = 0.2
+    mask = (torch.rand(n, 1024, generator=g, dtype=torch.float64) < keep).double() / keep
+    with torch.enable_grad():
+        course, stpp = O.stpp_forward(f64 * mask, scaling.double(), [2, 7, STEP_SEG])
+        raw_act = F.linear(course, heads["activity_fc.weight"], heads["activity_fc.bias"])
+        raw_comp = F.linear(stpp, heads["completeness_fc.weight"], heads["completeness_fc.bias"])
+        raw_reg = F.linear(stpp, heads["regressor_fc.weight"], heads["regressor_fc.bias"]).view(-1, STEP_K, 2)
+        t = prop_type.view(-1)
+        act_i, comp_i, reg_i = ((t == 0) | (t == 2)).nonzero().view(-1), ((t == 0) | (t == 1)).nonzero().view(-1), (t == 0).nonzero().view(-1)
+        tg, rt = target.view(-1), reg_target.view(-1, 2).double()
+        loss, _parts = O.total_loss((raw_act[act_i], tg[act_i], raw_comp[comp_i], tg[comp_i], raw_reg[reg_i], tg[reg_i], rt[reg_i]))
+        (d,) = torch.autograd.grad(loss, f64)
+    return d[:F_].float().to(feat.device)

@@ -5,8 +5,9 @@ training engine of tests/test_gpu_schedule.py, and the loss-scale guard:
     and at ragged ones; and their forward is bitwise the forward of a training engine;
   - bn_mode='partial' engines (bn1_train): conv1 raw, the training-mode BatchNorm of csrc/bn_train.cu (batch statistics,
     running statistics, dgamma / dbeta, dz and its operand planes), pool1 not folded into conv1;
-  - ssnb_grad_overflow: set when a gradient operand plane leaves the fp16 range under the loss scale (or a NaN arrives),
-    clear below it, and cleared on request.  The values involved are ordinary IEEE infinities / NaNs in the buffers.
+  - ssnb_grad_overflow: set when a NaN / inf arrives in dfeat or a gradient operand plane leaves the fp16 range, and cleared
+    on request; dfeat far outside fp16's range (x 2^+-40) is brought back by the backward's gradient exponent and gives
+    exactly scaled gradients.  The values involved are ordinary IEEE infinities / NaNs in the buffers.
 Run on an H100: pytest -m gpu -s tests/test_gpu_schedule_modes.py."""
 import os
 import time
@@ -210,65 +211,92 @@ def test_bn1_per_launch(precision, frames, in_channels, unfused):
 
 
 # ---- the loss-scale guard ------------------------------------------------------------------------------------------------
-def _grad_plane_max(eng, G):
-    """max |dz| over the gradient operand planes the backward wrote (un-scaled): every convolution output and the max-pool
-    branches of the stride-2 blocks (the block output's last writer splits them with the rest of the block)"""
-    names = [o["out"] for o in G.ops if o["kind"] == "conv"]
-    names += [v for v in G.branch if any(o["out"] == v and o["kind"] == "maxpool" for o in G.ops)]
-    return max(float(eng.read(v, grad=True, planes=True).abs().max()) for v in names)
+def _scaled_backward_flags(eng, dfeat, dw, db, extra=()):
+    """dfeat x 2^-40 and x 2^40: the backward brings the entry gradient back into range (its gradient exponent), so the flag
+    stays clear and every dW / db (and `extra`, e.g. dgamma / dbeta) is exactly 2^+-40 times the ordinary one"""
+    eng.backward(dfeat, dw, db)
+    ref = [t.clone() for t in list(dw) + list(db) + list(extra)]
+    flags, exact = {}, {}
+    for j in (-40, 40):
+        eng.backward(dfeat * 2.0 ** j, dw, db)
+        flags["dfeat x 2^%d" % j] = eng.grad_overflow()
+        exact["dfeat x 2^%d" % j] = all(torch.equal(a, b * 2.0 ** j) for a, b in zip(list(dw) + list(db) + list(extra), ref))
+    return flags, exact
+
+
+GUARD_CONV = "inception_5b_3x3_bn"
+
+
+def _conv_guard_flags(eng, precision, k):
+    """one convolution's backward on its own (run_op, which bypasses the entry) on a dy scaled so that the largest gradient
+    the tensor cores read (EXACT_TC: the planes of dz * grad_scale * 2^k, FAST: the fp16 storage) is 0.5x / 2x the fp16 range;
+    k: the gradient exponent of the last backward, whose units ssnb_value_write stores the gradient in"""
+    m = float(eng.read(GUARD_CONV, grad=True, planes=precision == "exact_tc").abs().max())
+    dy = eng.read(GUARD_CONV, grad=True)
+    op = [o for _kd, _i, o in eng.ops()].index(GUARD_CONV)
+    flags = {}
+    for f in (0.5, 2.0):
+        eng.write(GUARD_CONV, dy * (f * HALF_MAX / (m * GRAD_SCALE * 2.0 ** k)), grad=True)
+        eng.run_op(op, backward=True)
+        flags["%s backward %.1fx" % (GUARD_CONV, f)] = eng.grad_overflow()
+    return flags
 
 
 @pytest.mark.parametrize("bn1_train", [False, True], ids=["frozen", "bn1"])
-def test_overflow_guard_exact_tc(bn1_train):
-    """gradients are linear in dfeat: scaled so that the largest gradient plane times grad_scale is half the fp16 range the
-    flag stays clear; at twice the range it is raised, and reading it with clear=True clears it.  A NaN in dfeat raises it.
-    bn1: conv1's planes come from bn_bwd_apply_kernel, also checked on its own by re-running the BatchNorm backward on a dy
-    scaled across the same two limits"""
+def test_grad_guard_exact_tc(bn1_train):
+    """dfeat scaled by 2^+-40 raises no flag and scales every gradient exactly (the gradient exponent normalises the entry);
+    a NaN in dfeat raises the flag, and reading it with clear=True clears it.  The split passes still guard the planes: a
+    convolution's backward on its own (run_op, which bypasses the entry) on a dy scaled so that its largest plane is 0.5x / 2x
+    the fp16 range leaves the flag clear / raises it; bn1: the same for bn_bwd_apply_kernel and conv1's dz"""
+    from oracle import split_operands as SO
     dev = _cuda()
-    G = S.Graph(3, bn1_train=bn1_train)
     eng = _engine("exact_tc", 8, 3, True, dev, bn1_train=bn1_train)
     try:
+        extra = ()
         if bn1_train:
             bn, dgamma, dbeta = _bn1_module(3, dev)
             eng.set_bn1(bn, dgamma, dbeta)
+            extra = (dgamma, dbeta)
         x, dfeat = _inputs(8, 3, dev)
         dw, db = _grads(3, dev)
         feat = eng.forward(x)
         eng.backward(dfeat, dw, db)
-        assert not eng.grad_overflow()
-        m = _grad_plane_max(eng, G)
-        assert m > 0.0
-        flags = {}
+        flags = {"ordinary": eng.grad_overflow()}
+        # the planes hold dz * grad_scale * 2^k with k chosen from this dfeat; a write stores dy times the same 2^k
+        k = SO.grad_exponent(float(dfeat.abs().max()), GRAD_SCALE)
+        flags.update(_conv_guard_flags(eng, "exact_tc", k))
         if bn1_train:
             dy = eng.read(S.BN1_OUT, grad=True)
             mb = float(eng.read(S.BN1_RAW, grad=True, planes=True).abs().max())
-            bn_op = [k for k, _i, _o in eng.ops()].index("bn")
+            bn_op = [kd for kd, _i, _o in eng.ops()].index("bn")
             for f in (0.5, 2.0):
-                eng.write(S.BN1_OUT, dy * (f * HALF_MAX / (mb * GRAD_SCALE)), grad=True)
+                eng.write(S.BN1_OUT, dy * (f * HALF_MAX / (mb * GRAD_SCALE * 2.0 ** k)), grad=True)
                 eng.run_op(bn_op, backward=True)
                 flags["bn_bwd_apply %.1fx" % f] = eng.grad_overflow()
-        for f in (0.5, 2.0):
-            eng.backward(dfeat * (f * HALF_MAX / (m * GRAD_SCALE)), dw, db)
-            flags["backward %.1fx" % f] = eng.grad_overflow(clear=False)
-            flags["backward %.1fx, after clear" % f] = eng.grad_overflow(clear=True) and eng.grad_overflow()
+        f2, exact = _scaled_backward_flags(eng, dfeat, dw, db, extra)
+        flags.update(f2)
         nan = dfeat.clone()
         nan[0, int(feat[0].argmax())] = float("nan")      # a channel that is active in frame 0
         eng.backward(nan, dw, db)
-        flags["NaN in dfeat"] = eng.grad_overflow()
-        print("\nEXACT_TC F=8%s: max |dz| over the gradient planes %.3e; flags %s" % (" bn1" if bn1_train else "", m, flags))
-        want = {"backward 0.5x": False, "backward 0.5x, after clear": False, "backward 2.0x": True,
-                "backward 2.0x, after clear": False, "NaN in dfeat": True}
+        flags["NaN in dfeat"] = eng.grad_overflow(clear=False)
+        flags["NaN in dfeat, after clear"] = eng.grad_overflow(clear=True) and eng.grad_overflow()
+        print("\nEXACT_TC F=8%s: flags %s; exactly scaled gradients %s" % (" bn1" if bn1_train else "", flags, exact))
+        want = {"ordinary": False, "dfeat x 2^-40": False, "dfeat x 2^40": False, "NaN in dfeat": True, "NaN in dfeat, after clear": False,
+                GUARD_CONV + " backward 0.5x": False, GUARD_CONV + " backward 2.0x": True}
         if bn1_train:
             want.update({"bn_bwd_apply 0.5x": False, "bn_bwd_apply 2.0x": True})
         assert flags == want
+        assert all(exact.values()), exact
     finally:
         del eng
         torch.cuda.empty_cache()
 
 
-def test_overflow_guard_fast():
-    """FAST stores gradients as fp16 times grad_scale: a dfeat whose global-pool gradient dfeat * grad_scale / 49 is beyond
-    the fp16 range makes the weight-gradient sums non-finite and raises the flag; an ordinary dfeat does not"""
+def test_grad_guard_fast():
+    """FAST stores gradients in fp16 times grad_scale * 2^k: dfeat scaled by 2^+-40 raises no flag and scales every gradient
+    exactly; a NaN in dfeat raises the flag; an ordinary dfeat after it does not.  A convolution's backward on its own (run_op)
+    on a dy whose fp16 storage would be 0.5x / 2x the fp16 range: clear / raised (the weight-gradient sums of an inf)"""
+    from oracle import split_operands as SO
     dev = _cuda()
     eng = _engine("fast", 8, 3, True, dev)
     try:
@@ -276,13 +304,20 @@ def test_overflow_guard_fast():
         dw, db = _grads(3, dev)
         eng.forward(x)
         eng.backward(dfeat, dw, db)
-        normal = eng.grad_overflow()
-        eng.backward(torch.sign(dfeat) * (4 * HALF_MAX * 49 / GRAD_SCALE), dw, db)
-        big = eng.grad_overflow()
+        flags = {"ordinary": eng.grad_overflow()}
+        flags.update(_conv_guard_flags(eng, "fast", SO.grad_exponent(float(dfeat.abs().max()), GRAD_SCALE)))
+        f2, exact = _scaled_backward_flags(eng, dfeat, dw, db)
+        flags.update(f2)
+        nan = dfeat.clone()
+        nan[0, 0] = float("nan")
+        eng.backward(nan, dw, db)
+        flags["NaN in dfeat"] = eng.grad_overflow()
         eng.backward(dfeat, dw, db)
-        again = eng.grad_overflow()
-        print("\nFAST F=8: flag with an ordinary dfeat %s, beyond the fp16 range %s, ordinary again %s" % (normal, big, again))
-        assert (normal, big, again) == (False, True, False)
+        flags["ordinary again"] = eng.grad_overflow()
+        print("\nFAST F=8: flags %s; exactly scaled gradients %s" % (flags, exact))
+        assert flags == {"ordinary": False, "dfeat x 2^-40": False, "dfeat x 2^40": False, "NaN in dfeat": True, "ordinary again": False,
+                         GUARD_CONV + " backward 0.5x": False, GUARD_CONV + " backward 2.0x": True}
+        assert all(exact.values()), exact
     finally:
         del eng
         torch.cuda.empty_cache()
