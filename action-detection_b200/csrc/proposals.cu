@@ -23,6 +23,7 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
+#include "rank_key.cuh"
 
 namespace ssnb {
 namespace {
@@ -225,19 +226,8 @@ __global__ void __launch_bounds__(kSearchThreads) search_kernel(const VideoDesc*
   }
 }
 
-// descending score as an ascending radix key; -0 and +0 share a key, as they compare equal.  Every NaN, whatever its
-// sign or payload, gets key 0, ahead of +inf (key 0x007fffff): NaN-scored boxes rank first, as in the reference's
-// argsort()[::-1], and among themselves keep the search order.  key_score(0) is the NaN 0x7fffffff.
-__device__ __forceinline__ uint32_t score_key(float s) {
-  if (s != s) return 0u;
-  uint32_t u = __float_as_uint(s == 0.f ? 0.f : s);
-  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-  return ~u;
-}
-__device__ __forceinline__ float key_score(uint32_t key) {
-  const uint32_t u = ~key;
-  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
-}
+// score_key / key_score (rank_key.cuh): NaN-scored boxes rank first, as in the reference's argsort()[::-1], and among
+// themselves keep the search order
 
 __global__ void __launch_bounds__(kScoreThreads) score_kernel(const float* __restrict__ col, const VideoDesc* __restrict__ desc,
                                                               const int* __restrict__ seg_end, unsigned long long* __restrict__ vals,

@@ -38,6 +38,13 @@ class TagProposalsCfg(C.Structure):
                 ("thresholds", C.POINTER(C.c_double)), ("tolerances", C.POINTER(C.c_double))]
 
 
+class DetectBatchCfg(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("top_k", C.c_int32), ("n_sel", C.c_int32), ("softmax_before_filter", C.c_int32),
+                ("regress", C.c_int32), ("reserved", C.c_int32), ("nms_thresh", C.c_double)]
+
+
+DET_ALL, DET_TOPK, DET_CLS = 0, 1, 2
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 _pp = C.POINTER(C.c_void_p)
@@ -90,6 +97,12 @@ SIGNATURES = {
     "ssnb_timing_launches": (C.c_char_p, []),
     "ssnb_detect_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_detect_postprocess": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp]),
+    "ssnb_detect_batch_workspace_bytes": (_sz, [C.POINTER(DetectBatchCfg), _i, C.POINTER(C.c_int64), _i]),
+    "ssnb_detect_batch": (_i, [C.POINTER(DetectBatchCfg), _vp, _vp, _vp, _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp, _vp, _vp, _vp, _vp,
+                               _vp, _sz, _vp]),
+    "ssnb_detection_ap_workspace_bytes": (_sz, [_i, _i, C.c_int64, C.c_int64, _i]),
+    "ssnb_detection_ap": (_i, [_vp, _vp, _vp, _i, _i, C.c_int64, _vp, _vp, _vp, C.c_int64, C.POINTER(C.c_double), _i, _vp, _vp, _vp,
+                               _vp, _sz, _vp]),
     "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
     "ssnb_tag_proposals": (_i, [C.POINTER(TagProposalsCfg), _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp] + [_vp] * 10
                            + [_sz, _vp]),

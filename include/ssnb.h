@@ -228,6 +228,60 @@ int ssnb_detect_postprocess(const float* rel_props, const float* act_scores, con
                             int n_props, int num_class, double nms_thresh, int regress, float* detections, int* counts,
                             float* combined_ws, void* stream);
 
+/* ---- detection post-processing of many videos (eval_detection_results.py:91-145 gen_detection_results, all three branches;
+ *      :153-183 class-wise temporal_nms (ops/utils.py:56-82) and perform_regression (:162-174)) -------------------------------
+ * Video v owns proposal rows offsets[v] .. offsets[v+1]-1 of rel_props [sum N, 2], act [sum N, K+1], comp [sum N, K] and
+ * reg [sum N, K, 2] (NULL: zeros, the script's reg_scores = None; the boxes are still regressed when `regress`).  Per mode:
+ *   SSNB_DET_ALL   (:103-113)  softmax(act)[:, 1:] * exp(comp), every (proposal, class) pair;
+ *   SSNB_DET_TOPK  (:114-129)  softmax(act[:, 1:]) * exp(comp), the top_k pairs of the video (all when N*K < top_k);
+ *   SSNB_DET_CLS   (:130-145)  softmax(act)[:, 1:] * exp(comp) (softmax_before_filter) or act[:, 1:] * exp(comp), every
+ *                              proposal of the n_sel classes cls_sel[v, :] (device int32 [V, n_sel], distinct, in [0, K);
+ *                              others are ignored).
+ * then per non-empty (video, class): temporal NMS at nms_thresh and (regress) the location regression.  Ranking: NaN first,
+ * then descending score, equal scores by larger proposal index first (a stable ascending argsort reversed).
+ * Slots: video v has S_v = N_v*K (all), min(top_k, N_v*K) (top_k) or N_v*n_sel (cls) of them, starting at slot0[v] =
+ * S_0 + ... + S_{v-1}.  dets [sum S, 5] (t0, t1, score, loc, dur): video v's survivors from slot0[v] on, class by class in
+ * ascending class order, each class in kept (descending score) order; counts [V, K] int32.  Slots past the survivors are
+ * not written.  Optional traces (NULL: not written): combined [sum N, K] fp32 (the ranked scores) and sel [sum S] int32, the
+ * selected pairs row * K + class (global row) of video v at slots slot0[v] .. slot0[v] + S_v - 1 in ranking order.
+ * offsets (int64 [V+1], offsets[0] = 0, non-decreasing) are HOST memory; offsets_dev holds the same values on the device.
+ * Kernels only: no host synchronisation, no allocation, no copy from host memory (graph-capturable).  sum N * K and the
+ * slot total must fit in int32. */
+enum { SSNB_DET_ALL = 0, SSNB_DET_TOPK = 1, SSNB_DET_CLS = 2 };
+typedef struct {
+  int32_t mode;                   /* SSNB_DET_ALL | SSNB_DET_TOPK | SSNB_DET_CLS */
+  int32_t top_k;                  /* SSNB_DET_TOPK: >= 1 */
+  int32_t n_sel;                  /* SSNB_DET_CLS: classes per video, 1..K */
+  int32_t softmax_before_filter;  /* SSNB_DET_CLS: 1 = softmax(act)[:, 1:], 0 = act[:, 1:] */
+  int32_t regress;                /* 0: --no_regression */
+  int32_t reserved;
+  double nms_thresh;              /* not NaN */
+} ssnb_detect_batch_cfg;
+/* 0 for arguments ssnb_detect_batch would reject */
+size_t ssnb_detect_batch_workspace_bytes(const ssnb_detect_batch_cfg* cfg, int num_class, const int64_t* offsets, int n_videos);
+int ssnb_detect_batch(const ssnb_detect_batch_cfg* cfg, const float* rel_props, const float* act, const float* comp, const float* reg,
+                      int num_class, const int64_t* offsets, const int64_t* offsets_dev, int n_videos, const int32_t* cls_sel,
+                      float* dets, int32_t* counts, float* combined, int32_t* sel, void* workspace, size_t workspace_bytes,
+                      void* stream);
+
+/* ---- detection AP (anet_toolkit/Evaluation/eval_detection.py:160-235 compute_average_precision_detection, utils.py:14-51
+ *      interpolated_prec_rec / segment_iou), every class and tIoU threshold of eval_detection_results.py:216-237 in one call --
+ * Detections: ssnb_detect_batch's output for V videos (dets, counts [V, K], det_slot0 = device int64 [V+1], slot0[V] =
+ * n_slots).  Ground truth: n_gt rows of gt_cls int32 and gt_seg double [n_gt, 2] (t0, t1), packed per video: video v's rows
+ * are gt_offsets[v] .. gt_offsets[v+1]-1 (device int64 [V+1]); rows gt_offsets[V] .. n_gt-1 are ground truth of videos
+ * without detections, counted in npos only.  Classes outside [0, K) are ignored.  Per class: predictions sorted by
+ * descending score over all videos (NaN first; equal scores: the later (video, kept position) first); each is matched to
+ * the unlocked ground truth of its own video and class with the highest double tIoU not below the threshold (a NaN tIoU,
+ * from two zero-length segments, ranks first and matches; equal tIoU: larger ground-truth index first); precision and
+ * recall from the cumulative counts, ap = the interpolated sum.  No ground truth and >= 1 prediction: NaN; no prediction: 0.
+ * thresholds: host double [n_thr], 1..64.  ap: device double [K, n_thr].  Optional traces: rank [n_slots] int32 (a
+ * survivor's position in its class-wide order), tp [n_thr, n_slots] uint8 (1 = true positive, 0 = false positive), both
+ * written at survivor slots only.  Kernels only (graph-capturable), no host synchronisation, allocation or host copy. */
+size_t ssnb_detection_ap_workspace_bytes(int n_videos, int num_class, int64_t n_slots, int64_t n_gt, int n_thresholds);
+int ssnb_detection_ap(const float* dets, const int32_t* counts, const int64_t* det_slot0, int n_videos, int num_class, int64_t n_slots,
+                      const int64_t* gt_offsets, const int32_t* gt_cls, const double* gt_seg, int64_t n_gt, const double* thresholds,
+                      int n_thresholds, double* ap, int32_t* rank, uint8_t* tp, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- TAG bottom-up proposals of many videos (gen_bottom_up_proposals.py:116-142, ops/sequence_funcs.py:11-34,71-136) ----
  * Per video v with T_v = offsets[v+1] - offsets[v] ticks of the merged crop-mean score f_score [T_v, num_cols] (rows
  * offsets[v] .. offsets[v+1]-1 of one packed fp32 [offsets[V], num_cols] array): softmax (ops/metrics.py:8-11), column
