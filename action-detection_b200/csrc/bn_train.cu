@@ -13,20 +13,6 @@ namespace {
 
 constexpr int BN_THREADS = 256;
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __half2 h = __floats2half2_rn(a, b);
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-__device__ __forceinline__ void store_planes4(__half* hi, long long lo_off, const float4& v) {
-  uint2 h, l;
-  split2(v.x, v.y, h.x, l.x);
-  split2(v.z, v.w, h.y, l.y);
-  *reinterpret_cast<uint2*>(hi) = h;
-  *reinterpret_cast<uint2*>(reinterpret_cast<char*>(hi) + lo_off) = l;
-}
 
 // MODE 0: sum z                      -> partial[cta][C]
 // MODE 1: sum (z - mu)^2             -> partial[cta][C]            (stat[0..C) = mu)
@@ -158,7 +144,7 @@ __global__ void bn_bwd_apply_kernel(const float* __restrict__ z, int zpitch, int
   if (hi) {
     const float4 sv = make_float4(o[0] * scale, o[1] * scale, o[2] * scale, o[3] * scale);
     const float am = fmaxf(fmaxf(fabsf(sv.x), fabsf(sv.y)), fmaxf(fabsf(sv.z), fabsf(sv.w)));
-    if (flag && !(am <= 65504.f)) *flag = 1;
+    if (flag && !(am <= HALF_MAX)) *flag = 1;
     store_planes4(hi + r * zgpitch + zgcoff + g * 4, lo_off, sv);
   }
 }

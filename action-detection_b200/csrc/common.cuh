@@ -55,6 +55,24 @@ template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
 
+// SSNB_EXACT_TC operand format: an fp32 value x is carried as hi = fp16(x), lo = fp16(x - float(hi)) (tc_glue.cu)
+constexpr float HALF_MAX = 65504.f;
+__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
+  hi = *reinterpret_cast<const uint32_t*>(&h);
+  lo = *reinterpret_cast<const uint32_t*>(&l);
+}
+// 4 fp32 values -> 8 bytes of hi + 8 bytes of lo at the same element offset of the two planes
+__device__ __forceinline__ void store_planes4(__half* hi, long long lo_off, const float4& v) {
+  uint2 h, l;
+  split2(v.x, v.y, h.x, l.x);
+  split2(v.z, v.w, h.y, l.y);
+  *reinterpret_cast<uint2*>(hi) = h;
+  *reinterpret_cast<uint2*>(reinterpret_cast<char*>(hi) + lo_off) = l;
+}
+
 // ---- SIMT convolution family (simt_conv.cu) ---------------------------------------------------
 struct ConvArgs {
   const void* src; int SH, SW, Csrc, src_pitch, src_coff;   // x (fwd) or dz (dgrad)
@@ -148,16 +166,27 @@ struct FinalizeEntry {
 struct FinalizeTable { int n, total_blocks; int* flag; const float* unscale; FinalizeEntry e[FIN_MAX]; };
 int launch_wgrad_finalize_all(const FinalizeTable& t, float out_scale, int accumulate, cudaStream_t s);
 
-// FAST-mode vectorised glue (glue_fp16.cu)
-int launch_maxpool_fwd_h8(View src, View dst, int F, int k, int stride, int pad, uint8_t* argmax, cudaStream_t s);
-int launch_maxpool_bwd_h8(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate,
-                          cudaStream_t s);
-int launch_avgpool3_h8(View src, View dst, int F, int accumulate, cudaStream_t s);
-int launch_mask_bias_h8(View dy, View y, int F, const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas,
-                        float* db, int accumulate, cudaStream_t s);
-int launch_pool_mask_bias_h8(View dz, View y, View dpool, int F, int k, int stride, int pad, const uint8_t* argmax,
-                             const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
-                             cudaStream_t s);
+// Vectorised glue of the tensor-core modes (glue_vec.cu), T = float (SSNB_EXACT_TC) or __half (SSNB_FAST_FP16): every thread
+// moves VEC_WIDTH<T> channels (16 bytes), so C, pitch and coff must be multiples of it.  `*planes` views (base == nullptr: none)
+// receive the fp16 hi/lo operand planes; only the float launchers accept one.
+template <typename T> constexpr int VEC_WIDTH = 16 / (int)sizeof(T);
+template <typename T>
+int launch_maxpool_fwd_vec(View src, View dst, View dst_planes, int F, int k, int stride, int pad, uint8_t* argmax, cudaStream_t s);   // k = 3
+template <typename T>
+int launch_maxpool_bwd_vec(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate, cudaStream_t s);
+template <typename T> int launch_avgpool3_vec(View src, View dst, View dst_planes, int F, int accumulate, cudaStream_t s);
+// backward pass of a convolution's output gradient: dz = dy * (y > 0) (y.base == nullptr: no mask), bias-gradient column sums
+// into db (nullptr: none), planes of dz * scale; dz is written back to dy where the mask changed it and write_back is set.
+// partial must hold 64 + max_ctas * C floats (first 256 bytes: completion counter)
+template <typename T>
+int launch_mask_bias_vec(View dy, View y, View planes, float scale, int write_back, int* flag, int F, const float* mult, float out_scale,
+                         const float* unscale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
+// the same pass for a convolution whose only consumer is a k3/s2/pad0 max pool, with that pool's backward gather folded in:
+// dpool = gradient of the pool's output, argmax from its forward; dz is written whenever write_back is set
+template <typename T>
+int launch_pool_mask_bias_vec(View dz, View y, View dpool, View planes, float scale, int write_back, int* flag, int F, int k, int stride, int pad,
+                              const uint8_t* argmax, const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas,
+                              float* db, int accumulate, cudaStream_t s);
 // SSNB_EXACT_TC glue (tc_glue.cu): error-compensated fp16 operand planes of fp32 tensors.
 //   hi = fp16(x * scale), lo = fp16(x * scale - float(hi))  =>  hi + lo carries ~22 significand bits of x * scale
 // `flag` (device int, may be null) is set to 1 when |x * scale| exceeds the fp16 range (loss-scale overflow)
@@ -165,15 +194,6 @@ int launch_split_view(View src_f32, int F, float scale, View planes, int* flag, 
 int launch_planes_to_nchw(View planes, int F, float scale, float* dst, cudaStream_t s);
 int launch_nhwc_to_s2d_split(View src_f32, int F, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);
 int launch_nchw_to_s2d_split(const float* src, int F, int Cin, int H, int W, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);
-// SSNB_EXACT_TC vectorised fp32 glue (glue_fp32.cu); `*_planes` views (base == nullptr: none) receive the fp16 hi/lo operand planes
-int launch_maxpool_fwd_f4(View src, View dst, View dst_planes, int F, int k, int stride, int pad, uint8_t* argmax, cudaStream_t s);
-int launch_maxpool_bwd_f4(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate, cudaStream_t s);
-int launch_avgpool3_f4(View src, View dst, View dst_planes, int F, int accumulate, cudaStream_t s);
-int launch_mask_bias_split_f4(View dy, View y, View planes, float scale, int write_f32, int* flag, int F, const float* mult, float out_scale,
-                              const float* unscale, float* partial, int max_ctas, float* db, int accumulate, cudaStream_t s);
-int launch_pool_mask_bias_split_f4(View dz, View y, View dpool, View planes, float scale, int write_f32, int* flag, int F, const uint8_t* argmax,
-                                   const float* mult, float out_scale, const float* unscale, float* partial, int max_ctas, float* db, int accumulate,
-                                   cudaStream_t s);
 // training-mode BatchNorm + ReLU of the first layer (bn_train.cu); stat: 4*C floats, partial: max_ctas * 2 * C floats
 int launch_bn_train_fwd(View z, View y, View y_planes, int F, const float* gamma, const float* beta, float eps, float momentum, float* running_mean,
                         float* running_var, float* stat, float* partial, int max_ctas, cudaStream_t s);

@@ -410,7 +410,7 @@ static void plan(ssnb_engine* e) {
   }
   if (e->tensor_cores()) {
     // convolutions whose only consumer is a k3/s2/pad0 max pool: that pool's backward gather is folded into their mask pass,
-    // whose vector width (8 halves in FAST, 4 floats in EXACT_TC) must divide the channel count
+    // whose vector width must divide the channel count
     for (int i = 0; i < (int)e->ops.size(); ++i) {
       Op& po = e->ops[i];
       if (po.kind != OP_MAXPOOL || po.k != 3 || po.stride != 2 || po.pad != 0) continue;
@@ -419,7 +419,7 @@ static void plan(ssnb_engine* e) {
         if (e->ops[j].out_val == po.in_val && e->ops[j].kind == OP_CONV) producer = j;
         if (e->ops[j].in_val == po.in_val) ++consumers;
       }
-      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % (e->fast() ? 8 : 4) == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
+      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % (e->fast() ? VEC_WIDTH<__half> : VEC_WIDTH<float>) == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
     }
     // fp16 operand regions: one plane in FAST (the next region starts 1024-aligned behind it), hi + lo planes `plane`
     // bytes apart in EXACT_TC
@@ -505,11 +505,15 @@ static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* 
                                e->bn1_beta, e->bn1_eps, e->bn1_momentum, e->bn1_rmean, e->bn1_rvar, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, s);
   }
-  if (e->exact_tc() && (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) && e->bufs[e->vals[o.out_val].buf].plane) {
-    // vectorised fp32 pooling that also emits the output's operand planes (glue_fp32.cu)
-    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false), pl = e->planes(o.out_val, false);
-    if (o.kind == OP_MAXPOOL) return launch_maxpool_fwd_f4(in, out, pl, e->F, o.k, o.stride, o.pad, (uint8_t*)(e->ws + o.argmax_off), s);
-    return launch_avgpool3_f4(in, out, pl, e->F, 0, s);
+  if (e->tensor_cores() && (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL)) {
+    // vectorised pooling; in EXACT_TC it also emits the output's operand planes (glue_vec.cu)
+    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
+    const View pl = e->exact_tc() && e->bufs[e->vals[o.out_val].buf].plane ? e->planes(o.out_val, false) : View();
+    uint8_t* am = (uint8_t*)(e->ws + o.argmax_off);
+    if (o.kind == OP_MAXPOOL)
+      return DISPATCH(e, launch_maxpool_fwd_vec<float>(in, out, pl, e->F, o.k, o.stride, o.pad, am, s),
+                      launch_maxpool_fwd_vec<__half>(in, out, pl, e->F, o.k, o.stride, o.pad, am, s));
+    return DISPATCH(e, launch_avgpool3_vec<float>(in, out, pl, e->F, 0, s), launch_avgpool3_vec<__half>(in, out, pl, e->F, 0, s));
   }
   if (int rc = run_fwd_impl(e, o, input_nchw, feat, s)) return rc;
   return o.out_val >= 0 ? tc_split_value(e, o.out_val, false, 1.0f, s) : 0;
@@ -530,16 +534,9 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
   }
   if (o.kind == OP_MAXPOOL) {
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    uint8_t* am = (uint8_t*)(e->ws + o.argmax_off);
-    if (e->fast() && in.C % 8 == 0) return launch_maxpool_fwd_h8(in, out, F, o.k, o.stride, o.pad, am, s);
-    return DISPATCH(e, launch_maxpool_fwd<float>(in, out, F, o.k, o.stride, o.pad, am, s),
-                    launch_maxpool_fwd<__half>(in, out, F, o.k, o.stride, o.pad, am, s));
+    return launch_maxpool_fwd<float>(in, out, F, o.k, o.stride, o.pad, (uint8_t*)(e->ws + o.argmax_off), s);
   }
-  if (o.kind == OP_AVGPOOL) {
-    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    if (e->fast() && in.C % 8 == 0) return launch_avgpool3_h8(in, out, F, 0, s);
-    return DISPATCH(e, launch_avgpool3_fwd<float>(in, out, F, 0, s), launch_avgpool3_fwd<__half>(in, out, F, 0, s));
-  }
+  if (o.kind == OP_AVGPOOL) return launch_avgpool3_fwd<float>(e->view(o.in_val, false), e->view(o.out_val, false), F, 0, s);
   if (o.kind == OP_GPOOL) {
     if (!feat) return e->fail(SSNB_EINVAL, "global_pool needs the feat output pointer");
     const View in = e->view(o.in_val, false);
@@ -598,17 +595,15 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
     if (full && e->tensor_cores() && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
     const uint8_t* am = (const uint8_t*)(e->ws + o.argmax_off);
-    if (e->exact_tc() && din.C % 4 == 0) return launch_maxpool_bwd_f4(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
-    if (e->fast() && din.C % 8 == 0) return launch_maxpool_bwd_h8(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
-    return DISPATCH(e, launch_maxpool_bwd<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s),
-                    launch_maxpool_bwd<__half>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s));
+    if (!e->tensor_cores()) return launch_maxpool_bwd<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
+    return DISPATCH(e, launch_maxpool_bwd_vec<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s),
+                    launch_maxpool_bwd_vec<__half>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s));
   }
   if (o.kind == OP_AVGPOOL) {
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
-    if (e->exact_tc() && din.C % 4 == 0) return launch_avgpool3_f4(dout, din, View(), F, o.grad_accumulate, s);
-    if (e->fast() && din.C % 8 == 0) return launch_avgpool3_h8(dout, din, F, o.grad_accumulate, s);
-    return DISPATCH(e, launch_avgpool3_fwd<float>(dout, din, F, o.grad_accumulate, s),
-                    launch_avgpool3_fwd<__half>(dout, din, F, o.grad_accumulate, s));
+    if (!e->tensor_cores()) return launch_avgpool3_fwd<float>(dout, din, F, o.grad_accumulate, s);
+    return DISPATCH(e, launch_avgpool3_vec<float>(dout, din, View(), F, o.grad_accumulate, s),
+                    launch_avgpool3_vec<__half>(dout, din, View(), F, o.grad_accumulate, s));
   }
   // convolution: dz = dy * (y > 0); db, dW from dz; dx = dgrad(dz)
   const ConvSpec& c = e->convs[o.conv];
@@ -640,22 +635,26 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   const int max_ctas = (1024 * 512 - 64) / y.C;
   // 1. one pass over dy: ReLU mask + bias-gradient column sums.  FAST masks the fp16 dy in place.  EXACT_TC reads the fp32 dy,
   //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it.
+  const View dpool = pool ? e->view(pool->out_val, true) : View();
+  const uint8_t* pam = pool ? (const uint8_t*)(e->ws + pool->argmax_off) : nullptr;
   if (e->fast()) {
-    if (pool) rc = launch_pool_mask_bias_h8(dy, y, e->view(pool->out_val, true), F, pool->k, pool->stride, pool->pad, (const uint8_t*)(e->ws + pool->argmax_off),
-                                            scale, 1.0f / gst, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
-    else if (!bias_w) rc = launch_mask_bias_h8(dy, pre ? View() : y, F, scale, 1.0f / gst, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    if (pool) rc = launch_pool_mask_bias_vec<__half>(dy, y, dpool, View(), 1.0f, 1, nullptr, F, pool->k, pool->stride, pool->pad, pam,
+                                                    scale, 1.0f / gst, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+    else if (!bias_w) rc = launch_mask_bias_vec<__half>(dy, pre ? View() : y, View(), 1.0f, 1, nullptr, F, scale, 1.0f / gst, us, bpartial, max_ctas, dbp,
+                                                       e->grad_accumulate, s);
   } else {
     const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
     const View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
     if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz and its planes: only the bias sums are left
-      if (dbp) rc = launch_mask_bias_split_f4(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      if (dbp) rc = launch_mask_bias_vec<float>(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pre) {    // bias sums of the already masked fp32 dz only: no planes, nothing written back
-      if (!bias_w && dbp) rc = launch_mask_bias_split_f4(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      if (!bias_w && dbp) rc = launch_mask_bias_vec<float>(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pool) {
-      rc = launch_pool_mask_bias_split_f4(dy, y, e->view(pool->out_val, true), pl, gst, need_f32 ? 1 : 0, e->tc_flag, F, (const uint8_t*)(e->ws + pool->argmax_off),
-                                          scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      rc = launch_pool_mask_bias_vec<float>(dy, y, dpool, pl, gst, need_f32 ? 1 : 0, e->tc_flag, F, pool->k, pool->stride, pool->pad, pam,
+                                            scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else {
-      rc = launch_mask_bias_split_f4(dy, y, pl, gst, (need_f32 || !full) ? 1 : 0, e->tc_flag, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
+      rc = launch_mask_bias_vec<float>(dy, y, pl, gst, (need_f32 || !full) ? 1 : 0, e->tc_flag, F, scale, 1.0f, us, bpartial, max_ctas, dbp,
+                                       e->grad_accumulate, s);
     }
   }
   if (rc) return rc;

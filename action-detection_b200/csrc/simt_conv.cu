@@ -399,6 +399,5 @@ int launch_bias_grad(const void* dz, int rows, int C, int pitch, int coff, const
   return 0;
 }
 template int launch_bias_grad<float>(const void*, int, int, int, int, const float*, float, float*, int, float*, int, cudaStream_t);
-template int launch_bias_grad<__half>(const void*, int, int, int, int, const float*, float, float*, int, float*, int, cudaStream_t);
 
 }  // namespace ssnb

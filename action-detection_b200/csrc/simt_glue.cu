@@ -359,13 +359,14 @@ template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t 
 #define INST(T)                                                                                              \
   template int launch_nchw_to_nhwc<T>(const float*, int, int, int, int, View, float, cudaStream_t);                 \
   template int launch_nhwc_to_nchw<T>(View, int, float, float*, cudaStream_t);                               \
-  template int launch_maxpool_fwd<T>(View, View, int, int, int, int, uint8_t*, cudaStream_t);                \
-  template int launch_maxpool_bwd<T>(View, View, int, int, int, int, const uint8_t*, int, cudaStream_t);     \
-  template int launch_avgpool3_fwd<T>(View, View, int, int, cudaStream_t);                                   \
   template int launch_gpool_fwd<T>(View, int, float*, cudaStream_t);                                         \
-  template int launch_gpool_bwd<T>(const float*, float, const float*, View, int, const void*, cudaStream_t);              \
-  template int launch_relu_mask<T>(View, View, int, cudaStream_t);
+  template int launch_gpool_bwd<T>(const float*, float, const float*, View, int, const void*, cudaStream_t);
 INST(float)
 INST(__half)
+// EXACT_FP32 only: the tensor-core modes pool and mask with the vector kernels of glue_vec.cu
+template int launch_maxpool_fwd<float>(View, View, int, int, int, int, uint8_t*, cudaStream_t);
+template int launch_maxpool_bwd<float>(View, View, int, int, int, int, const uint8_t*, int, cudaStream_t);
+template int launch_avgpool3_fwd<float>(View, View, int, int, cudaStream_t);
+template int launch_relu_mask<float>(View, View, int, cudaStream_t);
 
 }  // namespace ssnb

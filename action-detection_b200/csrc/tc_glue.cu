@@ -12,15 +12,6 @@ namespace ssnb {
 namespace {
 
 constexpr int TPB = 256;
-constexpr float HALF_MAX = 65504.f;
-
-__device__ __forceinline__ void split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-  const __half2 h = __floats2half2_rn(a, b);
-  const float2 hf = __half22float2(h);
-  const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-  hi = *reinterpret_cast<const uint32_t*>(&h);
-  lo = *reinterpret_cast<const uint32_t*>(&l);
-}
 
 // one thread = 8 channels of one pixel: 2 x 16-byte fp32 loads -> 16 bytes of hi + 16 bytes of lo
 __global__ void split_view_kernel(const float* __restrict__ src, int spitch, int scoff, long long pixels, int C, float scale,
