@@ -97,19 +97,10 @@ int launch_wgrad_finalize(const float* partial, int splits, int taps, int Cout, 
                           float out_scale, float* dw_ref, int accumulate, cudaStream_t s, const float* bias_partial = nullptr,
                           float* db = nullptr, int* flag = nullptr,     // flag: set to 1 when a summed partial is inf / NaN
                           const float* unscale = nullptr);
-template <typename T>
-int launch_bias_grad(const void* dz, int rows, int C, int pitch, int coff, const float* mult, float out_scale,
-                     float* partial, int splits, float* db, int accumulate, cudaStream_t s);
 
 // ---- glue (simt_glue.cu) ------------------------------------------------------------------------
 template <typename T> int launch_nchw_to_nhwc(const float* src, int F, int C, int H, int W, View dst, float scale, cudaStream_t s);
 template <typename T> int launch_nhwc_to_nchw(View src, int F, float scale, float* dst, cudaStream_t s);
-template <typename T>
-int launch_maxpool_fwd(View src, View dst, int F, int k, int stride, int pad, uint8_t* argmax, cudaStream_t s);
-template <typename T>
-int launch_maxpool_bwd(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate,
-                       cudaStream_t s);
-template <typename T> int launch_avgpool3_fwd(View src, View dst, int F, int accumulate, cudaStream_t s);
 template <typename T> int launch_gpool_fwd(View src, int F, float* feat, cudaStream_t s);
 // d(in) = dfeat / HW * scale * (scale_dev ? *scale_dev : 1)
 template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, const float* scale_dev, View ddst, int F, const void* y,
@@ -120,7 +111,6 @@ template <typename T> int launch_gpool_bwd(const float* dfeat, float scale, cons
 // entry value on the H100 (tests/test_gpu_grad_range.py), so the planes stay 6x below the fp16 range
 constexpr int GRAD_EXP_TOP = 8, GRAD_EXP_MAX = 100;
 int launch_grad_exponent(const float* dfeat, long long n, float grad_scale, int HW, float* gscale, int* flag, cudaStream_t s);
-template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t s);
 
 // weight packing (simt_glue.cu), many layers per launch (block0 = first CTA of the entry; 256 threads per CTA): fold BN,
 // produce the kernel layouts wf [tap][ci][co], wd [tap][co][ci] in storage type T; bias' [co] fp32; scale [co] fp32;
@@ -166,7 +156,7 @@ struct FinalizeEntry {
 struct FinalizeTable { int n, total_blocks; int* flag; const float* unscale; FinalizeEntry e[FIN_MAX]; };
 int launch_wgrad_finalize_all(const FinalizeTable& t, float out_scale, int accumulate, cudaStream_t s);
 
-// Vectorised glue of the tensor-core modes (glue_vec.cu), T = float (SSNB_EXACT_TC) or __half (SSNB_FAST_FP16): every thread
+// Vectorised pooling and mask glue (glue_vec.cu), T = float (SSNB_EXACT_FP32, SSNB_EXACT_TC) or __half (SSNB_FAST_FP16): every thread
 // moves VEC_WIDTH<T> channels (16 bytes), so C, pitch and coff must be multiples of it.  `*planes` views (base == nullptr: none)
 // receive the fp16 hi/lo operand planes; only the float launchers accept one.
 template <typename T> constexpr int VEC_WIDTH = 16 / (int)sizeof(T);

@@ -505,7 +505,7 @@ static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* 
                                e->bn1_beta, e->bn1_eps, e->bn1_momentum, e->bn1_rmean, e->bn1_rvar, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, s);
   }
-  if (e->tensor_cores() && (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL)) {
+  if (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) {
     // vectorised pooling; in EXACT_TC it also emits the output's operand planes (glue_vec.cu)
     const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
     const View pl = e->exact_tc() && e->bufs[e->vals[o.out_val].buf].plane ? e->planes(o.out_val, false) : View();
@@ -532,11 +532,6 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
     tag_next(0, conv_flops(e, o), o.id.c_str());
     return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
   }
-  if (o.kind == OP_MAXPOOL) {
-    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    return launch_maxpool_fwd<float>(in, out, F, o.k, o.stride, o.pad, (uint8_t*)(e->ws + o.argmax_off), s);
-  }
-  if (o.kind == OP_AVGPOOL) return launch_avgpool3_fwd<float>(e->view(o.in_val, false), e->view(o.out_val, false), F, 0, s);
   if (o.kind == OP_GPOOL) {
     if (!feat) return e->fail(SSNB_EINVAL, "global_pool needs the feat output pointer");
     const View in = e->view(o.in_val, false);
@@ -592,16 +587,14 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
                                (float*)(e->ws + e->bn_partial_off), 1200, e->bn1_dgamma, e->bn1_dbeta, e->grad_unscale_dev(), e->grad_accumulate, s);
   }
   if (o.kind == OP_MAXPOOL) {
-    if (full && e->tensor_cores() && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass
+    if (full && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass (tensor-core modes)
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
     const uint8_t* am = (const uint8_t*)(e->ws + o.argmax_off);
-    if (!e->tensor_cores()) return launch_maxpool_bwd<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s);
     return DISPATCH(e, launch_maxpool_bwd_vec<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s),
                     launch_maxpool_bwd_vec<__half>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s));
   }
   if (o.kind == OP_AVGPOOL) {
     const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
-    if (!e->tensor_cores()) return launch_avgpool3_fwd<float>(dout, din, F, o.grad_accumulate, s);
     return DISPATCH(e, launch_avgpool3_vec<float>(dout, din, View(), F, o.grad_accumulate, s),
                     launch_avgpool3_vec<__half>(dout, din, View(), F, o.grad_accumulate, s));
   }
@@ -613,18 +606,8 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   float* dbp = (e->db.size() && e->db[o.conv]) ? e->db[o.conv] : nullptr;
   const bool want_w = e->dw.size() && e->dw[o.conv];
   const bool want_x = e->vals[o.in_val].name != "data" && !skip_dgrad;
-  if (!e->tensor_cores()) {
-    if (!o.raw && (rc = launch_relu_mask<float>(dy, y, F, s))) return rc;
-    if (dbp) {
-      const long long M = (long long)F * y.H * y.W;
-      int bs = (int)((M + 4095) / 4096); if (bs > 64) bs = 64; if (bs < 1) bs = 1;
-      if ((rc = launch_bias_grad<float>(dy.base, (int)M, y.C, dy.pitch, dy.coff, scale, 1.0f, bpartial, bs, dbp, e->grad_accumulate, s))) return rc;
-    }
-    if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
-    return want_x ? simt_dgrad(e, o, s) : 0;
-  }
-
-  // tensor-core modes; the tensor-core products read dz times the loss scale (FAST: the fp16 storage, EXACT_TC: the planes)
+  // the tensor-core products read dz times the loss scale (FAST: the fp16 storage, EXACT_TC: the planes); EXACT has no
+  // tensor-core plans
   const float gst = e->cfg.grad_scale;
   const float* us = e->grad_unscale_dev();
   const bool tc_w = want_w && o.umma_wgrad.enabled, tc_x = want_x && o.umma_dgrad.enabled;
@@ -634,7 +617,8 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   const Op* pool = (full && e->fold_pools && o.pool_consumer >= 0) ? &e->ops[o.pool_consumer] : nullptr;
   const int max_ctas = (1024 * 512 - 64) / y.C;
   // 1. one pass over dy: ReLU mask + bias-gradient column sums.  FAST masks the fp16 dy in place.  EXACT_TC reads the fp32 dy,
-  //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it.
+  //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it;
+  //    EXACT writes no planes and masks the fp32 dy in place for its SIMT kernels.
   const View dpool = pool ? e->view(pool->out_val, true) : View();
   const uint8_t* pam = pool ? (const uint8_t*)(e->ws + pool->argmax_off) : nullptr;
   if (e->fast()) {
@@ -645,7 +629,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   } else {
     const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
     const View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
-    if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz and its planes: only the bias sums are left
+    if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz (and its planes): only the bias sums are left
       if (dbp) rc = launch_mask_bias_vec<float>(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pre) {    // bias sums of the already masked fp32 dz only: no planes, nothing written back
       if (!bias_w && dbp) rc = launch_mask_bias_vec<float>(dy, y, View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
@@ -748,7 +732,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
   if (((uintptr_t)dev_ptr) % 1024) return h->fail(SSNB_EINVAL, "workspace must be 1024-byte aligned");
   h->ws = (char*)dev_ptr;
   h->weights_ready = false;
-  if (h->tensor_cores() && cudaMemset(h->ws + h->bpartial_off, 0, 256) != cudaSuccess) { cudaGetLastError(); /* no device (CPU-only planning) */ }
+  if (cudaMemset(h->ws + h->bpartial_off, 0, 256) != cudaSuccess) { cudaGetLastError(); /* no device (CPU-only planning) */ }
   h->tc_flag = (int*)(h->ws + h->tc_flag_off);
   if (cudaMemset(h->tc_flag, 0, 256) != cudaSuccess) cudaGetLastError();
   h->gscale = (float*)(h->ws + h->tc_flag_off + 16);

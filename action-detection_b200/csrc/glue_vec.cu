@@ -1,8 +1,9 @@
-// Memory-bound glue of the tensor-core modes over NHWC views, vectorised: every thread moves 16 bytes of channels, 4 fp32
-// channels in SSNB_EXACT_TC and 8 fp16 channels in SSNB_FAST_FP16.  Same semantics as the scalar kernels in simt_glue.cu
-// (Caffe ceil-mode pooling, model_zoo/bninception/layer_factory.py:41-53; first-max-wins arg-max; 3x3 average with
-// count_include_pad).  Each kernel is written once over the storage type; Vec<T> holds what differs between the two.  In
-// EXACT_TC the kernels that produce a convolution operand also write its fp16 hi / lo planes, so no separate split pass runs.
+// Memory-bound glue of every precision over NHWC views, vectorised: every thread moves 16 bytes of channels, 4 fp32
+// channels in SSNB_EXACT_FP32 and SSNB_EXACT_TC, 8 fp16 channels in SSNB_FAST_FP16.  Caffe ceil-mode pooling
+// (model_zoo/bninception/layer_factory.py:41-53) with a first-max-wins arg-max, the 3x3 average with count_include_pad, and
+// the ReLU mask + bias-gradient pass of a convolution's backward.  Each kernel is written once over the storage type; Vec<T>
+// holds what differs between the two.  In EXACT_TC the kernels that produce a convolution operand also write its fp16 hi / lo
+// planes, so no separate split pass runs; EXACT_FP32 passes no planes.
 #include <type_traits>
 
 #include "common.cuh"
@@ -15,7 +16,8 @@ __device__ __forceinline__ uint32_t zero_bytes(uint32_t x) { return (x - 0x01010
 
 template <typename T> struct Vec;
 
-// EXACT_TC: fp32 arithmetic throughout; the outputs that feed a tensor-core product also go out as hi / lo planes
+// EXACT_FP32 and EXACT_TC: fp32 arithmetic throughout; in EXACT_TC the outputs that feed a tensor-core product also go out as
+// hi / lo planes
 template <> struct Vec<float> {
   static constexpr int N = VEC_WIDTH<float>;
   static constexpr bool PLANES = true;
@@ -171,7 +173,7 @@ template <typename T> __device__ __forceinline__ typename Vec<T>::Raw ldv(const 
 
 // ---- max pooling ---------------------------------------------------------------------------------------------
 // every max pool of the network is 3x3: all nine loads are issued before the first compare; the compare order -- and with
-// it the first-max-wins / NaN rule -- is that of the scalar loop
+// it the first-max-wins / NaN rule -- is that of a row-major loop over the window
 template <typename T>
 __global__ void maxpool_fwd_vec(const T* __restrict__ src, int H, int W, int C, int spitch, int scoff, T* __restrict__ dst, int OH, int OW,
                                 int dpitch, int dcoff, __half* __restrict__ hi, long long lo_off, int stride, int pad, int F,

@@ -310,35 +310,6 @@ __global__ void wgrad_finalize_all_kernel(const __grid_constant__ FinalizeTable 
   *o = (accumulate ? *o : 0.f) + s * q.mult[co] * out_scale;
 }
 
-// column sums of dz: stage 1 partial[split][c], stage 2 db[c] = mult[c]*out_scale*sum
-template <typename T>
-__global__ void bias_grad_partial_kernel(const T* __restrict__ dz, long long rows, int C, int pitch, int coff,
-                                         long long rows_per_split, float* __restrict__ partial) {
-  __shared__ float red[8][32];
-  const int c = blockIdx.x * 32 + threadIdx.x;
-  const long long r0 = (long long)blockIdx.y * rows_per_split;
-  const long long r1 = (r0 + rows_per_split < rows) ? r0 + rows_per_split : rows;
-  float s = 0.f;
-  if (c < C)
-    for (long long r = r0 + threadIdx.y; r < r1; r += 8) s += to_f<T>(dz[r * pitch + coff + c]);
-  red[threadIdx.y][threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x];
-    partial[(long long)blockIdx.y * C + c] = t;
-  }
-}
-__global__ void bias_grad_final_kernel(const float* __restrict__ partial, int splits, int C,
-                                       const float* __restrict__ mult, float out_scale, float* __restrict__ db, int accumulate) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  float s = 0.f;
-  for (int i = 0; i < splits; ++i) s += partial[(long long)i * C + c];
-  db[c] = (accumulate ? db[c] : 0.f) + s * mult[c] * out_scale;
-}
-
 }  // namespace
 
 template <typename T> int launch_conv(const ConvArgs& a, cudaStream_t s) {
@@ -386,18 +357,5 @@ int launch_wgrad_finalize_all(const FinalizeTable& t, float out_scale, int accum
   SSNB_LAUNCH_CHECK("wgrad_finalize_all_kernel");
   return 0;
 }
-
-template <typename T>
-int launch_bias_grad(const void* dz, int rows, int C, int pitch, int coff, const float* mult, float out_scale,
-                     float* partial, int splits, float* db, int accumulate, cudaStream_t s) {
-  const long long rps = ((long long)rows + splits - 1) / splits;
-  dim3 grid((unsigned)((C + 31) / 32), (unsigned)splits), block(32, 8);
-  bias_grad_partial_kernel<T><<<grid, block, 0, s>>>(reinterpret_cast<const T*>(dz), rows, C, pitch, coff, rps, partial);
-  SSNB_LAUNCH_CHECK("bias_grad_partial_kernel");
-  bias_grad_final_kernel<<<(C + 127) / 128, 128, 0, s>>>(partial, splits, C, mult, out_scale, db, accumulate);
-  SSNB_LAUNCH_CHECK("bias_grad_final_kernel");
-  return 0;
-}
-template int launch_bias_grad<float>(const void*, int, int, int, int, const float*, float, float*, int, float*, int, cudaStream_t);
 
 }  // namespace ssnb

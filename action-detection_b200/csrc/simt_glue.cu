@@ -1,7 +1,6 @@
-// Memory-bound glue of the BNInception graph over NHWC views: layout conversion, max / average
-// pooling (Caffe ceil-mode semantics, model_zoo/bninception/layer_factory.py:41-53), 7x7 global
-// pooling (bn_inception.yaml:552), ReLU gradient masks, and BN-folding weight packing
-// (frozen BatchNorm2d, ssn_models.py:156-174).
+// Memory-bound glue of the BNInception graph over NHWC views: layout conversion, 7x7 global pooling
+// (bn_inception.yaml:552), the backward's gradient exponent, and BN-folding weight packing (frozen
+// BatchNorm2d, ssn_models.py:156-174).  Max / average pooling and the ReLU gradient mask are in glue_vec.cu.
 #include <cfloat>
 
 #include "common.cuh"
@@ -35,93 +34,6 @@ __global__ void nhwc_to_nchw_kernel(const T* __restrict__ src, int F, int C, int
   const int c = (int)((i / ((long long)H * W)) % C);
   const long long f = i / ((long long)H * W * C);
   dst[i] = to_f<T>(src[(f * H * W + yx) * pitch + coff + c]) * scale;
-}
-
-// max pooling, ceil_mode: OH = ceil((H + 2p - k)/s) + 1 (last window must start inside the padded input)
-template <typename T>
-__global__ void maxpool_fwd_kernel(const T* __restrict__ src, int H, int W, int C, int spitch, int scoff,
-                                   T* __restrict__ dst, int OH, int OW, int dpitch, int dcoff, int F, int k, int stride,
-                                   int pad, uint8_t* __restrict__ argmax) {
-  const long long total = (long long)F * OH * OW * C;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int c = (int)(i % C);
-  const long long p = i / C;
-  const int ox = (int)(p % OW), oy = (int)((p / OW) % OH);
-  const long long f = p / ((long long)OW * OH);
-  float best = -INFINITY;
-  int bi = 0;
-  bool first = true;
-  for (int r = 0; r < k; ++r) {
-    const int iy = oy * stride + r - pad;
-    if (iy < 0 || iy >= H) continue;
-    for (int s = 0; s < k; ++s) {
-      const int ix = ox * stride + s - pad;
-      if (ix < 0 || ix >= W) continue;
-      const float v = to_f<T>(src[((f * H + iy) * W + ix) * spitch + scoff + c]);
-      if (first || v > best || v != v) { best = v; bi = r * k + s; first = false; }   // first max wins (ATen)
-    }
-  }
-  dst[p * dpitch + dcoff + c] = from_f<T>(best);
-  argmax[i] = (uint8_t)bi;
-}
-
-template <typename T>
-__global__ void maxpool_bwd_kernel(T* __restrict__ dsrc, int H, int W, int C, int spitch, int scoff,
-                                   const T* __restrict__ ddst, int OH, int OW, int dpitch, int dcoff, int F, int k,
-                                   int stride, int pad, const uint8_t* __restrict__ argmax, int accumulate) {
-  const long long total = (long long)F * H * W * C;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int c = (int)(i % C);
-  const long long p = i / C;
-  const int ix = (int)(p % W), iy = (int)((p / W) % H);
-  const long long f = p / ((long long)W * H);
-  float g = 0.f;
-  for (int r = 0; r < k; ++r) {
-    const int ty = iy + pad - r;
-    if (ty < 0 || ty % stride) continue;
-    const int oy = ty / stride;
-    if (oy >= OH) continue;
-    for (int s = 0; s < k; ++s) {
-      const int tx = ix + pad - s;
-      if (tx < 0 || tx % stride) continue;
-      const int ox = tx / stride;
-      if (ox >= OW) continue;
-      const long long op = (f * OH + oy) * OW + ox;
-      if (argmax[op * C + c] == (uint8_t)(r * k + s)) g += to_f<T>(ddst[op * dpitch + dcoff + c]);
-    }
-  }
-  T* q = dsrc + p * spitch + scoff + c;
-  if (accumulate) g += to_f<T>(*q);
-  *q = from_f<T>(g);
-}
-
-// 3x3 stride-1 pad-1 average, count_include_pad (always /9); its own adjoint
-template <typename T>
-__global__ void avgpool3_kernel(const T* __restrict__ src, int H, int W, int C, int spitch, int scoff,
-                                T* __restrict__ dst, int dpitch, int dcoff, int F, int accumulate) {
-  const long long total = (long long)F * H * W * C;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int c = (int)(i % C);
-  const long long p = i / C;
-  const int x = (int)(p % W), y = (int)((p / W) % H);
-  const long long f = p / ((long long)W * H);
-  float s = 0.f;
-  for (int r = -1; r <= 1; ++r) {
-    const int yy = y + r;
-    if (yy < 0 || yy >= H) continue;
-    for (int q = -1; q <= 1; ++q) {
-      const int xx = x + q;
-      if (xx < 0 || xx >= W) continue;
-      s += to_f<T>(src[((f * H + yy) * W + xx) * spitch + scoff + c]);
-    }
-  }
-  s = s / 9.0f;
-  T* o = dst + p * dpitch + dcoff + c;
-  if (accumulate) s += to_f<T>(*o);
-  *o = from_f<T>(s);
 }
 
 template <typename T>
@@ -183,16 +95,6 @@ __global__ void __launch_bounds__(GE_THREADS) grad_exponent_kernel(const float* 
   }
   gscale[0] = ldexpf(1.0f, k);
   gscale[1] = ldexpf(1.0f, -k);
-}
-
-template <typename T>
-__global__ void relu_mask_kernel(T* __restrict__ dy, int dpitch, int dcoff, const T* __restrict__ y, int ypitch,
-                                 int ycoff, long long pixels, int C) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= pixels * C) return;
-  const int c = (int)(i % C);
-  const long long p = i / C;
-  if (!(to_f<T>(y[p * ypitch + ycoff + c]) > 0.f)) dy[p * dpitch + dcoff + c] = from_f<T>(0.f);
 }
 
 // all layers of the network in a few launches (69 per-layer launches would be mostly launch latency: the weights are
@@ -306,31 +208,6 @@ template <typename T> int launch_nhwc_to_nchw(View src, int F, float scale, floa
   SSNB_LAUNCH_CHECK("nhwc_to_nchw_kernel");
   return 0;
 }
-template <typename T>
-int launch_maxpool_fwd(View src, View dst, int F, int k, int stride, int pad, uint8_t* argmax, cudaStream_t s) {
-  const long long n = (long long)F * dst.H * dst.W * src.C;
-  maxpool_fwd_kernel<T><<<blocks_for(n), TPB, 0, s>>>(V(const T, src), src.H, src.W, src.C, src.pitch, src.coff, V(T, dst),
-                                                     dst.H, dst.W, dst.pitch, dst.coff, F, k, stride, pad, argmax);
-  SSNB_LAUNCH_CHECK("maxpool_fwd_kernel");
-  return 0;
-}
-template <typename T>
-int launch_maxpool_bwd(View dsrc, View ddst, int F, int k, int stride, int pad, const uint8_t* argmax, int accumulate,
-                       cudaStream_t s) {
-  const long long n = (long long)F * dsrc.H * dsrc.W * dsrc.C;
-  maxpool_bwd_kernel<T><<<blocks_for(n), TPB, 0, s>>>(V(T, dsrc), dsrc.H, dsrc.W, dsrc.C, dsrc.pitch, dsrc.coff,
-                                                     V(const T, ddst), ddst.H, ddst.W, ddst.pitch, ddst.coff, F, k, stride,
-                                                     pad, argmax, accumulate);
-  SSNB_LAUNCH_CHECK("maxpool_bwd_kernel");
-  return 0;
-}
-template <typename T> int launch_avgpool3_fwd(View src, View dst, int F, int accumulate, cudaStream_t s) {
-  const long long n = (long long)F * src.H * src.W * src.C;
-  avgpool3_kernel<T><<<blocks_for(n), TPB, 0, s>>>(V(const T, src), src.H, src.W, src.C, src.pitch, src.coff, V(T, dst),
-                                                  dst.pitch, dst.coff, F, accumulate);
-  SSNB_LAUNCH_CHECK("avgpool3_kernel");
-  return 0;
-}
 template <typename T> int launch_gpool_fwd(View src, int F, float* feat, cudaStream_t s) {
   gpool_fwd_kernel<T><<<blocks_for((long long)F * src.C), TPB, 0, s>>>(V(const T, src), src.H * src.W, src.C, src.pitch,
                                                                       src.coff, F, feat);
@@ -350,12 +227,6 @@ int launch_grad_exponent(const float* dfeat, long long n, float grad_scale, int 
   SSNB_LAUNCH_CHECK("grad_exponent_kernel");
   return 0;
 }
-template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t s) {
-  const long long px = (long long)F * dy.H * dy.W;
-  relu_mask_kernel<T><<<blocks_for(px * dy.C), TPB, 0, s>>>(V(T, dy), dy.pitch, dy.coff, V(const T, y), y.pitch, y.coff, px, dy.C);
-  SSNB_LAUNCH_CHECK("relu_mask_kernel");
-  return 0;
-}
 #define INST(T)                                                                                              \
   template int launch_nchw_to_nhwc<T>(const float*, int, int, int, int, View, float, cudaStream_t);                 \
   template int launch_nhwc_to_nchw<T>(View, int, float, float*, cudaStream_t);                               \
@@ -363,10 +234,5 @@ template <typename T> int launch_relu_mask(View dy, View y, int F, cudaStream_t 
   template int launch_gpool_bwd<T>(const float*, float, const float*, View, int, const void*, cudaStream_t);
 INST(float)
 INST(__half)
-// EXACT_FP32 only: the tensor-core modes pool and mask with the vector kernels of glue_vec.cu
-template int launch_maxpool_fwd<float>(View, View, int, int, int, int, uint8_t*, cudaStream_t);
-template int launch_maxpool_bwd<float>(View, View, int, int, int, int, const uint8_t*, int, cudaStream_t);
-template int launch_avgpool3_fwd<float>(View, View, int, int, cudaStream_t);
-template int launch_relu_mask<float>(View, View, int, cudaStream_t);
 
 }  // namespace ssnb
