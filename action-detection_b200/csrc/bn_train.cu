@@ -111,8 +111,8 @@ __global__ void bn_apply_relu_kernel(const float* __restrict__ z, int zpitch, in
   const long long r = i / G;
   const float4 zv = ld4(z + r * zpitch + zcoff + g * 4), m = ld4(stat + g * 4), s = ld4(stat + C + g * 4), ga = ld4(gamma + g * 4), be = ld4(beta + g * 4);
   float4 o;
-  o.x = fmaxf((zv.x - m.x) * s.x * ga.x + be.x, 0.f); o.y = fmaxf((zv.y - m.y) * s.y * ga.y + be.y, 0.f);
-  o.z = fmaxf((zv.z - m.z) * s.z * ga.z + be.z, 0.f); o.w = fmaxf((zv.w - m.w) * s.w * ga.w + be.w, 0.f);
+  o.x = relu((zv.x - m.x) * s.x * ga.x + be.x); o.y = relu((zv.y - m.y) * s.y * ga.y + be.y);
+  o.z = relu((zv.z - m.z) * s.z * ga.z + be.z); o.w = relu((zv.w - m.w) * s.w * ga.w + be.w);
   *reinterpret_cast<float4*>(y + r * ypitch + ycoff + g * 4) = o;
   if (hi) store_planes4(hi + r * ypitch + ycoff + g * 4, lo_off, o);
 }

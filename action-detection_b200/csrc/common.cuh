@@ -54,6 +54,8 @@ template <> __device__ __forceinline__ float to_f<__half>(__half v) { return __h
 template <typename T> __device__ __forceinline__ T from_f(float v);
 template <> __device__ __forceinline__ float from_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ __half from_f<__half>(float v) { return __float2half_rn(v); }
+// the ReLU of every forward epilogue: NaN stays NaN (torch.relu; fmaxf(NaN, 0) would be 0), -0 and +0 give +0
+__device__ __forceinline__ float relu(float v) { return v <= 0.f ? 0.f : v; }
 
 // SSNB_EXACT_TC operand format: an fp32 value x is carried as hi = fp16(x), lo = fp16(x - float(hi)) (tc_glue.cu)
 constexpr float HALF_MAX = 65504.f;

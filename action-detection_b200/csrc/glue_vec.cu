@@ -33,7 +33,7 @@ template <> struct Vec<float> {
       if (((am >> (8 * j)) & 0xFFu) == t) acc[j] += v[j];
   }
   static __device__ __forceinline__ uint32_t any_tag(Tags a, uint32_t t4) { return zero_bytes(a ^ t4); }
-  // running maximum of a window, per lane: first max wins, NaN propagates (ATen)
+  // running maximum of a window, per lane: first max wins, NaN propagates and the last NaN holds the arg-max (ATen)
   struct Max {
     float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
     uint32_t bi = 0u;
@@ -102,8 +102,8 @@ template <> struct Vec<__half> {
     }
   }
   static __device__ __forceinline__ uint32_t any_tag(Tags a, uint32_t t4) { return zero_bytes(a.x ^ t4) | zero_bytes(a.y ^ t4); }
-  // NaN-propagating half2 maximum; the tap index (16-bit, in the lanes of the half2 values) moves where the maximum changed
-  // (v > best, or a NaN arrived), or when nothing was taken yet: 3 instructions per half2
+  // NaN-propagating half2 maximum; the tap index (16-bit, in the lanes of the half2 values) moves where v > best or v is NaN
+  // (so a later NaN takes it from an earlier one, as in ATen), or when nothing was taken yet
   struct Max {
     uint32_t best[4] = {0u, 0u, 0u, 0u};
     uint32_t bi[4] = {0u, 0u, 0u, 0u};
@@ -115,7 +115,7 @@ template <> struct Vec<__half> {
         const __half2 hv = *reinterpret_cast<const __half2*>(&v[j]);
         const __half2 hb = *reinterpret_cast<const __half2*>(&best[j]);
         const __half2 hn = __hmax2_nan(hb, hv);
-        const uint32_t m = first ? 0xFFFFFFFFu : __hneu2_mask(hn, hb);
+        const uint32_t m = first ? 0xFFFFFFFFu : (__hgt2_mask(hv, hb) | __hneu2_mask(hv, hv));
         best[j] = first ? v[j] : *reinterpret_cast<const uint32_t*>(&hn);
         bi[j] = (tag & m) | (bi[j] & ~m);
       }

@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(NT) conv_kernel(ConvArgs a) {
     }
     if (a.relu) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) v[j] = fmaxf(v[j], 0.f);
+      for (int j = 0; j < 4; ++j) v[j] = relu(v[j]);
     }
     Vec4<T>::store(p, v);
   }

@@ -290,7 +290,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
               for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) v[b][h][j] = fmaxf(v[b][h][j], 0.f);
+                for (int j = 0; j < 4; ++j) v[b][h][j] = relu(v[b][h][j]);
           }
           if (p.mask32) {                              // ReLU gradient of the value this data gradient completes: keep where y > 0 (NaN -> 0)
             const float* m32 = p.mask32 + p.mask32_coff + col + q2;
@@ -335,7 +335,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
               for (int h = 0; h < 2; ++h)
 #pragma unroll
-                for (int j = 0; j < 4; ++j) v[b][h][j] = fmaxf(v[b][h][j], 0.f);
+                for (int j = 0; j < 4; ++j) v[b][h][j] = relu(v[b][h][j]);
           }
           if (p.mask_y) {
             const __half* my = p.mask_y + p.mask_coff + col + q2;

@@ -193,14 +193,22 @@ def fold(params, conv_id, device):
 
 
 def maxpool_route(x, g, k, s, p):
-    """vjp of a ceil-mode max pool with the kernels' rule: the gradient goes to the FIRST maximum of the window in row-major
-    tap order (a NaN counts as the maximum); padding never wins"""
+    """vjp of a ceil-mode max pool with the kernels' rule, ATen's: in row-major tap order a tap takes the gradient when it is
+    greater than the maximum so far or is NaN, so the FIRST maximum wins and, in a window with NaNs, the LAST NaN; padding
+    never wins (a window of -inf routes to its first real tap)"""
     n, c, h, w = x.shape
     oh, ow = g.shape[2:]
     hp, wp = (oh - 1) * s + k, (ow - 1) * s + k
-    xp = F.pad(x, (p, wp - w - p, p, hp - h - p), value=-math.inf)
-    cols = F.unfold(xp, k, stride=s).view(n, c, k * k, oh * ow)
-    idx = cols.argmax(2, keepdim=True)         # first maximal tap; NaN compares greater
+    pads = (p, wp - w - p, p, hp - h - p)
+    cols = F.unfold(F.pad(x, pads), k, stride=s).view(n, c, k * k, oh * ow)
+    real = F.unfold(F.pad(torch.ones_like(x[:1, :1]), pads), k, stride=s).view(1, 1, k * k, oh * ow) > 0
+    tap = torch.arange(k * k, device=x.device).view(1, 1, k * k, 1)
+    nan = cols.isnan() & real
+    num = real & ~nan
+    top = torch.where(num, cols, -math.inf).amax(2, keepdim=True)
+    first_max = torch.where(num & (cols == top), tap, k * k).amin(2, keepdim=True)
+    last_nan = torch.where(nan, tap, -1).amax(2, keepdim=True)
+    idx = torch.where(last_nan >= 0, last_nan, first_max)
     onehot = torch.zeros_like(cols).scatter_(2, idx, g.reshape(n, c, 1, oh * ow))
     dxp = F.fold(onehot.view(n, c * k * k, oh * ow), (hp, wp), k, stride=s)
     return dxp[:, :, p:p + h, p:p + w]

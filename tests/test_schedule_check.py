@@ -365,6 +365,30 @@ def test_max_pool_route_rule():
     assert d[0, 0, 2, 2] == 1 and d[0, 0, 2, 3] == 1 and d[0, 0, 3, 2] == 1 and d[0, 0, 3, 3] == 1 and d.sum() == 4
 
 
+@pytest.mark.parametrize("k,s,p,size", [(3, 2, 0, 7), (3, 2, 0, 8), (3, 1, 1, 7), (2, 1, 0, 5)])
+def test_max_pool_route_matches_aten_on_ties_and_non_finite(k, s, p, size):
+    """the route is float64 autograd of F.max_pool2d (ceil mode) on windows full of exact ties (+-0 among them), with two
+    NaNs in one window (the LAST one takes the gradient), NaN beside +-inf, and windows of -inf only"""
+    gen = torch.Generator().manual_seed(size * 10 + k + s + p)
+    vals = torch.tensor([-1.0, -0.5, -0.0, 0.0, 0.5, 1.0], dtype=torch.float64)
+    x = vals[torch.randint(0, len(vals), (2, 3, size, size), generator=gen)]
+    nan, inf = float("nan"), float("inf")
+    x[0, 0, 0, 0] = x[0, 0, 1, 1] = nan                 # two NaNs in the first window
+    x[0, 1, 0, 1], x[0, 1, 1, 0] = inf, nan              # NaN after +inf
+    x[0, 2, 0, 0], x[0, 2, 0, 1] = nan, -inf             # NaN before -inf
+    x[1, 0, :3, :3] = -inf                               # a window of -inf only (with padding around it at p = 1)
+    x[1, 1, -2:, -2:] = -inf                             # the partial last window
+    x[1, 2, -1, -1], x[1, 2, -1, 0], x[1, 2, 0, -1] = nan, nan, inf   # poison in the last row and column
+    x[1, 2, 2, 2] = inf
+    x[1, 2, 2, 3 % size] = inf                           # tied +inf
+    xr = x.clone().requires_grad_(True)
+    y = F.max_pool2d(xr, k, s, p, ceil_mode=True)
+    g = torch.randint(1, 9, y.shape, generator=gen).double()
+    y.backward(g)
+    d = S.maxpool_route(x, g, k, s, p)
+    assert torch.equal(d, xr.grad), (d - xr.grad).abs().nonzero()[:8]
+
+
 # ---- forward-only and bn_mode='partial' ---------------------------------------------------------------------------------
 BN1_PLANTS = {      # planted error -> the one record that must fail
     "no_xhat_term": (S.BN1_CONV, "dZ"),             # BatchNorm backward without xhat * sum(g * xhat) / M
