@@ -45,6 +45,20 @@ class DetectBatchCfg(C.Structure):
 
 DET_ALL, DET_TOPK, DET_CLS = 0, 1, 2
 
+
+class FrameCfg(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("channels", C.c_int32), ("out_size", C.c_int32), ("scale_size", C.c_int32),
+                ("invert_even", C.c_int32), ("n_mean", C.c_int32), ("mean", C.c_float * 8), ("std", C.c_float * 8)]
+
+
+class FrameGroup(C.Structure):
+    _fields_ = [("src_offset", C.c_int64), ("dst_offset", C.c_int64), ("scratch_offset", C.c_int64), ("first_image", C.c_int32),
+                ("height", C.c_int32), ("width", C.c_int32), ("images", C.c_int32), ("crop_x", C.c_int32), ("crop_y", C.c_int32),
+                ("crop_w", C.c_int32), ("crop_h", C.c_int32), ("flip", C.c_int32), ("reserved", C.c_int32)]
+
+
+FRAMES_TRAIN, FRAMES_OVERSAMPLE, FRAMES_CENTER = 0, 1, 2
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 _pp = C.POINTER(C.c_void_p)
@@ -106,6 +120,8 @@ SIGNATURES = {
     "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
     "ssnb_tag_proposals": (_i, [C.POINTER(TagProposalsCfg), _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp] + [_vp] * 10
                            + [_sz, _vp]),
+    "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
+    "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
     "ssnb_sgd_step": (_i, [_vp, _vp, _vp, _sz, _f, _f, _f, _f, _vp]),
     "ssnb_sgd_step_groups": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp]),
 }

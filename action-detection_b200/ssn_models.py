@@ -184,6 +184,30 @@ class _BNInceptionModel(torch.nn.Module):
         return torchvision.transforms.Compose([GroupMultiScaleCrop(self.input_size, scales),
                                                GroupRandomHorizontalFlip(is_flow=(self.modality == 'Flow'))])
 
+    def frame_transforms(self):
+        """The data-side transforms of the drivers on the GPU (ops/frame_transforms.py), with this model's scales, input_mean,
+        input_std and modality filled in.  Each transform takes uint8 frames (GroupToUint8 on the dataset side) and returns
+        the CUDA fp32 [frames, C, 224, 224] input that get_augmentation / GroupOverSample / GroupScale + GroupCenterCrop
+        followed by Stack, ToTorchFormatTensor(div=False) and GroupNormalize produce:
+          sample_train_params(sizes)     the crop and flip draws of get_augmentation(), one per group
+          train(frames, params)          get_augmentation() (training)
+          oversample(frames)             GroupOverSample(crop_size, scale_size) (10-crop test)
+          center_crop(frames)            GroupScale(scale_size) + GroupCenterCrop(crop_size) (1-crop test, validation)
+          to_uint8                       the dataset-side transform"""
+        import functools
+        import types
+        from ops import frame_transforms as T
+        is_flow = self.modality == 'Flow'
+        scales = [1, .875, .75] if is_flow else [1, .875, .75, .66]
+        fc = (2 if is_flow else 3) * self.new_length
+        common = dict(mean=self.input_mean, std=self.input_std, frame_channels=fc)
+        return types.SimpleNamespace(
+            sample_train_params=functools.partial(T.sample_train_params, scales=scales, input_size=self.input_size),
+            train=functools.partial(T.train_frames, input_size=self.input_size, is_flow=is_flow, **common),
+            oversample=functools.partial(T.oversample_frames, crop_size=self.crop_size, scale_size=self.scale_size, **common),
+            center_crop=functools.partial(T.center_crop_frames, crop_size=self.crop_size, scale_size=self.scale_size, **common),
+            to_uint8=T.GroupToUint8())
+
 
 class SSN(_BNInceptionModel):
     def __init__(self, num_class,

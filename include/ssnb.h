@@ -318,6 +318,56 @@ int ssnb_tag_proposals(const ssnb_tag_proposals_cfg* cfg, const float* f_score, 
                        uint32_t* labels, int32_t* raw_frames, float* raw_scores, int32_t* raw_counts, void* workspace,
                        size_t workspace_bytes, void* stream);
 
+/* ---- frame transforms: the PIL group transforms of the data pipeline (transforms.py:41-206) followed by Stack(roll=True),
+ *      ToTorchFormatTensor(div=False) and GroupNormalize (transforms.py:67-80,256-288), bitwise equal to PIL 8-bit BILINEAR --
+ * Modes (cfg->mode):
+ *   SSNB_FRAMES_TRAIN       GroupMultiScaleCrop (:135-206) + GroupRandomHorizontalFlip (:49-64) with the crop window and flip
+ *                           drawn on the host: each group's images are cropped to (crop_x, crop_y, crop_w, crop_h) and resized
+ *                           to out_size x out_size (get_augmentation, ssn_models.py; ssn_train.py:106-117)
+ *   SSNB_FRAMES_OVERSAMPLE  GroupOverSample(out_size, scale_size) (:99-132): GroupScale then the five fill_fix_offset(False)
+ *                           windows, each window's images plain then flipped (ssn_test.py / binary_test.py --test_crops 10)
+ *   SSNB_FRAMES_CENTER      GroupScale(scale_size) + GroupCenterCrop(out_size) (:41-46,83-96; ssn_test.py:107-110, val_loader)
+ * GroupScale is torchvision Resize of the shorter edge to scale_size (long = int(scale_size * long / short)); it is skipped when
+ * the shorter edge already equals scale_size.  A window that reaches outside the image reads zeros, as PIL's crop fills.
+ * Group g's images are src[src_offset ..] as uint8 [images, height, width, channels] (RGB or L).  Output: fp32 planes
+ * [out_size, out_size] from dst + dst_offset, plane ((crop * images + image) * channels + c) with c in BGR order for RGB,
+ * crop 0..9 (OVERSAMPLE: window crop / 2, flipped when odd) or 0; value (v - mean[p % n_mean]) / std[p % n_mean] in fp32,
+ * p the plane index within the group.  A flipped image at an even position of its group becomes 255 - v when invert_even
+ * is set (Flow, transforms.py:59-61,125-126).
+ * ssnb_frame_transform_workspace_bytes validates cfg and the HOST table, fills in each group's first_image, dst_offset and
+ * scratch_offset, and returns the workspace size and the floats dst must hold.  ssnb_frame_transform takes that host table
+ * (validated again, it sizes the launch) and groups_dev, a device copy of it that the kernels read: kernels only, no host
+ * synchronisation, allocation or host copy, so the call can be captured in a CUDA graph and replayed after new frames and
+ * new crop windows / flips are written to src and groups_dev (height, width, images and the layout fields must stay). */
+enum { SSNB_FRAMES_TRAIN = 0, SSNB_FRAMES_OVERSAMPLE = 1, SSNB_FRAMES_CENTER = 2 };
+typedef struct {
+  int32_t mode;         /* SSNB_FRAMES_TRAIN | SSNB_FRAMES_OVERSAMPLE | SSNB_FRAMES_CENTER */
+  int32_t channels;     /* 3 (RGB, written BGR) or 1 (L: Flow x / y planes) */
+  int32_t out_size;     /* crop size, 1..1024 (224) */
+  int32_t scale_size;   /* OVERSAMPLE / CENTER: GroupScale's shorter edge, out_size..4096 (256) */
+  int32_t invert_even;  /* 1: Flow */
+  int32_t n_mean;       /* 1..8 entries of mean / std, cycled over the stacked planes; images * channels % n_mean == 0 */
+  float mean[8];
+  float std[8];
+} ssnb_frame_cfg;
+typedef struct {
+  int64_t src_offset;      /* bytes */
+  int64_t dst_offset;      /* floats; filled in by ssnb_frame_transform_workspace_bytes */
+  int64_t scratch_offset;  /* workspace bytes of the GroupScale output; filled in likewise */
+  int32_t first_image;     /* images of the groups before this one; filled in likewise */
+  int32_t height, width;   /* 1..16384 */
+  int32_t images;          /* >= 1 */
+  int32_t crop_x, crop_y;  /* TRAIN: window offset (may be negative), |.| <= 16384 */
+  int32_t crop_w, crop_h;  /* TRAIN: window size, 1..16 * out_size */
+  int32_t flip;            /* TRAIN: 1 = GroupRandomHorizontalFlip flipped this group */
+  int32_t reserved;
+} ssnb_frame_group;
+int ssnb_frame_transform_workspace_bytes(const ssnb_frame_cfg* cfg, ssnb_frame_group* groups, int n_groups, size_t* workspace_bytes,
+                                         int64_t* dst_floats);
+int ssnb_frame_transform(const ssnb_frame_cfg* cfg, const ssnb_frame_group* groups, const ssnb_frame_group* groups_dev, int n_groups,
+                         const uint8_t* src, size_t src_bytes, float* dst, int64_t dst_floats, void* workspace, size_t workspace_bytes,
+                         void* stream);
+
 /* fused SGD-momentum step over flat fp32 buffers (ssn_train.py:141-144 torch.optim.SGD semantics):
  * g = grad*grad_mult + wd*p; buf = mom*buf + g; p -= lr*buf */
 int ssnb_sgd_step(float* param, const float* grad, float* momentum_buf, size_t n, float lr, float momentum,
