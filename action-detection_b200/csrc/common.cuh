@@ -25,12 +25,12 @@ void set_thread_error(const std::string& s);
 // on this thread, every launch records a CUDA event behind itself on its stream; a launch's time is the distance to the
 // previous event (launches are back to back on one stream).  The engine tags the launches it is about to make with the
 // pass they belong to, the algorithmic FLOPs of the convolution they compute and its op name; umma_conv_launch adds its
-// tile count and tile width.
+// tile count and tile width, umma_wgrad_launch its CTAs per pixel split and split count.
 struct LaunchTag {
   int phase = 3;                  // 0 forward, 1 data gradient, 2 weight gradient, 3 other
   double flop = 0.0;
   const char* op = nullptr;       // copied when the launch is recorded
-  int tiles = 0, block_n = 0;
+  int tiles = 0, block_n = 0;     // umma_wgrad_kernel: ctas, splits
 };
 extern thread_local bool t_timing;
 extern thread_local LaunchTag t_tag;

@@ -151,6 +151,7 @@ struct ssnb_engine {
   bool fold_pools = true;                            // SSNB_DISABLE_FUSION=1 also keeps the max-pool backward separate
   bool s2d_ready = false;                            // backbone_fwd converted the input directly
   int Cs = 0;                                        // channels of the space-to-depth input (4*Cin rounded up to 8)
+  int conv1_tsplits = 128;                           // tensor-core modes: bound of conv1's weight-gradient split count (sizes its partials)
   char* ws = nullptr;
   bool weights_ready = false;
   std::vector<float*> dw, db;
@@ -365,12 +366,13 @@ static void plan(ssnb_engine* e) {
         splits = (M + rows - 1) / rows;
         o.wsplits = (int)splits; o.wrows = (int)rows;
         // tensor-core path: one CTA per SM is resident, so the planner wants num_sms / (M tiles x N tiles x tap groups) pixel
-        // splits; the SIMT heuristic above used to cap it and left most SMs idle on most 3x3 layers
+        // splits, and whole waves more where a split would sum more than UMMA_WGRAD_MAX_PTILES pixel tiles; the SIMT
+        // heuristic above used to cap it and left most SMs idle on most 3x3 layers
         {
           const int chunks = (c.cin + 63) / 64, n_tiles = (chunks + 3) / 4, block_n = ((chunks + n_tiles - 1) / n_tiles) * 64;
           const int tpc = std::max(1, 4 / (block_n / 64));
           const int ctas = ((c.cout + 127) / 128) * n_tiles * ((taps + tpc - 1) / tpc);
-          o.tsplits = std::max(o.wsplits, std::min(128, std::max(1, device_sms() / ctas)));
+          o.tsplits = std::max(o.wsplits, std::min(128, umma_wgrad_splits(ctas, umma_wgrad_ptiles(ob.W, ob.H, e->F), device_sms())));
         }
         if (e->tensor_cores()) splits = std::max<long long>(splits, o.tsplits);
         const size_t need = (size_t)splits * taps * c.cout * c.cin * 4;
@@ -430,6 +432,15 @@ static void plan(ssnb_engine* e) {
       return at;
     };
     e->Cs = (4 * e->cfg.in_channels + 7) / 8 * 8;
+    // conv1's weight gradient (4 taps over the 4*Cs-channel space-to-depth input, one M tile): 128 splits, or as many whole
+    // waves as keep a split at most UMMA_WGRAD_MAX_PTILES pixel tiles long where 128 would not
+    {
+      const int chunks = (4 * e->Cs + 63) / 64, n_tiles = (chunks + 3) / 4, block_n = ((chunks + n_tiles - 1) / n_tiles) * 64;
+      const int tpc = std::min(4, std::max(1, 4 / (block_n / 64)));
+      const int ptiles = umma_wgrad_ptiles(112, 112, e->F);
+      if ((ptiles + UMMA_WGRAD_MAX_PTILES - 1) / UMMA_WGRAD_MAX_PTILES > 128)
+        e->conv1_tsplits = umma_wgrad_splits(n_tiles * ((4 + tpc - 1) / tpc), ptiles, device_sms());
+    }
     e->s2d_off = operand_region(F * 112 * 112 * 4 * e->Cs * 2, e->s2d_plane);      // packed: 4 horizontal neighbours per pixel
     e->s2d_w_off = operand_region((size_t)16 * 64 * e->Cs * 2, e->s2d_w_plane);
     if (e->cfg.training) {
@@ -440,7 +451,7 @@ static void plan(ssnb_engine* e) {
           up = std::max(up, F * ib.H * ib.W * (size_t)e->convs[o.conv].cout * 2);
         }
       e->up_off = operand_region(up, e->up_plane);
-      pmax = std::max(pmax, (size_t)128 * 16 * 64 * e->Cs * 4);
+      pmax = std::max(pmax, (size_t)e->conv1_tsplits * 16 * 64 * e->Cs * 4);
     }
   }
   e->partial_off = off; e->partial_bytes = pmax; off = align_up(off + pmax, 1024);
@@ -450,7 +461,7 @@ static void plan(ssnb_engine* e) {
         const ConvSpec& c = e->convs[o.conv];
         const int nsplit = e->tensor_cores() ? std::max(o.wsplits, o.tsplits) : o.wsplits;
         size_t need = (size_t)nsplit * c.k * c.k * c.cout * c.cin * 4;
-        if (o.conv == 0 && e->tensor_cores()) need = std::max(need, (size_t)128 * 16 * 64 * e->Cs * 4);
+        if (o.conv == 0 && e->tensor_cores()) need = std::max(need, (size_t)e->conv1_tsplits * 16 * 64 * e->Cs * 4);
         o.partial_off = off; off = align_up(off + need, 1024);
         o.bias_partial_off = off; off = align_up(off + (size_t)std::max(nsplit, 128) * c.cout * 4, 256);
       }
@@ -782,7 +793,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       if (rc) return h->fail(rc, "conv1 bind: " + ssnb::thread_error());
       tc_gate(o.umma);
       if (use_wgrad && (rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->operand(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
-                                                  (float*)(h->ws + o.partial_off), 128)))
+                                                  (float*)(h->ws + o.partial_off), h->conv1_tsplits)))
         return h->fail(rc, "conv1 wgrad bind: " + ssnb::thread_error());
       continue;
     }

@@ -132,6 +132,15 @@ struct UmmaWgradPlan {
   CUtensorMap tmap_dz_lo, tmap_x_lo;              // SSNB_EXACT_TC: LO planes (View::lo_off of the bound views)
   UmmaWgradParams p;
 };
+// Longest pixel range of one split, in 64-pixel tiles.  A split sums its pixels in the wgmma's fp32 accumulators, whose error
+// grows in proportion to the number of tiles summed: EXACT_TC's dW rel-L2 is about 1.6e-7 per tile (H100: conv2_3x3 1.1e-4 at
+// 642 tiles, 2.1e-4 at 1283; conv1 of Flow 2.1e-4 / 9.9e-5 / 6.3e-5 at 1711 / 856 / 571), so 768 keeps it near 1.3e-4.
+constexpr int UMMA_WGRAD_MAX_PTILES = 768;
+// pixel tiles of a weight gradient over a W x H x F dz (the box is chosen by W)
+int umma_wgrad_ptiles(int W, int H, int F);
+// split count before the caps of the bind (max_splits, the pixel tile count): `waves` waves of ctas-CTA splits (num_sms / ctas
+// per wave, at least 1), and as many more whole waves as keep every split at most UMMA_WGRAD_MAX_PTILES tiles long
+int umma_wgrad_splits(int ctas, int ptiles, int num_sms, int waves = 1);
 // returns the number of splits chosen through *splits (the caller sizes `partial` from it)
 int umma_wgrad_bind(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x, int F, int cin, int cout, int k, int pad,
                     float* partial, int max_splits, int x_stride = 1);

@@ -167,7 +167,30 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   }
 }
 
+// 64-pixel boxes whose rows are all real-or-zero-filled pixels (the pixel index is the reduction dim)
+void wgrad_box(int W, int& bw, int& bh, int& bf) {
+  if (W % 8 == 0) { bw = 8; bh = 8; bf = 1; }
+  else if (W % 4 == 0) { bw = 4; bh = 4; bf = 4; }
+  else if (W % 2 == 0) { bw = 2; bh = 2; bf = 16; }
+  else { bw = 1; bh = 1; bf = 64; }
+}
+
 }  // namespace
+
+int umma_wgrad_ptiles(int W, int H, int F) {
+  int bw, bh, bf;
+  wgrad_box(W, bw, bh, bf);
+  return ((W + bw - 1) / bw) * ((H + bh - 1) / bh) * ((F + bf - 1) / bf);
+}
+
+int umma_wgrad_splits(int ctas, int ptiles, int num_sms, int waves) {
+  // one CTA per SM is resident (192 KiB pipeline), so a second wave only runs after the first: ONE wave of CTAs with twice the
+  // pixels each does the same work with half the split-K partial traffic (every CTA writes its whole 128 x taps*N fp32
+  // accumulator: 100-250 KB) and no wave tail -- until a split gets longer than UMMA_WGRAD_MAX_PTILES tiles
+  const int per_wave = std::max(1, waves * num_sms / ctas);
+  const int need = (ptiles + UMMA_WGRAD_MAX_PTILES - 1) / UMMA_WGRAD_MAX_PTILES;
+  return std::max(1, (need + per_wave - 1) / per_wave) * per_wave;
+}
 
 int umma_wgrad_bind(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x, int F, int cin, int cout, int k, int pad,
                     float* partial, int max_splits, int x_stride) {
@@ -188,11 +211,7 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   UmmaWgradParams& p = plan.p;
   memset(&p, 0, sizeof(p));
   p.W = dz.W; p.H = dz.H; p.F = F; p.x_stride = x_stride;     // tiles enumerate dz (output) pixels
-  // 64-pixel boxes whose rows are all real-or-zero-filled pixels (the pixel index is the reduction dim)
-  if (dz.W % 8 == 0) { p.bw = 8; p.bh = 8; p.bf = 1; }
-  else if (dz.W % 4 == 0) { p.bw = 4; p.bh = 4; p.bf = 4; }
-  else if (dz.W % 2 == 0) { p.bw = 2; p.bh = 2; p.bf = 16; }
-  else { p.bw = 1; p.bh = 1; p.bf = 64; }
+  wgrad_box(dz.W, p.bw, p.bh, p.bf);
   p.tiles_w = (dz.W + p.bw - 1) / p.bw; p.tiles_h = (dz.H + p.bh - 1) / p.bh; p.tiles_f = (F + p.bf - 1) / p.bf;
   p.ntaps = ntaps;
   for (int t = 0; t < ntaps; ++t) { p.tap_dy[t] = tdy[t]; p.tap_dx[t] = tdx[t]; }
@@ -210,12 +229,8 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   p.taps_per_cta = (ntaps + p.tap_groups - 1) / p.tap_groups;        // balance the groups (9 taps: 3+3+3 rather than 4+4+1)
   const int ptiles = p.tiles_w * p.tiles_h * p.tiles_f;
   const int ctas = p.m_tiles * p.n_tiles * p.tap_groups;
-  // one CTA per SM is resident (192 KiB pipeline), so a second wave only runs after the first: ONE wave of CTAs with
-  // twice the pixels each does the same work with half the split-K partial traffic (every CTA writes its whole
-  // 128 x taps*N fp32 accumulator: 100-250 KB) and no wave tail
   const char* we = getenv("SSNB_WGRAD_WAVES");
-  int splits = ((we ? atoi(we) : 1) * ctx.num_sms) / ctas;
-  if (splits < 1) splits = 1;
+  int splits = umma_wgrad_splits(ctas, ptiles, ctx.num_sms, we ? atoi(we) : 1);
   if (splits > max_splits) splits = max_splits;
   if (splits > ptiles) splits = ptiles;
   if (splits < 1) splits = 1;
@@ -276,6 +291,7 @@ int umma_wgrad_launch(UmmaContext&, const UmmaWgradPlan& plan, cudaStream_t s, f
   if (!plan.enabled) { set_thread_error("umma wgrad: plan not bound"); return 3; }
   UmmaWgradParams p = plan.p;
   p.bias_partial = bias_partial;
+  t_tag.tiles = p.m_tiles * p.n_tiles * p.tap_groups; t_tag.block_n = p.splits;     // the launch log's grid: ctas x splits
   switch (p.taps_per_cta * (p.block_n / 64)) {
     case 1: return launch_nacc<1>(plan, p, s);
     case 2: return launch_nacc<2>(plan, p, s);

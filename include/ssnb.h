@@ -108,7 +108,8 @@ int ssnb_timing_begin(void* stream);
 const char* ssnb_timing_report(void);
 /* The same session launch by launch, in launch order: "kernel\tphase\top\tms\talgorithmic_flop\ttiles\tblock_n\n" with op the
  * engine's op name ("a+b+c" for a fused sibling launch, "-" for untagged glue) and tiles / block_n the tile count and tile
- * width of a umma_conv_kernel launch (0 otherwise).  Closes the session if it is still open; may follow ssnb_timing_report. */
+ * width of a umma_conv_kernel launch, the CTAs per pixel split and the split count (grid x and y) of a umma_wgrad_kernel
+ * launch (0 otherwise).  Closes the session if it is still open; may follow ssnb_timing_report. */
 const char* ssnb_timing_launches(void);
 /* per-kernel-family launch counters since creation (bench.py's gpu_launches claim) */
 int64_t ssnb_launch_count(ssnb_handle h);
