@@ -124,7 +124,9 @@ struct UmmaWgradParams {
   int taps_per_cta, tap_groups;   // taps sharing one dz tile per CTA (taps_per_cta * block_n <= 256 accumulator columns)
   int stages, stage_bytes;        // pipeline depth / stride
   float* partial;
-  int nseg;                       // 3: SSNB_EXACT_TC, every pixel tile runs (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi)
+  int nseg;                       // 3: SSNB_EXACT_TC, a stage holds the hi and lo planes of dz and x and the consumer issues
+                                  //    (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi) from it; 1: the plain fp16 product
+  int sub_dh, sub_df;             // EXACT_TC stages half a pixel tile: the second half starts sub_dh rows / sub_df frames on
 };
 struct UmmaWgradPlan {
   bool enabled = false;

@@ -3,7 +3,7 @@
 // a TMA box is [64 pixels][64 channels] (128-byte rows, SWIZZLE_128B) and the wgmma descriptors walk
 // it with 8-pixel groups every 1024 B (SBO).
 //
-//   CTA = (co tile of 128, ci tile of block_n <= 256, taps, pixel split); K loop over 64-pixel boxes.
+//   CTA = (co tile of 128, ci tile of block_n <= 256, taps, pixel split); K loop over 64-pixel boxes (EXACT_TC: 32-pixel halves).
 //   warpgroup 0: TMA producer; warpgroups 1, 2: co rows [64 * (wg - 1), +64), one m64nNk16 wgmma per 16 pixels covering
 //   every (tap, 64 input channels) block of the CTA, fp32 accumulators in registers -> split-K partials (reduced in fixed order by wgrad_finalize_kernel).
 #include <cstdio>
@@ -19,19 +19,29 @@ namespace {
 
 using namespace umma;
 constexpr int MAX_STAGES = 8;
-constexpr int BOX_BYTES = 64 * 128;                 // [64 px][64 ch] fp16
-constexpr int A_BYTES = 2 * BOX_BYTES;              // 128 output channels
-constexpr int STAGE_BYTES = A_BYTES + 4 * BOX_BYTES;        // 2 dz boxes + up to 4 x boxes (taps x 64-channel atoms)
-constexpr int STAGES = 4;
-constexpr int PIPE_BYTES = STAGES * STAGE_BYTES;            // 192 KiB of operand staging
+constexpr int BOX_BYTES = 64 * 128;                 // [64 px][64 ch] fp16: one pixel tile of one 64-channel atom
+constexpr int PIPE_BYTES = 192 * 1024;              // operand staging, cut into p.stages stages of p.stage_bytes
 constexpr int NUM_THREADS = 384;
 constexpr int ONES_OFF = PIPE_BYTES + 1024;                // [16 rows][64 px] of fp16 ones (bias-gradient operand), 1 KiB aligned
 constexpr int ONES_BYTES = 16 * 128;
 constexpr int SMEM_BYTES = PIPE_BYTES + 1024 /*align slack*/ + 1024 /*barriers*/ + ONES_BYTES;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory per block");
 
-// NACC = taps_per_cta * block_n / 64 accumulator blocks of 64 columns per consumer warpgroup
-template <int NACC>
+// D[64 co][NACC * 64] += dz^T x over the PX pixels of one stage: one m64n(64 NACC)k16 MMA per 16 pixel rows.  The x boxes of all
+// taps of the CTA are consecutive 64-channel N atoms PX * 128 bytes apart (the LBO), so the dz rows are read from shared memory
+// once per 16 pixels.
+template <int NACC, int PX>
+__device__ __forceinline__ void mma_px(float* acc, uint32_t dz, uint32_t x) {
+#pragma unroll
+  for (int k = 0; k < PX / MMA_K; ++k)
+    wgmma<NACC * MMA_N, 1, 1>(acc, make_desc_sw128(dz + k * (MMA_K * 128), PX * 128), make_desc_sw128(x + k * (MMA_K * 128), PX * 128));
+}
+
+// NACC = taps_per_cta * block_n / 64 accumulator blocks of 64 columns per consumer warpgroup.  NSEG = 3 (SSNB_EXACT_TC): a
+// stage holds the hi and lo planes of dz and x, [dz_hi | dz_lo | x_hi | x_lo], each fetched once, for half a pixel tile (32
+// pixels), so that a stage is no larger than FAST's one-plane stage of a whole tile and the ring keeps 4 to 8 stages: with
+// whole-tile four-plane stages (2 of 96 KiB) the weight gradient of the EXACT_TC step took 13.1 ms instead of 9.7.
+template <int NACC, int NSEG>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_constant__ CUtensorMap tmap_x,
                   const __grid_constant__ CUtensorMap tmap_dz_lo, const __grid_constant__ CUtensorMap tmap_x_lo,
@@ -41,6 +51,10 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + PIPE_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + MAX_STAGES;
+  constexpr int PLANES = NSEG == 3 ? 2 : 1;
+  constexpr int PX = NSEG == 3 ? 32 : 64;            // pixels per stage
+  constexpr int SUB = 64 / PX;                       // stages per pixel tile
+  constexpr int BOX = PX * 128;                      // one staged box: [PX px][64 ch]
 
   const int wg = threadIdx.x / 128;
   int id = blockIdx.x;
@@ -55,6 +69,8 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
   const int pt0 = split * p.ptiles_per_split;
   const int pt1 = min(pt0 + p.ptiles_per_split, ptiles);
   const int nboxes_b = p.block_n / 64;
+  const int nxb = p.taps_per_cta * nboxes_b;          // x box slots of a plane
+  const int x_off = 2 * PLANES * BOX;                 // stage: [dz_hi 2][dz_lo 2][x_hi nxb][x_lo nxb] boxes
   // CTAs of the first input tile / tap group also reduce dz over pixels: db[co] = sum_p dz[p, co] = dz^T * 1
   const bool do_bias = p.bias_partial != nullptr && nt == 0 && tgrp == 0;
 
@@ -77,26 +93,34 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
     producer_regs();
     if (threadIdx.x == 0) {
       uint32_t stage = 0, phase = 0;
-      const uint32_t tx_bytes = (uint32_t)(2 + nboxes_b * ntap) * BOX_BYTES;
       // pixel-tile coordinates advance by carries (no divisions in the loop)
       int tw = pt0 % p.tiles_w, th = (pt0 / p.tiles_w) % p.tiles_h, tf = pt0 / (p.tiles_w * p.tiles_h);
       for (int pt = pt0; pt < pt1; ++pt) {
-        const int w0 = tw * p.bw, h0 = th * p.bh, f0 = tf * p.bf;
-        // SSNB_EXACT_TC (nseg = 3): the tile is staged three times, (dz_lo, x_hi), (dz_hi, x_lo), (dz_hi, x_hi)
-        for (int seg = 3 - p.nseg; seg < 3; ++seg) {
-          const CUtensorMap* mdz = seg == 0 ? &tmap_dz_lo : &tmap_dz;
-          const CUtensorMap* mx = seg == 1 ? &tmap_x_lo : &tmap_x;
+#pragma unroll 1
+        for (int h = 0; h < SUB; ++h) {
+          // a half tile is the lower or upper half of the box in frames (bf > 1) or else in rows
+          const int w0 = tw * p.bw, h0 = th * p.bh + h * p.sub_dh, f0 = tf * p.bf + h * p.sub_df;
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          mbar_expect_tx(&full_bar[stage], tx_bytes);
-          tma_load_4d(sa, mdz, &full_bar[stage], m0, w0, h0, f0);
-          tma_load_4d(sa + BOX_BYTES, mdz, &full_bar[stage], m0 + 64, w0, h0, f0);
-          for (int t = 0; t < ntap; ++t)
-            for (int b = 0; b < nboxes_b; ++b)
-              tma_load_4d(sb + (t * nboxes_b + b) * BOX_BYTES, mx, &full_bar[stage], n0 + b * 64,
-                          w0 * p.x_stride + p.tap_dx[tap0 + t], h0 * p.x_stride + p.tap_dy[tap0 + t], f0);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          uint8_t* st = smem + stage * p.stage_bytes;
+          // the second 64-row dz box of a 128-row co tile lies wholly past Cout when Cout % 128 is in (0, 64]: not fetched
+          // (recomputed per stage: the producer runs on 40 registers)
+          const int ndz = m0 + 64 < p.Cout ? 2 : 1;
+          mbar_expect_tx(&full_bar[stage], (uint32_t)(PLANES * (ndz + nboxes_b * ntap) * BOX));
+#pragma unroll 1
+          for (int b = 0; b < ndz; ++b) {
+            tma_load_4d(st + b * BOX, &tmap_dz, &full_bar[stage], m0 + b * 64, w0, h0, f0);
+            if (NSEG == 3) tma_load_4d(st + (2 + b) * BOX, &tmap_dz_lo, &full_bar[stage], m0 + b * 64, w0, h0, f0);
+          }
+#pragma unroll 1
+          for (int t = 0; t < ntap; ++t) {
+            const int xw = w0 * p.x_stride + p.tap_dx[tap0 + t], xh = h0 * p.x_stride + p.tap_dy[tap0 + t];
+            for (int b = 0; b < nboxes_b; ++b) {
+              uint8_t* dst = st + x_off + (t * nboxes_b + b) * BOX;
+              tma_load_4d(dst, &tmap_x, &full_bar[stage], n0 + b * 64, xw, xh, f0);
+              if (NSEG == 3) tma_load_4d(dst + nxb * BOX, &tmap_x_lo, &full_bar[stage], n0 + b * 64, xw, xh, f0);
+            }
+          }
+          if (++stage == (uint32_t)p.stages) { stage = 0; phase ^= 1; }
         }
         if (++tw == p.tiles_w) { tw = 0; if (++th == p.tiles_h) { th = 0; ++tf; } }
       }
@@ -106,6 +130,18 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
     const int cw = wg - 1;
     const int warp = (threadIdx.x / 32) & 3, lane = threadIdx.x & 31;
     const int nacc = ntap * nboxes_b;                 // accumulator blocks in use (<= NACC)
+    uint32_t stage = 0, phase = 0, prev = 0;
+    const int nstages = (pt1 - pt0) * SUB;
+    if (m0 + cw * 64 >= p.Cout) {
+      // all 64 co rows of this warpgroup lie past Cout: no MMAs (they would multiply zero-filled rows), it only hands the
+      // stages it would have read back to the producer
+      for (int i = 0; i < nstages; ++i) {
+        mbar_wait(&full_bar[stage], phase);
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == (uint32_t)p.stages) { stage = 0; phase ^= 1; }
+      }
+      return;
+    }
     float acc[NACC][32], accb[8];
 #pragma unroll
     for (int j = 0; j < NACC; ++j)
@@ -114,26 +150,25 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
 #pragma unroll
     for (int i = 0; i < 8; ++i) accb[i] = 0.f;
     const uint32_t ones = smem_u32(smem + ONES_OFF);
-    uint32_t stage = 0, phase = 0, prev = 0;
     bool first = true;
-    for (int pt = pt0; pt < pt1; ++pt)
-    for (int seg = 3 - p.nseg; seg < 3; ++seg) {
+    for (int i = 0; i < nstages; ++i) {
       mbar_wait(&full_bar[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * BOX_BYTES;
-      const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
-      // the x boxes of all taps of this CTA are consecutive 64-channel N atoms BOX_BYTES apart (the LBO), so ONE m64n(64 NACC)k16
-      // MMA per 16 pixel rows takes them all and the dz rows are read from shared memory once.  A CTA of a short last tap
-      // group (nacc < NACC) multiplies stale atoms into accumulator blocks it never stores, which keeps the MMA sequence free
-      // of predication.
-      const bool bias_mma = do_bias && seg != 1;     // column sums of dz: hi and lo planes once each (seg 1 re-stages dz_hi)
+      const uint32_t st = smem_u32(smem + stage * p.stage_bytes);
+      const uint32_t dz_hi = st + cw * BOX, x_hi = st + x_off;
+      // A CTA of a short last tap group (nacc < NACC) multiplies stale atoms into accumulator blocks it never stores, which
+      // keeps the MMA sequence free of predication.
       wgmma_fence();
+      if constexpr (NSEG == 3) {                     // small terms first, into the same registers: lo.hi, hi.lo, hi.hi
+        mma_px<NACC, PX>(&acc[0][0], dz_hi + 2 * BOX, x_hi);
+        mma_px<NACC, PX>(&acc[0][0], dz_hi, x_hi + nxb * BOX);
+      }
+      mma_px<NACC, PX>(&acc[0][0], dz_hi, x_hi);
+      if (do_bias) {                                 // column sums of dz (lo plane, then hi); the ones operand is K-major
 #pragma unroll
-      for (int k = 0; k < 64 / MMA_K; ++k)           // 16 pixel rows (2 groups of 8) per instruction
-        wgmma<NACC * MMA_N, 1, 1>(&acc[0][0], make_desc_sw128(sa + k * (MMA_K * 128), BOX_BYTES), make_desc_sw128(sb + k * (MMA_K * 128), BOX_BYTES));
-      if (bias_mma) {                                // the ones operand is K-major
+        for (int q = PLANES - 1; q >= 0; --q)
 #pragma unroll
-        for (int k = 0; k < 64 / MMA_K; ++k)
-          wgmma<16, 1, 0>(accb, make_desc_sw128(sa + k * (MMA_K * 128), BOX_BYTES), make_desc_sw128(ones + k * MMA_K * 2));
+          for (int k = 0; k < PX / MMA_K; ++k)
+            wgmma<16, 1, 0>(accb, make_desc_sw128(dz_hi + q * 2 * BOX + k * (MMA_K * 128), PX * 128), make_desc_sw128(ones + k * MMA_K * 2));
       }
       wgmma_commit();
       // one group stays in flight: the previous stage's MMAs have retired, its smem slot goes back to the producer
@@ -141,7 +176,7 @@ umma_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __grid_cons
       if (!first && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
       first = false;
       prev = stage;
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      if (++stage == (uint32_t)p.stages) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
     if (!first && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
@@ -220,9 +255,8 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   const int chunks = (cin + 63) / 64;
   p.n_tiles = (chunks + 3) / 4;
   p.block_n = ((chunks + p.n_tiles - 1) / p.n_tiles) * 64;
-  // several taps per CTA share one dz tile: stage = 2 dz boxes + taps * (block_n/64) x boxes <= 6 boxes, which also
-  // bounds the register accumulators at 256 fp32 columns
-  p.stage_bytes = STAGE_BYTES; p.stages = STAGES;
+  // several taps per CTA share one dz tile: 2 dz boxes + taps * (block_n/64) <= 4 x boxes per plane, which also bounds the
+  // register accumulators at 256 fp32 columns
   p.taps_per_cta = std::max(1, 4 / (p.block_n / 64));
   if (p.taps_per_cta > ntaps) p.taps_per_cta = ntaps;
   p.tap_groups = (ntaps + p.taps_per_cta - 1) / p.taps_per_cta;
@@ -239,11 +273,17 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   p.partial = partial; p.bias_partial = nullptr;
   p.nseg = (dz.lo_off && x.lo_off) ? 3 : 1;
   if ((dz.lo_off != 0) != (x.lo_off != 0)) { set_thread_error("umma wgrad: both operands or neither must carry LO planes"); return 1; }
+  // a stage holds every operand box of one pixel tile (FAST) or both planes of each box of half a tile (EXACT_TC)
+  const int sub = p.nseg == 3 ? 2 : 1;       // stages per pixel tile: the kernel's SUB
+  const int sub_bh = p.bf > 1 ? p.bh : p.bh / sub, sub_bf = p.bf > 1 ? p.bf / sub : 1;
+  p.sub_dh = sub == 1 ? 0 : p.bh - sub_bh; p.sub_df = sub == 1 ? 0 : p.bf - sub_bf;
+  p.stage_bytes = (p.nseg == 3 ? 2 : 1) * (2 + p.taps_per_cta * (p.block_n / 64)) * BOX_BYTES / sub;
+  p.stages = std::min(PIPE_BYTES / p.stage_bytes, MAX_STAGES);
   auto lo_ptr = [](const View& v) { return reinterpret_cast<__half*>(reinterpret_cast<char*>(v.base) + v.lo_off) + v.coff; };
   {
     cuuint64_t dims[4] = {(cuuint64_t)cout, (cuuint64_t)dz.W, (cuuint64_t)dz.H, (cuuint64_t)F};
     cuuint64_t str[3] = {(cuuint64_t)dz.pitch * 2, (cuuint64_t)dz.W * dz.pitch * 2, (cuuint64_t)dz.H * dz.W * dz.pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)p.bf};
+    cuuint32_t box[4] = {64, (cuuint32_t)p.bw, (cuuint32_t)sub_bh, (cuuint32_t)sub_bf};
     if (int rc = umma_encode_f16(ctx, &plan.tmap_dz, 4, reinterpret_cast<__half*>(dz.base) + dz.coff, dims, str, box)) return rc;
     plan.tmap_dz_lo = plan.tmap_dz;
     if (p.nseg == 3) if (int rc = umma_encode_f16(ctx, &plan.tmap_dz_lo, 4, lo_ptr(dz), dims, str, box)) return rc;
@@ -251,7 +291,7 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
   {
     cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)x.W, (cuuint64_t)x.H, (cuuint64_t)F};
     cuuint64_t str[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.W * x.pitch * 2, (cuuint64_t)x.H * x.W * x.pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)(p.bw * x_stride), (cuuint32_t)(p.bh * x_stride), (cuuint32_t)p.bf};
+    cuuint32_t box[4] = {64, (cuuint32_t)(p.bw * x_stride), (cuuint32_t)(sub_bh * x_stride), (cuuint32_t)sub_bf};
     if (int rc = umma_encode_f16(ctx, &plan.tmap_x, 4, reinterpret_cast<__half*>(x.base) + x.coff, dims, str, box, x_stride)) return rc;
     plan.tmap_x_lo = plan.tmap_x;
     if (p.nseg == 3) if (int rc = umma_encode_f16(ctx, &plan.tmap_x_lo, 4, lo_ptr(x), dims, str, box, x_stride)) return rc;
@@ -261,10 +301,10 @@ int umma_wgrad_bind_taps(UmmaContext& ctx, UmmaWgradPlan& plan, View dz, View x,
 }
 
 namespace {
-template <int NACC>
+template <int NACC, int NSEG>
 int launch_nacc(const UmmaWgradPlan& plan, const UmmaWgradParams& p, cudaStream_t s) {
   static bool attr_set[64] = {};          // function attributes are per device
-  auto kern = umma_wgrad_kernel<NACC>;
+  auto kern = umma_wgrad_kernel<NACC, NSEG>;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
@@ -292,11 +332,15 @@ int umma_wgrad_launch(UmmaContext&, const UmmaWgradPlan& plan, cudaStream_t s, f
   UmmaWgradParams p = plan.p;
   p.bias_partial = bias_partial;
   t_tag.tiles = p.m_tiles * p.n_tiles * p.tap_groups; t_tag.block_n = p.splits;     // the launch log's grid: ctas x splits
-  switch (p.taps_per_cta * (p.block_n / 64)) {
-    case 1: return launch_nacc<1>(plan, p, s);
-    case 2: return launch_nacc<2>(plan, p, s);
-    case 3: return launch_nacc<3>(plan, p, s);
-    case 4: return launch_nacc<4>(plan, p, s);
+  switch (p.taps_per_cta * (p.block_n / 64) * 4 + p.nseg) {
+    case 5: return launch_nacc<1, 1>(plan, p, s);
+    case 9: return launch_nacc<2, 1>(plan, p, s);
+    case 13: return launch_nacc<3, 1>(plan, p, s);
+    case 17: return launch_nacc<4, 1>(plan, p, s);
+    case 7: return launch_nacc<1, 3>(plan, p, s);
+    case 11: return launch_nacc<2, 3>(plan, p, s);
+    case 15: return launch_nacc<3, 3>(plan, p, s);
+    case 19: return launch_nacc<4, 3>(plan, p, s);
   }
   set_thread_error("umma wgrad: unsupported tile width"); return 3;
 }

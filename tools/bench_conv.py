@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-launch times of the tensor-core convolution kernel (umma_conv_kernel) on one H100; prints ONE JSON line.
+"""Per-launch times of the tensor-core kernels (umma_conv_kernel, umma_wgrad_kernel) on one H100; prints ONE JSON line.
 
   python tools/bench_conv.py [--frames 288] [--reps 2] [--table FILE]
 
@@ -10,6 +10,14 @@ width, microseconds, algorithmic TFLOP/s, the epilogue's HBM bytes and the GB/s 
 the same launch: issued MMAs (padding included; EXACT_TC issues three per product) at 989 TFLOP/s dense fp16, and epilogue
 bytes at 3.35 TB/s HBM3 (H100 SXM data sheet, 700 W).  The model's epilogue bytes per output element: EXACT_TC forward 8
 (fp32 + hi + lo planes), data gradient 12 (also the old gradient or the fp32 mask); FAST forward 2, data gradient 4.
+For each umma_wgrad_kernel launch a second table lists op, CTAs, splits, microseconds, algorithmic TFLOP/s, the product
+MMAs the kernel issues (m64nNk16 units of 64 x 64 x 16, padding included: every 128-row co tile issues for each 64-row half
+that holds an output channel, over all block_n columns of all taps of its tap group, stale taps of a short last group
+included; three per product in EXACT_TC) and the bytes its TMA loads move into shared memory (every box of every pixel tile,
+each plane once), next to the model: those MMAs at 989 TFLOP/s.  Not counted: the bias-gradient m64n16k16 MMAs of layers
+whose bias gradient rides on the kernel (per pixel tile, 4 in FAST and 8 in EXACT_TC for each such 64-row half of the CTAs of
+the first ci tile and tap group, a quarter of a unit each), because which layers carry them is decided by the engine's mask
+fusion, not by the plan.  The plan comes from oracle/tile_plan.py, which restates the kernel's planner.
 The table goes to stdout (or FILE); the JSON line carries the totals per precision and pass.  Needs a CUDA device.
 """
 import argparse
@@ -29,6 +37,8 @@ PEAK_F16 = 989e12       # dense fp16 tensor FLOP/s, H100 SXM data sheet
 HBM = 3.35e12           # B/s, H100 SXM data sheet
 EPI_BYTES = {"exact_tc": (8, 12), "fast": (2, 4)}
 PHASES = {0: "fwd", 1: "dgrad"}
+MMA_UNIT = 64 * 64 * 16         # multiply-adds of one 64 x 64 x 16 slice of a wgmma
+BOX_BYTES = 64 * 128            # one [64 px][64 ch] fp16 TMA box
 
 
 def card_info():
@@ -56,6 +66,21 @@ def launch_model(op, phase, flop, tiles, block_n, spec, precision):
     return b, t_mma, b / HBM
 
 
+def wgrad_counts(plan, co, precision):
+    """(issued 64 x 64 x 16 product MMA units, TMA bytes) of one umma_wgrad_kernel launch (tile_plan.wgrad_plan's dict); the
+    bias-gradient MMAs are not included (module docstring)"""
+    nseg, planes = (3, 2) if precision == "exact_tc" else (1, 1)
+    nb, tpc, taps = plan["block_n"] // 64, plan["taps_per_cta"], plan["ntaps"]
+    mma = tma = 0
+    for mt in range(plan["m_tiles"]):
+        halves = sum(1 for h in range(2) if mt * 128 + h * 64 < co)       # 64-row halves holding an output channel
+        for g in range(plan["tap_groups"]):
+            ntap = min(tpc, taps - g * tpc)
+            mma += plan["n_tiles"] * halves * tpc * nb * 4 * nseg          # 4 k-steps of 16 pixels per tile
+            tma += plan["n_tiles"] * planes * (halves + ntap * nb) * BOX_BYTES
+    return mma * plan["ptiles"], tma * plan["ptiles"]
+
+
 def _split(flop, convs):
     w = [ci * co * k * k for (ci, co, k, s) in convs]
     return [flop * x / sum(w) for x in w]
@@ -75,13 +100,14 @@ def main():
     from ssn_b200.engine import BackboneEngine
     from oracle import ssn_oracle as O
     from oracle import synth
+    from oracle import tile_plan as T
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     spec = {n: (ci, co, k, s) for (n, ci, co, k, s, _p) in O.conv_layers(3)}
     bb = synth.synth_backbone(3, seed=0, calib_frames=2)
     x = synth.synth_frames(args.frames, 3, seed=1).to(dev)
     table = open(args.table, "w") if args.table else sys.stdout
-    result = {"metric": "umma_conv_kernel per-launch time, backbone fwd + bwd", "frames": args.frames, "card": card_info(), "modes": {}}
+    result = {"metric": "umma_conv_kernel and umma_wgrad_kernel per-launch time, backbone fwd + bwd", "frames": args.frames, "card": card_info(), "modes": {}}
     names = list(spec)
     for precision, prec in (("exact_tc", _lib.EXACT_TC), ("fast", _lib.FAST_FP16)):
         # the engine is driven from this thread: the timing session is per thread, and autograd would run the backward on
@@ -99,12 +125,16 @@ def main():
             e.backward(g, dw, db)
         step()
         torch.cuda.synchronize()
-        acc = {}
+        acc, wacc = {}, {}
         for _ in range(args.reps):
             _lib.lib.ssnb_timing_begin(C.c_void_p(torch.cuda.current_stream().cuda_stream))
             step()
             for i, ln in enumerate(_lib.lib.ssnb_timing_launches().decode().splitlines()):
                 c = ln.split("\t")
+                if c[0] == "umma_wgrad_kernel":
+                    a = wacc.setdefault((i, c[2]), {"ms": 0.0, "flop": float(c[4]), "ctas": int(c[5]), "splits": int(c[6])})
+                    a["ms"] += float(c[3]) / args.reps
+                    continue
                 if c[0] != "umma_conv_kernel" or int(c[1]) not in PHASES:
                     continue
                 key = (i, c[2], int(c[1]))
@@ -126,6 +156,20 @@ def main():
             if t_mma is not None:
                 t["model_mma_ms"] += t_mma * 1e3; t["model_epi_ms"] += t_epi * 1e3
                 t["model_serial_ms"] += (t_mma + t_epi) * 1e3; t["model_overlap_ms"] += max(t_mma, t_epi) * 1e3
+        plans = {l["op"]: l["plan"] for l in T.schedule(3, args.frames, precision, torch.cuda.get_device_properties(dev).multi_processor_count)
+                 if l["phase"] == 2}
+        print(file=table)
+        print("%-24s %5s %6s %9s %8s %10s %9s %9s %8s" % ("op (wgrad)", "ctas", "splits", "us", "TFLOP/s", "MMAs", "TMA MB", "TMA GB/s",
+                                                          "mdl mma"), file=table)
+        w = tot.setdefault("wgrad", {"launches": 0, "ms": 0.0, "flop": 0.0, "mmas": 0, "tma_bytes": 0.0, "model_mma_ms": 0.0})
+        for (i, op), a in sorted(wacc.items()):
+            mmas, tma = wgrad_counts(plans[op], spec[op][1], precision)
+            s = a["ms"] / 1e3
+            t_mma = 2.0 * mmas * MMA_UNIT / PEAK_F16
+            print("%-24s %5d %6d %9.1f %8.1f %10d %9.1f %9.0f %8.1f" % (op[:24], a["ctas"], a["splits"], s * 1e6, a["flop"] / s / 1e12, mmas,
+                                                                    tma / 1e6, tma / s / 1e9, t_mma * 1e6), file=table)
+            w["launches"] += 1; w["ms"] += a["ms"]; w["flop"] += a["flop"]; w["mmas"] += mmas; w["tma_bytes"] += tma
+            w["model_mma_ms"] += t_mma * 1e3
         for t in tot.values():
             t["tflops"] = t["flop"] / (t["ms"] / 1e3) / 1e12
         print(file=table)
