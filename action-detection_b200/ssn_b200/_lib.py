@@ -59,6 +59,16 @@ class FrameGroup(C.Structure):
 
 FRAMES_TRAIN, FRAMES_OVERSAMPLE, FRAMES_CENTER = 0, 1, 2
 
+
+class ProposalTargetsCfg(C.Structure):
+    _fields_ = [("fg_thresh", C.c_double), ("incomplete_iou_thresh", C.c_double), ("bg_iou_thresh", C.c_double),
+                ("bg_coverage_thresh", C.c_double), ("incomplete_overlap_thresh", C.c_double), ("exclude_empty", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+PROPFRAMES_SECONDS, PROPFRAMES_NORMALISED, PROPFRAMES_AS_GIVEN = 0, 1, 2
+TAG_FG, TAG_INCOMPLETE, TAG_BACKGROUND = 1, 2, 4
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 _pp = C.POINTER(C.c_void_p)
@@ -120,6 +130,14 @@ SIGNATURES = {
     "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
     "ssnb_tag_proposals": (_i, [C.POINTER(TagProposalsCfg), _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp] + [_vp] * 10
                            + [_sz, _vp]),
+    "ssnb_name_proposals": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp, C.c_double, _vp, _vp, _vp, _vp, _vp]),
+    "ssnb_proposal_recall": (_i, [_vp, C.POINTER(C.c_int64), _vp, _i, C.POINTER(C.c_double), _i, _vp, _vp, _vp]),
+    "ssnb_sliding_windows": (_i, [_vp, _i, C.POINTER(C.c_double), C.POINTER(C.c_double), _i, C.c_int64, C.c_int64, _vp, _vp, _vp, _vp,
+                                  _vp, _vp]),
+    "ssnb_proposal_frames": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
+    "ssnb_proposal_targets_workspace_bytes": (_sz, [_i]),
+    "ssnb_proposal_targets": (_i, [C.POINTER(ProposalTargetsCfg)] + [_vp] * 6 + [_i, _vp, C.POINTER(C.c_int64)] + [_vp] * 7 + [_sz, _vp]),
+    "ssnb_test_proposals": (_i, [_vp, _vp, _vp, _vp, _i, C.c_int64, _vp, _i, _i] + [_vp] * 7),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
     "ssnb_sgd_step": (_i, [_vp, _vp, _vp, _sz, _f, _f, _f, _f, _vp]),

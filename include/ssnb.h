@@ -319,6 +319,89 @@ int ssnb_tag_proposals(const ssnb_tag_proposals_cfg* cfg, const float* f_score, 
                        uint32_t* labels, int32_t* raw_frames, float* raw_scores, int32_t* raw_counts, void* workspace,
                        size_t workspace_bytes, void* stream);
 
+/* ---- proposal lists: labelling proposals against ground truth, recall, sliding windows, frame windows, the SSN data set's
+ *      training targets and test-time proposal inputs, many ragged videos per call (csrc/proposal_lists.cu) ------------------
+ * Packed layout shared by the calls below.  Proposals: boxes double [rows, 2] (start, end) with device first int64 [V] and
+ * count int32 [V]: video v owns rows first[v] .. first[v] + count[v] - 1.  That is the seconds / slot0 / counts of
+ * ssnb_tag_proposals read in place; a compact [sum N, 2] array is the case first = exclusive cumsum of count.  Per-row
+ * outputs are written at the row's own index; rows outside every video are not touched.  Ground truth: gt double [sum G, 2],
+ * gt_label int32 [sum G], video v's rows gt_offsets[v] .. gt_offsets[v+1]-1 (int64 [V+1], gt_offsets[0] = 0, ascending;
+ * HOST memory, validated; gt_offsets_dev is the device copy the kernels read).  max_count: a bound of count[v] known to the
+ * host that sizes the grid only -- any value >= 0 gives the same result.  No cap on N_v or G_v; V = 0, N_v = 0 and G_v = 0
+ * are valid.  Every call enqueues kernels and memsets only: no host synchronisation, allocation or host copy, so it can be
+ * captured in a CUDA graph.
+ *
+ * ssnb_name_proposals: name_proposal (ops/detection_metrics.py:54-76) of every proposal: label = gt_label + 1, max_overlap =
+ * temporal_iou (:7-20), overlap_self = overlap_over_b (:23-28) of the ground truth selected by `ov > thresh and ov >
+ * max_overlap` in ground-truth order (the first of equal overlaps; NaN never); 0 / 0 / 0 when none.  Bitwise the reference's
+ * doubles (Python min / max, one IEEE division).  gt_best double [sum G]: per ground truth the maximum tIoU over its video's
+ * proposals (0 without an overlapping one; NaN overlaps ignored), which answers temporal_recall (:31-51) at every threshold. */
+int ssnb_name_proposals(const double* boxes, const int64_t* first, const int32_t* count, int n_videos, int64_t max_count, const double* gt,
+                        const int32_t* gt_label, const int64_t* gt_offsets, const int64_t* gt_offsets_dev, double thresh, int32_t* label,
+                        double* max_overlap, double* overlap_self, double* gt_best, void* stream);
+/* get_temporal_proposal_recall (ops/detection_metrics.py:79-83) for n_thresholds (1..32, HOST) thresholds at once: hits int32
+ * [V, n_thresholds] = ground truth of video v with gt_best > threshold; totals int64 [2 * n_thresholds + 1] = per threshold
+ * the videos with hits == G_v (G_v = 0 counts, as 0 == 0 does), then per threshold the sum of hits, then sum G. */
+int ssnb_proposal_recall(const double* gt_best, const int64_t* gt_offsets, const int64_t* gt_offsets_dev, int n_videos, const double* thresholds,
+                         int n_thresholds, int32_t* hits, int64_t* totals, void* stream);
+/* gen_exponential_sw_proposal (ops/sequence_funcs.py:37-54) for V durations (device double [V]).  Level l (1..32 levels; HOST
+ * arrays): boxes (k * steps[l], k * steps[l] + t_spans[l]) for k * steps[l] < duration, kept when min(duration, end) - start
+ * >= 1; level-major, start ascending.  steps[l] = int(ceil(t_spans[l] * time_step * (1 - overlap))) is the caller's (an integer
+ * >= 1); the end uses t_span, not the span in seconds, as the reference does.  A duration that is not positive and finite has
+ * no windows.  Writes count [V], first [V] (exclusive cumsum), level_count int32 [V, n_levels], total int64 [1], and the boxes
+ * double [capacity, 2] (rows at or past capacity are dropped: compare total; capacity 0 only counts). */
+int ssnb_sliding_windows(const double* durations, int n_videos, const double* t_spans, const double* steps, int n_levels, int64_t max_count,
+                         int64_t capacity, double* boxes, int64_t* first, int32_t* count, int32_t* level_count, int64_t* total, void* stream);
+/* Frame windows.  SECONDS: dump_window_list (ops/io.py:109-127), int(x * real_fps) with real_fps = float(frame_cnt) /
+ * float(duration); NORMALISED: process_proposal_list (ops/io.py:44-47), int(float(x) * frame_cnt); AS_GIVEN: x holds frame
+ * integers already (a parsed list).  int() truncates toward zero; a product outside int64 saturates and NaN gives 0 (the
+ * reference raises).  frames int64 [rows, 2]: what the list file holds.  Optional (NULL: not written), SSNVideoRecord's rules
+ * (ssn_dataset.py:13-21,81-93): keep uint8 = end > start and start < frame_cnt; valid int64 [rows, 2] = (start, min(end,
+ * frame_cnt)); coverage double = (end - start) / frame_cnt with the unclipped end.  Ground truth goes through the same call
+ * with first = gt_offsets[:-1] and count = their differences. */
+enum { SSNB_PROPFRAMES_SECONDS = 0, SSNB_PROPFRAMES_NORMALISED = 1, SSNB_PROPFRAMES_AS_GIVEN = 2 };
+int ssnb_proposal_frames(const double* boxes, const int64_t* first, const int32_t* count, int n_videos, int64_t max_count, const double* durations,
+                         const int32_t* frame_cnt, int mode, int64_t* frames, int64_t* valid, double* coverage, uint8_t* keep, void* stream);
+/* What SSNDataSet._parse_prop_file derives (ssn_dataset.py:29-55,103-131,196-227,382-391) from kept rows only (valid frames,
+ * coverage, and best_iou / overlap_self as the caller chooses to pass them: the list's 4-decimal values or fresh ones):
+ *   tags uint8 [rows]: SSNB_TAG_FG best_iou > fg_thresh; SSNB_TAG_INCOMPLETE best_iou < incomplete_iou_thresh and overlap_self >
+ *     incomplete_overlap_thresh; SSNB_TAG_BACKGROUND not incomplete and best_iou < bg_iou_thresh and coverage >
+ *     bg_coverage_thresh (a row may be fg and incomplete, as the reference's two lists may both hold it);
+ *   reg double [rows, 2]: (loc_reg, size_reg) of every fg row against the first ground truth of maximum frame tIoU
+ *     (ops/utils.py:40-53, np.argmax), (0, 0) elsewhere.  The reference computes targets for the members of the fg list only,
+ *     so a row with best_iou == fg_thresh has none.  loc_reg is bitwise; size_reg is CUDA's double log;
+ *   pool_counts int32 [V, 4]: fg, incomplete, background proposals and ground truth of the video; totals int64 [5]: their sums
+ *     and the number of videos used; exclude_empty drops videos without ground truth from everything (tags 0), as the data
+ *     set does.  Without exclude_empty an fg row of a video without ground truth gets (0, 0) (np.argmax raises there);
+ *   stats double [4]: np.mean and np.std (population) of the fg rows' targets (mean loc, mean size, std loc, std size), summed
+ *     per video and then over the videos in a fixed order (repeatable to the bit; NaN when there is no fg row).
+ * gt_frames int64 [sum G, 2]: the kept ground truth's valid frames. */
+enum { SSNB_TAG_FG = 1, SSNB_TAG_INCOMPLETE = 2, SSNB_TAG_BACKGROUND = 4 };
+typedef struct {
+  double fg_thresh;                 /* fg_iou_thresh (0.7) */
+  double incomplete_iou_thresh;     /* 0.3 */
+  double bg_iou_thresh;             /* 0.01 */
+  double bg_coverage_thresh;        /* 0.02 */
+  double incomplete_overlap_thresh; /* 0.7 */
+  int32_t exclude_empty;            /* 1 */
+  int32_t reserved;
+} ssnb_proposal_targets_cfg;
+size_t ssnb_proposal_targets_workspace_bytes(int n_videos);
+int ssnb_proposal_targets(const ssnb_proposal_targets_cfg* cfg, const int64_t* frames, const double* best_iou, const double* overlap_self,
+                          const double* coverage, const int64_t* first, const int32_t* count, int n_videos, const int64_t* gt_frames,
+                          const int64_t* gt_offsets, const int64_t* gt_offsets_dev, uint8_t* tags, double* reg, int32_t* pool_counts,
+                          int64_t* totals, double* stats, void* workspace, size_t workspace_bytes, void* stream);
+/* get_test_data's proposal half (ssn_dataset.py:393-428) from kept rows' valid frames.  num_ticks int32 [V] =
+ * len(np.arange(0, frame_cnt - new_length, test_interval)).  Video v's output rows start at out_first[v] (device int64 [V];
+ * a video without proposals owns one row, the reference's fallback proposal (0, frame_cnt - 1), so out_first is the exclusive
+ * cumsum of max(count, 1)): rel_prop double [rows, 2], ticks int64 [rows, 4], scaling double [rows, 2], bitwise the
+ * reference's, each operation rounded on its own.  Optional ticks32 int32 [rows, 4] / scaling32 float [rows, 2]: the same
+ * values in the types ssnb_stpp_reorg and ssnb_stpp_reorg_prefix take.  A zero-length fallback (frame_cnt 1) divides by zero
+ * where the reference raises. */
+int ssnb_test_proposals(const int64_t* frames, const int64_t* first, const int32_t* count, const int64_t* out_first, int n_videos,
+                        int64_t max_count, const int32_t* frame_cnt, int new_length, int test_interval, int32_t* num_ticks, double* rel_prop,
+                        int64_t* ticks, double* scaling, int32_t* ticks32, float* scaling32, void* stream);
+
 /* ---- frame transforms: the PIL group transforms of the data pipeline (transforms.py:41-206) followed by Stack(roll=True),
  *      ToTorchFormatTensor(div=False) and GroupNormalize (transforms.py:67-80,256-288), bitwise equal to PIL 8-bit BILINEAR --
  * Modes (cfg->mode):
