@@ -18,4 +18,12 @@ __device__ __forceinline__ float key_score(uint32_t key) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
 
+// score_key for a double score (proposal_ar.cu): the same rule on 64 bits.  Every NaN gets key 0, -0 and +0 share a key.
+__device__ __forceinline__ uint64_t score_key64(double s) {
+  if (s != s) return 0ull;
+  uint64_t u = (uint64_t)__double_as_longlong(s == 0.0 ? 0.0 : s);
+  u = (u & 0x8000000000000000ull) ? ~u : (u | 0x8000000000000000ull);
+  return ~u;
+}
+
 }  // namespace ssnb

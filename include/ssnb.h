@@ -402,6 +402,33 @@ int ssnb_test_proposals(const int64_t* frames, const int64_t* first, const int32
                         int64_t max_count, const int32_t* frame_cnt, int new_length, int test_interval, int32_t* num_ticks, double* rel_prop,
                         int64_t* ticks, double* scaling, int32_t* ticks32, float* scaling32, void* stream);
 
+/* ---- ActivityNet proposal evaluation: average recall against the average number of proposals per video (AR-AN) of
+ *      anet_toolkit/Evaluation/eval_proposal.py:158-273 (segment_iou, utils.py:25-75), every video and threshold in one call
+ *      (csrc/proposal_ar.cu) ------------------------------------------------------------------------------------------------
+ * Proposals in the packed layout above: boxes double [rows, 2] (t0, t1) and scores double [rows], video v's rows first[v] ..
+ * first[v] + count[v] - 1 (device int64 / int32 [n_videos]).  Ground truth gt_seg double [sum G, 2], video v's instances
+ * gt_offsets[v] .. gt_offsets[v+1]-1 (int64 [n_videos + 1], HOST memory, validated; gt_offsets_dev is the device copy).  The
+ * evaluated videos are those with G_v > 0, in packed order (V of them); a video with G_v = 0 adds its count to P_all only,
+ * which is how proposals of videos outside the ground truth are passed.  Per evaluated video: the proposals ranked by the
+ * toolkit's score.argsort()[::-1] (NaN first, then descending score with -0 == +0, ties by descending row), the first
+ * nr_v = min(int(P_v * ratio), P_v) kept, ratio = max_avg * V / P_all in double, max_avg <= 0 meaning P_all / V; a video
+ * without proposals has one phantom column of tIoU 0.0.  tIoU is segment_iou with NaN-propagating max / min / clip (a 0 / 0
+ * union is NaN and matches nothing); an instance is matched at (t, j) when one of the first min(int(P'_v * pcn_j), P'_v)
+ * columns has tIoU >= thresholds[t], pcn_j = (j / 100.0) * (max_avg * V / total_nr), j = 1..100.
+ * thresholds: HOST double [n_thresholds], 1..64, not NaN; max_avg finite.  Outputs (device): recall double [n_thr, 100],
+ * avg_recall double [100] (recall summed over the thresholds in order, then / n_thr), proposals_per_video double [100]
+ * (pcn_j * (total_nr / V)), total_nr int64 [1]; all bitwise the toolkit's.  total_nr == 0 (the toolkit divides by zero):
+ * the three curves are NaN.  Optional traces (NULL: kept in the workspace): nr int32 [n_videos] (nr_v, 0 for videos without
+ * ground truth or proposals) and first_hit int32 [sum G, n_thr] (the first column with tIoU >= threshold, INT_MAX: none).
+ * rows <= INT_MAX and sum G <= INT_MAX / 64.  Kernels and memsets only: no host synchronisation, allocation or host copy, so
+ * the call can be captured in a CUDA graph.  The workspace (about 24 bytes per row plus 4 (n_thr + 1) per instance) is 0 for
+ * arguments ssnb_proposal_ar would reject. */
+size_t ssnb_proposal_ar_workspace_bytes(int n_videos, int64_t rows, const int64_t* gt_offsets, int n_thresholds);
+int ssnb_proposal_ar(const double* boxes, const double* scores, int64_t rows, const int64_t* first, const int32_t* count, int n_videos,
+                     const double* gt_seg, const int64_t* gt_offsets, const int64_t* gt_offsets_dev, const double* thresholds,
+                     int n_thresholds, double max_avg, double* recall, double* avg_recall, double* proposals_per_video,
+                     int64_t* total_nr, int32_t* nr, int32_t* first_hit, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- frame transforms: the PIL group transforms of the data pipeline (transforms.py:41-206) followed by Stack(roll=True),
  *      ToTorchFormatTensor(div=False) and GroupNormalize (transforms.py:67-80,256-288), bitwise equal to PIL 8-bit BILINEAR --
  * Modes (cfg->mode):
