@@ -184,16 +184,16 @@ int launch_pool_mask_bias_vec(View dz, View y, View dpool, View planes, float sc
 // `flag` (device int, may be null) is set to 1 when |x * scale| exceeds the fp16 range (loss-scale overflow)
 int launch_split_view(View src_f32, int F, float scale, View planes, int* flag, cudaStream_t s);
 int launch_planes_to_nchw(View planes, int F, float scale, float* dst, cudaStream_t s);
-int launch_nhwc_to_s2d_split(View src_f32, int F, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);
-int launch_nchw_to_s2d_split(const float* src, int F, int Cin, int H, int W, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s);
 // training-mode BatchNorm + ReLU of the first layer (bn_train.cu); stat: 4*C floats, partial: max_ctas * 2 * C floats
 int launch_bn_train_fwd(View z, View y, View y_planes, int F, const float* gamma, const float* beta, float eps, float momentum, float* running_mean,
                         float* running_var, float* stat, float* partial, int max_ctas, cudaStream_t s);
 int launch_bn_train_bwd(View z, View dy, View y, View dz, View dz_planes, float plane_scale, int* flag, int F, const float* gamma, float* stat,
                         float* partial, int max_ctas, float* dgamma, float* dbeta, const float* unscale, int accumulate, cudaStream_t s);
-// FAST-mode layout helpers (s2d_glue.cu)
-int launch_nhwc_to_s2d(View src, int F, __half* dst, int Cs, cudaStream_t s);
-int launch_nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, int Cs, cudaStream_t s);
+// tensor-core layout helpers (s2d_glue.cu).  conv1's packed space-to-depth operand from an NHWC view or NCHW fp32 frames:
+// lo_off == 0 (FAST) writes fp16 values (the NHWC view holds fp16); lo_off != 0 (EXACT_TC) writes the hi plane at dst and
+// the lo plane lo_off bytes after it (the NHWC view holds fp32)
+int launch_nhwc_to_s2d(View src, int F, __half* dst, long long lo_off, int Cs, cudaStream_t s);
+int launch_nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, long long lo_off, int Cs, cudaStream_t s);
 int launch_pack_conv1_s2d(const __half* wd, int Cout, int Cin, int Cs, __half* ws, cudaStream_t s);
 int launch_wgrad_finalize_s2d(const float* partial, int splits, int Cout, int Cin, int Cs, const float* mult, float out_scale,
                               const float* unscale, float* dw_ref, int accumulate, cudaStream_t s);

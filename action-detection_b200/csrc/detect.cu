@@ -358,8 +358,6 @@ using namespace ssnb;
 
 extern "C" {
 
-size_t ssnb_detect_workspace_bytes(int n_props, int num_class) { return (size_t)(n_props > 0 ? n_props : 0) * (num_class > 0 ? num_class : 0) * sizeof(float); }
-
 int ssnb_detect_postprocess(const float* rel_props, const float* act_scores, const float* comp_scores, const float* reg_scores, int n_props,
                             int num_class, double nms_thresh, int regress, float* detections, int* counts, float* combined_ws, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;

@@ -504,8 +504,7 @@ static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* 
     if (o.conv == 0 && !e->s2d_ready) {
       const View in = e->view(o.in_val, false);
       __half* s2d = (__half*)(e->ws + e->s2d_off);
-      if (int rc = e->exact_tc() ? launch_nhwc_to_s2d_split(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s) : launch_nhwc_to_s2d(in, e->F, s2d, e->Cs, s))
-        return rc;
+      if (int rc = launch_nhwc_to_s2d(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s)) return rc;
     }
     tag_next(0, conv_flops(e, o), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma, s);
@@ -1023,8 +1022,7 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
   const View d = h->view(h->val_by_name["data"], false);
   int rc;
   h->s2d_ready = h->tensor_cores() && h->ops[0].umma.enabled;
-  if (h->s2d_ready && h->exact_tc()) rc = launch_nchw_to_s2d_split(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
-  else if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), h->Cs, s);
+  if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
   else rc = h->fast() ? launch_nchw_to_nhwc<__half>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s)
                     : launch_nchw_to_nhwc<float>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s);
   if (rc) { h->s2d_ready = false; return h->fail(rc, "input layout: " + ssnb::thread_error()); }

@@ -266,38 +266,6 @@ __device__ __forceinline__ int reorg_tick(int left, double step, int q) {
   return (int)__dadd_rn(l, __dmul_rn((double)q, __dsub_rn(t1, l)));
 }
 
-__device__ void pspool_dev(const float* __restrict__ scores, int T, int D, int col0, int score_len, const int* tk,
-                           float s0, float s1, const ReorgCfg& cfg, float* __restrict__ out) {
-  // threads stride over the score_len output columns
-  for (int j = threadIdx.x; j < score_len; j += blockDim.x) {
-    float acc = 0.f;
-    int offset = 0;
-    for (int si = 0; si < 3; ++si) {
-      const float s = si == 0 ? s0 : (si == 2 ? s1 : 1.0f);
-      const int left = tk[si];
-      const int right = max(tk[si] + 1, tk[si + 1]);
-      if (right <= 0 || left >= T) { offset += cfg.cnt[si]; continue; }
-      for (int l = 0; l < cfg.nlev[si]; ++l) {
-        const int np_ = cfg.lev[si][l];
-        const double step = (double)(right - left) / (double)np_;
-        for (int q = 0; q < np_; ++q) {
-          const int pl = reorg_tick(left, step, q);
-          const int pr = reorg_tick(left, step, q + 1);
-          if (pr - pl >= 1) {
-            int a, b;
-            py_slice(pl, pr, T, a, b);
-            float sum = 0.f;
-            for (int r = a; r < b; ++r) sum += scores[(long long)r * D + col0 + offset * score_len + j];
-            acc += (sum / (float)(b - a)) * s;
-          }
-          ++offset;
-        }
-      }
-    }
-    out[j] = acc;
-  }
-}
-
 // ---- STPPReorgainzed through column prefix sums ---------------------------------------------------------------------------
 // Every pooled part is a mean over a contiguous row range of the [T, D] score table, and the 1000 proposals of a video overlap
 // heavily: one exclusive scan down the rows (fp64, so that P[b] - P[a] is exact to fp32 rounding of the part's own sum), then
@@ -359,27 +327,6 @@ __global__ void stpp_reorg_prefix_kernel(const double* __restrict__ P, int T, in
   }
   pspool_prefix_dev(P, T, D, act_len, comp_len, tk, s0, s1, cfg, out_comp + (long long)i * comp_len);
   pspool_prefix_dev(P, T, D, act_len + comp_len * mult, reg_len, tk, s0, s1, cfg, out_reg + (long long)i * reg_len);
-}
-
-__global__ void stpp_reorg_kernel(const float* __restrict__ scores, int T, int D, const int32_t* __restrict__ ticks,
-                                  const float* __restrict__ scaling, int N, int act_len, int comp_len, int reg_len,
-                                  ReorgCfg cfg, int mult, float* __restrict__ out_act, float* __restrict__ out_comp,
-                                  float* __restrict__ out_reg) {
-  const int i = blockIdx.x;
-  if (i >= N) return;
-  int tk[4] = {ticks[i * 4], ticks[i * 4 + 1], ticks[i * 4 + 2], ticks[i * 4 + 3]};
-  const float s0 = scaling[i * 2], s1 = scaling[i * 2 + 1];
-  {  // activity: mean of rows [t1, max(t1+1, t2)) of the first act_len columns
-    int a, b;
-    py_slice(tk[1], max(tk[1] + 1, tk[2]), T, a, b);
-    for (int j = threadIdx.x; j < act_len; j += blockDim.x) {
-      float sum = 0.f;
-      for (int r = a; r < b; ++r) sum += scores[(long long)r * D + j];
-      out_act[(long long)i * act_len + j] = sum / (float)(b - a);
-    }
-  }
-  pspool_dev(scores, T, D, act_len, comp_len, tk, s0, s1, cfg, out_comp + (long long)i * comp_len);
-  pspool_dev(scores, T, D, act_len + comp_len * mult, reg_len, tk, s0, s1, cfg, out_reg + (long long)i * reg_len);
 }
 
 // ---- linear ---------------------------------------------------------------------------------------
@@ -780,16 +727,6 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
     }
 }
 
-__global__ void sgd_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf, size_t n,
-                           float lr, float mom, float wd, float gm) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float gr = g[i] * gm + wd * p[i];
-  float b = mom * buf[i] + gr;
-  buf[i] = b;
-  p[i] -= lr * b;
-}
-
 // one launch for the whole model: the flat buffer is cut into segments (one per parameter tensor) carrying their group's
 // learning rate and weight decay (ssn_train.py:391-398 lr_mult / decay_mult); the segment of an element is found by
 // binary search over the cumulative ends staged in shared memory
@@ -915,27 +852,6 @@ int ssnb_gpool_stpp_fwd(ssnb_handle h, const float* drop_mask, const float* scal
   if (fp16) gpool_stpp_kernel<__half><<<(unsigned)((tot + 127) / 128), 128, 0, s>>>((const __half*)v.base, v.H * v.W, v.C, v.pitch, v.coff, n, n_seg, drop_mask, scaling, pt, feat, course_ft, stpp_ft);
   else gpool_stpp_kernel<float><<<(unsigned)((tot + 127) / 128), 128, 0, s>>>((const float*)v.base, v.H * v.W, v.C, v.pitch, v.coff, n, n_seg, drop_mask, scaling, pt, feat, course_ft, stpp_ft);
   SSNB_LAUNCH_CHECK("gpool_stpp_kernel");
-  return SSNB_OK;
-}
-
-int ssnb_stpp_reorg(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N, int act_len,
-                    int comp_len, int reg_len, const int* level_counts, const int* levels, float* out_act,
-                    float* out_comp, float* out_reg, void* stream) {
-  cudaStream_t s = (cudaStream_t)stream;
-  if (!scores || !ticks || !scaling || !out_act || !out_comp || !out_reg || T <= 0) { set_thread_error("stpp_reorg: bad argument"); return SSNB_EINVAL; }
-  ReorgCfg cfg; memset(&cfg, 0, sizeof(cfg));
-  cfg.nstage = 3;
-  int q = 0, mult = 0;
-  for (int s = 0; s < 3; ++s) {
-    if (level_counts[s] < 1 || level_counts[s] > 8) { set_thread_error("stpp_reorg: 1..8 pyramid levels per stage"); return SSNB_EINVAL; }
-    cfg.nlev[s] = level_counts[s];
-    for (int l = 0; l < level_counts[s]; ++l) { cfg.lev[s][l] = levels[q++]; cfg.cnt[s] += cfg.lev[s][l]; }
-    mult += cfg.cnt[s];
-  }
-  if (D != act_len + mult * (comp_len + reg_len)) { set_thread_error("stpp_reorg: D does not match act+M*(comp+reg)"); return SSNB_EINVAL; }
-  if (N == 0) return SSNB_OK;
-  stpp_reorg_kernel<<<N, 128, 0, s>>>(scores, T, D, ticks, scaling, N, act_len, comp_len, reg_len, cfg, mult, out_act, out_comp, out_reg);
-  SSNB_LAUNCH_CHECK("stpp_reorg_kernel");
   return SSNB_OK;
 }
 
@@ -1086,16 +1002,6 @@ int ssnb_heads_loss_fwd_bwd(const ssnb_heads_cfg* cfg, const float* course_ft, c
   if (cudaLaunchCooperativeKernel((const void*)heads_loss_kernel, dim3(slices), dim3(HL_THREADS), kargs, 0, s) != cudaSuccess) {
     set_thread_error(std::string("heads_loss_kernel cooperative launch: ") + cudaGetErrorString(cudaGetLastError())); return SSNB_ECUDA; }
   SSNB_LAUNCH_CHECK("heads_loss_kernel");
-  return SSNB_OK;
-}
-
-int ssnb_sgd_step(float* param, const float* grad, float* momentum_buf, size_t n, float lr, float momentum, float weight_decay,
-                  float grad_mult, void* stream) {
-  cudaStream_t s = (cudaStream_t)stream;
-  if (!param || !grad || !momentum_buf) { set_thread_error("sgd: null"); return SSNB_EINVAL; }
-  if (n == 0) return SSNB_OK;
-  sgd_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(param, grad, momentum_buf, n, lr, momentum, weight_decay, grad_mult);
-  SSNB_LAUNCH_CHECK("sgd_kernel");
   return SSNB_OK;
 }
 

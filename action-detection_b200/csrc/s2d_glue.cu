@@ -1,8 +1,10 @@
-// FAST-mode helpers that let every convolution of BNInception run on the stride-1 tensor-core kernels:
+// Layout helpers (FAST and EXACT_TC) that let every convolution of BNInception run on the stride-1 tensor-core kernels:
 //  * conv1 (7x7 stride 2 pad 3, bn_inception.yaml:3-5) as a 4x4 stride-1 convolution over the
 //    space-to-depth input  xs[f, i, j, (a*2+b)*Cin + c] = x[f, 2i+a, 2j+b, c]   (r = 2*dr + a - 1)
 //  * stride-2 3x3 layers (inception_3c/4e): backward through a zero-upsampled output gradient.
 #include "common.cuh"
+
+#include <type_traits>
 
 namespace ssnb {
 namespace {
@@ -11,8 +13,10 @@ namespace {
 //   x[f, 2*i + a, 2*(j + ds - 2) + b, c]      (zero outside the image / for the pad channels)
 // so the 7x7/2 convolution becomes FOUR vertical taps (dr = 0..3, dy = dr - 2) with K = 4*Cs each:
 //   r = 2*dr + a - 1,  s = 2*ds + b - 1.
-__global__ void nhwc_to_s2d_kernel(const __half* __restrict__ src, int F, int H, int W, int Cin, int spitch, int scoff,
-                                   __half* __restrict__ dst, int Cs) {
+// T = __half (FAST) copies the value; T = float (EXACT_TC) writes its hi plane at dst and its lo plane lo_off bytes further
+template <typename T>
+__global__ void nhwc_to_s2d_kernel(const T* __restrict__ src, int F, int H, int W, int Cin, int spitch, int scoff,
+                                   __half* __restrict__ dst, long long lo_off, int Cs) {
   const int H2 = H / 2, W2 = W / 2, Ck = 4 * Cs;
   const long long total = (long long)F * H2 * W2 * Ck;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -22,13 +26,19 @@ __global__ void nhwc_to_s2d_kernel(const __half* __restrict__ src, int F, int H,
   const int x2 = (int)(p % W2), y2 = (int)((p / W2) % H2);
   const long long f = p / ((long long)W2 * H2);
   const int ds = ch / Cs, q = ch % Cs;
-  __half v = __float2half_rn(0.f);
+  T v = 0.f;
   const int xs = x2 + ds - 2;
   if (q < 4 * Cin && xs >= 0 && xs < W2) {
     const int ab = q / Cin, c = q % Cin;
     v = src[((f * H + 2 * y2 + ab / 2) * W + 2 * xs + ab % 2) * spitch + scoff + c];
   }
-  dst[i] = v;
+  if constexpr (std::is_same_v<T, float>) {
+    const __half h = __float2half_rn(v);
+    dst[i] = h;
+    *reinterpret_cast<__half*>(reinterpret_cast<char*>(dst + i) + lo_off) = __float2half_rn(v - __half2float(h));
+  } else {
+    dst[i] = v;
+  }
 }
 
 // ws[dr][co][ds*Cs + (a*2+b)*Cin + c] = wd[(r*7+s)][co][c],  r = 2*dr+a-1, s = 2*ds+b-1 (0 outside 0..6)
@@ -70,9 +80,11 @@ __global__ void wgrad_finalize_s2d_kernel(const float* __restrict__ partial, int
 
 // fused input conversion: NCHW fp32 frames -> packed space-to-depth fp16; one thread per (pixel, ds block):
 // float2 reads coalesced along x, the Cs-channel block is assembled in registers and stored as 16-byte vectors
-// CIN > 0: compile-time channel count (RGB 3 / Flow 10): the channel loop unrolls and the staging array stays in registers
-template <int CS, int CIN>
-__global__ void nchw_to_s2d_kernel(const float* __restrict__ src, int F, int Cin_rt, int H, int W, __half* __restrict__ dst) {
+// CIN > 0: compile-time channel count (RGB 3 / Flow 10): the channel loop unrolls and the staging arrays stay in registers
+// LO (EXACT_TC): also writes the lo plane, lo_off bytes after the hi plane
+template <int CS, int CIN, bool LO>
+__global__ void nchw_to_s2d_kernel(const float* __restrict__ src, int F, int Cin_rt, int H, int W, __half* __restrict__ dst,
+                                   long long lo_off) {
   const int Cin = CIN ? CIN : Cin_rt;
   const int H2 = H / 2, W2 = W / 2;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -83,9 +95,13 @@ __global__ void nchw_to_s2d_kernel(const float* __restrict__ src, int F, int Cin
   const int x2 = (int)(pu % (unsigned)W2), y2 = (int)((pu / (unsigned)W2) % (unsigned)H2);
   const long long p = pu;
   const long long f = pu / (unsigned)(W2 * H2);
-  __align__(16) __half v[CS];
+  __align__(16) __half vh[CS];
+  __align__(16) __half vl[LO ? CS : 1];
 #pragma unroll
-  for (int c = 0; c < CS; ++c) v[c] = __float2half_rn(0.f);
+  for (int c = 0; c < CS; ++c) {
+    vh[c] = __float2half_rn(0.f);
+    if constexpr (LO) vl[c] = __float2half_rn(0.f);
+  }
   const int xs = x2 + ds - 2;
   if (xs >= 0 && xs < W2) {
 #pragma unroll
@@ -93,14 +109,23 @@ __global__ void nchw_to_s2d_kernel(const float* __restrict__ src, int F, int Cin
       const float* pl = src + ((f * Cin + c) * H + 2 * y2) * (long long)W + 2 * xs;
       const float2 r0 = __ldg(reinterpret_cast<const float2*>(pl));
       const float2 r1 = __ldg(reinterpret_cast<const float2*>(pl + W));
-      v[0 * Cin + c] = __float2half_rn(r0.x); v[1 * Cin + c] = __float2half_rn(r0.y);
-      v[2 * Cin + c] = __float2half_rn(r1.x); v[3 * Cin + c] = __float2half_rn(r1.y);
+      const float q[4] = {r0.x, r0.y, r1.x, r1.y};
+#pragma unroll
+      for (int ab = 0; ab < 4; ++ab) {
+        const __half h = __float2half_rn(q[ab]);
+        vh[ab * Cin + c] = h;
+        if constexpr (LO) vl[ab * Cin + c] = __float2half_rn(q[ab] - __half2float(h));
+      }
     }
   }
-  uint4* o = reinterpret_cast<uint4*>(dst + p * (4 * CS) + ds * CS);
-  const uint4* vv = reinterpret_cast<const uint4*>(v);
+  __half* o = dst + p * (4 * CS) + ds * CS;
+  uint4* oh = reinterpret_cast<uint4*>(o);
+  uint4* ol = reinterpret_cast<uint4*>(reinterpret_cast<char*>(o) + lo_off);
 #pragma unroll
-  for (int q = 0; q < CS / 8; ++q) o[q] = vv[q];
+  for (int q = 0; q < CS / 8; ++q) {
+    oh[q] = reinterpret_cast<const uint4*>(vh)[q];
+    if constexpr (LO) ol[q] = reinterpret_cast<const uint4*>(vl)[q];
+  }
 }
 
 // dst[f, y, x, c] = (y, x both even) ? src[f, y/2, x/2, c] : 0      (8 channels = 16 bytes per thread)
@@ -124,22 +149,28 @@ __global__ void upsample2_zero_kernel(const __half* __restrict__ src, int OH, in
 
 }  // namespace
 
-int launch_nhwc_to_s2d(View src, int F, __half* dst, int Cs, cudaStream_t s) {
+int launch_nhwc_to_s2d(View src, int F, __half* dst, long long lo_off, int Cs, cudaStream_t s) {
   const long long n = (long long)F * (src.H / 2) * (src.W / 2) * 4 * Cs;
-  nhwc_to_s2d_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const __half*)src.base, F, src.H, src.W, src.C, src.pitch, src.coff, dst, Cs);
+  const unsigned g = (unsigned)((n + 255) / 256);
+  if (lo_off) nhwc_to_s2d_kernel<float><<<g, 256, 0, s>>>((const float*)src.base, F, src.H, src.W, src.C, src.pitch, src.coff, dst, lo_off, Cs);
+  else nhwc_to_s2d_kernel<__half><<<g, 256, 0, s>>>((const __half*)src.base, F, src.H, src.W, src.C, src.pitch, src.coff, dst, lo_off, Cs);
   SSNB_LAUNCH_CHECK("nhwc_to_s2d_kernel");
   return 0;
 }
-int launch_nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, int Cs, cudaStream_t s) {
+template <bool LO>
+static int nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, long long lo_off, int Cs, cudaStream_t s) {
   const long long n = (long long)F * (H / 2) * (W / 2) * 4;
   const unsigned g = (unsigned)((n + 255) / 256);
-  if (Cs == 16 && Cin == 3) nchw_to_s2d_kernel<16, 3><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst);
-  else if (Cs == 40 && Cin == 10) nchw_to_s2d_kernel<40, 10><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst);
-  else if (Cs == 16) nchw_to_s2d_kernel<16, 0><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst);
-  else if (Cs == 40) nchw_to_s2d_kernel<40, 0><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst);
+  if (Cs == 16 && Cin == 3) nchw_to_s2d_kernel<16, 3, LO><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst, lo_off);
+  else if (Cs == 40 && Cin == 10) nchw_to_s2d_kernel<40, 10, LO><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst, lo_off);
+  else if (Cs == 16) nchw_to_s2d_kernel<16, 0, LO><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst, lo_off);
+  else if (Cs == 40) nchw_to_s2d_kernel<40, 0, LO><<<g, 256, 0, s>>>(src, F, Cin, H, W, dst, lo_off);
   else { set_thread_error("nchw_to_s2d: unsupported channel count (RGB 3 or Flow 10)"); return 1; }
   SSNB_LAUNCH_CHECK("nchw_to_s2d_kernel");
   return 0;
+}
+int launch_nchw_to_s2d(const float* src, int F, int Cin, int H, int W, __half* dst, long long lo_off, int Cs, cudaStream_t s) {
+  return lo_off ? nchw_to_s2d<true>(src, F, Cin, H, W, dst, lo_off, Cs, s) : nchw_to_s2d<false>(src, F, Cin, H, W, dst, lo_off, Cs, s);
 }
 int launch_pack_conv1_s2d(const __half* wd, int Cout, int Cin, int Cs, __half* ws, cudaStream_t s) {
   const long long n = 16LL * Cout * Cs;   // 4 taps x Cout x 4*Cs

@@ -262,39 +262,13 @@ __global__ void __launch_bounds__(NT) wgrad_kernel(WgradArgs a) {
   }
 }
 
-// threads enumerate the partial layout [tap][co][ci] (coalesced reads of every split), write the reference
-// layout [co][ci][tap]
-__global__ void wgrad_finalize_kernel(const float* __restrict__ partial, int splits, int taps, int Cout, int Cin,
-                                      const float* __restrict__ mult, float out_scale, float* __restrict__ dw, int accumulate,
-                                      const float* __restrict__ bias_partial, float* __restrict__ db, int* __restrict__ flag,
-                                      const float* __restrict__ unscale) {
-  const long long total = (long long)taps * Cout * Cin;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (unscale) out_scale *= __ldg(unscale);
-  if (bias_partial && db && i < Cout) {          // bias gradient from the weight-gradient kernel's ones-operand accumulator
-    float sb = 0.f;
-    for (int sp = 0; sp < splits; ++sp) sb += bias_partial[(long long)sp * Cout + i];
-    db[i] = (accumulate ? db[i] : 0.f) + sb * mult[i] * out_scale;
-  }
-  if (i >= total) return;
-  const int ci = (int)(i % Cin);
-  const int co = (int)((i / Cin) % Cout);
-  const int tap = (int)(i / ((long long)Cin * Cout));
-  float s = 0.f;
-  for (int sp = 0; sp < splits; ++sp) s += partial[(long long)sp * total + i];
-  if (flag && !(fabsf(s) <= 3.0e38f)) *flag = 1;         // inf / NaN: a gradient left the fp16 range under this loss scale
-  float* o = dw + ((long long)co * Cin + ci) * taps + tap;
-  *o = (accumulate ? *o : 0.f) + s * mult[co] * out_scale;
-}
-
-__global__ void wgrad_finalize_all_kernel(const __grid_constant__ FinalizeTable t, float out_scale, int accumulate) {
-  int ei = 0;
-  while (ei + 1 < t.n && (int)blockIdx.x >= t.e[ei + 1].block0) ++ei;       // <= 36 entries, uniform per block
-  const FinalizeEntry& q = t.e[ei];
+// one table entry's CTAs (from q.block0 on) enumerate the partial layout [tap][co][ci] (coalesced reads of every split) and
+// write the reference layout [co][ci][tap]
+__device__ __forceinline__ void wgrad_finalize_entry(const FinalizeEntry& q, const float* unscale, int* flag, float out_scale, int accumulate) {
   const long long total = (long long)q.taps * q.Cout * q.Cin;
   const long long i = (long long)(blockIdx.x - q.block0) * blockDim.x + threadIdx.x;
-  if (t.unscale) out_scale *= __ldg(t.unscale);
-  if (q.bias_partial && q.db && i < q.Cout) {
+  if (unscale) out_scale *= __ldg(unscale);
+  if (q.bias_partial && q.db && i < q.Cout) {     // bias gradient from the weight-gradient kernel's ones-operand accumulator
     float sb = 0.f;
     for (int sp = 0; sp < q.splits; ++sp) sb += q.bias_partial[(long long)sp * q.Cout + i];
     q.db[i] = (accumulate ? q.db[i] : 0.f) + sb * q.mult[i] * out_scale;
@@ -305,9 +279,23 @@ __global__ void wgrad_finalize_all_kernel(const __grid_constant__ FinalizeTable 
   const int tap = (int)(i / ((long long)q.Cin * q.Cout));
   float s = 0.f;
   for (int sp = 0; sp < q.splits; ++sp) s += q.partial[(long long)sp * total + i];
-  if (t.flag && !(fabsf(s) <= 3.0e38f)) *t.flag = 1;
+  if (flag && !(fabsf(s) <= 3.0e38f)) *flag = 1;         // inf / NaN: a gradient left the fp16 range under this loss scale
   float* o = q.dw + ((long long)co * q.Cin + ci) * q.taps + tap;
   *o = (accumulate ? *o : 0.f) + s * q.mult[co] * out_scale;
+}
+
+__global__ void wgrad_finalize_kernel(const float* __restrict__ partial, int splits, int taps, int Cout, int Cin,
+                                      const float* __restrict__ mult, float out_scale, float* __restrict__ dw, int accumulate,
+                                      const float* __restrict__ bias_partial, float* __restrict__ db, int* __restrict__ flag,
+                                      const float* __restrict__ unscale) {
+  const FinalizeEntry q{partial, mult, dw, bias_partial, db, splits, taps, Cout, Cin, 0, 0};
+  wgrad_finalize_entry(q, unscale, flag, out_scale, accumulate);
+}
+
+__global__ void wgrad_finalize_all_kernel(const __grid_constant__ FinalizeTable t, float out_scale, int accumulate) {
+  int ei = 0;
+  while (ei + 1 < t.n && (int)blockIdx.x >= t.e[ei + 1].block0) ++ei;       // <= 36 entries, uniform per block
+  wgrad_finalize_entry(t.e[ei], t.unscale, t.flag, out_scale, accumulate);
 }
 
 }  // namespace

@@ -5,7 +5,8 @@
 //     hi = fp16(x),  lo = fp16(x - float(hi))          (hi + lo == x to ~2^-22 relative, fp16 range permitting)
 // and a product a*b is evaluated as a_lo*b_hi + a_hi*b_lo + a_hi*b_hi on the tensor cores with fp32 accumulation
 // (umma_conv.cu / umma_wgrad.cu, nseg = 3).  The kernels here produce those planes for tensors that
-// do not come out of a convolution epilogue (pool outputs, the network input, masked output gradients, weights).
+// do not come out of a convolution epilogue (pool outputs, masked output gradients, weights); the network input's planes
+// come from the space-to-depth conversions of s2d_glue.cu.
 #include "common.cuh"
 
 namespace ssnb {
@@ -78,81 +79,7 @@ __global__ void planes_to_nchw_kernel(const __half* __restrict__ hi, long long l
   dst[i] = (__half2float(*hp) + __half2float(*lp)) * scale;
 }
 
-// NCHW fp32 frames -> conv1's packed space-to-depth operand planes (layout of s2d_glue.cu: channel = ds*Cs + (a*2+b)*Cin + c
-// holds x[f, 2i+a, 2(j+ds-2)+b, c]); one thread per (pixel, ds block)
-// CIN > 0: compile-time channel count (RGB 3 / Flow 10): the channel loop unrolls and the staging arrays stay in registers
-template <int CS, int CIN>
-__global__ void nchw_to_s2d_split_kernel(const float* __restrict__ src, int F, int Cin_rt, int H, int W, __half* __restrict__ dst,
-                                         long long lo_off) {
-  const int Cin = CIN ? CIN : Cin_rt;
-  const int H2 = H / 2, W2 = W / 2;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)F * H2 * W2 * 4) return;
-  const unsigned iu = (unsigned)i;
-  const int ds = (int)(iu & 3u);
-  const unsigned pu = iu >> 2;
-  const int x2 = (int)(pu % (unsigned)W2), y2 = (int)((pu / (unsigned)W2) % (unsigned)H2);
-  const long long p = pu;
-  const long long f = pu / (unsigned)(W2 * H2);
-  __align__(16) __half vh[CS];
-  __align__(16) __half vl[CS];
-#pragma unroll
-  for (int c = 0; c < CS; ++c) { vh[c] = __float2half_rn(0.f); vl[c] = __float2half_rn(0.f); }
-  const int xs = x2 + ds - 2;
-  if (xs >= 0 && xs < W2) {
-#pragma unroll
-    for (int c = 0; c < Cin; ++c) {
-      const float* pl = src + ((f * Cin + c) * H + 2 * y2) * (long long)W + 2 * xs;
-      const float2 r0 = __ldg(reinterpret_cast<const float2*>(pl));
-      const float2 r1 = __ldg(reinterpret_cast<const float2*>(pl + W));
-      const float q[4] = {r0.x, r0.y, r1.x, r1.y};
-#pragma unroll
-      for (int ab = 0; ab < 4; ++ab) {
-        const __half h = __float2half_rn(q[ab]);
-        vh[ab * Cin + c] = h;
-        vl[ab * Cin + c] = __float2half_rn(q[ab] - __half2float(h));
-      }
-    }
-  }
-  __half* o = dst + p * (4 * CS) + ds * CS;
-  uint4* oh = reinterpret_cast<uint4*>(o);
-  uint4* ol = reinterpret_cast<uint4*>(reinterpret_cast<char*>(o) + lo_off);
-#pragma unroll
-  for (int q = 0; q < CS / 8; ++q) { oh[q] = reinterpret_cast<const uint4*>(vh)[q]; ol[q] = reinterpret_cast<const uint4*>(vl)[q]; }
-}
-
-// fp32 NHWC view -> the same packed space-to-depth planes (per-layer tests: the input was written as a named value)
-__global__ void nhwc_to_s2d_split_kernel(const float* __restrict__ src, int F, int H, int W, int Cin, int spitch, int scoff,
-                                         __half* __restrict__ dst, long long lo_off, int Cs) {
-  const int H2 = H / 2, W2 = W / 2, Ck = 4 * Cs;
-  const long long total = (long long)F * H2 * W2 * Ck;
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int ch = (int)(i % Ck);
-  const long long p = i / Ck;
-  const int x2 = (int)(p % W2), y2 = (int)((p / W2) % H2);
-  const long long f = p / ((long long)W2 * H2);
-  const int ds = ch / Cs, q = ch % Cs;
-  float v = 0.f;
-  const int xs = x2 + ds - 2;
-  if (q < 4 * Cin && xs >= 0 && xs < W2) {
-    const int ab = q / Cin, c = q % Cin;
-    v = src[((f * H + 2 * y2 + ab / 2) * W + 2 * xs + ab % 2) * spitch + scoff + c];
-  }
-  const __half h = __float2half_rn(v);
-  dst[i] = h;
-  *reinterpret_cast<__half*>(reinterpret_cast<char*>(dst + i) + lo_off) = __float2half_rn(v - __half2float(h));
-}
-
 }  // namespace
-
-int launch_nhwc_to_s2d_split(View src, int F, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s) {
-  const long long n = (long long)F * (src.H / 2) * (src.W / 2) * 4 * Cs;
-  nhwc_to_s2d_split_kernel<<<(unsigned)((n + TPB - 1) / TPB), TPB, 0, s>>>((const float*)src.base, F, src.H, src.W, src.C, src.pitch, src.coff,
-                                                                         dst_hi, lo_off, Cs);
-  SSNB_LAUNCH_CHECK("nhwc_to_s2d_split_kernel");
-  return 0;
-}
 
 int launch_split_view(View src, int F, float scale, View planes, int* flag, cudaStream_t s) {
   if (src.C % 8 || src.pitch % 4 || src.coff % 4 || planes.pitch % 8 || planes.coff % 8 || planes.C != src.C || !planes.lo_off) {
@@ -175,17 +102,6 @@ int launch_planes_to_nchw(View planes, int F, float scale, float* dst, cudaStrea
   planes_to_nchw_kernel<<<(unsigned)((n + TPB - 1) / TPB), TPB, 0, s>>>((const __half*)planes.base, planes.lo_off, F, planes.C, planes.H, planes.W,
                                                                       planes.pitch, planes.coff, scale, dst);
   SSNB_LAUNCH_CHECK("planes_to_nchw_kernel");
-  return 0;
-}
-int launch_nchw_to_s2d_split(const float* src, int F, int Cin, int H, int W, __half* dst_hi, long long lo_off, int Cs, cudaStream_t s) {
-  const long long n = (long long)F * (H / 2) * (W / 2) * 4;
-  const unsigned g = (unsigned)((n + TPB - 1) / TPB);
-  if (Cs == 16 && Cin == 3) nchw_to_s2d_split_kernel<16, 3><<<g, TPB, 0, s>>>(src, F, Cin, H, W, dst_hi, lo_off);
-  else if (Cs == 40 && Cin == 10) nchw_to_s2d_split_kernel<40, 10><<<g, TPB, 0, s>>>(src, F, Cin, H, W, dst_hi, lo_off);
-  else if (Cs == 16) nchw_to_s2d_split_kernel<16, 0><<<g, TPB, 0, s>>>(src, F, Cin, H, W, dst_hi, lo_off);
-  else if (Cs == 40) nchw_to_s2d_split_kernel<40, 0><<<g, TPB, 0, s>>>(src, F, Cin, H, W, dst_hi, lo_off);
-  else { set_thread_error("nchw_to_s2d_split: unsupported channel count (RGB 3 or Flow 10)"); return 1; }
-  SSNB_LAUNCH_CHECK("nchw_to_s2d_split_kernel");
   return 0;
 }
 

@@ -56,7 +56,6 @@ class STPPReorgainzed:
     def __init__(self, feat_dim, act_score_len, comp_score_len, reg_score_len,
                  standalong_classifier=False, with_regression=True, stpp_cfg=(1, 1, 1)):
         self.sc = standalong_classifier
-        self.use_prefix_sums = True       # False: the direct row-loop kernel (same results to fp32 rounding)
         self.act_len = act_score_len
         self.comp_len = comp_score_len
         self.reg_len = reg_score_len
@@ -86,18 +85,12 @@ class STPPReorgainzed:
         counts = [len(p) for p in self.stpp_cfg]
         levels = [v for p in self.stpp_cfg for v in p]
         with torch.cuda.device(dev):
-            if self.use_prefix_sums:
-                # one fp64 column scan of the score table + a two-load gather per pooled part
-                ws = torch.empty(lib.ssnb_stpp_reorg_workspace_bytes(scores.size(0), scores.size(1)), dtype=torch.uint8, device=dev)
-                check(lib.ssnb_stpp_reorg_prefix(scores.data_ptr(), scores.size(0), scores.size(1), ticks.data_ptr(), sc.data_ptr(),
-                                                 n, self.act_len, self.comp_len, self.reg_len, _lib.int_array(counts),
-                                                 _lib.int_array(levels), out_act.data_ptr(), out_comp.data_ptr(),
-                                                 out_reg.data_ptr(), ws.data_ptr(), _stream()), None, "stpp_reorg_prefix")
-            else:
-                check(lib.ssnb_stpp_reorg(scores.data_ptr(), scores.size(0), scores.size(1), ticks.data_ptr(), sc.data_ptr(),
-                                          n, self.act_len, self.comp_len, self.reg_len, _lib.int_array(counts),
-                                          _lib.int_array(levels), out_act.data_ptr(), out_comp.data_ptr(),
-                                          out_reg.data_ptr(), _stream()), None, "stpp_reorg")
+            # one fp64 column scan of the score table + a two-load gather per pooled part
+            ws = torch.empty(lib.ssnb_stpp_reorg_workspace_bytes(scores.size(0), scores.size(1)), dtype=torch.uint8, device=dev)
+            check(lib.ssnb_stpp_reorg_prefix(scores.data_ptr(), scores.size(0), scores.size(1), ticks.data_ptr(), sc.data_ptr(),
+                                             n, self.act_len, self.comp_len, self.reg_len, _lib.int_array(counts),
+                                             _lib.int_array(levels), out_act.data_ptr(), out_comp.data_ptr(),
+                                             out_reg.data_ptr(), ws.data_ptr(), _stream()), None, "stpp_reorg_prefix")
         return out_act, out_comp, out_reg
 
 

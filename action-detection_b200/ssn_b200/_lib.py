@@ -101,7 +101,6 @@ SIGNATURES = {
     "ssnb_stpp_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _ip, _ip, _ip, _ip, _i, _i, _vp, _vp, _vp]),
     "ssnb_stpp_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _ip, _ip, _ip, _ip, _i, _i, _vp, _vp]),
     "ssnb_gpool_stpp_fwd": (_i, [_vp, _vp, _vp, _i, _i, _ip, _ip, _ip, _ip, _i, _i, _vp, _vp, _vp, _vp]),
-    "ssnb_stpp_reorg": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _ip, _ip, _vp, _vp, _vp, _vp]),
     "ssnb_stpp_reorg_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_stpp_reorg_prefix": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _ip, _ip, _vp, _vp, _vp, _vp, _vp]),
     "ssnb_linear_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
@@ -119,7 +118,6 @@ SIGNATURES = {
     "ssnb_timing_begin": (_i, [_vp]),
     "ssnb_timing_report": (C.c_char_p, []),
     "ssnb_timing_launches": (C.c_char_p, []),
-    "ssnb_detect_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_detect_postprocess": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_double, _i, _vp, _vp, _vp, _vp]),
     "ssnb_detect_batch_workspace_bytes": (_sz, [C.POINTER(DetectBatchCfg), _i, C.POINTER(C.c_int64), _i]),
     "ssnb_detect_batch": (_i, [C.POINTER(DetectBatchCfg), _vp, _vp, _vp, _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp, _vp, _vp, _vp, _vp,
@@ -143,7 +141,6 @@ SIGNATURES = {
                          + [_vp] * 7 + [_sz, _vp]),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
-    "ssnb_sgd_step": (_i, [_vp, _vp, _vp, _sz, _f, _f, _f, _f, _vp]),
     "ssnb_sgd_step_groups": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp]),
 }
 

@@ -135,12 +135,8 @@ int ssnb_gpool_stpp_fwd(ssnb_handle h, const float* drop_mask, const float* scal
 
 /* ---- STPPReorgainzed.forward (ops/ssn_ops.py:109-170), standalong_classifier + regression ----
  * scores [T, D] with D = act_len + M*comp_len + M*reg_len; ticks [N,4] int32; scaling [N,2];
- * stage_parts: 3 stages, parts-per-level lists flattened: level_counts[3] + levels[]. */
-int ssnb_stpp_reorg(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N,
-                    int act_len, int comp_len, int reg_len, const int* level_counts, const int* levels,
-                    float* out_act, float* out_comp, float* out_reg, void* stream);
-
-/* Same result through one fp64 exclusive column scan of scores (workspace: (T+1)*D doubles, ssnb_stpp_reorg_workspace_bytes)
+ * stage_parts: 3 stages, parts-per-level lists flattened: level_counts[3] + levels[].
+ * One fp64 exclusive column scan of scores (workspace: (T+1)*D doubles, ssnb_stpp_reorg_workspace_bytes)
  * + one gather per proposal: every part costs two loads instead of its row count (1000 heavily overlapping proposals/video). */
 size_t ssnb_stpp_reorg_workspace_bytes(int T, int D);
 int ssnb_stpp_reorg_prefix(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N, int act_len,
@@ -221,10 +217,9 @@ int ssnb_classifier_ce_fwd_bwd(const float* x, const float* w, const float* b, c
  * rel_props [N,2] (start, end in [0,1]), act_scores [N,K+1], comp_scores [N,K], reg_scores [N,K,2] (already de-normalised,
  * ssn_test.py:89-92) ->  per class c: combined score softmax(act)[:,c+1] * exp(comp[:,c]), greedy temporal NMS at
  * nms_thresh in descending score order, then (regress != 0) the location regression of the survivors.
- * detections [K, N, 5] rows (t0, t1, score, loc, dur) in kept order, counts [K] int32; combined_ws: N*K floats of scratch
- * (ssnb_detect_workspace_bytes).  N <= 8192.  act_scores == NULL: combined_ws already holds the [N,K] scores to rank by
+ * detections [K, N, 5] rows (t0, t1, score, loc, dur) in kept order, counts [K] int32; combined_ws: N*K floats of scratch.
+ * N <= 8192.  act_scores == NULL: combined_ws already holds the [N,K] scores to rank by
  * (plain class-wise temporal_nms, ops/utils.py:56-82). */
-size_t ssnb_detect_workspace_bytes(int n_props, int num_class);
 int ssnb_detect_postprocess(const float* rel_props, const float* act_scores, const float* comp_scores, const float* reg_scores,
                             int n_props, int num_class, double nms_thresh, int regress, float* detections, int* counts,
                             float* combined_ws, void* stream);
@@ -396,7 +391,7 @@ int ssnb_proposal_targets(const ssnb_proposal_targets_cfg* cfg, const int64_t* f
  * a video without proposals owns one row, the reference's fallback proposal (0, frame_cnt - 1), so out_first is the exclusive
  * cumsum of max(count, 1)): rel_prop double [rows, 2], ticks int64 [rows, 4], scaling double [rows, 2], bitwise the
  * reference's, each operation rounded on its own.  Optional ticks32 int32 [rows, 4] / scaling32 float [rows, 2]: the same
- * values in the types ssnb_stpp_reorg and ssnb_stpp_reorg_prefix take.  A zero-length fallback (frame_cnt 1) divides by zero
+ * values in the types ssnb_stpp_reorg_prefix takes.  A zero-length fallback (frame_cnt 1) divides by zero
  * where the reference raises. */
 int ssnb_test_proposals(const int64_t* frames, const int64_t* first, const int32_t* count, const int64_t* out_first, int n_videos,
                         int64_t max_count, const int32_t* frame_cnt, int new_length, int test_interval, int32_t* num_ticks, double* rel_prop,
@@ -479,15 +474,11 @@ int ssnb_frame_transform(const ssnb_frame_cfg* cfg, const ssnb_frame_group* grou
                          const uint8_t* src, size_t src_bytes, float* dst, int64_t dst_floats, void* workspace, size_t workspace_bytes,
                          void* stream);
 
-/* fused SGD-momentum step over flat fp32 buffers (ssn_train.py:141-144 torch.optim.SGD semantics):
- * g = grad*grad_mult + wd*p; buf = mom*buf + g; p -= lr*buf */
-int ssnb_sgd_step(float* param, const float* grad, float* momentum_buf, size_t n, float lr, float momentum,
-                  float weight_decay, float grad_mult, void* stream);
-
-/* The whole model in ONE launch: the flat buffers are cut into n_seg <= 512 segments (one per parameter tensor; seg_end =
- * cumulative element ends, device int64) with their parameter group's learning rate and weight decay (device fp32 arrays):
- * the per-group lr_mult / decay_mult of SSN.get_optim_policies (ssn_models.py:203-251) as applied by
- * adjust_learning_rate (ssn_train.py:391-398).  Same update rule as ssnb_sgd_step. */
+/* fused SGD-momentum step over flat fp32 buffers (ssn_train.py:141-144 torch.optim.SGD semantics), the whole model in ONE
+ * launch: the flat buffers are cut into n_seg <= 512 segments (one per parameter tensor; seg_end = cumulative element ends,
+ * device int64) with their parameter group's learning rate and weight decay (device fp32 arrays): the per-group lr_mult /
+ * decay_mult of SSN.get_optim_policies (ssn_models.py:203-251) as applied by adjust_learning_rate (ssn_train.py:391-398).
+ * Per element: g = grad*grad_mult + wd*p; buf = mom*buf + g; p -= lr*buf */
 int ssnb_sgd_step_groups(float* param, const float* grad, float* momentum_buf, size_t n, const int64_t* seg_end,
                          const float* seg_lr, const float* seg_wd, int n_seg, float momentum, float grad_mult, void* stream);
 

@@ -3,7 +3,7 @@
 What runs after the backbone at test time (ssn_test.py:80-87, eval_detection_results.py:91-183), op by op:
   crop mean folded into the test FC   (ssnb_test_fc_cropmean: linear_cropmean_kernel)
   plain test FC                       (ssnb_linear_fwd: linear_fwd_kernel)
-  re-organised STPP                   (ssnb_stpp_reorg_prefix: colscan_f64_kernel + stpp_reorg_prefix_kernel; ssnb_stpp_reorg)
+  re-organised STPP                   (ssnb_stpp_reorg_prefix: colscan_f64_kernel + stpp_reorg_prefix_kernel)
   combined scores, class-wise NMS, location regression   (ssnb_detect_postprocess: combined_scores_kernel + nms_regress_kernel)
 Each function takes what the kernel consumed, so one op's rounding never reaches the next.  The error of a quantity is the
 one of oracle/step_check.py (`Checker`): max |got - ref| over the tensor or the row, divided by max |ref| of the same, with
@@ -22,7 +22,6 @@ CROPMEAN_BAR = 2e-6      # linear_cropmean_kernel, per tick (row)               
 LINEAR_BAR = 3.5e-6      # linear_fwd_kernel, per row                                  [8.5e-7, out 2]
 REORG_BAR = 1.3e-6       # re-organised STPP through the fp64 column prefix, act / comp / reg per proposal (row)
                          #                                                             [3.3e-7, 8-level course stage, comp]
-REORG_DIRECT_BAR = 1.5e-5  # the direct kernel: fp32 sums down up to T rows           [3.7e-6, T = 20000, act]
 COMBINED_BAR = 4e-6      # combined scores, per proposal (row)                         [9.1e-7, K = 200]
 REGRESS_BAR = 4e-7       # regressed boxes of the survivors, per class                 [9.1e-8]
 

@@ -1,5 +1,5 @@
 """The test-time tail of SSN against float64 (oracle/infer_check.py): the crop-mean test FC and the plain test FC, the
-re-organised STPP through its prefix and direct kernels, and detection post-processing (combined scores, class-wise NMS,
+re-organised STPP through its column prefix sums, and detection post-processing (combined scores, class-wise NMS,
 regression), each fed what the previous kernel wrote, at the benchmarked shapes, ActivityNet's K = 200, the size limits
 and the edges.  Run on an H100: pytest -m gpu -s tests/test_gpu_infer_tail.py."""
 import math
@@ -58,8 +58,8 @@ def _lens(K):
     return K + 1, K, 2 * K
 
 
-def _reorg(scores, ticks, sc, K, cfg, prefix, n=None, fill=NAN):
-    """one ssnb_stpp_reorg_prefix / ssnb_stpp_reorg call -> (act, comp, reg, workspace, the three output buffers)"""
+def _reorg(scores, ticks, sc, K, cfg, n=None, fill=NAN):
+    """one ssnb_stpp_reorg_prefix call -> (act, comp, reg, workspace, the three output buffers)"""
     lib, check, int_array, _stream = _lib()
     dev = scores.device
     parts = [O.parse_stage_config(c)[0] for c in cfg]
@@ -69,12 +69,8 @@ def _reorg(scores, ticks, sc, K, cfg, prefix, n=None, fill=NAN):
     outs = [torch.full((max(n, 1), L), fill, device=dev) for L in _lens(K)]
     args = (scores.data_ptr(), scores.shape[0], scores.shape[1], tk.data_ptr(), s2.data_ptr(), n, *_lens(K),
             int_array([len(p) for p in parts]), int_array([v for p in parts for v in p]), *[o.data_ptr() for o in outs])
-    ws = None
-    if prefix:
-        ws = torch.full((lib.ssnb_stpp_reorg_workspace_bytes(scores.shape[0], scores.shape[1]),), 0xAB, dtype=torch.uint8, device=dev)
-        check(lib.ssnb_stpp_reorg_prefix(*args, ws.data_ptr(), _stream()), None, "stpp_reorg_prefix")
-    else:
-        check(lib.ssnb_stpp_reorg(*args, _stream()), None, "stpp_reorg")
+    ws = torch.full((lib.ssnb_stpp_reorg_workspace_bytes(scores.shape[0], scores.shape[1]),), 0xAB, dtype=torch.uint8, device=dev)
+    check(lib.ssnb_stpp_reorg_prefix(*args, ws.data_ptr(), _stream()), None, "stpp_reorg_prefix")
     torch.cuda.synchronize()
     return [o[:n] for o in outs] + [ws, outs]
 
@@ -221,33 +217,27 @@ REORG_CASES = ["bench", "dataset_ticks", "K200_T3000", "T20000_offset30", "T1", 
 
 @pytest.mark.parametrize("name", REORG_CASES)
 def test_stpp_reorg_vs_float64(name):
-    """stpp_reorg_prefix_kernel (after colscan_f64_kernel) and stpp_reorg_kernel vs reorg64, per proposal; both give the same
-    NaN positions; a repeated call gives the same bits"""
+    """stpp_reorg_prefix_kernel (after colscan_f64_kernel) vs reorg64, per proposal, NaN positions included; a repeated call
+    gives the same bits"""
     dev = _cuda()
     scores, ticks, sc, K, cfg = _reorg_case(name)
     sd = scores.to(dev)
     ref = IC.reorg64(scores, ticks, sc, *_lens(K), cfg)
     chk = IC.Checker()
-    got = {}
-    for prefix in (True, False):
-        kname = "prefix" if prefix else "direct"
-        got[kname] = _reorg(sd, ticks, sc, K, cfg, prefix)[:3]
-        IC.check_reorg(chk, "reorg %s %s" % (kname, name), scores, ticks, sc, *_lens(K), cfg, got[kname], ref=ref,
-                       bar=IC.REORG_BAR if prefix else IC.REORG_DIRECT_BAR)
-        again = _reorg(sd, ticks, sc, K, cfg, prefix)[:3]
-        for q, a, b in zip(("act", "comp", "reg"), got[kname], again):
-            assert _same(a, b), (kname, q, "repeat")
-    for q, a, b in zip(("act", "comp", "reg"), got["prefix"], got["direct"]):
-        assert torch.equal(torch.isnan(a), torch.isnan(b)), q
+    got = _reorg(sd, ticks, sc, K, cfg)[:3]
+    IC.check_reorg(chk, "reorg prefix %s" % name, scores, ticks, sc, *_lens(K), cfg, got, ref=ref, bar=IC.REORG_BAR)
+    again = _reorg(sd, ticks, sc, K, cfg)[:3]
+    for q, a, b in zip(("act", "comp", "reg"), got, again):
+        assert _same(a, b), (q, "repeat")
     if name == "edges":
-        assert torch.isnan(got["prefix"][0][1]).all() and torch.isnan(got["prefix"][0][5]).all()
+        assert torch.isnan(got[0][1]).all() and torch.isnan(got[0][5]).all()
     if name in NPOT_CASES:
         # the grid has teeth: part boundaries at left + q * step would be off at comp / reg, and only there
         with pytest.MonkeyPatch.context() as m:
             m.setattr(IC, "reorg_ticks", _naive_ticks)
             naive = IC.reorg64(scores, ticks, sc, *_lens(K), cfg)
         c2 = IC.Checker()
-        IC.check_reorg(c2, "naive", scores, ticks, sc, *_lens(K), cfg, got["prefix"], ref=naive)
+        IC.check_reorg(c2, "naive", scores, ticks, sc, *_lens(K), cfg, got, ref=naive)
         assert {q for _op, q in c2.failed()} == {"comp", "reg"}, c2.report()
     _report("re-organised STPP %s (T=%d, N=%d, K=%d, %s) vs float64" % (name, scores.shape[0], ticks.shape[0], K, cfg), chk)
     chk.assert_ok()
@@ -256,12 +246,10 @@ def test_stpp_reorg_vs_float64(name):
 def test_stpp_reorg_n0_writes_nothing():
     dev = _cuda()
     scores, ticks, sc, K, cfg = _reorg_case("edges")
-    for prefix in (True, False):
-        outs = _reorg(scores.to(dev), ticks, sc, K, cfg, prefix, n=0, fill=-7.0)
-        assert all(o.shape[0] == 0 for o in outs[:3])
-        assert all(bool(o.eq(-7.0).all()) for o in outs[4])
-        if prefix:
-            assert bool(outs[3].eq(0xAB).all())
+    outs = _reorg(scores.to(dev), ticks, sc, K, cfg, n=0, fill=-7.0)
+    assert all(o.shape[0] == 0 for o in outs[:3])
+    assert all(bool(o.eq(-7.0).all()) for o in outs[4])
+    assert bool(outs[3].eq(0xAB).all())
 
 
 # ---- (c) detection --------------------------------------------------------------------------------------------------------------
@@ -436,7 +424,7 @@ def test_bench_inference_tail_chained():
     ticks = torch.sort(torch.randint(0, T + 1, (N, 4), generator=g), dim=1)[0]
     sc = torch.rand(N, 2, generator=g)
     cfg = (1, (1, 2), 1)
-    act, comp, reg = _reorg(out, ticks, sc, K, cfg, True)[:3]
+    act, comp, reg = _reorg(out, ticks, sc, K, cfg)[:3]
     IC.check_reorg(chk, "reorg prefix", out, ticks, sc, *_lens(K), cfg, (act, comp, reg))
     props = (ticks[:, 1:3].float() / T).to(dev)
     _run_detect(chk, "detect", props, act, comp, reg.view(N, K, 2), 0.6)

@@ -114,14 +114,12 @@ def test_stpp_reorganized_golden(golden_dir, tag, cfg):
     K = 3
     scores = torch.tensor(z[tag + "_scores"], device=dev)
     st = STPPReorgainzed(scores.shape[1], K + 1, K, 2 * K, True, True, stpp_cfg=cfg)
-    for prefix in (True, False):
-        st.use_prefix_sums = prefix
-        a, c, r = st.forward(scores, torch.tensor(z[tag + "_ticks"]), torch.tensor(z[tag + "_sc"]))
-        for got, name in ((a, "_act"), (c, "_comp"), (r, "_reg")):
-            ref = z[tag + name]
-            got = got.cpu().numpy()
-            assert np.array_equal(np.isnan(got), np.isnan(ref))
-            np.testing.assert_allclose(np.nan_to_num(got), np.nan_to_num(ref), rtol=2e-6, atol=1e-6)
+    a, c, r = st.forward(scores, torch.tensor(z[tag + "_ticks"]), torch.tensor(z[tag + "_sc"]))
+    for got, name in ((a, "_act"), (c, "_comp"), (r, "_reg")):
+        ref = z[tag + name]
+        got = got.cpu().numpy()
+        assert np.array_equal(np.isnan(got), np.isnan(ref))
+        np.testing.assert_allclose(np.nan_to_num(got), np.nan_to_num(ref), rtol=2e-6, atol=1e-6)
 
 
 def test_stpp_reorganized_vs_oracle_big():
@@ -135,12 +133,10 @@ def test_stpp_reorganized_vs_oracle_big():
     ticks = torch.sort(torch.randint(0, T, (N, 4), generator=g), dim=1)[0]
     sc = torch.rand(N, 2, generator=g)
     ref = O.stpp_reorganized(scores, ticks, sc, K + 1, K, 2 * K, cfg)
-    for prefix in (True, False):          # fp64 column prefix sums + gather (default) and the direct row-loop kernel
-        mod = STPPReorgainzed(D, K + 1, K, 2 * K, True, True, stpp_cfg=cfg)
-        mod.use_prefix_sums = prefix
-        got = mod.forward(scores.to(dev), ticks, sc)
-        for a, b in zip(got, ref):
-            np.testing.assert_allclose(a.cpu().numpy(), b.numpy(), rtol=1e-5, atol=1e-6)
+    mod = STPPReorgainzed(D, K + 1, K, 2 * K, True, True, stpp_cfg=cfg)
+    got = mod.forward(scores.to(dev), ticks, sc)
+    for a, b in zip(got, ref):
+        np.testing.assert_allclose(a.cpu().numpy(), b.numpy(), rtol=1e-5, atol=1e-6)
 
 
 # ---- heads --------------------------------------------------------------------------------------------
