@@ -4,7 +4,8 @@ run against it unchanged.  The BNInception backbone, the segment mean and classi
 loss stays the caller's torch.nn.CrossEntropyLoss (binary_train.py:135), or BinaryClassifier.fused_step does the whole
 training step in the library.
 
-Only base_model='BNInception' with RGB / Flow input is accelerated; other backbones and modalities raise ValueError like
+base_model='BNInception' with RGB / Flow input is accelerated, and base_model='InceptionV3' at test time (scoring only);
+other backbones and modalities raise ValueError like
 the SSN drop-in does.  Construction, Flow conv1 expansion, bn_mode handling and the optimiser policies are SSN's
 (ssn_models._BNInceptionModel): the reference's two files repeat the same code.
 
@@ -89,6 +90,7 @@ class BinaryClassifier(_BNInceptionModel):
         gradient is multiplied by loss_scale (1/world for data parallel with equal rows per rank).  grad_sync
         (ssn_b200.dp.GradSync): exchange the gradients bucket by bucket while the backward of the lower layers is running.
         Keeps feat, course, logits and the dropout mask (None without dropout) of the step in self.last_fused."""
+        self._require_trainable_backbone()
         if not input.is_cuda:
             raise RuntimeError("BinaryClassifier(H100).fused_step needs CUDA tensors (libssn_b200 has no CPU path)")
         if self.base_model.bn1_training():

@@ -81,7 +81,7 @@ struct ConvArgs {
   void* dst;       int DH, DW, Cdst, dst_pitch, dst_coff;   // y (fwd) or dx (dgrad)
   const void* wgt;                                          // [tap][csrc][cdst], storage type
   const float* bias;                                        // [Cdst] or nullptr
-  int F, k, stride, pad;
+  int F, kh, kw, stride, pad_h, pad_w;                      // tap t = r * kw + s (r: row, s: column of the kernel)
   int relu, accumulate, dgrad;
 };
 struct WgradArgs {
@@ -120,15 +120,15 @@ int launch_grad_exponent(const float* dfeat, long long n, float grad_scale, int 
 constexpr int PACK_MAX = 32;
 constexpr int PACK_PER_THREAD = 4;     // element-wise path of pack_all_kernel (more than PACK_TILE_TAPS taps: conv1): 256 threads x 4 elements per CTA
 constexpr int PACK_TILE = 32, PACK_TILE_TAPS = 9;   // tiled path: one CTA per 32 output x 32 input channels x taps
-inline int pack_ctas(int cout, int cin, int k) {
-  if (k * k <= PACK_TILE_TAPS) return ((cout + PACK_TILE - 1) / PACK_TILE) * ((cin + PACK_TILE - 1) / PACK_TILE);
-  const long long n = (long long)cout * cin * k * k, per = 256LL * PACK_PER_THREAD;
+inline int pack_ctas(int cout, int cin, int taps) {
+  if (taps <= PACK_TILE_TAPS) return ((cout + PACK_TILE - 1) / PACK_TILE) * ((cin + PACK_TILE - 1) / PACK_TILE);
+  const long long n = (long long)cout * cin * taps, per = 256LL * PACK_PER_THREAD;
   return (int)(((n > cout ? n : cout) + per - 1) / per);
 }
 struct PackEntry {
   const float *w, *b, *gamma, *beta, *mean, *var;
   void *wf, *wd; float *bias, *scale, *absmax;
-  int cout, cin, k, block0;
+  int cout, cin, taps, block0;  // taps = kh * kw, the trailing extent of the reference layout [cout][cin][kh][kw]
   int nofold, pad_[3];          // nofold: scale = 1, bias' = b (the layer's BatchNorm runs in training mode, unfused)
   float* bias_b;                // optional second copy of the folded bias (stacked bias of a fused sibling block)
 };

@@ -538,7 +538,7 @@ static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, fl
     a.src = in.base; a.SH = in.H; a.SW = in.W; a.Csrc = in.C; a.src_pitch = in.pitch; a.src_coff = in.coff;
     a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
     a.wgt = e->ws + e->packed[o.conv].wf; a.bias = (const float*)(e->ws + e->packed[o.conv].bias);
-    a.F = F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = o.raw ? 0 : 1; a.accumulate = 0; a.dgrad = 0;
+    a.F = F; a.kh = a.kw = c.k; a.stride = c.stride; a.pad_h = a.pad_w = c.pad; a.relu = o.raw ? 0 : 1; a.accumulate = 0; a.dgrad = 0;
     tag_next(0, conv_flops(e, o), o.id.c_str());
     return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
   }
@@ -574,7 +574,7 @@ static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   a.src = dz.base; a.SH = dz.H; a.SW = dz.W; a.Csrc = dz.C; a.src_pitch = dz.pitch; a.src_coff = dz.coff;
   a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
   a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
-  a.F = e->F; a.k = c.k; a.stride = c.stride; a.pad = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
+  a.F = e->F; a.kh = a.kw = c.k; a.stride = c.stride; a.pad_h = a.pad_w = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
   tag_next(1, conv_flops(e, o), o.id.c_str());
   return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
 }
@@ -943,10 +943,10 @@ int ssnb_pack_weights(ssnb_handle h, const float* const* w, const float* const* 
       q.w = w[i]; q.b = b[i]; q.gamma = gamma[i]; q.beta = beta[i]; q.mean = mean[i]; q.var = var[i];
       q.wf = h->ws + p.wf; q.wd = h->ws + p.wd; q.bias = (float*)(h->ws + p.bias); q.scale = (float*)(h->ws + p.scale);
       q.absmax = h->exact_tc() ? (float*)(h->ws + p.wmax) : nullptr;
-      q.cout = c.cout; q.cin = c.cin; q.k = c.k; q.block0 = pblocks.back();
+      q.cout = c.cout; q.cin = c.cin; q.taps = c.k * c.k; q.block0 = pblocks.back();
       q.nofold = (h->bn1_train && i == 0) ? 1 : 0; q.pad_[0] = q.pad_[1] = q.pad_[2] = 0;
       q.bias_b = (h->exact_tc() && fb) ? (float*)(h->ws + fb->bias) + mb.row : nullptr;
-      pblocks.back() += pack_ctas(c.cout, c.cin, c.k);
+      pblocks.back() += pack_ctas(c.cout, c.cin, c.k * c.k);
       if (h->exact_tc()) {
         SplitEntry& e = stt.back().e[stt.back().n++];
         e.wf = (const float*)(h->ws + p.wf); e.wd = (const float*)(h->ws + p.wd);

@@ -86,7 +86,7 @@ __global__ void __launch_bounds__(NT) conv_kernel(ConvArgs a) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
 
-  const int taps = a.k * a.k;
+  const int taps = a.kh * a.kw;
   const int Ktot = taps * a.Csrc;
   const int nchunks = FLATK ? (Ktot + BK - 1) / BK : taps * (a.Csrc / BK);
   const int cpt = FLATK ? 1 : a.Csrc / BK;   // chunks per tap
@@ -95,10 +95,10 @@ __global__ void __launch_bounds__(NT) conv_kernel(ConvArgs a) {
     float av[8];
     if (!FLATK) {
       const int tap = ch / cpt, c0 = (ch % cpt) * BK;
-      const int tr = tap / a.k, ts = tap % a.k;
+      const int tr = tap / a.kw, ts = tap % a.kw;
       int sy, sx;
-      bool ok = row_ok && src_coord(ry, tr, a.stride, a.pad, a.SH, a.dgrad, sy) &&
-                src_coord(rx, ts, a.stride, a.pad, a.SW, a.dgrad, sx);
+      bool ok = row_ok && src_coord(ry, tr, a.stride, a.pad_h, a.SH, a.dgrad, sy) &&
+                src_coord(rx, ts, a.stride, a.pad_w, a.SW, a.dgrad, sx);
       if (ok) {
         const T* p = src + ((long long)(rf * a.SH + sy) * a.SW + sx) * a.src_pitch + a.src_coff + c0 + lhalf * 8;
         Vec8<T>::load(p, av);
@@ -114,8 +114,8 @@ __global__ void __launch_bounds__(NT) conv_kernel(ConvArgs a) {
         if (row_ok && kf < Ktot) {
           const int tap = kf / a.Csrc, c = kf % a.Csrc;
           int sy, sx;
-          if (src_coord(ry, tap / a.k, a.stride, a.pad, a.SH, a.dgrad, sy) &&
-              src_coord(rx, tap % a.k, a.stride, a.pad, a.SW, a.dgrad, sx))
+          if (src_coord(ry, tap / a.kw, a.stride, a.pad_h, a.SH, a.dgrad, sy) &&
+              src_coord(rx, tap % a.kw, a.stride, a.pad_w, a.SW, a.dgrad, sx))
             v = to_f<T>(src[((long long)(rf * a.SH + sy) * a.SW + sx) * a.src_pitch + a.src_coff + c]);
         }
         av[j] = v;

@@ -104,7 +104,7 @@ __global__ void pack_all_kernel(const __grid_constant__ PackTable t) {
   int ei = 0;
   while (ei + 1 < t.n && (int)blockIdx.x >= t.e[ei + 1].block0) ++ei;       // <= 32 entries, uniform per block
   const PackEntry& q = t.e[ei];
-  const int taps = q.k * q.k;
+  const int taps = q.taps;
   const long long total = (long long)q.cout * q.cin * taps;
   float av = 0.f;
   __shared__ float wmax[TPB / 32];

@@ -496,20 +496,22 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
                 int a_stride = 1, const UmmaTcOpts* tc = nullptr) {
   plan.enabled = false;
   if (int rc = resolve_encode(ctx)) return rc;
-  if (a_stride == 2) {
-    // strided TMA: tiles enumerate OUTPUT pixels, the A box steps over the input with stride 2
+  if (a_stride == 2 || (a_stride == 1 && (a.H != o.H || a.W != o.W))) {
+    // tiles enumerate OUTPUT pixels and the A map keeps the input's dims: stride 2 (the A box steps over the input with TMA
+    // element stride 2), or a valid stride-1 layer whose output is smaller than its input (taps with non-negative shifts)
     View ao = a; ao.H = o.H; ao.W = o.W;
     if (int rc = bind_common(ctx, plan, ao, o, F, K, N, ntaps, w, 1, tc)) return rc;
     plan.enabled = false;
     UmmaConvParams& q = plan.p;
-    q.a_stride = 2;
+    q.a_stride = a_stride;
     cuuint64_t dims[4] = {(cuuint64_t)K, (cuuint64_t)a.W, (cuuint64_t)a.H, (cuuint64_t)F};
     cuuint64_t str[3] = {(cuuint64_t)a.pitch * 2, (cuuint64_t)a.W * a.pitch * 2, (cuuint64_t)a.H * a.W * a.pitch * 2};
-    cuuint32_t box[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)(2 * q.bw), (cuuint32_t)(2 * q.bh), (cuuint32_t)q.bf};
-    if (int rc = encode(ctx, &plan.tmap_a, 4, reinterpret_cast<__half*>(a.base) + a.coff, dims, str, box, 2)) return rc;
+    cuuint32_t box[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)(a_stride * q.bw), (cuuint32_t)(a_stride * q.bh), (cuuint32_t)q.bf};
+    if (int rc = encode(ctx, &plan.tmap_a, 4, reinterpret_cast<__half*>(a.base) + a.coff, dims, str, box, a_stride)) return rc;
     plan.tmap_a_lo = plan.tmap_a;
     if (a.lo_off)
-      if (int rc = encode(ctx, &plan.tmap_a_lo, 4, reinterpret_cast<__half*>(reinterpret_cast<char*>(a.base) + a.lo_off) + a.coff, dims, str, box, 2)) return rc;
+      if (int rc = encode(ctx, &plan.tmap_a_lo, 4, reinterpret_cast<__half*>(reinterpret_cast<char*>(a.base) + a.lo_off) + a.coff, dims, str, box, a_stride))
+        return rc;
     plan.tmap_a2 = plan.tmap_a; plan.tmap_a2_lo = plan.tmap_a_lo;
     plan.enabled = true;
     return 0;
@@ -595,8 +597,9 @@ void umma_context_init(UmmaContext&) {}
 void umma_context_destroy(UmmaContext&) {}
 
 int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int ntaps,
-                        const int* dy, const int* dx, const __half* w_tap_n_k, const float* bias, int relu, const UmmaTcOpts* tc) {
-  if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, ntaps, w_tap_n_k, 1, tc)) return rc;
+                        const int* dy, const int* dx, const __half* w_tap_n_k, const float* bias, int relu, const UmmaTcOpts* tc, int stride) {
+  if (stride != 1 && stride != 2) { set_thread_error("umma conv: stride must be 1 or 2"); return 1; }
+  if (int rc = bind_common(ctx, plan, in, out, F, cin, cout, ntaps, w_tap_n_k, stride, tc)) return rc;
   for (int t = 0; t < ntaps; ++t) { plan.p.tap_dy[t] = dy[t]; plan.p.tap_dx[t] = dx[t]; }
   plan.p.bias = bias; plan.p.relu = relu; plan.p.accumulate = 0;
   mark_tc_ok(plan, in.W, false);

@@ -14,7 +14,7 @@
 
 namespace ssnb {
 
-constexpr int UMMA_MAX_TAPS = 16;
+constexpr int UMMA_MAX_TAPS = 25;         // a 5x5 kernel in one launch (InceptionV3)
 
 struct UmmaContext {
   void* encode_tiled = nullptr;   // cuTensorMapEncodeTiled, resolved through cudaGetDriverEntryPoint
@@ -87,9 +87,12 @@ void umma_context_destroy(UmmaContext& ctx);
 // forward convolution plan (stride 1): in/out views, weights wd = [tap][cout][cin] fp16
 int umma_conv_bind_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int k, int pad,
                        int stride, const __half* w_tap_n_k, const float* bias, const UmmaTcOpts* tc = nullptr);
-// generic tap table variant (conv1 in space-to-depth form: 16 taps of a 4x4 stride-1 convolution)
+// generic tap table variant (BNInception's conv1 in space-to-depth form: 4 taps over the packed input; InceptionV3's
+// kh x kw layers).  Tiles run at the output's geometry; the A map keeps the input's dims, so an output smaller than the input
+// (valid padding) reads in[out * stride + (dy, dx)] with TMA zero fill outside the image.  stride: 1 or 2
 int umma_conv_bind_taps(UmmaContext& ctx, UmmaConvPlan& plan, View in, View out, int F, int cin, int cout, int ntaps,
-                        const int* dy, const int* dx, const __half* w_tap_n_k, const float* bias, int relu, const UmmaTcOpts* tc = nullptr);
+                        const int* dy, const int* dx, const __half* w_tap_n_k, const float* bias, int relu, const UmmaTcOpts* tc = nullptr,
+                        int stride = 1);
 // data-gradient plan (stride 1): dz/dx gradient views, weights wf = [tap][cin][cout] fp16
 int umma_conv_bind_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz, View dx, int F, int cin, int cout, int k, int pad,
                          const __half* w_tap_k_n, int accumulate, const UmmaTcOpts* tc = nullptr);

@@ -24,6 +24,10 @@ class Config(C.Structure):
                 ("training", C.c_int32), ("grad_scale", C.c_float), ("bn1_train", C.c_int32), ("reserved", C.c_int32 * 2)]
 
 
+class IV3Config(C.Structure):
+    _fields_ = [("in_channels", C.c_int32), ("frames", C.c_int32), ("precision", C.c_int32), ("reserved", C.c_int32)]
+
+
 class HeadsCfg(C.Structure):
     _fields_ = [("n", C.c_int32), ("props_per_video", C.c_int32), ("num_class", C.c_int32),
                 ("feat_dim", C.c_int32), ("feat_mult", C.c_int32), ("fg_per_video", C.c_int32),
@@ -141,6 +145,20 @@ SIGNATURES = {
                          + [_vp] * 7 + [_sz, _vp]),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
+    "ssnb_iv3_num_convs": (_i, []),
+    "ssnb_iv3_conv_info": (_i, [_i, _i, C.c_char_p, _i] + [_ip] * 7),
+    "ssnb_iv3_create": (_i, [C.POINTER(IV3Config), C.POINTER(_vp)]),
+    "ssnb_iv3_destroy": (_i, [_vp]),
+    "ssnb_iv3_workspace_bytes": (_sz, [_vp]),
+    "ssnb_iv3_set_workspace": (_i, [_vp, _vp, _sz]),
+    "ssnb_iv3_pack_weights": (_i, [_vp, _pp, _pp, _pp, _pp, _pp, _pp, _vp]),
+    "ssnb_iv3_forward": (_i, [_vp, _vp, _vp, _vp]),
+    "ssnb_iv3_num_ops": (_i, [_vp]),
+    "ssnb_iv3_op_info": (_i, [_vp, _i, C.c_char_p, _i, C.c_char_p, _i, C.c_char_p, _i, _ip, _ip, _ip, _ip]),
+    "ssnb_iv3_value_info": (_i, [_vp, C.c_char_p, _ip, _ip, _ip, C.c_char_p, _i, _ip]),
+    "ssnb_iv3_value_write": (_i, [_vp, C.c_char_p, _vp, _vp]),
+    "ssnb_iv3_value_read": (_i, [_vp, C.c_char_p, _i, _vp, _vp]),
+    "ssnb_iv3_run_op": (_i, [_vp, _i, _vp, _vp]),
     "ssnb_sgd_step_groups": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp]),
 }
 

@@ -2,8 +2,9 @@
 attributes and state_dict keys, so the loops in ssn_train.py:191-253 / ssn_test.py:68-96 run
 against it unchanged.  The BNInception backbone, STPP and the heads execute in libssn_b200.so.
 
-Only base_model='BNInception' with RGB / Flow input is accelerated (the hot path this repo
-covers); other backbones raise ValueError like an unknown name does in the reference (:153-154).
+base_model='BNInception' with RGB / Flow input is accelerated (the hot path this repo covers), and
+base_model='InceptionV3' at test time (forward only); other backbones raise ValueError like an unknown name does in the
+reference (:153-154).
 """
 import torch
 from torch import nn
@@ -29,8 +30,9 @@ class _BNInceptionModel(torch.nn.Module):
 
     # ---- construction (ssn_models.py:69-154) ------------------------------------------------------
     def _prepare_base_model(self, base_model):
-        if base_model != 'BNInception':
-            raise ValueError('Unknown base model: {} (the H100 hot path implements BNInception)'.format(base_model))
+        if base_model not in ('BNInception', 'InceptionV3'):
+            raise ValueError('Unknown base model: {} (the H100 hot path implements BNInception and, at test time, '
+                             'InceptionV3)'.format(base_model))
         if self.modality == 'RGB':
             in_ch = 3 * self.new_length
         elif self.modality == 'Flow':
@@ -38,15 +40,17 @@ class _BNInceptionModel(torch.nn.Module):
         else:
             raise ValueError('modality {} is outside the accelerated path (RGB, Flow)'.format(self.modality))
         import model_zoo
+        net = getattr(model_zoo, base_model)
         if self.modality == 'Flow':
             # like the reference: build the 3-channel network (this is where pretrained RGB weights would be loaded) and swap
-            # conv1 for the mean-expanded 2*new_length-channel kernel (_construct_flow_model, ssn_models.py:318-343)
-            self.base_model = self._construct_flow_model(model_zoo.BNInception(in_channels=3))
+            # the first convolution for the mean-expanded 2*new_length-channel kernel (_construct_flow_model, ssn_models.py:318-343)
+            self.base_model = self._construct_flow_model(net(in_channels=3))
             assert self.base_model.in_channels() == in_ch
         else:
-            self.base_model = model_zoo.BNInception(in_channels=in_ch)
-        self.base_model.last_layer_name = 'fc'
-        self.input_size = 224
+            self.base_model = net(in_channels=in_ch)
+        # BNInception (ssn_models.py:121-132) and InceptionV3 (:133-144) differ in the last layer's name and the input size only
+        self.base_model.last_layer_name = 'fc' if base_model == 'BNInception' else 'top_cls_fc'
+        self.input_size = 224 if base_model == 'BNInception' else 299
         self.input_mean = [104, 117, 128]
         self.input_std = [1]
         if self.modality == 'Flow':
@@ -133,6 +137,12 @@ class _BNInceptionModel(torch.nn.Module):
             {'params': normal_bias, 'lr_mult': 2, 'decay_mult': 0, 'name': "normal_bias"},
             {'params': bn, 'lr_mult': 1, 'decay_mult': 0, 'name': "BN scale/shift"},
         ]
+
+    def _require_trainable_backbone(self):
+        from model_zoo import InceptionV3
+        if isinstance(self.base_model, InceptionV3):
+            raise NotImplementedError("fused_step trains the BNInception backbone; InceptionV3 runs at test time only: "
+                                      "training InceptionV3 (backward schedule, fused_step) is a follow-up")
 
     def _frames(self, input):
         sample_len = (3 if self.modality == "RGB" else 2) * self.new_length
@@ -330,7 +340,7 @@ class SSN(_BNInceptionModel):
         assert F_ % num_crop == 0, "frame count must be a multiple of the crop count"
         nt = F_ // num_crop
         with torch.no_grad():
-            base_out = self.base_model(frames).contiguous()          # [F, 1024]: fc is Identity / eval-mode Dropout at test time
+            base_out = self.base_model(frames).contiguous()          # [F, 1024 | 2048]: fc is Identity / eval-mode Dropout at test time
         out = torch.empty(nt, self.test_fc.out_features, dtype=torch.float32, device=base_out.device)
         from ssn_b200.engine import _stream
         with torch.cuda.device(base_out.device):
@@ -347,6 +357,7 @@ class SSN(_BNInceptionModel):
         gradients bucket by bucket while the backward of the lower layers is still running."""
         import ctypes as C
         from ssn_b200.engine import _stream
+        self._require_trainable_backbone()
         assert self.with_regression, "fused_step implements the regression configuration"
         if not input.is_cuda:
             raise RuntimeError("SSN(H100).fused_step needs CUDA tensors (libssn_b200 has no CPU path)")

@@ -474,6 +474,51 @@ int ssnb_frame_transform(const ssnb_frame_cfg* cfg, const ssnb_frame_group* grou
                          const uint8_t* src, size_t src_bytes, float* dst, int64_t dst_floats, void* workspace, size_t workspace_bytes,
                          void* stream);
 
+/* ---- InceptionV3 backbone at test time: replaces model_zoo.InceptionV3 (pytorch_load.py:64-67, inceptionv3.yaml) as used by
+ *      SSN.test_forward and BinaryClassifier scoring with --arch InceptionV3 (ssn_models.py:133-139, binary_model.py:175-178) ----
+ * Forward only, frozen BatchNorm folded into each convolution, in every precision: EXACT_FP32 (fp32 SIMT convolutions),
+ * FAST_FP16 and EXACT_TC (every convolution on the wgmma kernel; EXACT_TC with split operands, an fp32 epilogue and the
+ * output's operand planes).  A handle of its own: the BNInception functions above do not take it, and errors are read with
+ * ssnb_last_error(NULL).  Creation only plans (no device call), so the plan can be inspected without a
+ * GPU.  Activations are NHWC fp32; the branch ends of every inception block are channel slices of the block's concat buffer
+ * ("<block>_join"), so no concat runs; each value has a buffer of its own (no reuse across the pass). */
+typedef struct ssnb_iv3* ssnb_iv3_handle;
+typedef struct {
+  int32_t in_channels; /* 3 (RGB) or 10 (Flow 2x5) */
+  int32_t frames;      /* F images per call, >= 1 */
+  int32_t precision;   /* SSNB_EXACT_FP32 | SSNB_FAST_FP16 | SSNB_EXACT_TC */
+  int32_t reserved;
+} ssnb_iv3_config;
+/* the 94 convolutions in graph order; name is the yaml's blob (conv id "<name>_Conv2D", BatchNorm id "<name>_batchnorm") */
+int ssnb_iv3_num_convs(void);
+int ssnb_iv3_conv_info(int idx, int in_channels, char* name, int name_cap, int* cin, int* cout, int* kh, int* kw, int* stride, int* pad_h,
+                       int* pad_w);
+int ssnb_iv3_create(const ssnb_iv3_config* cfg, ssnb_iv3_handle* out);
+int ssnb_iv3_destroy(ssnb_iv3_handle h);
+size_t ssnb_iv3_workspace_bytes(ssnb_iv3_handle h);
+/* dev_ptr 1024-byte aligned, at least ssnb_iv3_workspace_bytes; packed weights must be set again afterwards */
+int ssnb_iv3_set_workspace(ssnb_iv3_handle h, void* dev_ptr, size_t bytes);
+/* arrays of 94 device pointers in graph order, reference shapes: w [cout, cin, kh, kw], b / gamma / beta / mean / var [cout]
+ * (BatchNorm eps 1e-5).  Call again whenever a parameter changes. */
+int ssnb_iv3_pack_weights(ssnb_iv3_handle h, const float* const* w, const float* const* b, const float* const* gamma,
+                          const float* const* beta, const float* const* mean, const float* const* var, void* stream);
+/* input [F, C, 299, 299] fp32 NCHW -> feat [F, 2048] fp32 (top_cls_pool, the 8x8 average pool; top_cls_fc is replaced by
+ * Identity / Dropout) */
+int ssnb_iv3_forward(ssnb_iv3_handle h, const float* input_nchw, float* feat, void* stream);
+/* introspection for the plan and the launch-by-launch tests: op kinds "conv" | "maxpool" | "avgpool" | "gpool", the names of the
+ * values an op reads and writes (the yaml's blob names; the last op writes "top_cls_global_pool", the feat output), its
+ * convolution index (-1 for pools) and a pool's window, stride and pad (0 / 1 / 0 for convolutions).  A value's shape, its buffer and its channel offset in that buffer. */
+int ssnb_iv3_num_ops(ssnb_iv3_handle h);
+int ssnb_iv3_op_info(ssnb_iv3_handle h, int op, char* kind, int kind_cap, char* in_name, int in_cap, char* out_name, int out_cap, int* conv,
+                     int* k, int* stride, int* pad);
+int ssnb_iv3_value_info(ssnb_iv3_handle h, const char* name, int* c, int* hh, int* ww, char* buffer, int buffer_cap, int* coff);
+/* NCHW fp32 [F, C, H, W] copies in and out of a value (FAST: of its fp16 storage; EXACT_TC: a write also refreshes its operand
+ * planes); planes = 1 (EXACT_TC only) reads hi + lo of the value's operand planes instead.  ssnb_iv3_run_op runs one op on
+ * what the workspace holds (feat: the last op's output, else unused) */
+int ssnb_iv3_value_write(ssnb_iv3_handle h, const char* name, const float* src_nchw, void* stream);
+int ssnb_iv3_value_read(ssnb_iv3_handle h, const char* name, int planes, float* dst_nchw, void* stream);
+int ssnb_iv3_run_op(ssnb_iv3_handle h, int op, float* feat, void* stream);
+
 /* fused SGD-momentum step over flat fp32 buffers (ssn_train.py:141-144 torch.optim.SGD semantics), the whole model in ONE
  * launch: the flat buffers are cut into n_seg <= 512 segments (one per parameter tensor; seg_end = cumulative element ends,
  * device int64) with their parameter group's learning rate and weight decay (device fp32 arrays): the per-group lr_mult /
