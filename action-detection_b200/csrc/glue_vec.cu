@@ -102,8 +102,9 @@ template <> struct Vec<__half> {
     }
   }
   static __device__ __forceinline__ uint32_t any_tag(Tags a, uint32_t t4) { return zero_bytes(a.x ^ t4) | zero_bytes(a.y ^ t4); }
-  // NaN-propagating half2 maximum; the tap index (16-bit, in the lanes of the half2 values) moves where v > best or v is NaN
-  // (so a later NaN takes it from an earlier one, as in ATen), or when nothing was taken yet
+  // NaN-propagating half2 maximum; value and tap index (16-bit, in the lanes of the half2 values) move together where
+  // v > best or v is NaN (so a later NaN takes them from an earlier one, as in ATen), or when nothing was taken yet.  The
+  // value is the taken tap's bits: __hmax2_nan would give +0 for a window whose first maximum is -0.
   struct Max {
     uint32_t best[4] = {0u, 0u, 0u, 0u};
     uint32_t bi[4] = {0u, 0u, 0u, 0u};
@@ -114,9 +115,8 @@ template <> struct Vec<__half> {
       for (int j = 0; j < 4; ++j) {
         const __half2 hv = *reinterpret_cast<const __half2*>(&v[j]);
         const __half2 hb = *reinterpret_cast<const __half2*>(&best[j]);
-        const __half2 hn = __hmax2_nan(hb, hv);
         const uint32_t m = first ? 0xFFFFFFFFu : (__hgt2_mask(hv, hb) | __hneu2_mask(hv, hv));
-        best[j] = first ? v[j] : *reinterpret_cast<const uint32_t*>(&hn);
+        best[j] = (v[j] & m) | (best[j] & ~m);
         bi[j] = (tag & m) | (bi[j] & ~m);
       }
     }

@@ -19,7 +19,9 @@ on one launch's plan; `regimes(launch)` is the set a launch is in.
 
 Every gated EXACT_TC plan passes UmmaConvParams::tc_ok in this network (engine.cu: ssnb_set_workspace), so the list is the
 same for FAST and EXACT_TC except for `stages` (EXACT_TC stages hold both operand planes).  bn_mode='partial' runs the same
-launches (conv1 raw changes its epilogue, not its tiles).  CPU only; nothing here touches a device.
+launches (conv1 raw changes its epilogue, not its tiles).  `iv3_schedule(frames, precision, sms)` lists the InceptionV3
+test-time engine's forward launches the same way; `reached` / `greedy_cover` take it as `sched`.  CPU only; nothing here
+touches a device.
 """
 import functools
 
@@ -283,6 +285,54 @@ def schedule(in_channels, frames, precision, sms=SMS_H100_SXM, training=True, wa
     return launches
 
 
+# ---- the InceptionV3 test-time engine ----------------------------------------------------------------------------------
+# The frame counts tests/test_gpu_inception_v3.py checks every launch at: the small and ragged ones, the benchmarked 40 ticks
+# x 10 crops, and 89 / 129, which reach the one_and_two_tiles pairs of mixed_8's stride-2 outputs and the 8x8 layers of
+# mixed_9 / mixed_10 that the others miss (129 also leaves one frame alone in the second 128-frame box of the 1x1x128
+# tiles).  Together they reach every (precision, launch, regime) of the forward that a frame count in [1, FRAME_RANGE]
+# reaches on a 132-SM H100 (tests/test_tile_regimes.py holds them to it).
+IV3_FRAME_SET = (1, 10, 37, 400, 89, 129)
+IV3_STEM_K = 16                 # inception_v3.cu kStemK: the stem's 3 or 10 input channels zero-padded for the wgmma kernel
+
+
+@functools.lru_cache(maxsize=None)
+def _iv3_convs():
+    """[(name, cin, cout, kh, kw, out_h, out_w)] of the 94 convolutions in the yaml's (the engine's) order, geometry walked
+    through oracle/inception_v3_oracle.layers (in_channels only changes the stem's cin, which the plan pads to 16)"""
+    from . import inception_v3_oracle as IV
+    hw = {"data": (IV.INPUT_SIZE, IV.INPUT_SIZE)}
+    ch = {"data": 3}
+    out = []
+    for id_, op, o, ins, a in IV.layers(3):
+        if op == "Convolution":
+            h, w = hw[ins[0]]
+            oh = (h + 2 * a["pad_h"] - a["kernel_h"]) // a["stride_h"] + 1
+            ow = (w + 2 * a["pad_w"] - a["kernel_w"]) // a["stride_w"] + 1
+            out.append((o[:-len("_Conv2D")], ch[ins[0]], a["num_output"], a["kernel_h"], a["kernel_w"], oh, ow))
+            hw[o], ch[o] = (oh, ow), a["num_output"]
+        elif op == "Pooling":
+            h, w = hw[ins[0]]
+            k, s, p = a["kernel_size"], a["stride"], a["pad"]
+            hw[o], ch[o] = (_cdiv(h + 2 * p - k, s) + 1, _cdiv(w + 2 * p - k, s) + 1), ch[ins[0]]      # ceil mode
+        elif op == "Concat":
+            hw[o], ch[o] = hw[ins[0]], sum(ch[i] for i in ins)
+        elif op in ("BN", "ReLU"):
+            hw[o], ch[o] = hw[ins[0]], ch[ins[0]]
+    return tuple(out)
+
+
+def iv3_schedule(frames, precision, sms=SMS_H100_SXM):
+    """[launch dict] of one InceptionV3 forward (inception_v3.cu: bind_plans, run_op), as `schedule`'s: one umma_conv_kernel
+    launch per convolution in engine order, each planned at its output geometry (valid stride-1 and stride-2 layers tile
+    output pixels, bind_common), K = the stem's 16 padded channels or cin, N = cout, kh * kw taps"""
+    if precision not in ("exact_tc", "fast"):
+        raise ValueError("only the tensor-core precisions run the wgmma kernels")
+    split = precision == "exact_tc"
+    return [dict(kernel="umma_conv_kernel", phase=0, op=name,
+                 plan=conv_plan(ow, oh, frames, IV3_STEM_K if i == 0 else cin, cout, kh * kw, split, sms))
+            for i, (name, cin, cout, kh, kw, oh, ow) in enumerate(_iv3_convs())]
+
+
 def log_key(launch):
     """what ssnb_timing_launches reports for the launch: (kernel, phase, op, a, b) with (a, b) = (tiles, block_n) for
     umma_conv_kernel and (ctas, splits) for umma_wgrad_kernel"""
@@ -313,20 +363,21 @@ def regimes(launch):
     return {name for name, pred in table.items() if pred(launch["plan"])}
 
 
-def reached(in_channels, frames, sms, precisions=("exact_tc", "fast")):
-    """{(precision, launch id, regime)} of the training schedule at this frame count"""
+def reached(in_channels, frames, sms, precisions=("exact_tc", "fast"), sched=None):
+    """{(precision, launch id, regime)} of the training schedule at this frame count; sched(frames, precision, sms): another
+    launch list (iv3_schedule; in_channels is then unused)"""
     out = set()
     for prec in precisions:
-        for l in schedule(in_channels, frames, prec, sms):
+        for l in (schedule(in_channels, frames, prec, sms) if sched is None else sched(frames, prec, sms)):
             out |= {(prec, launch_id(l), r) for r in regimes(l)}
     return out
 
 
-def greedy_cover(in_channels, frame_range, sms, cost=lambda f: f):
+def greedy_cover(in_channels, frame_range, sms, cost=lambda f: f, sched=None):
     """greedy weighted set cover of every (precision, launch, regime) reached somewhere in frame_range: repeatedly the frame
     count with the most newly reached pairs per cost (ties: the smaller frame count).  Returns (chosen frame counts in the
     order picked, the union of reached pairs, {frame count: its pairs})"""
-    per = {f: reached(in_channels, f, sms) for f in frame_range}
+    per = {f: reached(in_channels, f, sms, sched=sched) for f in frame_range}
     universe = set().union(*per.values())
     left, chosen = set(universe), []
     while left:

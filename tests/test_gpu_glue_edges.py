@@ -21,6 +21,7 @@ pytestmark = pytest.mark.gpu
 from oracle import schedule_check as S
 from oracle import ssn_oracle as O
 from oracle import synth
+from oracle.edge_inputs import edge_input as _edge_input, same_bits
 
 GRAD_SCALE = 4096.0
 PRECISIONS = ("exact", "exact_tc", "fast")
@@ -77,32 +78,6 @@ def _grads(dev):
 
 
 # ---- A: every pool op on its own ------------------------------------------------------------------------------------------
-DYADIC = torch.tensor([-2.0, -1.0, -0.5, -0.0, 0.0, 0.5, 1.0, 2.0])       # exact in fp16: windows full of exact ties
-
-
-def _edge_input(frames, c, h, w, stride, pad, gen):
-    """dyadic values; per channel one edge case, in the first and the last frame (the others: plain dyadic values)"""
-    x = DYADIC[torch.randint(0, len(DYADIC), (frames, c, h, w), generator=gen)]
-    x[:, 0::16] = 0.5                                                      # constant: every window tied
-    x[:, 1::16] = torch.where(torch.rand(x[:, 1::16].shape, generator=gen) < 0.5, -0.0, 0.0)    # +-0 only
-    y0 = x0 = stride - pad                    # the window of output (1, 1): tap t reads input (y0 + t // 3, x0 + t % 3)
-    for f in sorted({0, frames - 1}):
-        for t in range(9):
-            x[f, 2 + t, y0 + t // 3, x0 + t % 3] = NAN                   # one NaN at each of the 9 taps
-        x[f, 11, y0, x0] = x[f, 11, y0 + 2, x0 + 1] = NAN                # two NaNs in one window
-        x[f, 12, y0, x0 + 1], x[f, 12, y0 + 1, x0 + 2] = INF, NAN        # NaN after +inf
-        x[f, 13, y0, x0], x[f, 13, y0 + 2, x0 + 2] = NAN, -INF           # NaN before -inf
-        x[f, 14, y0 + 1, x0 + 1], x[f, 14, y0 + 2, x0] = INF, -INF       # +inf and -inf (average: NaN)
-        x[f, 15, :5, :5] = -INF                                           # windows of -inf only, padding around some
-        x[f, 15, h // 2:h // 2 + 5, w // 2:w // 2 + 5] = -INF
-        x[f, 17, -1, -1], x[f, 17, -1, 0], x[f, 17, 0, -1] = NAN, INF, -INF      # poison in the last row and column
-        x[f, 17, -1, w // 2], x[f, 17, h // 2, -1] = NAN, INF
-        x[f, 18, -2:, -2:] = -INF                                         # (part of) the partial last window
-        x[f, 19, -1, -3:] = NAN                                           # NaNs side by side in the last row
-        x[f, 20, 2:7, 2:7] = INF                                          # tied +inf
-    return x
-
-
 def _pool_ops(eng):
     """[(op index, kind, input, output, attrs, accumulates)]; accumulates: a later op reads the same input, so its gradient
     is already in d(input) when this op's backward runs"""
@@ -114,10 +89,6 @@ def _pool_ops(eng):
         if kind in ("maxpool", "avgpool"):
             out.append((i, kind, inp, o, G.ops[i]["a"], any(e[1] == inp for e in ops[i + 1:])))
     return out
-
-
-def _same(got, ref):
-    return (got == ref) | (got.isnan() & ref.isnan())
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -143,8 +114,8 @@ def test_pool_ops_on_ties_and_non_finite(precision, frames):
             xr = x.double().requires_grad_(True)
             ref = pool(xr, k, s, p, ceil_mode=True)
             if kind == "maxpool":
-                if not _same(y, ref.detach()).all():
-                    bad.append("%s fwd: %d values differ" % (out, int((~_same(y, ref.detach())).sum())))
+                if not same_bits(y, ref.detach()).all():       # the sign of a tied zero included
+                    bad.append("%s fwd: %d values differ" % (out, int((~same_bits(y, ref.detach())).sum())))
             else:
                 r = ref.detach()
                 masks = [(t(y) == t(r)).all() for t in (torch.isnan, torch.isposinf, torch.isneginf)]

@@ -109,3 +109,63 @@ def test_plan_invariants(frames, sms):
 def test_launch_ids_are_unique():
     ids = [(p, T.launch_id(l)) for p in ("exact_tc", "fast") for l in T.schedule(3, 1, p)]
     assert len(ids) == len(set(ids)) == len(_launch_ids())
+
+
+# ---- the InceptionV3 test-time engine ------------------------------------------------------------------------------------
+_IV3_PER = {}
+
+
+def _iv3_per_frame(sms):
+    if sms not in _IV3_PER:
+        _IV3_PER[sms] = {f: T.reached(None, f, sms, sched=T.iv3_schedule) for f in FRAMES}
+    return _IV3_PER[sms]
+
+
+def test_iv3_frame_set_reaches_every_regime():
+    """every (precision, launch, regime) of the InceptionV3 forward that some frame count in [1, 640] reaches at 132 SMs is
+    reached by IV3_FRAME_SET, the frame counts tests/test_gpu_inception_v3.py checks every launch at"""
+    per = _iv3_per_frame(T.SMS_H100_SXM)
+    universe = set().union(*per.values())
+    covered = set().union(*(per[f] for f in T.IV3_FRAME_SET))
+    print("\nInceptionV3, 132 SMs: frame set %s, %d of %d (precision, launch, regime) pairs" % (
+        list(T.IV3_FRAME_SET), len(covered), len(universe)))
+    print("    %-24s %5s %5s" % ("regime", "reach", "set"), *_table(universe, covered), sep="\n")
+    missing = sorted(universe - covered)
+    assert not missing, "IV3_FRAME_SET misses %d pairs: %s" % (len(missing), ", ".join("%s %s %s" % m for m in missing))
+    assert {r for (_p, _l, r) in covered} == set(T.CONV_REGIMES)
+    assert len(T.IV3_FRAME_SET) == len(set(T.IV3_FRAME_SET)) and all(1 <= f <= T.FRAME_RANGE for f in T.IV3_FRAME_SET)
+
+
+def test_iv3_coverage_at_114_sms():
+    """IV3_FRAME_SET's coverage on an H100 PCIe (114 SMs), reported"""
+    per = _iv3_per_frame(T.SMS_H100_PCIE)
+    universe = set().union(*per.values())
+    covered = set().union(*(per[f] for f in T.IV3_FRAME_SET))
+    missing = sorted(universe - covered)
+    print("\nInceptionV3, 114 SMs: frame set %s reaches %d of %d pairs (%.1f %%)%s" % (
+        list(T.IV3_FRAME_SET), len(covered), len(universe), 100.0 * len(covered) / len(universe),
+        "; missed: " + ", ".join("%s %s %s" % m for m in missing) if missing else ""))
+    print("    %-24s %5s %5s" % ("regime", "reach", "set"), *_table(universe, covered), sep="\n")
+    assert {r for (_p, _l, r) in universe} == set(T.CONV_REGIMES)
+
+
+@pytest.mark.parametrize("sms", [T.SMS_H100_SXM, T.SMS_H100_PCIE])
+@pytest.mark.parametrize("frames", sorted(T.IV3_FRAME_SET))
+def test_iv3_plan_invariants(frames, sms):
+    """one launch per convolution, in the engine's order with its channel counts and taps (the stem's K padded to 16), the
+    boxes pick_box gives InceptionV3's widths, and the same tiles for both precisions"""
+    from ssn_b200.inception_v3 import conv_table
+    for cin in (3, 10):
+        table = conv_table(cin)
+        for prec in ("exact_tc", "fast"):
+            ls = T.iv3_schedule(frames, prec, sms)
+            assert [l["op"] for l in ls] == [c[0] for c in table]
+            for i, (l, (_n, ci, co, kh, kw, _s, _ph, _pw)) in enumerate(zip(ls, table)):
+                p = l["plan"]
+                assert (p["kchunks"], p["ntaps"]) == (-(-(16 if i == 0 else ci) // 64), kh * kw)
+                assert p["n_tiles"] * p["block_n"] >= co and p["block_n"] % 16 == 0 and p["block_n"] <= 128
+                assert 1 <= p["grid"] <= min(sms, p["total"]) and sum(t * n for t, n in p["per_cta"].items()) == p["total"]
+        assert [T.log_key(l) for l in T.iv3_schedule(frames, "exact_tc", sms)] == \
+            [T.log_key(l) for l in T.iv3_schedule(frames, "fast", sms)]
+    boxes = collections.Counter(l["plan"]["box"] for l in T.iv3_schedule(frames, "fast", sms))
+    assert boxes == {(1, 1, 128): 74, (4, 4, 8): 20}, boxes
