@@ -8,7 +8,7 @@ FLAGS="$ARCH -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -I../../
 mkdir -p build
 pids=()
 for f in engine simt_conv simt_glue heads classifier umma_conv umma_wgrad s2d_glue glue_vec tc_glue detect detection_ap proposals proposal_lists proposal_ar bn_train frames inception_v3; do
-  if [ ! -f build/$f.o ] || [ $f.cu -nt build/$f.o ] || [ common.cuh -nt build/$f.o ] || [ umma_conv.cuh -nt build/$f.o ] || [ umma_dev.cuh -nt build/$f.o ] || [ rank_key.cuh -nt build/$f.o ] || [ ../../include/ssnb.h -nt build/$f.o ] || [ build.sh -nt build/$f.o ]; then
+  if [ ! -f build/$f.o ] || [ $f.cu -nt build/$f.o ] || [ common.cuh -nt build/$f.o ] || [ graph.cuh -nt build/$f.o ] || [ umma_conv.cuh -nt build/$f.o ] || [ umma_dev.cuh -nt build/$f.o ] || [ rank_key.cuh -nt build/$f.o ] || [ ../../include/ssnb.h -nt build/$f.o ] || [ build.sh -nt build/$f.o ]; then
     $NVCC $FLAGS ${PTXAS_V:+-Xptxas -v} -c $f.cu -o build/$f.o &
     pids+=($!)
   fi

@@ -20,6 +20,7 @@ struct View {
 
 extern std::atomic<long long> g_launches;  // every kernel launch of this library bumps it
 void set_thread_error(const std::string& s);
+const std::string& thread_error();
 
 // Per-launch device timing (ssnb_timing_begin / ssnb_timing_report, bench.py's roofline): while a timing session is open
 // on this thread, every launch records a CUDA event behind itself on its stream; a launch's time is the distance to the

@@ -14,6 +14,7 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
+#include "graph.cuh"
 #include "umma_conv.cuh"
 
 namespace ssnb {
@@ -63,36 +64,31 @@ static const BlockSpec kBlocks[10] = {
     {"4d", 96, 128, 192, 160, 192, 192, 0, 128, 1}, {"4e", 0, 128, 192, 192, 256, 256, 1, 0, 2},
     {"5a", 352, 192, 320, 160, 224, 224, 0, 128, 1}, {"5b", 352, 192, 320, 192, 224, 224, 1, 128, 1}};
 
-struct ConvSpec { std::string id; int cin, cout, k, stride, pad; };
-
-static std::vector<ConvSpec> conv_table(int in_ch) {
-  std::vector<ConvSpec> v;
-  v.push_back({"conv1_7x7_s2", in_ch, 64, 7, 2, 3});
-  v.push_back({"conv2_3x3_reduce", 64, 64, 1, 1, 0});
-  v.push_back({"conv2_3x3", 64, 192, 3, 1, 1});
+// every convolution is square: k x k, stride, padding pad on all sides
+static std::vector<Conv> conv_table(int in_ch) {
+  std::vector<Conv> v;
+  auto add = [&](const std::string& id, int cin, int cout, int k, int stride, int pad) { v.push_back({id, cin, cout, k, k, stride, pad, pad}); };
+  add("conv1_7x7_s2", in_ch, 64, 7, 2, 3);
+  add("conv2_3x3_reduce", 64, 64, 1, 1, 0);
+  add("conv2_3x3", 64, 192, 3, 1, 1);
   int cx = 192;
   for (const BlockSpec& b : kBlocks) {
     std::string p = std::string("inception_") + b.name + "_";
-    if (b.c1) v.push_back({p + "1x1", cx, b.c1, 1, 1, 0});
-    v.push_back({p + "3x3_reduce", cx, b.c3r, 1, 1, 0});
-    v.push_back({p + "3x3", b.c3r, b.c3, 3, b.stride, 1});
-    v.push_back({p + "double_3x3_reduce", cx, b.cdr, 1, 1, 0});
-    v.push_back({p + "double_3x3_1", b.cdr, b.cd1, 3, 1, 1});
-    v.push_back({p + "double_3x3_2", b.cd1, b.cd2, 3, b.stride, 1});
-    if (b.cproj) v.push_back({p + "pool_proj", cx, b.cproj, 1, 1, 0});
+    if (b.c1) add(p + "1x1", cx, b.c1, 1, 1, 0);
+    add(p + "3x3_reduce", cx, b.c3r, 1, 1, 0);
+    add(p + "3x3", b.c3r, b.c3, 3, b.stride, 1);
+    add(p + "double_3x3_reduce", cx, b.cdr, 1, 1, 0);
+    add(p + "double_3x3_1", b.cdr, b.cd1, 3, 1, 1);
+    add(p + "double_3x3_2", b.cd1, b.cd2, 3, b.stride, 1);
+    if (b.cproj) add(p + "pool_proj", cx, b.cproj, 1, 1, 0);
     cx = b.c1 + b.c3 + b.cd2 + (b.cproj ? b.cproj : cx);
   }
   return v;
 }
 
 // ---- planned objects -----------------------------------------------------------------------------
-struct Buffer { std::string name; int H, W, C; size_t off = 0, goff = 0; size_t hoff = 0, ghoff = 0, plane = 0; };   // EXACT_TC: fp16 hi/lo operand planes (lo = hi + plane)
-struct Value { std::string name; int buf, coff, C; };
-enum OpKind { OP_CONV = 0, OP_MAXPOOL = 1, OP_AVGPOOL = 2, OP_GPOOL = 3, OP_BN1 = 4 };   // OP_BN1: training-mode BatchNorm + ReLU behind conv1 (bn_mode='partial')
-struct Op {
-  OpKind kind; std::string id; int in_val, out_val;
-  int conv = -1, k = 0, stride = 1, pad = 0;
-  size_t argmax_off = 0;
+// the forward fields (graph.cuh) and what the training schedule and the tensor-core binding add
+struct Op : GraphOp {
   int grad_accumulate = 0;  // backward: dIn += (another consumer wrote first)
   int wsplits = 1, wrows = 0;
   int tsplits = 1;                // upper bound of the split count the tensor-core weight-gradient planner may pick (sizes `partial`)
@@ -102,14 +98,13 @@ struct Op {
   UmmaWgradPlan umma_wgrad; // tensor-core weight-gradient plan
   int pool_consumer = -1;   // conv whose only consumer is a k3/s2 max pool: that pool's op index (backward gather is folded in)
   bool folded_into_conv = false;   // max pool whose backward runs inside its producer conv's mask+bias pass
-  bool dgrad_masks = false; // this op's data gradient is the LAST writer of d(in_val): it applies the ReLU mask of in_val
+  bool dgrad_masks = false; // this op's data gradient is the LAST writer of d(in): it applies the ReLU mask of in
   bool bias_in_wgrad = false;// conv: bias gradient comes out of the tensor-core weight-gradient kernel (ones operand)
   bool dy_premasked = false;// conv: d(out) arrives already masked, the backward pass only needs the bias column sums
   bool raw = false;         // conv whose BatchNorm runs unfused in training mode: no fold, no ReLU in the epilogue, no ReLU mask in backward
   int fuse_role = 0;        // sibling 1x1 fusion: 1 = leader (launches the fused kernels), 2 = follower
   int fuse_block = -1;
 };
-struct PackedConv { size_t wf, wd, bias, scale; size_t wf16 = 0, wd16 = 0, wplane = 0, wmax = 0; };   // EXACT_TC: fp16 hi planes of wf / wd, lo = hi + wplane
 // the 1x1 convolutions of one inception block that read the block input (1x1, 3x3_reduce, double_3x3_reduce)
 struct FusedBlock {
   int op1 = -1, op_r3 = -1, op_rd = -1;   // op indices (op1 = -1 for 3c/4e)
@@ -124,13 +119,11 @@ struct FusedBlock {
 
 using namespace ssnb;
 
-struct ssnb_engine {
+struct ssnb_engine : ssnb::Graph<ssnb::Op> {
   ssnb_config cfg;
-  int F = 0;
-  size_t esz = 4;
   size_t up_plane = 0, s2d_plane = 0, s2d_w_plane = 0;
   int* tc_flag = nullptr;           // device int: set when a split pass saw |x * grad_scale| beyond the fp16 range
-  size_t tc_flag_off = 0, wmax_off = 0;
+  size_t tc_flag_off = 0;
   // tensor-core modes: the backward's gradient exponent, [0] = 2^k, [1] = 2^-k (launch_grad_exponent, at the start of every
   // backward).  Every gradient buffer holds dz * 2^k (FAST: times grad_scale as well); the global pool's backward multiplies
   // by 2^k and every kernel that writes a gradient the caller sees (dW, db, dgamma, dbeta) by 2^-k
@@ -139,12 +132,6 @@ struct ssnb_engine {
   const float *bn1_gamma = nullptr, *bn1_beta = nullptr; float *bn1_rmean = nullptr, *bn1_rvar = nullptr, *bn1_dgamma = nullptr, *bn1_dbeta = nullptr;
   float bn1_momentum = 0.1f, bn1_eps = 1e-5f;
   size_t bn_stat_off = 0, bn_partial_off = 0;
-  std::vector<ConvSpec> convs;
-  std::vector<Buffer> bufs;
-  std::vector<Value> vals;
-  std::map<std::string, int> val_by_name;
-  std::vector<Op> ops;
-  std::vector<PackedConv> packed;
   std::vector<FusedBlock> fused;
   size_t ws_bytes = 0, partial_off = 0, partial_bytes = 0, bpartial_off = 0;
   size_t s2d_off = 0, s2d_w_off = 0, up_off = 0;   // tensor-core modes: space-to-depth input + weights, zero-upsampled dz
@@ -152,7 +139,6 @@ struct ssnb_engine {
   bool s2d_ready = false;                            // backbone_fwd converted the input directly
   int Cs = 0;                                        // channels of the space-to-depth input (4*Cin rounded up to 8)
   int conv1_tsplits = 128;                           // tensor-core modes: bound of conv1's weight-gradient split count (sizes its partials)
-  char* ws = nullptr;
   bool weights_ready = false;
   std::vector<float*> dw, db;
   std::vector<int> pending_finalize;  // conv ops whose partials wait for the batched finalize of this backward
@@ -162,31 +148,9 @@ struct ssnb_engine {
   UmmaContext umma_ctx;
 
   int fail(int code, const std::string& msg) { error = msg; return code; }
-  bool fast() const { return cfg.precision == SSNB_FAST_FP16; }          // fp16 storage, fp16 operands
-  bool exact_tc() const { return cfg.precision == SSNB_EXACT_TC; }       // fp32 storage, convolutions on split (hi/lo fp16) operand planes
-  bool tensor_cores() const { return cfg.precision != SSNB_EXACT_FP32; } // either of the two: the wgmma schedule
   const float* grad_scale_dev() const { return tensor_cores() ? gscale : nullptr; }      // 2^k (nullptr: 1)
   const float* grad_unscale_dev() const { return tensor_cores() ? gscale + 1 : nullptr; }  // 2^-k
   int nplanes() const { return exact_tc() ? 2 : 1; }                     // fp16 operand planes per tensor-core operand
-  View view(int val, bool grad) const {
-    const Value& v = vals[val];
-    const Buffer& b = bufs[v.buf];
-    View w;
-    w.base = ws + (grad ? b.goff : b.off);
-    w.H = b.H; w.W = b.W; w.C = v.C; w.pitch = b.C; w.coff = v.coff;
-    return w;
-  }
-  // EXACT_TC: the fp16 hi/lo operand planes of a value (activation or gradient)
-  View planes(int val, bool grad) const {
-    const Value& v = vals[val];
-    const Buffer& b = bufs[v.buf];
-    View w;
-    w.base = ws + (grad ? b.ghoff : b.hoff);
-    w.H = b.H; w.W = b.W; w.C = v.C; w.pitch = b.C; w.coff = v.coff; w.lo_off = (long long)b.plane;
-    return w;
-  }
-  // what the tensor-core kernels read and write for a value: the fp16 storage in FAST, the operand planes in EXACT_TC
-  View operand(int val, bool grad) const { return exact_tc() ? planes(val, grad) : view(val, grad); }
   // tensor-core weight operands of a convolution: forward [tap][co][ci], data gradient [tap][ci][co]
   const __half* w_fwd(const PackedConv& p) const { return (const __half*)(ws + (exact_tc() ? p.wd16 : p.wd)); }
   const __half* w_dgrad(const PackedConv& p) const { return (const __half*)(ws + (exact_tc() ? p.wf16 : p.wf)); }
@@ -201,7 +165,6 @@ struct ssnb_engine {
 
 namespace ssnb {
 
-static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 // profiling aid: SSNB_PROFILE_FWD_OPS / SSNB_PROFILE_BWD_OPS = comma-separated op ids; the engine brackets those ops of a whole
 // forward / backward pass with cudaProfilerStart/Stop (use with `ncu --profile-from-start off`)
 static bool profiled_op(const char* env, const std::string& id) {
@@ -225,137 +188,86 @@ static int device_sms() {
   return sms;
 }
 
-static int pool_out(int h, int k, int s, int p) {   // ceil_mode (layer_factory.py:46-50)
-  int o = (h + 2 * p - k + s - 1) / s + 1;
-  if ((o - 1) * s >= h + p) --o;
-  return o;
-}
-
-static int add_buffer(ssnb_engine* e, const std::string& name, int H, int W, int C) {
-  e->bufs.push_back({name, H, W, C});
-  return (int)e->bufs.size() - 1;
-}
-static int add_value(ssnb_engine* e, const std::string& name, int buf, int coff, int C) {
-  e->vals.push_back({name, buf, coff, C});
-  e->val_by_name[name] = (int)e->vals.size() - 1;
-  return (int)e->vals.size() - 1;
-}
-
 static void build_graph(ssnb_engine* e) {
   const int cin = e->cfg.in_channels;
   e->convs = conv_table(cin);
   int ci = 0;
-  auto conv_op = [&](int in_val, int out_val) {
-    const ConvSpec& c = e->convs[ci];
-    Op o; o.kind = OP_CONV; o.id = c.id; o.in_val = in_val; o.out_val = out_val; o.conv = ci;
-    o.k = c.k; o.stride = c.stride; o.pad = c.pad;
+  auto conv_op = [&](int in, int out) {
+    const Conv& c = e->convs[ci];
+    Op o; o.kind = OP_CONV; o.id = c.id; o.in = in; o.out = out; o.conv = ci;
+    o.k = c.kh; o.stride = c.stride; o.pad = c.ph;
     e->ops.push_back(o);
     ++ci;
   };
-  auto pool_op = [&](OpKind kind, const std::string& id, int in_val, int out_val, int k, int s, int p) {
-    Op o; o.kind = kind; o.id = id; o.in_val = in_val; o.out_val = out_val; o.k = k; o.stride = s; o.pad = p;
+  auto pool_op = [&](OpKind kind, const std::string& id, int in, int out, int k, int s, int p) {
+    Op o; o.kind = kind; o.id = id; o.in = in; o.out = out; o.k = k; o.stride = s; o.pad = p;
     e->ops.push_back(o);
   };
-  auto whole = [&](const std::string& name, int H, int W, int C) {
-    return add_value(e, name, add_buffer(e, name, H, W, C), 0, C);
-  };
-  int x = whole("data", 224, 224, cin);
+  int x = e->whole("data", 224, 224, cin);
   int v;
   if (e->bn1_train) {
-    const int raw = whole("conv1_7x7_s2_raw", 112, 112, 64); conv_op(x, raw); e->ops.back().raw = true;
-    v = whole("conv1_7x7_s2_bn", 112, 112, 64);
+    const int raw = e->whole("conv1_7x7_s2_raw", 112, 112, 64); conv_op(x, raw); e->ops.back().raw = true;
+    v = e->whole("conv1_7x7_s2_bn", 112, 112, 64);
     pool_op(OP_BN1, "conv1_7x7_s2_bn", raw, v, 0, 1, 0); x = v;
   } else {
-    v = whole("conv1_7x7_s2_bn", 112, 112, 64); conv_op(x, v); x = v;
+    v = e->whole("conv1_7x7_s2_bn", 112, 112, 64); conv_op(x, v); x = v;
   }
-  v = whole("pool1_3x3_s2", 56, 56, 64); pool_op(OP_MAXPOOL, "pool1_3x3_s2", x, v, 3, 2, 0); x = v;
-  v = whole("conv2_3x3_reduce_bn", 56, 56, 64); conv_op(x, v); x = v;
-  v = whole("conv2_3x3_bn", 56, 56, 192); conv_op(x, v); x = v;
-  v = whole("pool2_3x3_s2", 28, 28, 192); pool_op(OP_MAXPOOL, "pool2_3x3_s2", x, v, 3, 2, 0); x = v;
+  v = e->whole("pool1_3x3_s2", 56, 56, 64); pool_op(OP_MAXPOOL, "pool1_3x3_s2", x, v, 3, 2, 0); x = v;
+  v = e->whole("conv2_3x3_reduce_bn", 56, 56, 64); conv_op(x, v); x = v;
+  v = e->whole("conv2_3x3_bn", 56, 56, 192); conv_op(x, v); x = v;
+  v = e->whole("pool2_3x3_s2", 28, 28, 192); pool_op(OP_MAXPOOL, "pool2_3x3_s2", x, v, 3, 2, 0); x = v;
   int H = 28, cx = 192;
   for (const BlockSpec& b : kBlocks) {
     const std::string p = std::string("inception_") + b.name + "_";
     const int OHW = (b.stride == 2) ? pool_out(H, 3, 2, 0) : H;
     const int ctot = b.c1 + b.c3 + b.cd2 + (b.cproj ? b.cproj : cx);
-    const int cat = add_buffer(e, p + "output", OHW, OHW, ctot);
-    const int red = add_buffer(e, p + "reduce", H, H, b.c3r + b.cdr);
+    const int cat = e->add_buffer(p + "output", OHW, OHW, ctot);
+    const int red = e->add_buffer(p + "reduce", H, H, b.c3r + b.cdr);
     int off = 0;
-    if (b.c1) { v = add_value(e, p + "1x1_bn", cat, off, b.c1); conv_op(x, v); off += b.c1; }
-    int r3 = add_value(e, p + "3x3_reduce_bn", red, 0, b.c3r); conv_op(x, r3);
-    v = add_value(e, p + "3x3_bn", cat, off, b.c3); conv_op(r3, v); off += b.c3;
-    int rd = add_value(e, p + "double_3x3_reduce_bn", red, b.c3r, b.cdr); conv_op(x, rd);
-    int d1 = whole(p + "double_3x3_1_bn", H, H, b.cd1); conv_op(rd, d1);
-    v = add_value(e, p + "double_3x3_2_bn", cat, off, b.cd2); conv_op(d1, v); off += b.cd2;
+    if (b.c1) { v = e->add_value(p + "1x1_bn", cat, off, b.c1); conv_op(x, v); off += b.c1; }
+    int r3 = e->add_value(p + "3x3_reduce_bn", red, 0, b.c3r); conv_op(x, r3);
+    v = e->add_value(p + "3x3_bn", cat, off, b.c3); conv_op(r3, v); off += b.c3;
+    int rd = e->add_value(p + "double_3x3_reduce_bn", red, b.c3r, b.cdr); conv_op(x, rd);
+    int d1 = e->whole(p + "double_3x3_1_bn", H, H, b.cd1); conv_op(rd, d1);
+    v = e->add_value(p + "double_3x3_2_bn", cat, off, b.cd2); conv_op(d1, v); off += b.cd2;
     if (b.stride == 2) {
-      v = add_value(e, p + "pool", cat, off, cx);
+      v = e->add_value(p + "pool", cat, off, cx);
       pool_op(OP_MAXPOOL, p + "pool", x, v, 3, 2, 0);
     } else {
-      int pl = whole(p + "pool", H, H, cx);
+      int pl = e->whole(p + "pool", H, H, cx);
       pool_op(b.pool_max ? OP_MAXPOOL : OP_AVGPOOL, p + "pool", x, pl, 3, 1, 1);
-      v = add_value(e, p + "pool_proj_bn", cat, off, b.cproj); conv_op(pl, v);
+      v = e->add_value(p + "pool_proj_bn", cat, off, b.cproj); conv_op(pl, v);
     }
-    x = add_value(e, p + "output", cat, 0, ctot);
+    x = e->add_value(p + "output", cat, 0, ctot);
     H = OHW; cx = ctot;
   }
   // global_pool writes the caller's feat tensor; it has no workspace buffer
-  Op g; g.kind = OP_GPOOL; g.id = "global_pool"; g.in_val = x; g.out_val = -1; g.k = 7;
+  Op g; g.kind = OP_GPOOL; g.id = "global_pool"; g.in = x; g.out = -1; g.k = 7;
   e->ops.push_back(g);
 }
 
+// The fixed-size slots first (their sizes are multiples of 1024, so every region behind them keeps its alignment), then the
+// shared forward storage (graph.cuh) with one extra (absmax, 1 / scale) slot per fused sibling block, then the training and
+// tensor-core regions of this engine.
 static void plan(ssnb_engine* e) {
   const size_t F = (size_t)e->F;
   size_t off = 0;
-  for (Buffer& b : e->bufs) { b.off = off; off = align_up(off + F * b.H * b.W * b.C * e->esz, 1024); }
-  if (e->cfg.training)
-    for (Buffer& b : e->bufs) { b.goff = off; off = align_up(off + F * b.H * b.W * b.C * e->esz, 1024); }
-  if (e->exact_tc()) {
-    for (Buffer& b : e->bufs) {
-      if (b.C % 8) continue;                              // the network input (3 / 10 channels) has no planes: conv1 reads its own packed copy
-      b.plane = align_up(F * b.H * b.W * b.C * 2, 1024);
-      b.hoff = off; off += 2 * b.plane;
-      if (e->cfg.training) { b.ghoff = off; off += 2 * b.plane; }
-    }
-  }
   e->tc_flag_off = off; off = align_up(off + 256, 1024);      // gradient overflow flag (every mode), gradient exponent
   if (e->bn1_train) { e->bn_stat_off = off; off = align_up(off + 4 * 64 * 4, 1024); e->bn_partial_off = off; off = align_up(off + (size_t)1200 * 2 * 64 * 4, 1024); }
-  for (Op& o : e->ops)
-    if (o.kind == OP_MAXPOOL) {
-      const Buffer& ob = e->bufs[e->vals[o.out_val].buf];
-      o.argmax_off = off;
-      off = align_up(off + F * ob.H * ob.W * e->vals[o.out_val].C, 1024);
-    }
-  e->packed.resize(e->convs.size());
-  for (size_t i = 0; i < e->convs.size(); ++i) {
-    const ConvSpec& c = e->convs[i];
-    const size_t n = (size_t)c.cout * c.cin * c.k * c.k;
-    e->packed[i].wf = off; off = align_up(off + n * e->esz, 1024);
-    e->packed[i].wd = off; off = align_up(off + n * e->esz, 1024);
-    e->packed[i].bias = off; off = align_up(off + c.cout * 4, 256);
-    e->packed[i].scale = off; off = align_up(off + c.cout * 4, 256);
-    if (e->exact_tc()) {
-      e->packed[i].wplane = align_up(n * 2, 1024);
-      e->packed[i].wf16 = off; off += 2 * e->packed[i].wplane;
-      e->packed[i].wd16 = off; off += 2 * e->packed[i].wplane;
-    }
-  }
-  if (e->exact_tc()) {      // per layer: [0] max |folded weight| (atomicMax target, zeroed before every pack), [1] 1 / plane scale (the kernels' alpha_dev)
-    e->wmax_off = off;
-    for (size_t i = 0; i < e->convs.size(); ++i) e->packed[i].wmax = off + i * 8;
-    off = align_up(off + (e->convs.size() + 16) * 8, 1024);     // + one shared slot per fused sibling block
-  }
+  off = e->plan_storage(off, e->cfg.training != 0, e->convs[0].cin, 16);
   // backward bookkeeping: accumulate flags + split-K sizing
   size_t pmax = 0;
   if (e->cfg.training) {
     std::vector<char> written(e->vals.size(), 0);
     for (int i = (int)e->ops.size() - 1; i >= 0; --i) {
       Op& o = e->ops[i];
-      o.grad_accumulate = written[o.in_val];
-      written[o.in_val] = 1;
+      o.grad_accumulate = written[o.in];
+      written[o.in] = 1;
       if (o.kind == OP_CONV) {
-        const ConvSpec& c = e->convs[o.conv];
-        const Buffer& ob = e->bufs[e->vals[o.out_val].buf];
+        const Conv& c = e->convs[o.conv];
+        const Buffer& ob = e->bufs[e->vals[o.out].buf];
         const long long M = (long long)F * ob.H * ob.W;
-        const int taps = c.k * c.k;
+        const int taps = c.kh * c.kw;
         const bool flat = c.cin < 16;
         const long long tiles = (long long)((c.cout + 63) / 64) * (flat ? (taps * c.cin + 63) / 64 : ((c.cin + 63) / 64) * taps);
         long long splits = (592 + tiles - 1) / tiles;
@@ -418,10 +330,10 @@ static void plan(ssnb_engine* e) {
       if (po.kind != OP_MAXPOOL || po.k != 3 || po.stride != 2 || po.pad != 0) continue;
       int producer = -1, consumers = 0;
       for (int j = 0; j < (int)e->ops.size(); ++j) {
-        if (e->ops[j].out_val == po.in_val && e->ops[j].kind == OP_CONV) producer = j;
-        if (e->ops[j].in_val == po.in_val) ++consumers;
+        if (e->ops[j].out == po.in && e->ops[j].kind == OP_CONV) producer = j;
+        if (e->ops[j].in == po.in) ++consumers;
       }
-      if (producer >= 0 && consumers == 1 && e->vals[po.in_val].C % (e->fast() ? VEC_WIDTH<__half> : VEC_WIDTH<float>) == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
+      if (producer >= 0 && consumers == 1 && e->vals[po.in].C % (e->fast() ? VEC_WIDTH<__half> : VEC_WIDTH<float>) == 0) { e->ops[producer].pool_consumer = i; po.folded_into_conv = true; }
     }
     // fp16 operand regions: one plane in FAST (the next region starts 1024-aligned behind it), hi + lo planes `plane`
     // bytes apart in EXACT_TC
@@ -447,7 +359,7 @@ static void plan(ssnb_engine* e) {
       size_t up = 0;
       for (const Op& o : e->ops)
         if (o.kind == OP_CONV && o.stride == 2 && o.conv != 0) {
-          const Buffer& ib = e->bufs[e->vals[o.in_val].buf];
+          const Buffer& ib = e->bufs[e->vals[o.in].buf];
           up = std::max(up, F * ib.H * ib.W * (size_t)e->convs[o.conv].cout * 2);
         }
       e->up_off = operand_region(up, e->up_plane);
@@ -458,9 +370,9 @@ static void plan(ssnb_engine* e) {
   if (e->cfg.training)
     for (Op& o : e->ops)
       if (o.kind == OP_CONV) {
-        const ConvSpec& c = e->convs[o.conv];
+        const Conv& c = e->convs[o.conv];
         const int nsplit = e->tensor_cores() ? std::max(o.wsplits, o.tsplits) : o.wsplits;
-        size_t need = (size_t)nsplit * c.k * c.k * c.cout * c.cin * 4;
+        size_t need = (size_t)nsplit * c.kh * c.kw * c.cout * c.cin * 4;
         if (o.conv == 0 && e->tensor_cores()) need = std::max(need, (size_t)e->conv1_tsplits * 16 * 64 * e->Cs * 4);
         o.partial_off = off; off = align_up(off + need, 1024);
         o.bias_partial_off = off; off = align_up(off + (size_t)std::max(nsplit, 128) * c.cout * 4, 256);
@@ -472,12 +384,7 @@ static void plan(ssnb_engine* e) {
 // ---- op execution --------------------------------------------------------------------------------
 #define DISPATCH(e, call_f, call_h) ((e)->fast() ? (call_h) : (call_f))
 
-// timing tags (common.cuh): the next launch is the convolution `o` in pass `phase`
-static double conv_flops(const ssnb_engine* e, const Op& o) {
-  const ConvSpec& c = e->convs[o.conv];
-  const Buffer& ob = e->bufs[e->vals[o.out_val].buf];
-  return 2.0 * e->F * ob.H * ob.W * (double)c.cout * c.cin * c.k * c.k;
-}
+// timing tags (common.cuh): the next launch is in pass `phase`, `flop` the algorithmic FLOPs of the convolution op `op`
 static inline void tag_next(int phase, double flop, const char* op = nullptr) { t_tag.phase = phase; t_tag.flop = flop; t_tag.op = op; }
 // a fused sibling launch is named after its convolutions, "a+b+c"
 static thread_local std::string t_fused_name;
@@ -489,93 +396,62 @@ static const char* fused_name(const ssnb_engine* e, const FusedBlock& fb) {
   return t_fused_name.c_str();
 }
 
-// EXACT_TC: operand planes of a value produced by a kernel that only wrote fp32 (pools, SIMT convolutions, value_write)
-static int tc_split_value(ssnb_engine* e, int val, bool grad, float scale, cudaStream_t s) {
-  if (!e->exact_tc() || !e->bufs[e->vals[val].buf].plane) return 0;
-  return launch_split_view(e->view(val, grad), e->F, scale, e->planes(val, grad), grad ? e->tc_flag : nullptr, s);
-}
-
-static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s);
-static int run_fwd(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s) {
+static int run_fwd(ssnb_engine* e, const Op& o, float* feat, cudaStream_t s) {
   tag_next(0, 0.0);
   if (o.kind == OP_CONV && o.umma.enabled) {
     // tensor-core convolution (EXACT_TC: reads the input's hi/lo planes, writes fp32 + the output's planes); conv1 runs as a
     // 4x4 stride-1 convolution over the space-to-depth input
     if (o.conv == 0 && !e->s2d_ready) {
-      const View in = e->view(o.in_val, false);
+      const View in = e->view(o.in, false);
       __half* s2d = (__half*)(e->ws + e->s2d_off);
       if (int rc = launch_nhwc_to_s2d(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s)) return rc;
     }
-    tag_next(0, conv_flops(e, o), o.id.c_str());
+    tag_next(0, e->conv_flops(o), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma, s);
   }
   if (o.kind == OP_BN1) {
     if (!e->bn1_gamma || !e->bn1_beta) { set_thread_error("bn1_train engine: call ssnb_set_bn1 first"); return SSNB_ESTATE; }
-    return launch_bn_train_fwd(e->view(o.in_val, false), e->view(o.out_val, false), e->exact_tc() ? e->planes(o.out_val, false) : View(), e->F, e->bn1_gamma,
+    return launch_bn_train_fwd(e->view(o.in, false), e->view(o.out, false), e->exact_tc() ? e->planes(o.out, false) : View(), e->F, e->bn1_gamma,
                                e->bn1_beta, e->bn1_eps, e->bn1_momentum, e->bn1_rmean, e->bn1_rvar, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, s);
   }
-  if (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) {
-    // vectorised pooling; in EXACT_TC it also emits the output's operand planes (glue_vec.cu)
-    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    const View pl = e->exact_tc() && e->bufs[e->vals[o.out_val].buf].plane ? e->planes(o.out_val, false) : View();
-    uint8_t* am = (uint8_t*)(e->ws + o.argmax_off);
-    if (o.kind == OP_MAXPOOL)
-      return DISPATCH(e, launch_maxpool_fwd_vec<float>(in, out, pl, e->F, o.k, o.stride, o.pad, am, s),
-                      launch_maxpool_fwd_vec<__half>(in, out, pl, e->F, o.k, o.stride, o.pad, am, s));
-    return DISPATCH(e, launch_avgpool3_vec<float>(in, out, pl, e->F, 0, s), launch_avgpool3_vec<__half>(in, out, pl, e->F, 0, s));
-  }
-  if (int rc = run_fwd_impl(e, o, input_nchw, feat, s)) return rc;
-  return o.out_val >= 0 ? tc_split_value(e, o.out_val, false, 1.0f, s) : 0;
-}
-
-static int run_fwd_impl(ssnb_engine* e, const Op& o, const float* input_nchw, float* feat, cudaStream_t s) {
-  const int F = e->F;
-  if (o.kind == OP_CONV) {
-    const ConvSpec& c = e->convs[o.conv];
-    const View in = e->view(o.in_val, false), out = e->view(o.out_val, false);
-    ConvArgs a;
-    a.src = in.base; a.SH = in.H; a.SW = in.W; a.Csrc = in.C; a.src_pitch = in.pitch; a.src_coff = in.coff;
-    a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
-    a.wgt = e->ws + e->packed[o.conv].wf; a.bias = (const float*)(e->ws + e->packed[o.conv].bias);
-    a.F = F; a.kh = a.kw = c.k; a.stride = c.stride; a.pad_h = a.pad_w = c.pad; a.relu = o.raw ? 0 : 1; a.accumulate = 0; a.dgrad = 0;
-    tag_next(0, conv_flops(e, o), o.id.c_str());
-    return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
-  }
+  if (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) return e->pool_fwd(o, s);     // EXACT_TC: and the output's operand planes
   if (o.kind == OP_GPOOL) {
     if (!feat) return e->fail(SSNB_EINVAL, "global_pool needs the feat output pointer");
-    const View in = e->view(o.in_val, false);
-    return DISPATCH(e, launch_gpool_fwd<float>(in, F, feat, s), launch_gpool_fwd<__half>(in, F, feat, s));
+    return e->gpool_fwd(o, feat, s);
   }
-  return SSNB_EINVAL;
+  // SIMT convolution; the raw conv1 of a bn1_train engine has no ReLU
+  if (int rc = e->simt_conv_fwd(o, o.raw ? 0 : 1, s)) return rc;
+  if (!e->exact_tc() || !e->bufs[e->vals[o.out].buf].plane) return 0;     // EXACT_TC: the output's operand planes
+  return launch_split_view(e->view(o.out), e->F, 1.0f, e->planes(o.out), nullptr, s);
 }
 
 // SIMT convolution backward (EXACT_FP32, and layers or passes without a tensor-core plan), reading the masked fp32 / fp16
 // dz = d(out): weight gradient into the layer's split-K partials + finalize; data gradient into d(in)
 static int simt_wgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
-  const ConvSpec& c = e->convs[o.conv];
-  const View x = e->view(o.in_val, false), dz = e->view(o.out_val, true);
+  const Conv& c = e->convs[o.conv];
+  const View x = e->view(o.in, false), dz = e->view(o.out, true);
   float* partial = (float*)(e->ws + o.partial_off);
   WgradArgs w;
   w.dz = dz.base; w.OH = dz.H; w.OW = dz.W; w.Cout = dz.C; w.dz_pitch = dz.pitch; w.dz_coff = dz.coff;
   w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
-  w.partial = partial; w.F = e->F; w.k = c.k; w.stride = c.stride; w.pad = c.pad;
+  w.partial = partial; w.F = e->F; w.k = c.kh; w.stride = c.stride; w.pad = c.ph;
   w.rows_per_split = o.wrows; w.splits = o.wsplits;
-  tag_next(2, conv_flops(e, o), o.id.c_str());
+  tag_next(2, e->conv_flops(o), o.id.c_str());
   if (int rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s))) return rc;
   const float out_scale = e->fast() ? 1.0f / e->cfg.grad_scale : 1.0f;      // FAST stores gradients times the loss scale
-  return launch_wgrad_finalize(partial, o.wsplits, c.k * c.k, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
+  return launch_wgrad_finalize(partial, o.wsplits, c.kh * c.kw, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
                                e->dw[o.conv], e->grad_accumulate, s, nullptr, nullptr, nullptr, e->grad_unscale_dev());
 }
 static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
-  const ConvSpec& c = e->convs[o.conv];
-  const View dz = e->view(o.out_val, true), dx = e->view(o.in_val, true);
+  const Conv& c = e->convs[o.conv];
+  const View dz = e->view(o.out, true), dx = e->view(o.in, true);
   ConvArgs a;
   a.src = dz.base; a.SH = dz.H; a.SW = dz.W; a.Csrc = dz.C; a.src_pitch = dz.pitch; a.src_coff = dz.coff;
   a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
   a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
-  a.F = e->F; a.kh = a.kw = c.k; a.stride = c.stride; a.pad_h = a.pad_w = c.pad; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
-  tag_next(1, conv_flops(e, o), o.id.c_str());
+  a.F = e->F; a.kh = a.kw = c.kh; a.stride = c.stride; a.pad_h = a.pad_w = c.ph; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
+  tag_next(1, e->conv_flops(o), o.id.c_str());
   return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
 }
 
@@ -586,36 +462,36 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   tag_next(3, 0.0);
   if (o.kind == OP_GPOOL) {
     if (!dfeat) return e->fail(SSNB_EINVAL, "global_pool backward needs dfeat");
-    const View din = e->view(o.in_val, true);
-    const void* ym = (full && e->fold_pools && o.dgrad_masks) ? e->view(o.in_val, false).base : nullptr;
+    const View din = e->view(o.in, true);
+    const void* ym = (full && e->fold_pools && o.dgrad_masks) ? e->view(o.in, false).base : nullptr;
     const float* gsd = e->grad_scale_dev();
     return DISPATCH(e, launch_gpool_bwd<float>(dfeat, gs, gsd, din, F, ym, s), launch_gpool_bwd<__half>(dfeat, gs, gsd, din, F, ym, s));
   }
   if (o.kind == OP_BN1) {
-    return launch_bn_train_bwd(e->view(o.in_val, false), e->view(o.out_val, true), e->view(o.out_val, false), e->view(o.in_val, true),
-                               e->exact_tc() ? e->planes(o.in_val, true) : View(), e->cfg.grad_scale, e->tc_flag, F, e->bn1_gamma, (float*)(e->ws + e->bn_stat_off),
+    return launch_bn_train_bwd(e->view(o.in, false), e->view(o.out, true), e->view(o.out, false), e->view(o.in, true),
+                               e->exact_tc() ? e->planes(o.in, true) : View(), e->cfg.grad_scale, e->tc_flag, F, e->bn1_gamma, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, e->bn1_dgamma, e->bn1_dbeta, e->grad_unscale_dev(), e->grad_accumulate, s);
   }
   if (o.kind == OP_MAXPOOL) {
     if (full && e->fold_pools && o.folded_into_conv) return 0;      // gathered by the producer conv's mask+bias pass (tensor-core modes)
-    const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
+    const View din = e->view(o.in, true), dout = e->view(o.out, true);
     const uint8_t* am = (const uint8_t*)(e->ws + o.argmax_off);
     return DISPATCH(e, launch_maxpool_bwd_vec<float>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s),
                     launch_maxpool_bwd_vec<__half>(din, dout, F, o.k, o.stride, o.pad, am, o.grad_accumulate, s));
   }
   if (o.kind == OP_AVGPOOL) {
-    const View din = e->view(o.in_val, true), dout = e->view(o.out_val, true);
+    const View din = e->view(o.in, true), dout = e->view(o.out, true);
     return DISPATCH(e, launch_avgpool3_vec<float>(dout, din, View(), F, o.grad_accumulate, s),
                     launch_avgpool3_vec<__half>(dout, din, View(), F, o.grad_accumulate, s));
   }
   // convolution: dz = dy * (y > 0); db, dW from dz; dx = dgrad(dz)
-  const ConvSpec& c = e->convs[o.conv];
-  const View x = e->view(o.in_val, false), y = e->view(o.out_val, false), dy = e->view(o.out_val, true);
+  const Conv& c = e->convs[o.conv];
+  const View x = e->view(o.in, false), y = e->view(o.out, false), dy = e->view(o.out, true);
   const float* scale = (const float*)(e->ws + e->packed[o.conv].scale);
   float* bpartial = (float*)(e->ws + e->bpartial_off);
   float* dbp = (e->db.size() && e->db[o.conv]) ? e->db[o.conv] : nullptr;
   const bool want_w = e->dw.size() && e->dw[o.conv];
-  const bool want_x = e->vals[o.in_val].name != "data" && !skip_dgrad;
+  const bool want_x = e->vals[o.in].name != "data" && !skip_dgrad;
   // the tensor-core products read dz times the loss scale (FAST: the fp16 storage, EXACT_TC: the planes); EXACT has no
   // tensor-core plans
   const float gst = e->cfg.grad_scale;
@@ -629,7 +505,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   // 1. one pass over dy: ReLU mask + bias-gradient column sums.  FAST masks the fp16 dy in place.  EXACT_TC reads the fp32 dy,
   //    writes the hi/lo planes of dz * grad_scale and writes the masked fp32 dz back only when a SIMT kernel will read it;
   //    EXACT writes no planes and masks the fp32 dy in place for its SIMT kernels.
-  const View dpool = pool ? e->view(pool->out_val, true) : View();
+  const View dpool = pool ? e->view(pool->out, true) : View();
   const uint8_t* pam = pool ? (const uint8_t*)(e->ws + pool->argmax_off) : nullptr;
   if (e->fast()) {
     if (pool) rc = launch_pool_mask_bias_vec<__half>(dy, y, dpool, View(), 1.0f, 1, nullptr, F, pool->k, pool->stride, pool->pad, pam,
@@ -638,7 +514,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
                                                        e->grad_accumulate, s);
   } else {
     const bool need_f32 = (want_w && !tc_w) || (want_x && !tc_x);
-    const View pl = (tc_w || tc_x) ? e->planes(o.out_val, true) : View();
+    const View pl = (tc_w || tc_x) ? e->planes(o.out, true) : View();
     if (o.raw) {         // the training-mode BatchNorm behind this convolution produced dz (and its planes): only the bias sums are left
       if (dbp) rc = launch_mask_bias_vec<float>(dy, View(), View(), gst, 0, nullptr, F, scale, 1.0f, us, bpartial, max_ctas, dbp, e->grad_accumulate, s);
     } else if (pre) {    // bias sums of the already masked fp32 dz only: no planes, nothing written back
@@ -654,7 +530,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   if (rc) return rc;
   // 2. a stride-2 data gradient reads dz zero-upsampled to the input resolution, every operand plane
   if (tc_x && c.stride == 2 && o.conv != 0) {
-    View dz = e->operand(o.out_val, true);
+    View dz = e->operand(o.out, true);
     for (int p = 0; p < e->nplanes(); ++p, dz.base = (char*)dz.base + dz.lo_off)
       if ((rc = launch_upsample2_zero(dz, (__half*)(e->ws + e->up_off + p * e->up_plane), x.H, x.W, F, s))) return rc;
   }
@@ -663,18 +539,18 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   if (tc_w) {
     float* partial = (float*)(e->ws + o.partial_off);
     float* bp = bias_w ? (float*)(e->ws + o.bias_partial_off) : nullptr;
-    tag_next(2, conv_flops(e, o), o.id.c_str());
+    tag_next(2, e->conv_flops(o), o.id.c_str());
     if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bp))) return rc;
     if (full && o.conv != 0) e->pending_finalize.push_back((int)(&o - e->ops.data()));
     else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, us, e->dw[o.conv],
                                                          e->grad_accumulate, s);
-    else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.k * c.k, c.cout, c.cin, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s,
+    else rc = launch_wgrad_finalize(partial, o.umma_wgrad.p.splits, c.kh * c.kw, c.cout, c.cin, scale, 1.0f / gst, e->dw[o.conv], e->grad_accumulate, s,
                                     nullptr, nullptr, e->tc_flag, us);
     if (rc) return rc;
   } else if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
   // 4. data gradient; as the last writer of d(in) the wgmma epilogue applies in's ReLU mask
   if (tc_x) {
-    tag_next(1, conv_flops(e, o), o.id.c_str());
+    tag_next(1, e->conv_flops(o), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
   }
   return want_x ? simt_dgrad(e, o, s) : 0;
@@ -682,7 +558,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
 
 int engine_tail_view(ssnb_handle h, View* v, int* F, int* fp16) {
   if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
-  *v = h->view(h->ops.back().in_val, false);
+  *v = h->view(h->ops.back().in, false);
   *F = h->F; *fp16 = h->fast() ? 1 : 0;
   return 0;
 }
@@ -699,11 +575,11 @@ const char* ssnb_last_error(ssnb_handle h) { return h ? h->error.c_str() : ssnb:
 int ssnb_num_convs(void) { return 69; }
 
 int ssnb_conv_info(int idx, int in_channels, char* name, int name_cap, int* cin, int* cout, int* k, int* stride, int* pad) {
-  std::vector<ConvSpec> t = conv_table(in_channels);
+  std::vector<Conv> t = conv_table(in_channels);
   if (idx < 0 || idx >= (int)t.size()) { set_thread_error("ssnb_conv_info: index out of range"); return SSNB_EINVAL; }
   if (name && name_cap > 0) { snprintf(name, name_cap, "%s", t[idx].id.c_str()); }
-  if (cin) *cin = t[idx].cin; if (cout) *cout = t[idx].cout; if (k) *k = t[idx].k;
-  if (stride) *stride = t[idx].stride; if (pad) *pad = t[idx].pad;
+  if (cin) *cin = t[idx].cin; if (cout) *cout = t[idx].cout; if (k) *k = t[idx].kh;
+  if (stride) *stride = t[idx].stride; if (pad) *pad = t[idx].ph;
   return SSNB_OK;
 }
 
@@ -715,6 +591,7 @@ int ssnb_create(const ssnb_config* cfg, ssnb_handle* out) {
   e->cfg = *cfg;
   if (!(e->cfg.grad_scale > 0.f)) e->cfg.grad_scale = 1.0f;
   e->F = cfg->frames;
+  e->precision = cfg->precision;
   e->bn1_train = cfg->bn1_train != 0;
   if (e->bn1_train && e->fast()) { delete e; set_thread_error("ssnb_create: bn1_train (bn_mode='partial') needs EXACT_FP32 or EXACT_TC"); return SSNB_ENOSUPPORT; }
   e->esz = e->fast() ? 2 : 4;
@@ -777,7 +654,7 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
   };
   for (Op& o : h->ops) {
     if (o.kind != OP_CONV || !use_tc) continue;
-    const ConvSpec& c = h->convs[o.conv];
+    const Conv& c = h->convs[o.conv];
     const PackedConv& pk = h->packed[o.conv];
     UmmaTcOpts tf, tg;
     int rc = 0;
@@ -787,34 +664,34 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
       View xs; xs.base = h->ws + h->s2d_off; xs.H = 112; xs.W = 112; xs.C = Ck; xs.pitch = Ck; xs.coff = 0; xs.lo_off = (long long)h->s2d_plane;
       int dy[4], dx[4];
       for (int t = 0; t < 4; ++t) { dy[t] = t - 2; dx[t] = 0; }
-      rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, h->operand(o.out_val, false), h->F, Ck, c.cout, 4, dy, dx, (const __half*)(h->ws + h->s2d_w_off),
-                               (const float*)(h->ws + pk.bias), o.raw ? 0 : 1, h->tc_opts(tf, h->s2d_w_plane, h->view(o.out_val, false).base, 1.0f, pk.wmax));
+      rc = umma_conv_bind_taps(h->umma_ctx, o.umma, xs, h->operand(o.out, false), h->F, Ck, c.cout, 4, dy, dx, (const __half*)(h->ws + h->s2d_w_off),
+                               (const float*)(h->ws + pk.bias), o.raw ? 0 : 1, h->tc_opts(tf, h->s2d_w_plane, h->view(o.out, false).base, 1.0f, pk.wmax));
       if (rc) return h->fail(rc, "conv1 bind: " + ssnb::thread_error());
       tc_gate(o.umma);
-      if (use_wgrad && (rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->operand(o.out_val, true), xs, h->F, Ck, c.cout, 4, dy, dx,
+      if (use_wgrad && (rc = umma_wgrad_bind_taps(h->umma_ctx, o.umma_wgrad, h->operand(o.out, true), xs, h->F, Ck, c.cout, 4, dy, dx,
                                                   (float*)(h->ws + o.partial_off), h->conv1_tsplits)))
         return h->fail(rc, "conv1 wgrad bind: " + ssnb::thread_error());
       continue;
     }
-    if (c.cin % 8 != 0 || c.k * c.k > UMMA_MAX_TAPS) continue;
-    rc = umma_conv_bind_fwd(h->umma_ctx, o.umma, h->operand(o.in_val, false), h->operand(o.out_val, false), h->F, c.cin, c.cout, c.k, c.pad,
-                            c.stride, h->w_fwd(pk), (const float*)(h->ws + pk.bias), h->tc_opts(tf, pk.wplane, h->view(o.out_val, false).base, 1.0f, pk.wmax));
+    if (c.cin % 8 != 0 || c.kh * c.kw > UMMA_MAX_TAPS) continue;
+    rc = umma_conv_bind_fwd(h->umma_ctx, o.umma, h->operand(o.in, false), h->operand(o.out, false), h->F, c.cin, c.cout, c.kh, c.ph,
+                            c.stride, h->w_fwd(pk), (const float*)(h->ws + pk.bias), h->tc_opts(tf, pk.wplane, h->view(o.out, false).base, 1.0f, pk.wmax));
     if (rc) return h->fail(rc, "bind_fwd(" + c.id + "): " + ssnb::thread_error());
     if (!training) continue;
     // data gradient: stride-2 layers read the zero-upsampled dz at input resolution.  EXACT_TC writes the fp32 d(in) only:
     // its consumer masks and splits it.
-    const View in = h->view(o.in_val, false);
-    View dz = h->operand(o.out_val, true);
+    const View in = h->view(o.in, false);
+    View dz = h->operand(o.out, true);
     if (c.stride == 2) { dz.base = h->ws + h->up_off; dz.H = in.H; dz.W = in.W; dz.C = c.cout; dz.pitch = c.cout; dz.coff = 0; dz.lo_off = (long long)h->up_plane; }
-    View dx = h->view(o.in_val, true);
+    View dx = h->view(o.in, true);
     const UmmaTcOpts* og = h->tc_opts(tg, pk.wplane, dx.base, 1.0f / gs, pk.wmax);
     if (og) dx.base = nullptr;
-    rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, dx, h->F, c.cin, c.cout, c.k, c.pad, h->w_dgrad(pk), o.grad_accumulate, og);
+    rc = umma_conv_bind_dgrad(h->umma_ctx, o.umma_dgrad, dz, dx, h->F, c.cin, c.cout, c.kh, c.ph, h->w_dgrad(pk), o.grad_accumulate, og);
     if (rc) return h->fail(rc, "bind_dgrad(" + c.id + "): " + ssnb::thread_error());
     tc_gate(o.umma_dgrad);
     // weight gradient: stride-2 layers read dz at its own (output) resolution, the x boxes step over the input with element stride 2
-    if (use_wgrad && (rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->operand(o.out_val, true), h->operand(o.in_val, false), h->F, c.cin, c.cout,
-                                           c.k, c.pad, (float*)(h->ws + o.partial_off), o.tsplits, c.stride)))
+    if (use_wgrad && (rc = umma_wgrad_bind(h->umma_ctx, o.umma_wgrad, h->operand(o.out, true), h->operand(o.in, false), h->F, c.cin, c.cout,
+                                           c.kh, c.ph, (float*)(h->ws + o.partial_off), o.tsplits, c.stride)))
       return h->fail(rc, "wgrad_bind(" + c.id + "): " + ssnb::thread_error());
   }
   // horizontal fusion of the sibling 1x1 convolutions of each inception block: ONE forward launch (stacked weights; the first
@@ -825,26 +702,26 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
     const Op& o3 = h->ops[fb.op_r3]; const Op& od = h->ops[fb.op_rd];
     if (!o3.umma.enabled || !od.umma.enabled) continue;
     const int nr = fb.c3r + fb.cdr;                  // both reduce outputs: adjacent slices of one buffer
-    const View x = h->operand(o3.in_val, false);
-    View red = h->operand(o3.out_val, false); red.C = nr;
+    const View x = h->operand(o3.in, false);
+    View red = h->operand(o3.out, false); red.C = nr;
     UmmaTcOpts tf, tg;
     int rc;
     if (fb.op1 >= 0) {
-      const int v1 = h->ops[fb.op1].out_val;
+      const int v1 = h->ops[fb.op1].out;
       const UmmaTcOpts* of = h->tc_opts(tf, fb.w_fwd_plane, h->view(v1, false).base, 1.0f, fb.wmax);
-      tf.out32_2 = (float*)h->view(o3.out_val, false).base;
+      tf.out32_2 = (float*)h->view(o3.out, false).base;
       rc = umma_conv_bind_fused_fwd(h->umma_ctx, fb.fwd, x, h->operand(v1, false), red, h->F, fb.cx, fb.c1, nr, (const __half*)(h->ws + fb.w_fwd),
                                     (const float*)(h->ws + fb.bias), of);
     } else {
       rc = umma_conv_bind_fwd(h->umma_ctx, fb.fwd, x, red, h->F, fb.cx, nr, 1, 0, 1, (const __half*)(h->ws + fb.w_fwd), (const float*)(h->ws + fb.bias),
-                              h->tc_opts(tf, fb.w_fwd_plane, h->view(o3.out_val, false).base, 1.0f, fb.wmax));
+                              h->tc_opts(tf, fb.w_fwd_plane, h->view(o3.out, false).base, 1.0f, fb.wmax));
     }
     if (rc) return h->fail(rc, "fused fwd bind(" + o3.id + "): " + ssnb::thread_error());
     if (!tc_gate(fb.fwd)) continue;
     if (training) {
-      View dred = h->operand(o3.out_val, true); dred.C = nr;
-      const View d1 = fb.op1 >= 0 ? h->operand(h->ops[fb.op1].out_val, true) : dred;
-      View dx = h->view(o3.in_val, true);
+      View dred = h->operand(o3.out, true); dred.C = nr;
+      const View d1 = fb.op1 >= 0 ? h->operand(h->ops[fb.op1].out, true) : dred;
+      View dx = h->view(o3.in, true);
       const UmmaTcOpts* og = h->tc_opts(tg, fb.w_dg_plane, dx.base, 1.0f / gs, fb.wmax);
       if (og) dx.base = nullptr;
       rc = umma_conv_bind_fused_dgrad(h->umma_ctx, fb.dgrad, d1, dred, dx, h->F, fb.cx, fb.c1, nr, (const __half*)(h->ws + fb.w_dg), od.grad_accumulate, og);
@@ -866,13 +743,13 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
   if (use_tc && training && fuse) {
     std::vector<int> first_consumer(h->vals.size(), -1);
     for (int i = 0; i < (int)h->ops.size(); ++i)
-      if (first_consumer[h->ops[i].in_val] < 0) first_consumer[h->ops[i].in_val] = i;
+      if (first_consumer[h->ops[i].in] < 0) first_consumer[h->ops[i].in] = i;
     for (size_t v = 0; v < h->vals.size(); ++v) {
       const int fc = first_consumer[v];
       if (fc < 0 || h->vals[v].name == "data") continue;
       if (h->exact_tc() && !h->bufs[h->vals[v].buf].plane) continue;      // no operand planes to emit
       bool conv_made = false;                    // only buffers that hold convolution outputs have a ReLU to differentiate
-      for (const Op& q : h->ops) conv_made = conv_made || (q.kind == OP_CONV && h->vals[q.out_val].buf == h->vals[v].buf);
+      for (const Op& q : h->ops) conv_made = conv_made || (q.kind == OP_CONV && h->vals[q.out].buf == h->vals[v].buf);
       if (!conv_made) continue;
       Op& c = h->ops[fc];
       UmmaConvPlan* dg = nullptr;
@@ -892,9 +769,9 @@ int ssnb_set_workspace(ssnb_handle h, void* dev_ptr, size_t bytes) {
     }
     for (Op& o : h->ops) {
       if (o.kind != OP_CONV) continue;
-      int w = o.out_val;
+      int w = o.out;
       if (first_consumer[w] < 0) {               // a slice of a concat buffer: gradients are written through the whole-buffer value
-        const Value& ov = h->vals[o.out_val];
+        const Value& ov = h->vals[o.out];
         for (size_t v = 0; v < h->vals.size(); ++v)
           if (h->vals[v].buf == ov.buf && h->vals[v].coff == 0 && h->vals[v].C == h->bufs[ov.buf].C && first_consumer[v] >= 0) { w = (int)v; break; }
       }
@@ -909,70 +786,40 @@ int ssnb_pack_weights(ssnb_handle h, const float* const* w, const float* const* 
                       const float* const* beta, const float* const* mean, const float* const* var, void* stream) {
   if (!h || !h->ws) return h ? h->fail(SSNB_ESTATE, "set_workspace first") : SSNB_EINVAL;
   cudaStream_t s = (cudaStream_t)stream;
-  if (h->exact_tc() && cudaMemsetAsync(h->ws + h->wmax_off, 0, (h->convs.size() + 16) * 8, s) != cudaSuccess) return h->fail(SSNB_ECUDA, "pack_weights: memset");
-  {
-    // fold + re-layout of all 69 layers in a few launches (PACK_MAX entries per launch); EXACT_TC: every fold launch first (the
-    // layers of a fused sibling block share one absmax slot), then the hi/lo splits
-    struct Member { int block = -1, row = 0, col = 0; };
-    std::vector<Member> member(h->convs.size());
-    for (size_t bi = 0; bi < h->fused.size(); ++bi) {
-      const FusedBlock& fb = h->fused[bi];
-      if (!fb.enabled) continue;
-      const int k1p = (fb.c1 + 63) / 64 * 64;
-      int row = 0, col = 0;
-      for (int j : {fb.op1, fb.op_r3, fb.op_rd}) {
-        if (j < 0) continue;
-        const int ci = h->ops[j].conv;
-        member[ci].block = (int)bi; member[ci].row = row; member[ci].col = col;
-        row += h->convs[ci].cout;
-        col += (j == fb.op1) ? k1p : h->convs[ci].cout;
-      }
+  // the members of each fused sibling block: their rows in its stacked forward weights, their columns in its K-concatenated
+  // data-gradient weights
+  struct Member { int block = -1, row = 0, col = 0; };
+  std::vector<Member> member(h->convs.size());
+  for (size_t bi = 0; bi < h->fused.size(); ++bi) {
+    const FusedBlock& fb = h->fused[bi];
+    if (!fb.enabled) continue;
+    const int k1p = (fb.c1 + 63) / 64 * 64;
+    int row = 0, col = 0;
+    for (int j : {fb.op1, fb.op_r3, fb.op_rd}) {
+      if (j < 0) continue;
+      const int ci = h->ops[j].conv;
+      member[ci].block = (int)bi; member[ci].row = row; member[ci].col = col;
+      row += h->convs[ci].cout;
+      col += (j == fb.op1) ? k1p : h->convs[ci].cout;
     }
-    std::vector<PackTable> pt(1);
-    std::vector<SplitTable> stt(1);
-    std::vector<int> pblocks(1, 0), sblocks(1, 0);
-    pt[0].n = 0; pt[0].pad_ = 0; stt[0].n = 0; stt[0].pad_ = 0;
-    for (size_t i = 0; i < h->convs.size(); ++i) {
-      const ConvSpec& c = h->convs[i];
-      const PackedConv& p = h->packed[i];
-      const long long n = (long long)c.cout * c.cin * c.k * c.k;
-      if (pt.back().n == PACK_MAX) { pt.emplace_back(); pt.back().n = 0; pt.back().pad_ = 0; pblocks.push_back(0); stt.emplace_back(); stt.back().n = 0; stt.back().pad_ = 0; sblocks.push_back(0); }
-      const Member& mb = member[i];
-      const FusedBlock* fb = mb.block >= 0 ? &h->fused[mb.block] : nullptr;
-      PackEntry& q = pt.back().e[pt.back().n++];
-      q.w = w[i]; q.b = b[i]; q.gamma = gamma[i]; q.beta = beta[i]; q.mean = mean[i]; q.var = var[i];
-      q.wf = h->ws + p.wf; q.wd = h->ws + p.wd; q.bias = (float*)(h->ws + p.bias); q.scale = (float*)(h->ws + p.scale);
-      q.absmax = h->exact_tc() ? (float*)(h->ws + p.wmax) : nullptr;
-      q.cout = c.cout; q.cin = c.cin; q.taps = c.k * c.k; q.block0 = pblocks.back();
-      q.nofold = (h->bn1_train && i == 0) ? 1 : 0; q.pad_[0] = q.pad_[1] = q.pad_[2] = 0;
-      q.bias_b = (h->exact_tc() && fb) ? (float*)(h->ws + fb->bias) + mb.row : nullptr;
-      pblocks.back() += pack_ctas(c.cout, c.cin, c.k * c.k);
-      if (h->exact_tc()) {
-        SplitEntry& e = stt.back().e[stt.back().n++];
-        e.wf = (const float*)(h->ws + p.wf); e.wd = (const float*)(h->ws + p.wd);
-        e.wf16 = (__half*)(h->ws + p.wf16); e.wd16 = (__half*)(h->ws + p.wd16); e.plane_bytes = (long long)p.wplane; e.n = n;
-        e.absmax = (const float*)(h->ws + p.wmax); e.inv_scale = (float*)(h->ws + p.wmax) + 1; e.block0 = sblocks.back(); e.pad_ = 0;
-        e.wd16_b = nullptr; e.wf16_b = nullptr; e.b_plane_bytes = 0; e.b_pitch = 0; e.cout = c.cout;
-        if (fb) {
-          const int kf = (fb->c1 + 63) / 64 * 64 + fb->c3r + fb->cdr;
-          e.wd16_b = (__half*)(h->ws + fb->w_fwd) + (size_t)mb.row * fb->cx;      // stacked forward rows [n][cx]
-          e.wf16_b = (__half*)(h->ws + fb->w_dg) + mb.col;                         // column block of [cx][kf]
-          e.b_pitch = kf;
-          // both fused buffers are written through ONE plane distance per entry: the kernel applies it to wd16_b and wf16_b alike,
-          // so the two buffers are planned with equal plane sizes (max of the two)
-          e.b_plane_bytes = (long long)std::max(fb->w_fwd_plane, fb->w_dg_plane);
-        }
-        sblocks.back() += (int)((n + 255) / 256);
-      }
-    }
-    for (size_t k = 0; k < pt.size(); ++k) {
-      int rc = h->fast() ? launch_pack_all<__half>(pt[k], pblocks[k], s) : launch_pack_all<float>(pt[k], pblocks[k], s);
-      if (rc) return h->fail(rc, "pack_weights: " + ssnb::thread_error());
-    }
-    if (h->exact_tc())
-      for (size_t k = 0; k < stt.size(); ++k)
-        if (int rc = launch_split_all(stt[k], sblocks[k], s)) return h->fail(rc, "pack_weights split: " + ssnb::thread_error());
   }
+  // bn1_train: conv1 is not folded.  EXACT_TC: the layers of a fused sibling block share one absmax slot, and the fold and
+  // split launches also write the block's fused operands
+  auto adjust = [&](size_t i, PackEntry& q, SplitEntry* e) {
+    q.nofold = (h->bn1_train && i == 0) ? 1 : 0;
+    const Member& mb = member[i];
+    if (!h->exact_tc() || mb.block < 0) return;
+    const FusedBlock& fb = h->fused[mb.block];
+    q.bias_b = (float*)(h->ws + fb.bias) + mb.row;
+    const int kf = (fb.c1 + 63) / 64 * 64 + fb.c3r + fb.cdr;
+    e->wd16_b = (__half*)(h->ws + fb.w_fwd) + (size_t)mb.row * fb.cx;      // stacked forward rows [n][cx]
+    e->wf16_b = (__half*)(h->ws + fb.w_dg) + mb.col;                         // column block of [cx][kf]
+    e->b_pitch = kf;
+    // both fused buffers are written through ONE plane distance per entry: the kernel applies it to wd16_b and wf16_b alike,
+    // so the two buffers are planned with equal plane sizes (max of the two)
+    e->b_plane_bytes = (long long)std::max(fb.w_fwd_plane, fb.w_dg_plane);
+  };
+  if (int rc = h->pack_weights(w, b, gamma, beta, mean, var, h->convs[0].cin, adjust, "pack_weights", s)) return h->fail(rc, ssnb::thread_error());
   if (h->ops.size() && h->ops[0].umma.enabled) {      // conv1's space-to-depth weights, every operand plane
     const PackedConv& p = h->packed[0];
     for (int pl = 0; pl < h->nplanes(); ++pl) {
@@ -1023,8 +870,7 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
   int rc;
   h->s2d_ready = h->tensor_cores() && h->ops[0].umma.enabled;
   if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
-  else rc = h->fast() ? launch_nchw_to_nhwc<__half>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s)
-                    : launch_nchw_to_nhwc<float>(input_nchw, h->F, d.C, d.H, d.W, d, 1.0f, s);
+  else rc = h->value_write(h->val_by_name["data"], false, input_nchw, 1.0f, s);
   if (rc) { h->s2d_ready = false; return h->fail(rc, "input layout: " + ssnb::thread_error()); }
   for (size_t i = 0; i < h->ops.size(); ++i) {
     const Op& o = h->ops[i];
@@ -1035,10 +881,10 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
     if (o.fuse_role == 1) {
       const FusedBlock& fb = h->fused[o.fuse_block];
       double fl = 0.0;
-      for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += conv_flops(h, h->ops[j]);
+      for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j]);
       tag_next(0, fl, fused_name(h, fb));
       r = umma_conv_launch(h->umma_ctx, fb.fwd, s);
-    } else r = run_fwd(h, o, input_nchw, feat, s);
+    } else r = run_fwd(h, o, feat, s);
     if (prof) cudaProfilerStop();
     if (r) { h->s2d_ready = false; return h->fail(r, "fwd " + o.id + ": " + ssnb::thread_error()); }
   }
@@ -1074,7 +920,7 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
       if (!rc && o.fuse_role == 1) {                                   // ... one fused data gradient
         const FusedBlock& fb = h->fused[o.fuse_block];
         double fl = 0.0;
-        for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += conv_flops(h, h->ops[j]);
+        for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j]);
         tag_next(1, fl, fused_name(h, fb));
         rc = umma_conv_launch(h->umma_ctx, fb.dgrad, s, h->fold_pools && o.dgrad_masks);
       }
@@ -1089,12 +935,12 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
     auto flush = [&]() -> int { int rc = launch_wgrad_finalize_all(t, 1.0f / gs, h->grad_accumulate, s); t.n = 0; t.total_blocks = 0; return rc; };
     for (int oi : h->pending_finalize) {
       const Op& o = h->ops[oi];
-      const ConvSpec& c = h->convs[o.conv];
+      const Conv& c = h->convs[o.conv];
       FinalizeEntry& q = t.e[t.n];
       q.partial = (const float*)(h->ws + o.partial_off); q.mult = (const float*)(h->ws + h->packed[o.conv].scale); q.dw = h->dw[o.conv];
       const bool bias_w = o.dy_premasked && o.bias_in_wgrad && h->db.size() && h->db[o.conv];
       q.bias_partial = bias_w ? (const float*)(h->ws + o.bias_partial_off) : nullptr; q.db = bias_w ? h->db[o.conv] : nullptr;
-      q.splits = o.umma_wgrad.p.splits; q.taps = c.k * c.k; q.Cout = c.cout; q.Cin = c.cin; q.block0 = t.total_blocks; q.pad_ = 0;
+      q.splits = o.umma_wgrad.p.splits; q.taps = c.kh * c.kw; q.Cout = c.cout; q.Cin = c.cin; q.block0 = t.total_blocks; q.pad_ = 0;
       t.total_blocks += (int)(((long long)q.taps * q.Cout * q.Cin + 255) / 256);
       if (++t.n == FIN_MAX) if (int rc = flush()) { h->pending_finalize.clear(); return h->fail(rc, "finalize: " + ssnb::thread_error()); }
     }
@@ -1107,8 +953,8 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
   if (op_lo < 0 || op_lo > op_hi) return h->fail(SSNB_EINVAL, "backbone_bwd_range: bad op range");
   // the range that starts at the global pool reads dfeat: choose the gradient exponent of this backward from it first
   if (op_hi == last && h->tensor_cores()) {
-    if (int rc = launch_grad_exponent(dfeat, (long long)h->F * h->vals[h->ops[last].in_val].C, h->cfg.grad_scale,
-                                      h->bufs[h->vals[h->ops[last].in_val].buf].H * h->bufs[h->vals[h->ops[last].in_val].buf].W, h->gscale, h->tc_flag, s))
+    if (int rc = launch_grad_exponent(dfeat, (long long)h->F * h->vals[h->ops[last].in].C, h->cfg.grad_scale,
+                                      h->bufs[h->vals[h->ops[last].in].buf].H * h->bufs[h->vals[h->ops[last].in].buf].W, h->gscale, h->tc_flag, s))
       return h->fail(rc, "gradient exponent: " + ssnb::thread_error());
   }
   if (int rc = run_range(op_hi, op_lo)) return rc;
@@ -1125,20 +971,19 @@ int ssnb_num_ops(ssnb_handle h) { return h ? (int)h->ops.size() : 0; }
 
 int ssnb_op_info(ssnb_handle h, int op, char* kind, int kind_cap, char* in_name, int in_cap, char* out_name, int out_cap) {
   if (!h || op < 0 || op >= (int)h->ops.size()) return SSNB_EINVAL;
-  static const char* kn[] = {"conv", "maxpool", "avgpool", "gpool", "bn"};
   const Op& o = h->ops[op];
-  if (kind) snprintf(kind, kind_cap, "%s", kn[o.kind]);
-  if (in_name) snprintf(in_name, in_cap, "%s", h->vals[o.in_val].name.c_str());
-  if (out_name) snprintf(out_name, out_cap, "%s", o.out_val >= 0 ? h->vals[o.out_val].name.c_str() : "feat");
+  if (kind) snprintf(kind, kind_cap, "%s", kOpKindName[o.kind]);
+  if (in_name) snprintf(in_name, in_cap, "%s", h->vals[o.in].name.c_str());
+  if (out_name) snprintf(out_name, out_cap, "%s", o.out >= 0 ? h->vals[o.out].name.c_str() : "feat");
   return SSNB_OK;
 }
 
 int ssnb_value_shape(ssnb_handle h, const char* name, int* c, int* hh, int* ww) {
   if (!h || !name) return SSNB_EINVAL;
-  auto it = h->val_by_name.find(name);
-  if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
-  const View v = h->view(it->second, false);
-  if (c) *c = v.C; if (hh) *hh = v.H; if (ww) *ww = v.W;
+  const int v = h->value_of(name);
+  if (v < 0) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
+  const View w = h->view(v, false);
+  if (c) *c = w.C; if (hh) *hh = w.H; if (ww) *ww = w.W;
   return SSNB_OK;
 }
 
@@ -1152,33 +997,28 @@ static float host_gscale(ssnb_handle h, int which, cudaStream_t s) {
 
 int ssnb_value_write(ssnb_handle h, const char* name, int grad, const float* src_nchw, void* stream) {
   if (!h || !name || !src_nchw || !h->ws) return SSNB_EINVAL;
-  auto it = h->val_by_name.find(name);
-  if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
+  const int v = h->value_of(name);
+  if (v < 0) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
   if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
-  const View v = h->view(it->second, grad != 0);
   // a gradient is stored in the units of the last backward: times 2^k (FAST: and grad_scale)
   const float sc = grad ? (h->fast() ? h->cfg.grad_scale : 1.0f) * host_gscale(h, 0, (cudaStream_t)stream) : 1.0f;
-  int rc = h->fast() ? launch_nchw_to_nhwc<__half>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream)
-                   : launch_nchw_to_nhwc<float>(src_nchw, h->F, v.C, v.H, v.W, v, sc, (cudaStream_t)stream);
-  if (!rc && h->exact_tc() && !grad) rc = tc_split_value(h, it->second, false, 1.0f, (cudaStream_t)stream);   // activation planes follow the fp32 value
+  const int rc = h->value_write(v, grad != 0, src_nchw, sc, (cudaStream_t)stream);
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
 }
 
 int ssnb_value_read(ssnb_handle h, const char* name, int grad, float* dst_nchw, void* stream) {
   if (!h || !name || !dst_nchw || !h->ws) return SSNB_EINVAL;
-  auto it = h->val_by_name.find(name);
-  if (it == h->val_by_name.end()) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
+  const int v = h->value_of(name);
+  if (v < 0) return h->fail(SSNB_EINVAL, std::string("unknown value ") + name);
   if ((grad & 1) && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");     // grad = 2: an activation's planes
   if (grad & 2) {       // diagnostic: read hi + lo of the value's EXACT_TC operand planes (bit 0: gradient planes, un-scaled)
-    if (!h->exact_tc() || !h->bufs[h->vals[it->second].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
+    if (!h->exact_tc() || !h->bufs[h->vals[v].buf].plane) return h->fail(SSNB_ESTATE, "value has no operand planes");
     const float sc = (grad & 1) ? host_gscale(h, 1, (cudaStream_t)stream) / h->cfg.grad_scale : 1.0f;
-    int rc = launch_planes_to_nchw(h->planes(it->second, (grad & 1) != 0), h->F, sc, dst_nchw, (cudaStream_t)stream);
+    const int rc = h->planes_read(v, (grad & 1) != 0, sc, dst_nchw, (cudaStream_t)stream);
     return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
   }
-  const View v = h->view(it->second, grad != 0);
   const float sc = grad ? host_gscale(h, 1, (cudaStream_t)stream) / (h->fast() ? h->cfg.grad_scale : 1.0f) : 1.0f;
-  int rc = h->fast() ? launch_nhwc_to_nchw<__half>(v, h->F, sc, dst_nchw, (cudaStream_t)stream)
-                   : launch_nhwc_to_nchw<float>(v, h->F, sc, dst_nchw, (cudaStream_t)stream);
+  const int rc = h->value_read(v, grad != 0, sc, dst_nchw, (cudaStream_t)stream);
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
 }
 
@@ -1187,7 +1027,7 @@ int ssnb_run_op(ssnb_handle h, int op, int backward, void* stream) {
   if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
   const Op& o = h->ops[op];
   if (o.kind == OP_GPOOL) return h->fail(SSNB_ENOSUPPORT, "run_op: global_pool runs through backbone_fwd/bwd");
-  int rc = backward ? run_bwd(h, o, nullptr, (cudaStream_t)stream) : run_fwd(h, o, nullptr, nullptr, (cudaStream_t)stream);
+  int rc = backward ? run_bwd(h, o, nullptr, (cudaStream_t)stream) : run_fwd(h, o, nullptr, (cudaStream_t)stream);
   return rc ? h->fail(rc, o.id + ": " + ssnb::thread_error()) : SSNB_OK;
 }
 

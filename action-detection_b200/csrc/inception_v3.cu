@@ -1,37 +1,24 @@
-// InceptionV3 test-time engine: graph table, workspace planner and forward schedule of the second backbone the reference
-// offers (--arch InceptionV3: ssn_models.py:133-139, binary_model.py:175-178; graph model_zoo/bninception/inceptionv3.yaml,
-// class model_zoo/bninception/pytorch_load.py:64-67).  Forward only, frozen BatchNorm folded into every convolution, in the
+// InceptionV3 test-time engine: graph table and forward schedule of the second backbone the reference offers (--arch
+// InceptionV3: ssn_models.py:133-139, binary_model.py:175-178; graph model_zoo/bninception/inceptionv3.yaml, class
+// model_zoo/bninception/pytorch_load.py:64-67).  Forward only, frozen BatchNorm folded into every convolution, in the
 // three precisions of the BNInception engine: EXACT_FP32 on the SIMT kernels of simt_conv.cu, FAST_FP16 and EXACT_TC on the
 // wgmma kernel of umma_conv.cu (every convolution, through its tap-table bind: valid stride-1 / stride-2 layers tile at the
 // output's geometry with the A map at the input's dims, 1x3 / 3x1 / 1x7 / 7x1 and 25-tap 5x5 tables, and the 3- / 10-channel
-// stem over an input zero-padded to 16 channels with its weights padded to match).  It reuses the BNInception engine's kernels
-// (convolutions, weight packing and splitting, vectorised pools, global pool, layout conversion) and shares no state with it.
+// stem over an input zero-padded to 16 channels with its weights padded to match).  The graph records, workspace planner,
+// weight pack, pools and value I/O are the BNInception engine's (graph.cuh); this file adds the block table, the stem
+// padding and the tap-table binds.  Its handle and ABI section (ssnb_iv3_*) are its own.
 #include <cstdio>
-#include <map>
 #include <string>
 #include <vector>
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
+#include "graph.cuh"
 #include "umma_conv.cuh"
-
-namespace ssnb {
-const std::string& thread_error();
-}
 
 namespace {
 
 using namespace ssnb;
-
-// one convolution + BN + ReLU of inceptionv3.yaml; `id` is the blob it writes (the yaml's `<id>_Conv2D` / `<id>_batchnorm`)
-struct Conv { std::string id; int cin, cout, kh, kw, stride, ph, pw; };
-struct Buf { std::string name; int H, W, C; size_t off = 0, hoff = 0, plane = 0; };   // EXACT_TC: fp16 hi / lo planes (lo = hi + plane)
-struct Val { std::string name; int buf, coff, C; };
-enum Kind { K_CONV = 0, K_MAXPOOL = 1, K_AVGPOOL = 2, K_GPOOL = 3 };
-const char* const kKindName[] = {"conv", "maxpool", "avgpool", "gpool"};
-struct Op { Kind kind; std::string id; int in, out; int conv = -1; int k = 0, stride = 1, pad = 0; size_t argmax_off = 0; };
-// EXACT_TC: wf16 / wd16 hi planes (lo = hi + wplane); wmax: [0] max |folded weight|, [1] 1 / the power-of-two plane scale
-struct Packed { size_t wf, wd, bias, scale; size_t wf16 = 0, wd16 = 0, wplane = 0, wmax = 0; };
 
 constexpr int kInput = 299;
 // tensor-core modes: the stem's input channels as the wgmma kernel reads them (K % 8 == 0 and 32-byte pixels), zeros past
@@ -40,86 +27,47 @@ constexpr int kStemK = 16;
 
 }  // namespace
 
-struct ssnb_iv3 {
+struct ssnb_iv3 : ssnb::Graph<ssnb::GraphOp> {
   ssnb_iv3_config cfg;
-  std::vector<Conv> convs;
-  std::vector<Buf> bufs;
-  std::vector<Val> vals;
-  std::map<std::string, int> val_by_name;
-  std::vector<Op> ops;
-  std::vector<Packed> packed;
   std::vector<UmmaConvPlan> plans;    // tensor-core modes: one forward plan per convolution (bound by ssnb_iv3_set_workspace)
   UmmaContext umma_ctx;
-  size_t esz = 4;
   size_t w0pad = 0;                   // tensor-core modes: the stem's weights zero-padded to kStemK input channels (fp32)
-  size_t wmax_off = 0;                // EXACT_TC: the per-layer weight maxima / plane scales
   size_t ws_bytes = 0;
-  char* ws = nullptr;
   bool weights_ready = false;
 
-  bool fast() const { return cfg.precision == SSNB_FAST_FP16; }
-  bool exact_tc() const { return cfg.precision == SSNB_EXACT_TC; }
-  bool tensor_cores() const { return cfg.precision != SSNB_EXACT_FP32; }
-  // input channels of convolution i as the kernels read them
-  int conv_k(int i) const { return (tensor_cores() && i == 0) ? kStemK : convs[i].cin; }
-
-  View view(int v) const {
-    const Val& x = vals[v];
-    const Buf& b = bufs[x.buf];
-    View w;
-    w.base = ws + b.off; w.H = b.H; w.W = b.W; w.C = x.C; w.pitch = b.C; w.coff = x.coff;
-    return w;
-  }
-  // EXACT_TC: the value's fp16 hi / lo operand planes
-  View planes(int v) const {
-    View w = view(v);
-    w.base = ws + bufs[vals[v].buf].hoff; w.lo_off = (long long)bufs[vals[v].buf].plane;
-    return w;
-  }
-  // what the wgmma kernel reads and writes: the fp16 storage (FAST) or the operand planes (EXACT_TC)
-  View operand(int v) const { return exact_tc() ? planes(v) : view(v); }
+  // input channels of convolution 0 as the kernels read them
+  int stem_k() const { return tensor_cores() ? kStemK : convs[0].cin; }
 };
 
 namespace {
 
 int fail(int code, const std::string& msg) { set_thread_error(msg); return code; }
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-int conv_out(int h, int k, int s, int p) { return (h + 2 * p - k) / s + 1; }
-// every pool of the graph divides evenly, so Caffe's ceil mode (layer_factory.py:41-53) gives the floor size
-int pool_out(int h, int k, int s, int p) { return (h + 2 * p - k + s - 1) / s + 1; }
 
 // Builds the graph of inceptionv3.yaml in its layer order.  Convolution outputs that are branch ends of a block are
 // channel slices of the block's concat buffer (`<block>_join`), in the yaml's concat order, so no concat runs.
 struct Builder {
   ssnb_iv3* e;
-  int add_buf(const std::string& name, int H, int W, int C) { e->bufs.push_back({name, H, W, C}); return (int)e->bufs.size() - 1; }
-  int add_val(const std::string& name, int buf, int coff, int C) {
-    e->vals.push_back({name, buf, coff, C});
-    e->val_by_name[name] = (int)e->vals.size() - 1;
-    return (int)e->vals.size() - 1;
-  }
-  int whole(const std::string& name, int H, int W, int C) { return add_val(name, add_buf(name, H, W, C), 0, C); }
   int H(int v) const { return e->bufs[e->vals[v].buf].H; }
   int W(int v) const { return e->bufs[e->vals[v].buf].W; }
   int C(int v) const { return e->vals[v].C; }
   // conv kh x kw / stride, pads (ph, pw); dst: -1 = a buffer of its own, else the concat buffer and channel offset
   int conv(const std::string& id, int in, int cout, int kh, int kw, int stride, int ph, int pw, int dst = -1, int coff = 0) {
     const int oh = conv_out(H(in), kh, stride, ph), ow = conv_out(W(in), kw, stride, pw);
-    const int v = dst < 0 ? whole(id, oh, ow, cout) : add_val(id, dst, coff, cout);
+    const int v = dst < 0 ? e->whole(id, oh, ow, cout) : e->add_value(id, dst, coff, cout);
     e->convs.push_back({id, C(in), cout, kh, kw, stride, ph, pw});
-    Op o; o.kind = K_CONV; o.id = id; o.in = in; o.out = v; o.conv = (int)e->convs.size() - 1; o.stride = stride;
+    GraphOp o; o.kind = OP_CONV; o.id = id; o.in = in; o.out = v; o.conv = (int)e->convs.size() - 1; o.stride = stride;
     e->ops.push_back(o);
     return v;
   }
-  int pool(Kind kind, const std::string& id, int in, int k, int s, int p, int dst = -1, int coff = 0) {
+  int pool(OpKind kind, const std::string& id, int in, int k, int s, int p, int dst = -1, int coff = 0) {
     const int oh = pool_out(H(in), k, s, p), ow = pool_out(W(in), k, s, p);
-    const int v = dst < 0 ? whole(id, oh, ow, C(in)) : add_val(id, dst, coff, C(in));
-    Op o; o.kind = kind; o.id = id; o.in = in; o.out = v; o.k = k; o.stride = s; o.pad = p;
+    const int v = dst < 0 ? e->whole(id, oh, ow, C(in)) : e->add_value(id, dst, coff, C(in));
+    GraphOp o; o.kind = kind; o.id = id; o.in = in; o.out = v; o.k = k; o.stride = s; o.pad = p;
     e->ops.push_back(o);
     return v;
   }
-  int join(const std::string& p, int HW, int C) { return add_buf(p + "_join", HW, HW, C); }
-  int join_val(const std::string& p, int buf) { return add_val(p + "_join", buf, 0, e->bufs[buf].C); }
+  int join(const std::string& p, int HW, int C) { return e->add_buffer(p + "_join", HW, HW, C); }
+  int join_val(const std::string& p, int buf) { return e->add_value(p + "_join", buf, 0, e->bufs[buf].C); }
 
   // 35x35 blocks mixed, mixed_1, mixed_2: 1x1 | 1x1 -> 5x5 | 1x1 -> 3x3 -> 3x3 | avg pool -> 1x1
   int block_a(const std::string& p, int x, int proj) {
@@ -130,7 +78,7 @@ struct Builder {
     t = conv(p + "_tower_1_conv", x, 64, 1, 1, 1, 0, 0);
     t = conv(p + "_tower_1_conv_1", t, 96, 3, 3, 1, 1, 1);
     conv(p + "_tower_1_conv_2", t, 96, 3, 3, 1, 1, 1, j, 128);
-    t = pool(K_AVGPOOL, p + "_tower_2_pool", x, 3, 1, 1);
+    t = pool(OP_AVGPOOL, p + "_tower_2_pool", x, 3, 1, 1);
     conv(p + "_tower_2_conv", t, proj, 1, 1, 1, 0, 0, j, 224);
     return join_val(p, j);
   }
@@ -141,7 +89,7 @@ struct Builder {
     int t = conv(p + "_tower_conv", x, 64, 1, 1, 1, 0, 0);
     t = conv(p + "_tower_conv_1", t, 96, 3, 3, 1, 1, 1);
     conv(p + "_tower_conv_2", t, 96, 3, 3, 2, 0, 0, j, 384);
-    pool(K_MAXPOOL, p + "_pool", x, 3, 2, 0, j, 480);
+    pool(OP_MAXPOOL, p + "_pool", x, 3, 2, 0, j, 480);
     return join_val(p, j);
   }
   // 17x17 blocks mixed_4 .. mixed_7 (c7 = 128, 160, 160, 192): 1x1 | 1x1 -> 7x1 -> 1x7 | 1x1 -> 1x7 -> 7x1 -> 1x7 -> 7x1 |
@@ -157,7 +105,7 @@ struct Builder {
     t = conv(p + "_tower_1_conv_2", t, c7, 7, 1, 1, 3, 0);
     t = conv(p + "_tower_1_conv_3", t, c7, 1, 7, 1, 0, 3);
     conv(p + "_tower_1_conv_4", t, 192, 7, 1, 1, 3, 0, j, 384);
-    t = pool(K_AVGPOOL, p + "_tower_2_pool", x, 3, 1, 1);
+    t = pool(OP_AVGPOOL, p + "_tower_2_pool", x, 3, 1, 1);
     conv(p + "_tower_2_conv", t, 192, 1, 1, 1, 0, 0, j, 576);
     return join_val(p, j);
   }
@@ -170,12 +118,12 @@ struct Builder {
     t = conv(p + "_tower_1_conv_1", t, 192, 7, 1, 1, 3, 0);
     t = conv(p + "_tower_1_conv_2", t, 192, 1, 7, 1, 0, 3);
     conv(p + "_tower_1_conv_3", t, 192, 3, 3, 2, 0, 0, j, 320);
-    pool(K_MAXPOOL, p + "_pool", x, 3, 2, 0, j, 512);
+    pool(OP_MAXPOOL, p + "_pool", x, 3, 2, 0, j, 512);
     return join_val(p, j);
   }
   // 8x8 blocks mixed_9 (avg pool) and mixed_10 (max pool 3x3/1/1): 1x1 | 1x1 -> (3x1 | 1x3) | 1x1 -> 3x3 -> (3x1 | 1x3) |
   // pool -> 1x1
-  int block_e(const std::string& p, int x, Kind pool_kind) {
+  int block_e(const std::string& p, int x, OpKind pool_kind) {
     const int hw = H(x), j = join(p, hw, 320 + 4 * 384 + 192);
     conv(p + "_conv", x, 320, 1, 1, 1, 0, 0, j, 0);
     int t = conv(p + "_tower_conv", x, 384, 1, 1, 1, 0, 0);
@@ -191,14 +139,14 @@ struct Builder {
   }
 
   void build(int in_ch) {
-    int x = add_val("data", add_buf("data", kInput, kInput, e->tensor_cores() ? kStemK : in_ch), 0, in_ch);
+    int x = e->add_value("data", e->add_buffer("data", kInput, kInput, e->tensor_cores() ? kStemK : in_ch), 0, in_ch);
     x = conv("conv", x, 32, 3, 3, 2, 0, 0);
     x = conv("conv_1", x, 32, 3, 3, 1, 0, 0);
     x = conv("conv_2", x, 64, 3, 3, 1, 1, 1);
-    x = pool(K_MAXPOOL, "pool", x, 3, 2, 0);
+    x = pool(OP_MAXPOOL, "pool", x, 3, 2, 0);
     x = conv("conv_3", x, 80, 1, 1, 1, 0, 0);
     x = conv("conv_4", x, 192, 3, 3, 1, 0, 0);
-    x = pool(K_MAXPOOL, "pool_1", x, 3, 2, 0);
+    x = pool(OP_MAXPOOL, "pool_1", x, 3, 2, 0);
     x = block_a("mixed", x, 32);
     x = block_a("mixed_1", x, 64);
     x = block_a("mixed_2", x, 64);
@@ -208,46 +156,17 @@ struct Builder {
     x = block_c("mixed_6", x, 160);
     x = block_c("mixed_7", x, 192);
     x = block_d("mixed_8", x);
-    x = block_e("mixed_9", x, K_AVGPOOL);
-    x = block_e("mixed_10", x, K_MAXPOOL);
+    x = block_e("mixed_9", x, OP_AVGPOOL);
+    x = block_e("mixed_10", x, OP_MAXPOOL);
     // top_cls_pool (8x8 average) writes the caller's feat [F, 2048]; it has no workspace buffer
-    Op g; g.kind = K_GPOOL; g.id = "top_cls_pool"; g.in = x; g.out = -1; g.k = H(x);
+    GraphOp g; g.kind = OP_GPOOL; g.id = "top_cls_pool"; g.in = x; g.out = -1; g.k = H(x);
     e->ops.push_back(g);
   }
 };
 
+// the shared forward storage, then the stem's padded weights
 void plan(ssnb_iv3* e) {
-  const size_t F = (size_t)e->cfg.frames;
-  size_t off = 0;
-  e->esz = e->fast() ? 2 : 4;
-  for (Buf& b : e->bufs) { b.off = off; off = align_up(off + F * b.H * b.W * b.C * e->esz, 1024); }
-  if (e->exact_tc())
-    for (Buf& b : e->bufs) { b.plane = align_up(F * b.H * b.W * b.C * 2, 1024); b.hoff = off; off += 2 * b.plane; }
-  for (Op& o : e->ops)
-    if (o.kind == K_MAXPOOL) {       // the vectorised max pool records its arg-max (one byte per output element)
-      const View out = e->view(o.out);
-      o.argmax_off = off; off = align_up(off + F * out.H * out.W * out.C, 1024);
-    }
-  e->packed.resize(e->convs.size());
-  for (size_t i = 0; i < e->convs.size(); ++i) {
-    const Conv& c = e->convs[i];
-    const size_t n = (size_t)c.cout * e->conv_k((int)i) * c.kh * c.kw;
-    Packed& p = e->packed[i];
-    p.wf = off; off = align_up(off + n * e->esz, 1024);
-    p.wd = off; off = align_up(off + n * e->esz, 1024);
-    p.bias = off; off = align_up(off + c.cout * 4, 256);
-    p.scale = off; off = align_up(off + c.cout * 4, 256);
-    if (e->exact_tc()) {
-      p.wplane = align_up(n * 2, 1024);
-      p.wf16 = off; off += 2 * p.wplane;
-      p.wd16 = off; off += 2 * p.wplane;
-    }
-  }
-  if (e->exact_tc()) {      // one 8-byte (absmax, 1 / scale) slot per convolution, contiguous: zeroed by one memset before every pack
-    e->wmax_off = off;
-    for (size_t i = 0; i < e->convs.size(); ++i) e->packed[i].wmax = off + i * 8;
-    off = align_up(off + e->convs.size() * 8, 1024);
-  }
+  size_t off = e->plan_storage(0, false, e->stem_k(), 0);
   if (e->tensor_cores()) {
     const Conv& c = e->convs[0];
     e->w0pad = off; off = align_up(off + (size_t)c.cout * kStemK * c.kh * c.kw * 4, 1024);
@@ -291,15 +210,16 @@ int launch_pad_weights(const float* w, int cout, int cin, int taps, int cp, floa
 // which tests/test_gpu_inception_v3.py checks launch by launch at the EXACT_TC and FAST bars.
 int bind_plans(ssnb_iv3* e) {
   e->plans.assign(e->convs.size(), UmmaConvPlan());
-  for (const Op& o : e->ops) {
-    if (o.kind != K_CONV) continue;
+  for (const GraphOp& o : e->ops) {
+    if (o.kind != OP_CONV) continue;
     const Conv& c = e->convs[o.conv];
-    const Packed& pk = e->packed[o.conv];
+    const PackedConv& pk = e->packed[o.conv];
+    const int ck = o.conv == 0 ? kStemK : c.cin;
     int dy[UMMA_MAX_TAPS], dx[UMMA_MAX_TAPS];
     for (int r = 0; r < c.kh; ++r)
       for (int q = 0; q < c.kw; ++q) { dy[r * c.kw + q] = r - c.ph; dx[r * c.kw + q] = q - c.pw; }
     View in = e->operand(o.in);
-    in.C = e->conv_k(o.conv);
+    in.C = ck;
     UmmaTcOpts tc;
     const UmmaTcOpts* opts = nullptr;
     if (e->exact_tc()) {
@@ -308,52 +228,30 @@ int bind_plans(ssnb_iv3* e) {
       opts = &tc;
     }
     const __half* w = (const __half*)(e->ws + (e->exact_tc() ? pk.wd16 : pk.wd));
-    if (int rc = umma_conv_bind_taps(e->umma_ctx, e->plans[o.conv], in, e->operand(o.out), e->cfg.frames, e->conv_k(o.conv), c.cout, c.kh * c.kw,
+    if (int rc = umma_conv_bind_taps(e->umma_ctx, e->plans[o.conv], in, e->operand(o.out), e->F, ck, c.cout, c.kh * c.kw,
                                      dy, dx, w, (const float*)(e->ws + pk.bias), 1, opts, c.stride))
       return fail(rc, "bind(" + c.id + "): " + thread_error());
   }
   return SSNB_OK;
 }
 
-const Conv* conv_at(const ssnb_iv3* e, int idx) { return (idx >= 0 && idx < (int)e->convs.size()) ? &e->convs[idx] : nullptr; }
-
-int run_op(ssnb_iv3* e, const Op& o, float* feat, cudaStream_t s) {
-  const int F = e->cfg.frames;
-  if (o.kind == K_CONV && e->tensor_cores()) {
-    const Conv& c = e->convs[o.conv];
-    const View out = e->view(o.out);
-    t_tag.phase = 0; t_tag.flop = 2.0 * F * out.H * out.W * (double)c.cout * c.cin * c.kh * c.kw; t_tag.op = o.id.c_str();
+int run_op(ssnb_iv3* e, const GraphOp& o, float* feat, cudaStream_t s) {
+  if (o.kind == OP_CONV && e->tensor_cores()) {
+    t_tag.phase = 0; t_tag.flop = e->conv_flops(o); t_tag.op = o.id.c_str();
     return umma_conv_launch(e->umma_ctx, e->plans[o.conv], s);
   }
-  if (o.kind == K_CONV) {
-    const Conv& c = e->convs[o.conv];
-    const View in = e->view(o.in), out = e->view(o.out);
-    ConvArgs a;
-    a.src = in.base; a.SH = in.H; a.SW = in.W; a.Csrc = in.C; a.src_pitch = in.pitch; a.src_coff = in.coff;
-    a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
-    a.wgt = e->ws + e->packed[o.conv].wf; a.bias = (const float*)(e->ws + e->packed[o.conv].bias);
-    a.F = F; a.kh = c.kh; a.kw = c.kw; a.stride = c.stride; a.pad_h = c.ph; a.pad_w = c.pw; a.relu = 1; a.accumulate = 0; a.dgrad = 0;
-    t_tag.phase = 0; t_tag.flop = 2.0 * F * out.H * out.W * (double)c.cout * c.cin * c.kh * c.kw; t_tag.op = o.id.c_str();
-    return launch_conv<float>(a, s);
-  }
+  if (o.kind == OP_CONV) return e->simt_conv_fwd(o, 1, s);
   t_tag.phase = 0; t_tag.flop = 0.0; t_tag.op = o.id.c_str();
-  // EXACT_TC: the pools also write their output's operand planes (the next convolution's A operand)
-  const View pl = (e->exact_tc() && o.out >= 0) ? e->planes(o.out) : View();
-  uint8_t* am = (uint8_t*)(e->ws + o.argmax_off);
-  if (o.kind == K_MAXPOOL)
-    return e->fast() ? launch_maxpool_fwd_vec<__half>(e->view(o.in), e->view(o.out), pl, F, o.k, o.stride, o.pad, am, s)
-                     : launch_maxpool_fwd_vec<float>(e->view(o.in), e->view(o.out), pl, F, o.k, o.stride, o.pad, am, s);
-  if (o.kind == K_AVGPOOL)
-    return e->fast() ? launch_avgpool3_vec<__half>(e->view(o.in), e->view(o.out), pl, F, 0, s)
-                     : launch_avgpool3_vec<float>(e->view(o.in), e->view(o.out), pl, F, 0, s);
+  if (o.kind != OP_GPOOL) return e->pool_fwd(o, s);
   if (!feat) return fail(SSNB_EINVAL, "top_cls_pool needs the feat output pointer");
-  return e->fast() ? launch_gpool_fwd<__half>(e->view(o.in), F, feat, s) : launch_gpool_fwd<float>(e->view(o.in), F, feat, s);
+  return e->gpool_fwd(o, feat, s);
 }
 
-int value_of(const ssnb_iv3* e, const char* name) {
-  if (!name) return -1;
-  auto it = e->val_by_name.find(name);
-  return it == e->val_by_name.end() ? -1 : it->second;
+// the graph of in_channels, planned for cfg
+void build(ssnb_iv3* e, const ssnb_iv3_config& cfg) {
+  e->cfg = cfg;
+  e->F = cfg.frames; e->precision = cfg.precision; e->esz = e->fast() ? 2 : 4;
+  Builder{e}.build(cfg.in_channels);
 }
 
 }  // namespace
@@ -365,18 +263,17 @@ int ssnb_iv3_num_convs(void) { return 94; }
 int ssnb_iv3_conv_info(int idx, int in_channels, char* name, int name_cap, int* cin, int* cout, int* kh, int* kw, int* stride, int* pad_h,
                        int* pad_w) {
   ssnb_iv3 e;
-  e.cfg.in_channels = in_channels; e.cfg.frames = 1; e.cfg.precision = SSNB_EXACT_FP32; e.cfg.reserved = 0;
-  Builder{&e}.build(in_channels);
-  const Conv* c = conv_at(&e, idx);
-  if (!c) return fail(SSNB_EINVAL, "ssnb_iv3_conv_info: index out of range");
-  if (name && name_cap > 0) snprintf(name, name_cap, "%s", c->id.c_str());
-  if (cin) *cin = c->cin;
-  if (cout) *cout = c->cout;
-  if (kh) *kh = c->kh;
-  if (kw) *kw = c->kw;
-  if (stride) *stride = c->stride;
-  if (pad_h) *pad_h = c->ph;
-  if (pad_w) *pad_w = c->pw;
+  build(&e, ssnb_iv3_config{in_channels, 1, SSNB_EXACT_FP32, 0});
+  if (idx < 0 || idx >= (int)e.convs.size()) return fail(SSNB_EINVAL, "ssnb_iv3_conv_info: index out of range");
+  const Conv& c = e.convs[idx];
+  if (name && name_cap > 0) snprintf(name, name_cap, "%s", c.id.c_str());
+  if (cin) *cin = c.cin;
+  if (cout) *cout = c.cout;
+  if (kh) *kh = c.kh;
+  if (kw) *kw = c.kw;
+  if (stride) *stride = c.stride;
+  if (pad_h) *pad_h = c.ph;
+  if (pad_w) *pad_w = c.pw;
   return SSNB_OK;
 }
 
@@ -388,8 +285,7 @@ int ssnb_iv3_create(const ssnb_iv3_config* cfg, ssnb_iv3_handle* out) {
   if (cfg->precision != SSNB_EXACT_FP32 && cfg->precision != SSNB_FAST_FP16 && cfg->precision != SSNB_EXACT_TC)
     return fail(SSNB_EINVAL, "ssnb_iv3_create: unknown precision");
   ssnb_iv3* e = new ssnb_iv3();
-  e->cfg = *cfg;
-  Builder{e}.build(cfg->in_channels);
+  build(e, *cfg);
   plan(e);
   *out = e;
   return SSNB_OK;
@@ -416,46 +312,16 @@ int ssnb_iv3_pack_weights(ssnb_iv3_handle h, const float* const* w, const float*
     if (!w[i] || !b[i] || !gamma[i] || !beta[i] || !mean[i] || !var[i])
       return fail(SSNB_EINVAL, "ssnb_iv3_pack_weights: null tensor for " + h->convs[i].id);
   cudaStream_t s = (cudaStream_t)stream;
-  const float* w0 = w[0];
+  std::vector<const float*> ws(w, w + h->convs.size());
   if (h->tensor_cores()) {       // the stem's kernels over the zero-padded input channels
     const Conv& c = h->convs[0];
     if (int rc = launch_pad_weights(w[0], c.cout, c.cin, c.kh * c.kw, kStemK, (float*)(h->ws + h->w0pad), s))
       return fail(rc, "ssnb_iv3_pack_weights: " + thread_error());
-    w0 = (const float*)(h->ws + h->w0pad);
+    ws[0] = (const float*)(h->ws + h->w0pad);
   }
-  if (h->exact_tc() && cudaMemsetAsync(h->ws + h->wmax_off, 0, h->convs.size() * 8, s) != cudaSuccess)
-    return fail(SSNB_ECUDA, "ssnb_iv3_pack_weights: memset failed");
-  PackTable t;
-  SplitTable st;
-  int blocks = 0, sblocks = 0;
-  t.n = 0; t.pad_ = 0; st.n = 0; st.pad_ = 0;
-  for (size_t i = 0; i < h->convs.size(); ++i) {
-    const Conv& c = h->convs[i];
-    const Packed& p = h->packed[i];
-    const int ck = h->conv_k((int)i), taps = c.kh * c.kw;
-    PackEntry& q = t.e[t.n++];
-    q.w = i == 0 ? w0 : w[i]; q.b = b[i]; q.gamma = gamma[i]; q.beta = beta[i]; q.mean = mean[i]; q.var = var[i];
-    q.wf = h->ws + p.wf; q.wd = h->ws + p.wd; q.bias = (float*)(h->ws + p.bias); q.scale = (float*)(h->ws + p.scale);
-    q.absmax = h->exact_tc() ? (float*)(h->ws + p.wmax) : nullptr;
-    q.cout = c.cout; q.cin = ck; q.taps = taps; q.block0 = blocks;
-    q.nofold = 0; q.pad_[0] = q.pad_[1] = q.pad_[2] = 0; q.bias_b = nullptr;
-    blocks += pack_ctas(c.cout, ck, taps);
-    if (h->exact_tc()) {        // hi / lo planes of both layouts with the layer's power-of-two scale (tc_glue.cu)
-      const long long n = (long long)c.cout * ck * taps;
-      SplitEntry& se = st.e[st.n++];
-      se.wf = (const float*)(h->ws + p.wf); se.wd = (const float*)(h->ws + p.wd);
-      se.wf16 = (__half*)(h->ws + p.wf16); se.wd16 = (__half*)(h->ws + p.wd16); se.plane_bytes = (long long)p.wplane; se.n = n;
-      se.absmax = (const float*)(h->ws + p.wmax); se.inv_scale = (float*)(h->ws + p.wmax) + 1; se.block0 = sblocks; se.pad_ = 0;
-      se.wd16_b = nullptr; se.wf16_b = nullptr; se.b_plane_bytes = 0; se.b_pitch = 0; se.cout = c.cout;
-      sblocks += (int)((n + 255) / 256);
-    }
-    if (t.n == PACK_MAX || i + 1 == h->convs.size()) {
-      int rc = h->fast() ? launch_pack_all<__half>(t, blocks, s) : launch_pack_all<float>(t, blocks, s);
-      if (rc) return fail(rc, "ssnb_iv3_pack_weights: " + thread_error());
-      if (h->exact_tc() && (rc = launch_split_all(st, sblocks, s))) return fail(rc, "ssnb_iv3_pack_weights split: " + thread_error());
-      t.n = 0; blocks = 0; st.n = 0; sblocks = 0;
-    }
-  }
+  if (int rc = h->pack_weights(ws.data(), b, gamma, beta, mean, var, h->stem_k(), [](size_t, PackEntry&, SplitEntry*) {},
+                               "ssnb_iv3_pack_weights", s))
+    return rc;
   h->weights_ready = true;
   return SSNB_OK;
 }
@@ -468,18 +334,18 @@ int ssnb_iv3_forward(ssnb_iv3_handle h, const float* input_nchw, float* feat, vo
   const View d = h->view(dv);
   int rc;
   if (!h->tensor_cores()) {
-    rc = launch_nchw_to_nhwc<float>(input_nchw, h->cfg.frames, d.C, d.H, d.W, d, 1.0f, s);
+    rc = h->value_write(dv, false, input_nchw, 1.0f, s);
   } else {      // every kStemK channels of a pixel written, the padding as zeros
-    rc = h->fast() ? launch_nchw_to_nhwc_pad<__half>(input_nchw, h->cfg.frames, d.C, d.H * d.W, d.pitch, (__half*)d.base, s)
-                   : launch_nchw_to_nhwc_pad<float>(input_nchw, h->cfg.frames, d.C, d.H * d.W, d.pitch, (float*)d.base, s);
+    rc = h->fast() ? launch_nchw_to_nhwc_pad<__half>(input_nchw, h->F, d.C, d.H * d.W, d.pitch, (__half*)d.base, s)
+                   : launch_nchw_to_nhwc_pad<float>(input_nchw, h->F, d.C, d.H * d.W, d.pitch, (float*)d.base, s);
     if (!rc && h->exact_tc()) {
       View x = d, xp = h->planes(dv);
       x.C = xp.C = d.pitch;
-      rc = launch_split_view(x, h->cfg.frames, 1.0f, xp, nullptr, s);
+      rc = launch_split_view(x, h->F, 1.0f, xp, nullptr, s);
     }
   }
   if (rc) return fail(rc, "input layout: " + thread_error());
-  for (const Op& o : h->ops)
+  for (const GraphOp& o : h->ops)
     if (int rc = run_op(h, o, feat, s)) return fail(rc, o.id + ": " + thread_error());
   return SSNB_OK;
 }
@@ -489,8 +355,8 @@ int ssnb_iv3_num_ops(ssnb_iv3_handle h) { return h ? (int)h->ops.size() : 0; }
 int ssnb_iv3_op_info(ssnb_iv3_handle h, int op, char* kind, int kind_cap, char* in_name, int in_cap, char* out_name, int out_cap, int* conv,
                      int* k, int* stride, int* pad) {
   if (!h || op < 0 || op >= (int)h->ops.size()) return fail(SSNB_EINVAL, "ssnb_iv3_op_info: op out of range");
-  const Op& o = h->ops[op];
-  if (kind && kind_cap > 0) snprintf(kind, kind_cap, "%s", kKindName[o.kind]);
+  const GraphOp& o = h->ops[op];
+  if (kind && kind_cap > 0) snprintf(kind, kind_cap, "%s", kOpKindName[o.kind]);
   if (in_name && in_cap > 0) snprintf(in_name, in_cap, "%s", h->vals[o.in].name.c_str());
   if (out_name && out_cap > 0) snprintf(out_name, out_cap, "%s", o.out >= 0 ? h->vals[o.out].name.c_str() : "top_cls_global_pool");
   if (conv) *conv = o.conv;
@@ -502,9 +368,9 @@ int ssnb_iv3_op_info(ssnb_iv3_handle h, int op, char* kind, int kind_cap, char* 
 
 int ssnb_iv3_value_info(ssnb_iv3_handle h, const char* name, int* c, int* hh, int* ww, char* buffer, int buffer_cap, int* coff) {
   if (!h) return fail(SSNB_EINVAL, "null handle");
-  const int v = value_of(h, name);
+  const int v = h->value_of(name);
   if (v < 0) return fail(SSNB_EINVAL, std::string("ssnb_iv3_value_info: unknown value ") + (name ? name : "(null)"));
-  const Buf& b = h->bufs[h->vals[v].buf];
+  const Buffer& b = h->bufs[h->vals[v].buf];
   if (c) *c = h->vals[v].C;
   if (hh) *hh = b.H;
   if (ww) *ww = b.W;
@@ -515,35 +381,20 @@ int ssnb_iv3_value_info(ssnb_iv3_handle h, const char* name, int* c, int* hh, in
 
 int ssnb_iv3_value_write(ssnb_iv3_handle h, const char* name, const float* src_nchw, void* stream) {
   if (!h || !src_nchw || !h->ws) return fail(SSNB_EINVAL, "ssnb_iv3_value_write: null argument or no workspace");
-  const int v = value_of(h, name);
+  const int v = h->value_of(name);
   if (v < 0) return fail(SSNB_EINVAL, std::string("ssnb_iv3_value_write: unknown value ") + (name ? name : "(null)"));
-  const View w = h->view(v);
-  cudaStream_t s = (cudaStream_t)stream;
-  int rc = h->fast() ? launch_nchw_to_nhwc<__half>(src_nchw, h->cfg.frames, w.C, w.H, w.W, w, 1.0f, s)
-                     : launch_nchw_to_nhwc<float>(src_nchw, h->cfg.frames, w.C, w.H, w.W, w, 1.0f, s);
-  if (!rc && h->exact_tc()) {       // the operand planes follow the value (the stem's input: all kStemK channels of a pixel)
-    View x = w, xp = h->planes(v);
-    if (w.C % 8) x.C = xp.C = w.pitch;
-    rc = launch_split_view(x, h->cfg.frames, 1.0f, xp, nullptr, s);
-  }
+  const int rc = h->value_write(v, false, src_nchw, 1.0f, (cudaStream_t)stream);
   return rc ? fail(rc, thread_error()) : SSNB_OK;
 }
 
 int ssnb_iv3_value_read(ssnb_iv3_handle h, const char* name, int planes, float* dst_nchw, void* stream) {
   if (!h || !dst_nchw || !h->ws) return fail(SSNB_EINVAL, "ssnb_iv3_value_read: null argument or no workspace");
-  const int v = value_of(h, name);
+  const int v = h->value_of(name);
   if (v < 0) return fail(SSNB_EINVAL, std::string("ssnb_iv3_value_read: unknown value ") + (name ? name : "(null)"));
+  if (planes && !h->exact_tc()) return fail(SSNB_ESTATE, "ssnb_iv3_value_read: operand planes exist in EXACT_TC only");
   cudaStream_t s = (cudaStream_t)stream;
-  int rc;
-  if (planes) {
-    if (!h->exact_tc()) return fail(SSNB_ESTATE, "ssnb_iv3_value_read: operand planes exist in EXACT_TC only");
-    rc = launch_planes_to_nchw(h->planes(v), h->cfg.frames, 1.0f, dst_nchw, s);
-  } else {
-    rc = h->fast() ? launch_nhwc_to_nchw<__half>(h->view(v), h->cfg.frames, 1.0f, dst_nchw, s)
-                   : launch_nhwc_to_nchw<float>(h->view(v), h->cfg.frames, 1.0f, dst_nchw, s);
-  }
-  if (rc) return fail(rc, thread_error());
-  return SSNB_OK;
+  const int rc = planes ? h->planes_read(v, false, 1.0f, dst_nchw, s) : h->value_read(v, false, 1.0f, dst_nchw, s);
+  return rc ? fail(rc, thread_error()) : SSNB_OK;
 }
 
 int ssnb_iv3_run_op(ssnb_iv3_handle h, int op, float* feat, void* stream) {

@@ -12,17 +12,20 @@ from torch import nn
 from ssn_b200 import _lib
 from ssn_b200.engine import BackboneEngine, BackboneFunction, conv_table
 
+from .backbone import EngineBackbone
 
-class BNInception(nn.Module):
+
+class BNInception(EngineBackbone):
     def __init__(self, model_path=None, num_classes=101, weight_url=None, in_channels=3):
         super(BNInception, self).__init__()
         # model_path / weight_url are accepted for signature compatibility; the graph is built into
         # the library and there is no network access for pretrained weights.
-        self._conv_names = []
+        self._conv_names, self._bn_names = [], []
         for (name, cin, cout, k, stride, pad) in conv_table(in_channels):
             setattr(self, name, nn.Conv2d(cin, cout, k, stride, pad, bias=True))
             setattr(self, name + "_bn", nn.BatchNorm2d(cout, momentum=0.1))
             self._conv_names.append(name)
+            self._bn_names.append(name + "_bn")
         self.fc = nn.Linear(1024, 1000)
         self.last_layer_name = "fc"
         self.precision = _lib.EXACT_FP32
@@ -41,32 +44,9 @@ class BNInception(nn.Module):
             self.grad_scale = float(grad_scale)
         self._engines = {}
 
-    def _convs(self):
-        return [getattr(self, n) for n in self._conv_names]
-
-    def _bns(self):
-        return [getattr(self, n + "_bn") for n in self._conv_names]
-
-    def in_channels(self):
-        return getattr(self, self._conv_names[0]).in_channels
-
     def grad_overflow(self, clear=True):
         """True when a gradient left the fp16 range under grad_scale in any engine since the last call (device sync)."""
         return any([e.grad_overflow(clear) for e in self._engines.values()])
-
-    def _weights_version(self):
-        v = 0
-        for c, b in zip(self._convs(), self._bns()):
-            v += c.weight._version + c.bias._version + b.weight._version + b.bias._version \
-                + b.running_mean._version + b.running_var._version
-        return (v, id(self._convs()[0].weight), self._convs()[0].weight.data_ptr())
-
-    def invalidate_packed(self):
-        """The kernels read BN-folded, re-laid-out copies of the weights.  They are refreshed automatically when a parameter's
-        Tensor._version moves (optimizer.step(), in-place ops); writes that bypass the version counter -- `p.data.copy_()`,
-        the fused SGD kernel, a raw pointer -- need this call."""
-        for eng in self._engines.values():
-            eng.packed_version = None
 
     def bn1_training(self):
         """bn_mode='partial' (ssn_models.py:95-105): the first BatchNorm2d stays in training mode, every other one is frozen.
@@ -81,17 +61,8 @@ class BNInception(nn.Module):
         if bn1_train and self.precision == _lib.FAST_FP16:
             raise NotImplementedError("bn_mode='partial' runs in EXACT_FP32 / EXACT_TC precision (fp32 activations), not FAST_FP16")
         key = (frames, bool(training), self.precision, self.in_channels(), str(device), bool(bn1_train))
-        eng = self._engines.get(key)
-        if eng is None:
-            eng = BackboneEngine(self.in_channels(), frames, self.precision, training, self.grad_scale, device, bn1_train=bn1_train)
-            self._engines[key] = eng
-        ver = self._weights_version()
-        if eng.packed_version != ver:
-            cs, bs = self._convs(), self._bns()
-            eng.pack([c.weight.data for c in cs], [c.bias.data for c in cs], [b.weight.data for b in bs],
-                     [b.bias.data for b in bs], [b.running_mean for b in bs], [b.running_var for b in bs])
-            eng.packed_version = ver
-        return eng
+        return self._packed_engine(key, lambda: BackboneEngine(self.in_channels(), frames, self.precision, training, self.grad_scale,
+                                                               device, bn1_train=bn1_train))
 
     def forward(self, input):
         if not input.is_cuda:

@@ -15,18 +15,20 @@ from torch import nn
 from ssn_b200 import _lib
 from ssn_b200.inception_v3 import FEAT_DIM, InceptionV3Engine, conv_table
 
+from .backbone import EngineBackbone
+
 _GPOOL_ID = "top_cls_pool"
 FOLLOW_UP = "training InceptionV3 (backward schedule, fused_step) is a follow-up"
 
 
-class InceptionV3(nn.Module):
+class InceptionV3(EngineBackbone):
     def __init__(self, model_path=None, num_classes=101, weight_url=None, in_channels=3):
         super(InceptionV3, self).__init__()
         # model_path / weight_url are accepted for signature compatibility; the graph is built into the library and there
         # is no network access for pretrained weights.
         convs = {c[0]: c for c in conv_table(in_channels)}
         plan = InceptionV3Engine(in_channels, 1)          # plans on the host only: the op order and pool geometry
-        self._conv_names = []
+        self._conv_names, self._bn_names = [], []
         for (kind, _in, out, conv, k, stride, pad) in plan.ops():
             if kind == "conv":
                 name, cin, cout, kh, kw, st, ph, pw = convs[out]
@@ -34,6 +36,7 @@ class InceptionV3(nn.Module):
                 setattr(self, name + "_batchnorm", nn.BatchNorm2d(cout, momentum=0.1))
                 setattr(self, name, nn.ReLU(inplace=True))
                 self._conv_names.append(name + "_Conv2D")
+                self._bn_names.append(name + "_batchnorm")
             elif kind == "maxpool":
                 setattr(self, out, nn.MaxPool2d(k, stride, pad, ceil_mode=True))
             elif kind == "avgpool":
@@ -54,45 +57,15 @@ class InceptionV3(nn.Module):
         self.precision = precision
         self._engines = {}
 
-    def _convs(self):
-        return [getattr(self, n) for n in self._conv_names]
-
-    def _bns(self):
-        return [getattr(self, n[:-len("_Conv2D")] + "_batchnorm") for n in self._conv_names]
-
-    def in_channels(self):
-        return getattr(self, self._conv_names[0]).in_channels
-
     def bn1_training(self):
         """False: every BatchNorm2d is frozen.  Raises for a training-mode BatchNorm2d (bn_mode 'partial' / 'full' in train())."""
         if any(b.training for b in self._bns()):
             raise NotImplementedError("InceptionV3 runs with frozen BatchNorm2d layers (eval mode); " + FOLLOW_UP)
         return False
 
-    def _weights_version(self):
-        v = 0
-        for c, b in zip(self._convs(), self._bns()):
-            v += c.weight._version + c.bias._version + b.weight._version + b.bias._version + b.running_mean._version + b.running_var._version
-        return (v, id(self._convs()[0].weight), self._convs()[0].weight.data_ptr())
-
-    def invalidate_packed(self):
-        """Refresh the BN-folded copies of the weights after writes that bypass Tensor._version (`p.data.copy_()`, raw pointers)."""
-        for eng in self._engines.values():
-            eng.packed_version = None
-
     def engine_for(self, frames, device):
         key = (frames, self.precision, self.in_channels(), str(device))
-        eng = self._engines.get(key)
-        if eng is None:
-            eng = InceptionV3Engine(self.in_channels(), frames, self.precision, device)
-            self._engines[key] = eng
-        ver = self._weights_version()
-        if eng.packed_version != ver:
-            cs, bs = self._convs(), self._bns()
-            eng.pack([c.weight.data for c in cs], [c.bias.data for c in cs], [b.weight.data for b in bs], [b.bias.data for b in bs],
-                     [b.running_mean for b in bs], [b.running_var for b in bs])
-            eng.packed_version = ver
-        return eng
+        return self._packed_engine(key, lambda: InceptionV3Engine(self.in_channels(), frames, self.precision, device))
 
     def forward(self, input):
         if not input.is_cuda:

@@ -28,8 +28,44 @@ def conv_table(in_channels):
     return out
 
 
-class BackboneEngine:
+class PlannedEngine:
+    """A planned backbone engine handle `h` of `workspace_bytes` and what every such handle needs: its workspace on `device`
+    (1024-byte aligned, as the library requires), the BatchNorm-folded weight pack, and destruction with the object.  A
+    subclass names its library functions and says where the library keeps its errors: on the handle (ssnb_*) or per
+    thread (ssnb_iv3_*, read with ssnb_last_error(NULL))."""
+    _set_workspace_fn = _pack_fn = _destroy_fn = None
+    _errors_on_handle = True
+
+    def _err(self):
+        return self.h if self._errors_on_handle else None
+
+    def _call(self, fn, *args):
+        check(getattr(lib, fn)(self.h, *args), self._err(), fn[len("ssnb_"):])
+
+    def _set_workspace(self):
+        with torch.cuda.device(self.device):
+            self._ws = torch.empty(self.workspace_bytes + 1024, dtype=torch.uint8, device=self.device)
+            base = self._ws.data_ptr()
+            self.ws_ptr = base + ((-base) % 1024)
+            self._call(self._set_workspace_fn, C.c_void_p(self.ws_ptr), self.workspace_bytes)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                getattr(lib, self._destroy_fn)(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+    def pack(self, w, b, gamma, beta, mean, var):
+        """lists of one tensor per convolution each, reference shapes (graph order)"""
+        with torch.cuda.device(self.device):
+            self._call(self._pack_fn, *[_lib.ptr_array(x) for x in (w, b, gamma, beta, mean, var)], _stream())
+
+
+class BackboneEngine(PlannedEngine):
     """One planned BNInception instance for a fixed frame count (ssnb_create .. ssnb_destroy)."""
+    _set_workspace_fn, _pack_fn, _destroy_fn = "ssnb_set_workspace", "ssnb_pack_weights", "ssnb_destroy"
 
     def __init__(self, in_channels, frames, precision, training, grad_scale, device, bn1_train=False):
         self.device = torch.device(device)
@@ -38,36 +74,16 @@ class BackboneEngine:
         cfg = _lib.Config(in_channels, frames, precision, 1 if training else 0, float(grad_scale), 1 if bn1_train else 0)
         self.h = C.c_void_p()
         check(lib.ssnb_create(C.byref(cfg), C.byref(self.h)), None, "ssnb_create")
-        nbytes = lib.ssnb_workspace_bytes(self.h)
-        with torch.cuda.device(self.device):
-            self._ws = torch.empty(nbytes + 1024, dtype=torch.uint8, device=self.device)
-            base = self._ws.data_ptr()
-            self.ws_ptr = base + ((-base) % 1024)
-            check(lib.ssnb_set_workspace(self.h, C.c_void_p(self.ws_ptr), nbytes), self.h, "set_workspace")
-        self.workspace_bytes = nbytes
+        self.workspace_bytes = lib.ssnb_workspace_bytes(self.h)
+        self._set_workspace()
         self.packed_version = None
         self.generation = 0        # bumped by every forward: the saved activations belong to the latest one only
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.ssnb_destroy(self.h)
-                self.h = None
-        except Exception:
-            pass
 
     def set_bn1(self, bn, dgamma=None, dbeta=None):
         """bn1_train engines: the first BatchNorm2d module's tensors (training-mode statistics, running-stat update, gradients)"""
         check(lib.ssnb_set_bn1(self.h, bn.weight.data_ptr(), bn.bias.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
                                None if dgamma is None else dgamma.data_ptr(), None if dbeta is None else dbeta.data_ptr(),
                                float(bn.momentum if bn.momentum is not None else 0.1), float(bn.eps)), self.h, "set_bn1")
-
-    # weights: lists of 69 tensors each, reference shapes
-    def pack(self, w, b, gamma, beta, mean, var):
-        with torch.cuda.device(self.device):
-            check(lib.ssnb_pack_weights(self.h, _lib.ptr_array(w), _lib.ptr_array(b), _lib.ptr_array(gamma),
-                                        _lib.ptr_array(beta), _lib.ptr_array(mean), _lib.ptr_array(var), _stream()),
-                  self.h, "pack_weights")
 
     def forward(self, x):
         _need_cuda(x, "input")

@@ -6,7 +6,7 @@ import torch
 
 from . import _lib
 from ._lib import lib, check
-from .engine import _need_cuda, _stream
+from .engine import PlannedEngine, _need_cuda, _stream
 
 INPUT_SIZE, FEAT_DIM = 299, 2048
 
@@ -22,9 +22,11 @@ def conv_table(in_channels):
     return out
 
 
-class InceptionV3Engine:
+class InceptionV3Engine(PlannedEngine):
     """One planned InceptionV3 forward for a fixed frame count (ssnb_iv3_create .. ssnb_iv3_destroy).  device=None plans
     without allocating (the plan needs no GPU)."""
+    _set_workspace_fn, _pack_fn, _destroy_fn = "ssnb_iv3_set_workspace", "ssnb_iv3_pack_weights", "ssnb_iv3_destroy"
+    _errors_on_handle = False
 
     def __init__(self, in_channels, frames, precision=_lib.EXACT_FP32, device=None):
         self.frames, self.in_channels, self.precision = frames, in_channels, precision
@@ -35,25 +37,7 @@ class InceptionV3Engine:
         self.device = None if device is None else torch.device(device)
         self.packed_version = None
         if self.device is not None:
-            with torch.cuda.device(self.device):
-                self._ws = torch.empty(self.workspace_bytes + 1024, dtype=torch.uint8, device=self.device)
-                base = self._ws.data_ptr()
-                self.ws_ptr = base + ((-base) % 1024)
-                check(lib.ssnb_iv3_set_workspace(self.h, C.c_void_p(self.ws_ptr), self.workspace_bytes), None, "iv3_set_workspace")
-
-    def __del__(self):
-        try:
-            if getattr(self, "h", None):
-                lib.ssnb_iv3_destroy(self.h)
-                self.h = None
-        except Exception:
-            pass
-
-    def pack(self, w, b, gamma, beta, mean, var):
-        """lists of 94 tensors each, reference shapes (graph order)"""
-        with torch.cuda.device(self.device):
-            check(lib.ssnb_iv3_pack_weights(self.h, _lib.ptr_array(w), _lib.ptr_array(b), _lib.ptr_array(gamma), _lib.ptr_array(beta),
-                                            _lib.ptr_array(mean), _lib.ptr_array(var), _stream()), None, "iv3_pack_weights")
+            self._set_workspace()
 
     def forward(self, x):
         _need_cuda(x, "input")

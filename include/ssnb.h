@@ -478,8 +478,8 @@ int ssnb_frame_transform(const ssnb_frame_cfg* cfg, const ssnb_frame_group* grou
  *      SSN.test_forward and BinaryClassifier scoring with --arch InceptionV3 (ssn_models.py:133-139, binary_model.py:175-178) ----
  * Forward only, frozen BatchNorm folded into each convolution, in every precision: EXACT_FP32 (fp32 SIMT convolutions),
  * FAST_FP16 and EXACT_TC (every convolution on the wgmma kernel; EXACT_TC with split operands, an fp32 epilogue and the
- * output's operand planes).  A handle of its own: the BNInception functions above do not take it, and errors are read with
- * ssnb_last_error(NULL).  Creation only plans (no device call), so the plan can be inspected without a
+ * output's operand planes).  Planned and run by the same host-side graph core as the BNInception engine, under a handle of
+ * its own: the BNInception functions above do not take it, and errors are read with ssnb_last_error(NULL).  Creation only plans (no device call), so the plan can be inspected without a
  * GPU.  Activations are NHWC fp32; the branch ends of every inception block are channel slices of the block's concat buffer
  * ("<block>_join"), so no concat runs; each value has a buffer of its own (no reuse across the pass). */
 typedef struct ssnb_iv3* ssnb_iv3_handle;
