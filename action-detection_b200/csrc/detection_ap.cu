@@ -15,7 +15,7 @@
 //                         and each threshold, the unlocked ground truth of the highest tIoU that is not below it (the walk of
 //                         eval_detection.py:209-223), tp / fp flags at the prediction's rank
 //   ap_sum_kernel         one CTA per (class, threshold): cumulative tp, precision / recall as numpy divides them, suffix
-//                         maximum of precision and the interpolated sum, walked from the last tile to the first
+//                         maximum of precision and the interpolated sum, walked from the last tile to the first (interp_ap.cuh)
 #include <cub/cub.cuh>
 
 #include <climits>
@@ -23,12 +23,13 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
+#include "interp_ap.cuh"
 #include "rank_key.cuh"
 
 namespace ssnb {
 namespace {
 
-constexpr int kMaxClass = 1024, kMaxThr = 64, kKeyThreads = 128, kSumThreads = 256, kMatchWarps = 8;
+constexpr int kMaxClass = 1024, kMaxThr = 64, kKeyThreads = 128, kMatchWarps = 8;
 
 struct ApParams {
   int V, K, n_thr, n_slots;
@@ -177,65 +178,13 @@ __global__ void __launch_bounds__(32 * kMatchWarps) ap_match_kernel(const float*
   }
 }
 
-struct MaxOp {
-  __device__ __forceinline__ double operator()(double a, double b) const { return b > a ? b : a; }
-};
-
-// one CTA per (class, threshold).  Ranked prediction e: cum_e = tp count at ranks <= e, prec_e = cum_e / (e + 1) (tp + fp =
-// e + 1 exactly), rec_e = cum_e / npos, both double divisions as numpy does them.  interpolated_prec_rec sums
-// (mrec[i] - mrec[i-1]) * max(mprec[i:]) over the i where recall changes, which are the true positives (the closing
-// (1 - rec_last) * 0 adds +0).  Tiles are walked from the last to the first with thread t on rank base + 255 - t, so a prefix
-// over threads is a suffix over ranks.
+// one CTA per (class, threshold): interp_ap_cta over the class's ranked flags of threshold k
 __global__ void ap_sum_kernel(const unsigned char* __restrict__ tp_ranked, const int* __restrict__ cls_begin,
-                                                              const int* __restrict__ cls_end, const int* __restrict__ npos_arr, ApParams p,
-                                                              double* __restrict__ ap) {
-  using IScan = cub::BlockScan<int, kSumThreads>;
-  using DScan = cub::BlockScan<double, kSumThreads>;
-  using IRed = cub::BlockReduce<int, kSumThreads>;
-  using DRed = cub::BlockReduce<double, kSumThreads>;
-  __shared__ union {
-    typename IScan::TempStorage is;
-    typename DScan::TempStorage ds;
-    typename IRed::TempStorage ir;
-    typename DRed::TempStorage dr;
-  } tmp;
-  __shared__ int s_total;
+                              const int* __restrict__ cls_end, const int* __restrict__ npos_arr, ApParams p, double* __restrict__ ap) {
   const int c = blockIdx.x / p.n_thr, k = blockIdx.x % p.n_thr;
   const int b = cls_begin[c], n = cls_end[c] - b, npos = npos_arr[c];
-  if (n == 0 || npos == 0) {                                  // no prediction: mrec = [0, 1], mprec = [0, 0]; no ground truth: rec = 0/0
-    if (threadIdx.x == 0) ap[c * p.n_thr + k] = n == 0 ? 0.0 : __longlong_as_double(0x7ff8000000000000LL);
-    return;
-  }
-  const unsigned char* f = tp_ranked + (long long)k * p.n_slots + b;
-  int mine = 0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) mine += f[i];
-  const int total = IRed(tmp.ir).Sum(mine);
-  if (threadIdx.x == 0) s_total = total;
-  __syncthreads();
-  const int T = s_total;
-  const double dn = (double)npos;
-  int later = 0;
-  double carry = 0.0, acc = 0.0;
-  for (int base = ((n - 1) / kSumThreads) * kSumThreads; base >= 0; base -= kSumThreads) {
-    const int e = base + kSumThreads - 1 - threadIdx.x;
-    const int flag = e < n ? f[e] : 0;
-    int after, tile_tp;
-    IScan(tmp.is).ExclusiveSum(flag, after, tile_tp);
-    __syncthreads();
-    const int cum = T - later - after;
-    const double prec = e < n ? (double)cum / (double)(e + 1) : 0.0;
-    double smax, tile_max;
-    DScan(tmp.ds).InclusiveScan(prec, smax, MaxOp(), tile_max);
-    __syncthreads();
-    smax = MaxOp()(smax, carry);
-    const double term = flag ? ((double)cum / dn - (double)(cum - 1) / dn) * smax : 0.0;
-    const double tile_sum = DRed(tmp.dr).Sum(term);
-    __syncthreads();
-    acc += tile_sum;                                          // thread 0's value is the one written
-    carry = MaxOp()(carry, tile_max);
-    later += tile_tp;
-  }
-  if (threadIdx.x == 0) ap[c * p.n_thr + k] = acc;
+  const double r = interp_ap_cta(tp_ranked + (long long)k * p.n_slots + b, n, npos);
+  if (threadIdx.x == 0) ap[c * p.n_thr + k] = r;
 }
 
 size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
@@ -352,7 +301,7 @@ int ssnb_detection_ap(const float* dets, const int32_t* counts, const int64_t* d
         dets, vb.Current(), cvb.Current(), cv_begin, cv_end, gt_offsets, gt_cls, gt_seg, p, (unsigned char*)(ws + L.lock), tp_ranked, tp);
     SSNB_LAUNCH_CHECK("ap_match_kernel");
   }
-  ap_sum_kernel<<<p.K * p.n_thr, kSumThreads, 0, s>>>(tp_ranked, cls_begin, cls_end, npos, p, ap);
+  ap_sum_kernel<<<p.K * p.n_thr, kApSumThreads, 0, s>>>(tp_ranked, cls_begin, cls_end, npos, p, ap);
   SSNB_LAUNCH_CHECK("ap_sum_kernel");
   return SSNB_OK;
 }

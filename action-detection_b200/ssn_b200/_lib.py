@@ -143,6 +143,8 @@ SIGNATURES = {
     "ssnb_proposal_ar_workspace_bytes": (_sz, [_i, C.c_int64, C.POINTER(C.c_int64), _i]),
     "ssnb_proposal_ar": (_i, [_vp, _vp, C.c_int64, _vp, _vp, _i, _vp, C.POINTER(C.c_int64), _vp, C.POINTER(C.c_double), _i, C.c_double]
                          + [_vp] * 7 + [_sz, _vp]),
+    "ssnb_classification_ap_workspace_bytes": (_sz, [C.c_int64, C.c_int64, _i, _i]),
+    "ssnb_classification_ap": (_i, [_vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_int64, _i, _i, _i] + [_vp] * 7 + [_sz, _vp]),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
     "ssnb_iv3_num_convs": (_i, []),

@@ -424,6 +424,30 @@ int ssnb_proposal_ar(const double* boxes, const double* scores, int64_t rows, co
                      int n_thresholds, double max_avg, double* recall, double* avg_recall, double* proposals_per_video,
                      int64_t* total_nr, int32_t* nr, int32_t* first_hit, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- ActivityNet untrimmed video classification: per-class average precision and video hit@k of
+ *      anet_toolkit/Evaluation/eval_classification.py:124-249 (and eval_kinetics.py, the same code), every class and video in
+ *      one call (csrc/classification_ap.cu) -----------------------------------------------------------------------------
+ * Predictions: rows of video int32, label int32 and score double (device [rows]).  Ground truth: n_gt (video, label) pairs
+ * gt_video / gt_label int32 (device [n_gt]); repeated pairs count once (drop_duplicates).  Videos are 0..n_videos-1, classes
+ * 0..num_class-1; a row or pair outside them is ignored.  Ranking: the toolkit's score.argsort()[::-1] -- NaN first, then
+ * descending score (-0 == +0), equal scores the later row first -- over a class's rows for AP and over a video's rows for
+ * hit@k.  Per class c: a row is a true positive when (its video, c) is ground truth and no higher-ranked row of c has the
+ * same video, else a false positive; npos = distinct ground-truth videos of c; ap[c] = interpolated_prec_rec of cumsum(tp) /
+ * npos and tp / (tp + fp) (no row: 0; rows but npos = 0: NaN).  Per video v with ground truth: hits[v] = its distinct
+ * ground-truth labels found among its top_k ranked rows (a duplicate row takes a place); hit_at_k = the fraction of these
+ * videos with hits > 0 (exact), avg_hit_at_k = the mean of hits[v] / labels[v] (summed in a fixed order; NaN without a
+ * ground-truth video).  num_class 1..1024, num_class * n_videos < INT_MAX, rows and n_gt < INT_MAX, top_k >= 1.
+ * Outputs (device): ap double [num_class], hit_at_k double [1], avg_hit_at_k double [1].  Optional traces (NULL: not
+ * written): hits int32 [n_videos], gt_labels int32 [n_videos] (distinct ground-truth labels per video), tp uint8 [rows] (1:
+ * the row is a true positive).  Kernels, memsets and device copies only: no host synchronisation, allocation or host copy, so
+ * the call can be captured in a CUDA graph.  The workspace (about 70 bytes per row, 8 per pair, 12 per video and class) is 0
+ * for arguments ssnb_classification_ap would reject. */
+size_t ssnb_classification_ap_workspace_bytes(int64_t rows, int64_t n_gt, int n_videos, int num_class);
+int ssnb_classification_ap(const int32_t* video, const int32_t* label, const double* score, int64_t rows, const int32_t* gt_video,
+                           const int32_t* gt_label, int64_t n_gt, int n_videos, int num_class, int top_k, double* ap, double* hit_at_k,
+                           double* avg_hit_at_k, int32_t* hits, int32_t* gt_labels, uint8_t* tp, void* workspace, size_t workspace_bytes,
+                           void* stream);
+
 /* ---- frame transforms: the PIL group transforms of the data pipeline (transforms.py:41-206) followed by Stack(roll=True),
  *      ToTorchFormatTensor(div=False) and GroupNormalize (transforms.py:67-80,256-288), bitwise equal to PIL 8-bit BILINEAR --
  * Modes (cfg->mode):
