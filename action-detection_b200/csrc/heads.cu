@@ -1,6 +1,7 @@
 // STPP, the three linear heads, and the multi-task loss of SSN — all fp32 (HBM/latency-bound work).
 // Reference: ops/ssn_ops.py:22-79 (STPP), :82-170 (STPPReorgainzed), :173-258 (losses);
 // ssn_models.py:272-289 (heads + row selection); ssn_train.py:210-214 (loss mix).
+#include <climits>
 #include <cstring>
 
 #include "../../include/ssnb.h"
@@ -270,19 +271,41 @@ __device__ __forceinline__ int reorg_tick(int left, double step, int q) {
 // Every pooled part is a mean over a contiguous row range of the [T, D] score table, and the 1000 proposals of a video overlap
 // heavily: one exclusive scan down the rows (fp64, so that P[b] - P[a] is exact to fp32 rounding of the part's own sum), then
 // each part costs two loads instead of (b - a).  P has T + 1 rows.
-__global__ void colscan_f64_kernel(const float* __restrict__ scores, int T, int D, double* __restrict__ P) {
-  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+// Many videos per launch: video v's ticks are rows tick_off[v] .. tick_off[v+1]-1 of the packed scores and its table is rows
+// tick_off[v] + v .. tick_off[v+1] + v of P; its proposals are rows off[v] .. off[v+1]-1.  tick_off == NULL: one video of
+// T ticks (and off == NULL: its N proposals), the single-video call.
+struct ReorgVideo { const double* P; int T; };
+
+__device__ __forceinline__ ReorgVideo reorg_video(const double* P, int T, int D, const int64_t* tick_off, int v) {
+  if (!tick_off) return {P, T};
+  const long long t0 = tick_off[v];
+  return {P + (t0 + v) * D, (int)(tick_off[v + 1] - t0)};
+}
+
+// grid (V, ceil(D / 128)): one thread per (video, column)
+__global__ void colscan_f64_kernel(const float* __restrict__ scores, int T, int D, const int64_t* __restrict__ tick_off,
+                                   double* __restrict__ P) {
+  const int d = blockIdx.y * blockDim.x + threadIdx.x;
   if (d >= D) return;
+  const int v = blockIdx.x;
+  const long long t0 = tick_off ? tick_off[v] : 0;
+  const int Tv = tick_off ? (int)(tick_off[v + 1] - t0) : T;
+  double* Pv = P + (t0 + v) * D;
+  const float* sv = scores + t0 * D;
   double s = 0.0;
-  P[d] = 0.0;
-  for (int r = 0; r < T; ++r) {
-    s += (double)scores[(long long)r * D + d];
-    P[(long long)(r + 1) * D + d] = s;
+  Pv[d] = 0.0;
+  for (int r = 0; r < Tv; ++r) {
+    s += (double)sv[(long long)r * D + d];
+    Pv[(long long)(r + 1) * D + d] = s;
   }
 }
 
+// ssn_test.py:89-92 de-normalisation of the regression columns by the checkpoint's reg_stats (means, stds): column 2k is
+// location, 2k + 1 size; torch's two fp32 ops, each rounded on its own (no FMA)
+struct RegStats { int on; float mean[2]; float std[2]; };
+
 __device__ void pspool_prefix_dev(const double* __restrict__ P, int T, int D, int col0, int score_len, const int* tk, float s0, float s1,
-                                  const ReorgCfg& cfg, float* __restrict__ out) {
+                                  const ReorgCfg& cfg, float* __restrict__ out, RegStats stats) {
   for (int j = threadIdx.x; j < score_len; j += blockDim.x) {
     float acc = 0.f;
     int offset = 0;
@@ -308,25 +331,44 @@ __device__ void pspool_prefix_dev(const double* __restrict__ P, int T, int D, in
         }
       }
     }
+    if (stats.on) {
+      const bool size = j & 1;
+      acc = __fadd_rn(__fmul_rn(acc, size ? stats.std[1] : stats.std[0]), size ? stats.mean[1] : stats.mean[0]);
+    }
     out[j] = acc;
   }
 }
 
-__global__ void stpp_reorg_prefix_kernel(const double* __restrict__ P, int T, int D, const int32_t* __restrict__ ticks,
+// one CTA per proposal row i of the packed proposals; its video is the last v with off[v] <= i (empty videos own no row)
+__global__ void stpp_reorg_prefix_kernel(const double* __restrict__ Pall, int T_one, int D, const int64_t* __restrict__ tick_off,
+                                         const int64_t* __restrict__ off, int V, const int32_t* __restrict__ ticks,
                                          const float* __restrict__ scaling, int N, int act_len, int comp_len, int reg_len, ReorgCfg cfg, int mult,
-                                         float* __restrict__ out_act, float* __restrict__ out_comp, float* __restrict__ out_reg) {
+                                         RegStats stats, float* __restrict__ out_act, float* __restrict__ out_comp, float* __restrict__ out_reg) {
   const int i = blockIdx.x;
   if (i >= N) return;
-  int tk[4] = {ticks[i * 4], ticks[i * 4 + 1], ticks[i * 4 + 2], ticks[i * 4 + 3]};
-  const float s0 = scaling[i * 2], s1 = scaling[i * 2 + 1];
+  int v = 0;
+  if (off) {
+    int lo = 0, hi = V - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (off[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    v = lo;
+  }
+  const ReorgVideo vid = reorg_video(Pall, T_one, D, tick_off, v);
+  const double* P = vid.P;
+  const int T = vid.T;
+  const long long i4 = (long long)i * 4, i2 = (long long)i * 2;
+  int tk[4] = {ticks[i4], ticks[i4 + 1], ticks[i4 + 2], ticks[i4 + 3]};
+  const float s0 = scaling[i2], s1 = scaling[i2 + 1];
   {
     int a, b;
     py_slice(tk[1], max(tk[1] + 1, tk[2]), T, a, b);
     for (int j = threadIdx.x; j < act_len; j += blockDim.x)
       out_act[(long long)i * act_len + j] = (float)(P[(long long)b * D + j] - P[(long long)a * D + j]) / (float)(b - a);
   }
-  pspool_prefix_dev(P, T, D, act_len, comp_len, tk, s0, s1, cfg, out_comp + (long long)i * comp_len);
-  pspool_prefix_dev(P, T, D, act_len + comp_len * mult, reg_len, tk, s0, s1, cfg, out_reg + (long long)i * reg_len);
+  pspool_prefix_dev(P, T, D, act_len, comp_len, tk, s0, s1, cfg, out_comp + (long long)i * comp_len, RegStats{0, {0.f, 0.f}, {0.f, 0.f}});
+  pspool_prefix_dev(P, T, D, act_len + comp_len * mult, reg_len, tk, s0, s1, cfg, out_reg + (long long)i * reg_len, stats);
 }
 
 // ---- linear ---------------------------------------------------------------------------------------
@@ -857,14 +899,12 @@ int ssnb_gpool_stpp_fwd(ssnb_handle h, const float* drop_mask, const float* scal
 
 size_t ssnb_stpp_reorg_workspace_bytes(int T, int D) { return (size_t)(T > 0 ? T + 1 : 0) * (size_t)(D > 0 ? D : 0) * sizeof(double); }
 
-int ssnb_stpp_reorg_prefix(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N, int act_len,
-                           int comp_len, int reg_len, const int* level_counts, const int* levels, float* out_act,
-                           float* out_comp, float* out_reg, void* workspace, void* stream) {
-  cudaStream_t s = (cudaStream_t)stream;
-  if (!scores || !ticks || !scaling || !out_act || !out_comp || !out_reg || !workspace || T <= 0) { set_thread_error("stpp_reorg_prefix: bad argument"); return SSNB_EINVAL; }
-  ReorgCfg cfg; memset(&cfg, 0, sizeof(cfg));
+// the three stages' pyramid levels (level_counts[3] + the flattened levels) -> cfg and M; D must be act + M * (comp + reg)
+static int reorg_cfg(const int* level_counts, const int* levels, int D, int act_len, int comp_len, int reg_len, ReorgCfg& cfg, int& mult) {
+  memset(&cfg, 0, sizeof(cfg));
   cfg.nstage = 3;
-  int q = 0, mult = 0;
+  int q = 0;
+  mult = 0;
   for (int st = 0; st < 3; ++st) {
     if (level_counts[st] < 1 || level_counts[st] > 8) { set_thread_error("stpp_reorg: 1..8 pyramid levels per stage"); return SSNB_EINVAL; }
     cfg.nlev[st] = level_counts[st];
@@ -872,11 +912,79 @@ int ssnb_stpp_reorg_prefix(const float* scores, int T, int D, const int32_t* tic
     mult += cfg.cnt[st];
   }
   if (D != act_len + mult * (comp_len + reg_len)) { set_thread_error("stpp_reorg: D does not match act+M*(comp+reg)"); return SSNB_EINVAL; }
+  return SSNB_OK;
+}
+
+int ssnb_stpp_reorg_prefix(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N, int act_len,
+                           int comp_len, int reg_len, const int* level_counts, const int* levels, float* out_act,
+                           float* out_comp, float* out_reg, void* workspace, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!scores || !ticks || !scaling || !out_act || !out_comp || !out_reg || !workspace || T <= 0) { set_thread_error("stpp_reorg_prefix: bad argument"); return SSNB_EINVAL; }
+  ReorgCfg cfg;
+  int mult = 0;
+  if (int rc = reorg_cfg(level_counts, levels, D, act_len, comp_len, reg_len, cfg, mult)) return rc;
   if (N == 0) return SSNB_OK;
+  // one video: the V = 1 case of the batch kernels, without offsets
   double* P = reinterpret_cast<double*>(workspace);
-  colscan_f64_kernel<<<(D + 127) / 128, 128, 0, s>>>(scores, T, D, P);
+  colscan_f64_kernel<<<dim3(1, (D + 127) / 128), 128, 0, s>>>(scores, T, D, nullptr, P);
   SSNB_LAUNCH_CHECK("colscan_f64_kernel");
-  stpp_reorg_prefix_kernel<<<N, 128, 0, s>>>(P, T, D, ticks, scaling, N, act_len, comp_len, reg_len, cfg, mult, out_act, out_comp, out_reg);
+  stpp_reorg_prefix_kernel<<<N, 128, 0, s>>>(P, T, D, nullptr, nullptr, 1, ticks, scaling, N, act_len, comp_len, reg_len, cfg, mult,
+                                             RegStats{0, {0.f, 0.f}, {0.f, 0.f}}, out_act, out_comp, out_reg);
+  SSNB_LAUNCH_CHECK("stpp_reorg_prefix_kernel");
+  return SSNB_OK;
+}
+
+// host offsets [V + 1]: offsets[0] = 0, non-decreasing; -> the total, or -1
+static long long reorg_offsets_total(const int64_t* offsets, int V) {
+  if (!offsets || offsets[0] != 0) return -1;
+  for (int v = 0; v < V; ++v)
+    if (offsets[v + 1] < offsets[v]) return -1;
+  return offsets[V];
+}
+
+static constexpr int kReorgMaxD = 65535 * 128;       // column blocks of the scan on grid y
+
+size_t ssnb_stpp_reorg_batch_workspace_bytes(const int64_t* tick_offsets, int n_videos, int D) {
+  if (n_videos < 0 || D <= 0 || D > kReorgMaxD) return 0;
+  const long long T = reorg_offsets_total(tick_offsets, n_videos);
+  if (T < 0) return 0;
+  return (size_t)(T + n_videos) * (size_t)D * sizeof(double);
+}
+
+int ssnb_stpp_reorg_batch(const float* scores, int D, const int64_t* tick_offsets, const int64_t* tick_offsets_dev, const int32_t* ticks,
+                          const float* scaling, const int64_t* offsets, const int64_t* offsets_dev, int n_videos, int act_len, int comp_len,
+                          int reg_len, const int* level_counts, const int* levels, const double* reg_stats, float* out_act, float* out_comp,
+                          float* out_reg, void* workspace, size_t workspace_bytes, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  const int V = n_videos;
+  if (V < 0 || D <= 0 || act_len < 0 || comp_len < 0 || reg_len < 0 || !level_counts || !levels) {
+    set_thread_error("stpp_reorg_batch: bad argument (n_videos, D, score lengths or level table)"); return SSNB_EINVAL; }
+  if (D > kReorgMaxD) { set_thread_error("stpp_reorg_batch: D above 65535 * 128"); return SSNB_ENOSUPPORT; }
+  const long long sumT = reorg_offsets_total(tick_offsets, V), sumN = reorg_offsets_total(offsets, V);
+  if (sumT < 0 || sumN < 0) {
+    set_thread_error("stpp_reorg_batch: tick_offsets and offsets must be host int64 [V + 1], starting at 0, non-decreasing"); return SSNB_EINVAL; }
+  for (int v = 0; v < V; ++v)
+    if (tick_offsets[v + 1] - tick_offsets[v] > INT_MAX) { set_thread_error("stpp_reorg_batch: a video with more than INT_MAX ticks"); return SSNB_ENOSUPPORT; }
+  if (sumN > INT_MAX) { set_thread_error("stpp_reorg_batch: more than INT_MAX proposal rows; split the batch"); return SSNB_ENOSUPPORT; }
+  ReorgCfg cfg;
+  int mult = 0;
+  if (int rc = reorg_cfg(level_counts, levels, D, act_len, comp_len, reg_len, cfg, mult)) return rc;
+  for (int st = 0; st < 3; ++st)
+    for (int l = 0; l < cfg.nlev[st]; ++l)
+      if (cfg.lev[st][l] < 1) { set_thread_error("stpp_reorg_batch: a pyramid level with no part"); return SSNB_EINVAL; }
+  if (reg_stats && reg_len % 2) { set_thread_error("stpp_reorg_batch: reg_stats needs (location, size) column pairs: reg_len even"); return SSNB_EINVAL; }
+  if (sumN > 0 && (!tick_offsets_dev || !offsets_dev || !ticks || !scaling || !out_act || !out_comp || !out_reg || !workspace || (sumT > 0 && !scores))) {
+    set_thread_error("stpp_reorg_batch: NULL input, output, offsets or workspace pointer"); return SSNB_EINVAL; }
+  if (sumN > 0 && workspace_bytes < (size_t)(sumT + V) * (size_t)D * sizeof(double)) {
+    set_thread_error("stpp_reorg_batch: workspace too small (ssnb_stpp_reorg_batch_workspace_bytes)"); return SSNB_EINVAL; }
+  if (sumN == 0) return SSNB_OK;
+  RegStats st{0, {0.f, 0.f}, {0.f, 0.f}};
+  if (reg_stats) st = RegStats{1, {(float)reg_stats[0], (float)reg_stats[1]}, {(float)reg_stats[2], (float)reg_stats[3]}};
+  double* P = reinterpret_cast<double*>(workspace);
+  colscan_f64_kernel<<<dim3((unsigned)V, (D + 127) / 128), 128, 0, s>>>(scores, 0, D, tick_offsets_dev, P);
+  SSNB_LAUNCH_CHECK("colscan_f64_kernel");
+  stpp_reorg_prefix_kernel<<<(unsigned)sumN, 128, 0, s>>>(P, 0, D, tick_offsets_dev, offsets_dev, V, ticks, scaling, (int)sumN, act_len,
+                                                          comp_len, reg_len, cfg, mult, st, out_act, out_comp, out_reg);
   SSNB_LAUNCH_CHECK("stpp_reorg_prefix_kernel");
   return SSNB_OK;
 }

@@ -94,6 +94,67 @@ class STPPReorgainzed:
         return out_act, out_comp, out_reg
 
 
+def _host_offsets(offsets, what):
+    o = [int(x) for x in offsets]
+    if not o or o[0] != 0 or any(b < a for a, b in zip(o, o[1:])):
+        raise ValueError("%s must be V + 1 non-decreasing ints starting at 0" % what)
+    return o
+
+
+def reorg_packed(scores, tick_offsets, ticks32, scaling32, offsets, stpp_cfg, act_len, comp_len, reg_len, reg_stats=None):
+    """The tail of ssn_test.py's worker loop (:87-92) for V videos in one library call (ssnb_stpp_reorg_batch):
+    STPPReorgainzed.forward of every video (standalong_classifier, with_regression), then, with reg_stats, the regression
+    de-normalisation.  scores [sum T, D] CUDA fp32, video v's ticks at rows tick_offsets[v] .. tick_offsets[v+1]-1; ticks32
+    [sum N, 4] / scaling32 [sum N, 2] and offsets (V + 1 row offsets) as ops.proposal_lists.test_proposals returns them;
+    stpp_cfg e.g. (1, (1, 2), 1); reg_stats: the checkpoint's [2, 2] (means, then stds), or None.
+    -> device tensors (act [sum N, act_len], comp [sum N, comp_len], reg) ready for ops.detection.detections_packed, reg
+    [sum N, reg_len // 2, 2] de-normalised when reg_stats is given, else the raw [sum N, reg_len].  Each video's rows are
+    bitwise STPPReorgainzed.forward's for that video alone followed by the reference's two torch lines.
+    Memory: the call holds (sum T + V) * D doubles of prefix tables beside the sum T * D fp32 scores, 12.8 KB + 6.4 KB per
+    tick at K = 100 with (1, (1, 2), 1) (D = 1601): batch the videos so that a call fits (INTEGRATION.md)."""
+    toff, off = _host_offsets(tick_offsets, "tick_offsets"), _host_offsets(offsets, "offsets")
+    if len(toff) != len(off):
+        raise ValueError("tick_offsets and offsets describe %d and %d videos" % (len(toff) - 1, len(off) - 1))
+    V, T, N = len(off) - 1, toff[-1], off[-1]
+    parts = [parse_stage_config(c)[0] for c in stpp_cfg]
+    if len(parts) != 3:
+        raise ValueError("stpp_cfg has three stages (starting, course, ending)")
+    mult = sum(sum(p) for p in parts)
+    if scores.dim() != 2 or scores.shape[0] != T:
+        raise ValueError("scores must be [tick_offsets[-1] = %d, D], got %s" % (T, tuple(scores.shape)))
+    D = scores.shape[1]
+    if D != act_len + mult * (comp_len + reg_len):
+        raise ValueError("D = %d does not match act_len + M * (comp_len + reg_len) with M = %d" % (D, mult))
+    if tuple(ticks32.shape) != (N, 4) or tuple(scaling32.shape) != (N, 2):
+        raise ValueError("ticks32 must be [offsets[-1] = %d, 4] and scaling32 [%d, 2]" % (N, N))
+    stats = None
+    if reg_stats is not None:
+        stats = torch.as_tensor(reg_stats, dtype=torch.float64).cpu()
+        if tuple(stats.shape) != (2, 2) or reg_len % 2:
+            raise ValueError("reg_stats must be [2, 2] (means, then stds) and reg_len even")
+        stats = (C.c_double * 4)(*stats.reshape(-1).tolist())
+    for t, nm in ((scores, "scores"), (ticks32, "ticks32"), (scaling32, "scaling32")):
+        _need_cuda(t, nm)
+    dev = scores.device
+    scores = scores.contiguous().float()
+    ticks = ticks32.to(device=dev, dtype=torch.int32).contiguous()
+    sc = scaling32.to(device=dev, dtype=torch.float32).contiguous()
+    outs = [torch.empty(max(N, 1), L, dtype=torch.float32, device=dev) for L in (act_len, comp_len, reg_len)]
+    c_toff, c_off = (C.c_int64 * (V + 1))(*toff), (C.c_int64 * (V + 1))(*off)
+    ws_bytes = lib.ssnb_stpp_reorg_batch_workspace_bytes(c_toff, V, D)
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+    toff_dev = torch.tensor(toff, dtype=torch.int64, device=dev)
+    off_dev = torch.tensor(off, dtype=torch.int64, device=dev)
+    counts = [len(p) for p in parts]
+    levels = [v for p in parts for v in p]
+    with torch.cuda.device(dev):
+        check(lib.ssnb_stpp_reorg_batch(scores.data_ptr(), D, c_toff, toff_dev.data_ptr(), ticks.data_ptr(), sc.data_ptr(), c_off,
+                                        off_dev.data_ptr(), V, act_len, comp_len, reg_len, _lib.int_array(counts), _lib.int_array(levels),
+                                        stats, *[o.data_ptr() for o in outs], ws.data_ptr(), ws_bytes, _stream()), None, "stpp_reorg_batch")
+    act, comp, reg = (o[:N] for o in outs)
+    return act, comp, (reg if stats is None else reg.view(N, reg_len // 2, 2))
+
+
 class OHEMHingeLoss(torch.autograd.Function):
     """Class-wise hinge loss with online hard example mining; apply(pred, labels, is_positive,
     ohem_ratio, group_size) -> tensor of shape [1]; gradient only w.r.t. pred."""

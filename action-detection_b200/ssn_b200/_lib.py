@@ -107,6 +107,9 @@ SIGNATURES = {
     "ssnb_gpool_stpp_fwd": (_i, [_vp, _vp, _vp, _i, _i, _ip, _ip, _ip, _ip, _i, _i, _vp, _vp, _vp, _vp]),
     "ssnb_stpp_reorg_workspace_bytes": (_sz, [_i, _i]),
     "ssnb_stpp_reorg_prefix": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _i, _ip, _ip, _vp, _vp, _vp, _vp, _vp]),
+    "ssnb_stpp_reorg_batch_workspace_bytes": (_sz, [C.POINTER(C.c_int64), _i, _i]),
+    "ssnb_stpp_reorg_batch": (_i, [_vp, _i, C.POINTER(C.c_int64), _vp, _vp, _vp, C.POINTER(C.c_int64), _vp, _i, _i, _i, _i, _ip, _ip,
+                                   C.POINTER(C.c_double), _vp, _vp, _vp, _vp, _sz, _vp]),
     "ssnb_linear_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     "ssnb_test_fc_cropmean": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     "ssnb_linear_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp]),

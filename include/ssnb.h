@@ -142,6 +142,28 @@ size_t ssnb_stpp_reorg_workspace_bytes(int T, int D);
 int ssnb_stpp_reorg_prefix(const float* scores, int T, int D, const int32_t* ticks, const float* scaling, int N, int act_len,
                            int comp_len, int reg_len, const int* level_counts, const int* levels, float* out_act,
                            float* out_comp, float* out_reg, void* workspace, void* stream);
+/* ---- the per-video tail of ssn_test.py's worker loop (ssn_test.py:87-92) for V videos in one call: STPPReorgainzed.forward
+ *      (ops/ssn_ops.py:109-170) of every video, then the regression de-normalisation by the checkpoint's reg_stats ----------
+ * Video v owns ticks tick_offsets[v] .. tick_offsets[v+1]-1 of the packed score table scores [sum T, D] (fp32, D = act_len +
+ * M*comp_len + M*reg_len) and proposal rows offsets[v] .. offsets[v+1]-1 of ticks [sum N, 4] int32 and scaling [sum N, 2]
+ * fp32 (ssnb_test_proposals' ticks32 / scaling32 in its row layout).  Writes act [sum N, act_len], comp [sum N, comp_len] and
+ * reg [sum N, reg_len] in the same row order, the layout ssnb_detect_batch reads.  Each video's rows are bitwise what
+ * ssnb_stpp_reorg_prefix gives for that video alone, which is this call with V = 1 (same kernels: one fp64 exclusive column
+ * scan per video segment, one gather per proposal).  A video with N_v = 0 writes nothing; one with T_v = 0 pools empty
+ * slices (NaN), as the reference's slices of an empty table do.
+ * reg_stats: NULL, or HOST double [4] = {mean loc, mean size, std loc, std size} (the [2, 2] reg_stats, means then stds):
+ * reg[:, 2k] = fp32(fp32(x * (float)std loc) + (float)mean loc), reg[:, 2k+1] likewise with the size pair, each op rounded
+ * on its own as torch runs ssn_test.py:90-92 (reg_len must be even).
+ * tick_offsets and offsets (int64 [V+1], [0] = 0, non-decreasing) are HOST memory: validated, they size the call;
+ * tick_offsets_dev / offsets_dev hold the same values on the device.  Workspace: (sum T + V) * D doubles, the per-video
+ * prefix tables (ssnb_stpp_reorg_batch_workspace_bytes; 0 for arguments the call rejects).  At K = 100 and (1,(1,2),1),
+ * D = 1601: 12.8 KB of workspace per tick beside the 6.4 KB of scores.  Bad arguments are refused before any launch.
+ * Kernels only: no host synchronisation, allocation or host copy (graph-capturable). */
+size_t ssnb_stpp_reorg_batch_workspace_bytes(const int64_t* tick_offsets, int n_videos, int D);
+int ssnb_stpp_reorg_batch(const float* scores, int D, const int64_t* tick_offsets, const int64_t* tick_offsets_dev, const int32_t* ticks,
+                          const float* scaling, const int64_t* offsets, const int64_t* offsets_dev, int n_videos, int act_len, int comp_len,
+                          int reg_len, const int* level_counts, const int* levels, const double* reg_stats, float* out_act, float* out_comp,
+                          float* out_reg, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- heads: activity_fc / completeness_fc / regressor_fc (ssn_models.py:272-283) ------------- */
 int ssnb_linear_fwd(const float* x, const float* w, const float* b, int n, int in_dim, int out_dim, float* y,
