@@ -64,6 +64,19 @@ class FrameGroup(C.Structure):
 FRAMES_TRAIN, FRAMES_OVERSAMPLE, FRAMES_CENTER = 0, 1, 2
 
 
+class JpegInput(C.Structure):
+    _fields_ = [("offset", C.c_int64), ("bytes", C.c_int64), ("channels", C.c_int32), ("reserved", C.c_int32)]
+
+
+class JpegImageInfo(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("components", C.c_int32), ("h_samp", C.c_int32),
+                ("v_samp", C.c_int32), ("channels", C.c_int32), ("restart_interval", C.c_int32), ("intervals", C.c_int32),
+                ("scan_offset", C.c_int64), ("scan_bytes", C.c_int64), ("out_offset", C.c_int64)]
+
+
+JPEG_OK, JPEG_TRUNCATED, JPEG_BAD_CODE, JPEG_BAD_RUN, JPEG_BAD_RESTART = 0, 1, 2, 3, 4
+
+
 class ProposalTargetsCfg(C.Structure):
     _fields_ = [("fg_thresh", C.c_double), ("incomplete_iou_thresh", C.c_double), ("bg_iou_thresh", C.c_double),
                 ("bg_coverage_thresh", C.c_double), ("incomplete_overlap_thresh", C.c_double), ("exclude_empty", C.c_int32),
@@ -150,6 +163,12 @@ SIGNATURES = {
     "ssnb_classification_ap": (_i, [_vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_int64, _i, _i, _i] + [_vp] * 7 + [_sz, _vp]),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
+    "ssnb_jpeg_plan_create": (_i, [_vp, _sz, C.POINTER(JpegInput), _i, C.POINTER(_vp), _ip]),
+    "ssnb_jpeg_plan_destroy": (_i, [_vp]),
+    "ssnb_jpeg_plan_sizes": (_i, [_vp, C.POINTER(_sz), C.POINTER(_sz), C.POINTER(C.c_int64)]),
+    "ssnb_jpeg_plan_image": (_i, [_vp, _i, C.POINTER(JpegImageInfo)]),
+    "ssnb_jpeg_plan_write_table": (_i, [_vp, _vp, _sz]),
+    "ssnb_jpeg_decode": (_i, [_vp, _vp, _vp, _sz, _vp, C.c_int64, _vp, _vp, _sz, _vp]),
     "ssnb_iv3_num_convs": (_i, []),
     "ssnb_iv3_conv_info": (_i, [_i, _i, C.c_char_p, _i] + [_ip] * 7),
     "ssnb_iv3_create": (_i, [C.POINTER(IV3Config), C.POINTER(_vp)]),

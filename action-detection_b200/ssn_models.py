@@ -203,10 +203,13 @@ class _BNInceptionModel(torch.nn.Module):
           train(frames, params)          get_augmentation() (training)
           oversample(frames)             GroupOverSample(crop_size, scale_size) (10-crop test)
           center_crop(frames)            GroupScale(scale_size) + GroupCenterCrop(crop_size) (1-crop test, validation)
-          to_uint8                       the dataset-side transform"""
+          to_uint8                       the dataset-side transform
+          decode(byte_groups)            decode_jpeg of the frame files' bytes (ops/jpeg.py): 'RGB', or 'L' for Flow; uint8
+                                         groups the transforms above take"""
         import functools
         import types
         from ops import frame_transforms as T
+        from ops import jpeg as J
         is_flow = self.modality == 'Flow'
         scales = [1, .875, .75] if is_flow else [1, .875, .75, .66]
         fc = (2 if is_flow else 3) * self.new_length
@@ -216,7 +219,8 @@ class _BNInceptionModel(torch.nn.Module):
             train=functools.partial(T.train_frames, input_size=self.input_size, is_flow=is_flow, **common),
             oversample=functools.partial(T.oversample_frames, crop_size=self.crop_size, scale_size=self.scale_size, **common),
             center_crop=functools.partial(T.center_crop_frames, crop_size=self.crop_size, scale_size=self.scale_size, **common),
-            to_uint8=T.GroupToUint8())
+            to_uint8=T.GroupToUint8(),
+            decode=functools.partial(J.decode_jpeg, mode='L' if is_flow else 'RGB'))
 
 
 class SSN(_BNInceptionModel):

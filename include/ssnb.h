@@ -520,6 +520,50 @@ int ssnb_frame_transform(const ssnb_frame_cfg* cfg, const ssnb_frame_group* grou
                          const uint8_t* src, size_t src_bytes, float* dst, int64_t dst_floats, void* workspace, size_t workspace_bytes,
                          void* stream);
 
+/* ---- JPEG decode: the frame loading of the data sets, Image.open(path).convert('RGB') for RGB frames and .convert('L') for
+ * the x / y planes of Flow (SSNDataSet._load_image, ssn_dataset.py:187-194; BinaryDataSet._load_image,
+ * load_binary_score.py:198-205), bitwise equal to Pillow over libjpeg-turbo.  Huffman-coded sequential 8-bit JPEG (SOF0 /
+ * SOF1), grayscale or YCbCr with luma sampling 1x1, 2x1 or 2x2 over 1x1 chroma, any size, restart intervals; the islow IDCT,
+ * fancy upsampling, libjpeg's YCbCr -> RGB tables and PIL's RGB -> L.
+ *
+ * ssnb_jpeg_plan_create parses every image of a call from HOST bytes into one table: geometry, dequantisation and expanded
+ * Huffman tables (identical tables are stored once), restart intervals with their byte ranges, the output offsets.  A stream
+ * the decoder does not support (progressive, lossless, hierarchical, arithmetic-coded, 12-bit, CMYK / YCCK, Adobe RGB, other
+ * sampling factors, multi-scan) is refused with SSNB_ENOSUPPORT, a malformed or truncated header or a scan that references an
+ * undefined table with SSNB_EINVAL; *bad_image gets the image's index and ssnb_last_error(NULL) "jpeg: image i: reason".
+ * Nothing is launched.
+ * ssnb_jpeg_plan_write_table writes the plan's device table (table_bytes) to host memory; the caller copies it to the device
+ * together with the bytes.  ssnb_jpeg_decode then only enqueues: a memset of status, the entropy decode (one thread per restart
+ * interval), the IDCT of every block and the upsampling / colour conversion into out: image i is uint8 [height, width,
+ * channels] at info.out_offset, images back to back in call order.  src_dev holds the call's bytes at the offsets the plan was
+ * made with.  status int32 [n]: 0, or the largest SSNB_JPEG_* code of a corrupt entropy-coded segment of that image; the bit
+ * reader never reads outside an image's segment and every other image of the call decodes as if alone. */
+typedef struct {
+  int64_t offset;          /* the image's first byte in src */
+  int64_t bytes;
+  int32_t channels;        /* 3: convert('RGB'), 1: convert('L') */
+  int32_t reserved;
+} ssnb_jpeg_input;
+typedef struct {
+  int32_t width, height;
+  int32_t components;      /* 1 grayscale, 3 YCbCr */
+  int32_t h_samp, v_samp;  /* luma sampling over 1x1 chroma (1, 1 for grayscale) */
+  int32_t channels;
+  int32_t restart_interval, intervals;  /* MCUs per interval (0: none), intervals of the scan */
+  int64_t scan_offset, scan_bytes;      /* the entropy-coded segment in src */
+  int64_t out_offset;                   /* first output byte */
+} ssnb_jpeg_image_info;
+enum { SSNB_JPEG_OK = 0, SSNB_JPEG_TRUNCATED = 1, SSNB_JPEG_BAD_CODE = 2, SSNB_JPEG_BAD_RUN = 3, SSNB_JPEG_BAD_RESTART = 4 };
+typedef struct ssnb_jpeg_plan_s* ssnb_jpeg_plan;
+int ssnb_jpeg_plan_create(const uint8_t* src, size_t src_bytes, const ssnb_jpeg_input* images, int n, ssnb_jpeg_plan* plan,
+                          int* bad_image);
+int ssnb_jpeg_plan_destroy(ssnb_jpeg_plan plan);
+int ssnb_jpeg_plan_sizes(ssnb_jpeg_plan plan, size_t* table_bytes, size_t* workspace_bytes, int64_t* out_bytes);
+int ssnb_jpeg_plan_image(ssnb_jpeg_plan plan, int i, ssnb_jpeg_image_info* info);
+int ssnb_jpeg_plan_write_table(ssnb_jpeg_plan plan, void* dst, size_t dst_bytes);
+int ssnb_jpeg_decode(ssnb_jpeg_plan plan, const void* table_dev, const uint8_t* src_dev, size_t src_bytes, uint8_t* out, int64_t out_bytes,
+                     int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- InceptionV3 backbone at test time: replaces model_zoo.InceptionV3 (pytorch_load.py:64-67, inceptionv3.yaml) as used by
  *      SSN.test_forward and BinaryClassifier scoring with --arch InceptionV3 (ssn_models.py:133-139, binary_model.py:175-178) ----
  * Forward only, frozen BatchNorm folded into each convolution, in every precision: EXACT_FP32 (fp32 SIMT convolutions),
