@@ -161,6 +161,12 @@ SIGNATURES = {
                          + [_vp] * 7 + [_sz, _vp]),
     "ssnb_classification_ap_workspace_bytes": (_sz, [C.c_int64, C.c_int64, _i, _i]),
     "ssnb_classification_ap": (_i, [_vp, _vp, _vp, C.c_int64, _vp, _vp, C.c_int64, _i, _i, _i] + [_vp] * 7 + [_sz, _vp]),
+    "ssnb_video_aggregate_workspace_bytes": (_sz, [C.POINTER(C.c_int64), _i, _i, _i, _i, _i, _i, _ip, _i, C.c_double, _i, _i]),
+    "ssnb_video_aggregate": (_i, [_vp, C.POINTER(C.c_int64), _vp, _i, _i, _i, _i, _i, _i, _i, _ip, _i, C.c_double, _i, _i, _vp, _vp,
+                                  _sz, _vp]),
+    "ssnb_video_fuse": (_i, [_vp, _pp, C.POINTER(C.c_double), _i, C.c_int64, _i, _i, C.c_double, _vp, _vp]),
+    "ssnb_video_metrics_workspace_bytes": (_sz, [_i, _i]),
+    "ssnb_video_metrics": (_i, [_vp, _i, _i, _i, _vp, _vp, C.c_int64, _vp, _i] + [_vp] * 8 + [_vp, _sz, _vp]),
     "ssnb_frame_transform_workspace_bytes": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_frame_transform": (_i, [C.POINTER(FrameCfg), C.POINTER(FrameGroup), _vp, _i, _vp, _sz, _vp, C.c_int64, _vp, _sz, _vp]),
     "ssnb_jpeg_plan_create": (_i, [_vp, _sz, C.POINTER(JpegInput), _i, C.POINTER(_vp), _ip]),

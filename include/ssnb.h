@@ -470,6 +470,56 @@ int ssnb_classification_ap(const int32_t* video, const int32_t* label, const dou
                            double* avg_hit_at_k, int32_t* hits, int32_t* gt_labels, uint8_t* tp, void* workspace, size_t workspace_bytes,
                            void* stream);
 
+/* ---- video-level classification from snippet scores: the aggregation and fusion functions of the reference's
+ *      ops/video_funcs.py and the metrics of ops/metrics.py, many ragged videos per call (csrc/video_agg.cu) --------------
+ * Scores: packed fp32 [sum T, crops, D] (device), video v's ticks at tick_offsets[v] .. tick_offsets[v+1] (int64 [V+1], [0] = 0,
+ * every video at least one tick).  tick_offsets is HOST memory: validated, it sizes the call; tick_offsets_dev holds the same
+ * values on the device.  Modes and their output out [V, K] (device):
+ *   SSNB_VAGG_DEFAULT  default_aggregation_func (:8-18): crop reduction, mean over ticks                  fp32, K = D
+ *   SSNB_VAGG_TOP_K    top_k_aggregation_func (:21-26): crop reduction, mean of the top_k largest ticks   fp32, K = D
+ *                      per class (all T when top_k > T)
+ *   SSNB_VAGG_SLIDING  sliding_window_aggregation_func (:29-57): crop MEAN; per span s (spans[i] * fps ticks) the maxima of  fp32, K = D
+ *                      the windows [i, i + s) clipped at T, i in range(0, T, ceil(s * (1 - overlap))); the mean of their
+ *                      max(15, n_windows // 4) largest; the mean over spans
+ *   SSNB_VAGG_TPP      tpp_aggregation_func (:60-70): crop mean; tick t adds its stage int(t * (stage / T)) of the       float64, K = num_class
+ *                      D = stage * num_class columns, in float64 from 0; divided by T
+ * crop_agg: SSNB_CROP_MEAN or SSNB_CROP_MAX (default and top-k only); normalize (not tpp): metrics.softmax of each output row.
+ * The fp32 sums run in numpy's order (crops, then ticks, then the top k from the k-th largest up, then spans, each from its
+ * first term; the softmax denominator by numpy's pairwise rule) and every fp32 operation is rounded on its own, so only the
+ * softmax's expf differs from numpy (a few ulp).  NaN propagates as numpy's max and sort put it; top-k and sliding-window
+ * take at most 32768 ticks per video.  Workspace (ssnb_video_aggregate_workspace_bytes; 0 for arguments the call rejects):
+ * 4 sum T * D bytes for top-k and sliding window, 1 otherwise.  Bad arguments are refused before any launch; kernels only: no
+ * host synchronisation, allocation or copy (graph-capturable). */
+enum { SSNB_VAGG_DEFAULT = 0, SSNB_VAGG_TOP_K = 1, SSNB_VAGG_SLIDING = 2, SSNB_VAGG_TPP = 3 };
+enum { SSNB_CROP_MEAN = 0, SSNB_CROP_MAX = 1 };
+size_t ssnb_video_aggregate_workspace_bytes(const int64_t* tick_offsets, int n_videos, int crops, int D, int mode, int crop_agg, int top_k,
+                                            const int32_t* spans, int n_spans, double overlap, int fps, int num_class);
+int ssnb_video_aggregate(const float* scores, const int64_t* tick_offsets, const int64_t* tick_offsets_dev, int n_videos, int crops, int D,
+                         int mode, int crop_agg, int normalize, int top_k, const int32_t* spans, int n_spans, double overlap, int fps,
+                         int num_class, void* out, void* workspace, size_t workspace_bytes, void* stream);
+/* default_fusion_func (:73-80) over rows x num_class fp32 streams (device): out = major, then out += others[i] * (float)weights[i]
+ * in stream order (each product and sum rounded to fp32, numpy's rule for a Python float weight), then with normalize the
+ * softmax exp((x - max) * temperature) / sum of each row (metrics.softmax; temperature 1 for the fusion).  others and weights
+ * are HOST arrays of at most 8; out may be major.  Kernels only (graph-capturable). */
+int ssnb_video_fuse(const float* major, const float* const* others, const double* weights, int n_others, int64_t rows, int num_class,
+                    int normalize, double temperature, float* out, void* stream);
+/* metrics.py over video scores [V, K] (device, fp32, or float64 with scores_f64) and the (label_video, label) pairs (device
+ * int32 [n_labels]; repeated pairs count once, pairs outside 0..V-1 / 0..K-1 are ignored).  Each video's classes are ranked by
+ * descending score with NaN first (rank_key.cuh) and equal scores the HIGHER class first (a stable ascending argsort's
+ * [-k:]); top_k_idx (optional, int32 [V, min(top_k, K)]) is that ranking's head, best first.  hits[v] = labels of v among
+ * them, label_count[v] = distinct labels of v (top_k_acc); top_k_accuracy = videos with a hit / V (top_k_accuracy).  ap [K]:
+ * sklearn's average_precision_score per class (the step AP over distinct thresholds; 0 for a class without a positive);
+ * mean_ap = their mean (video_mean_ap, average='macro').  class_label (optional, int32 [V]) gives mean_class_accuracy:
+ * np.argmax per video (the first NaN, else the first maximum), confusion (optional, int32 [3, K]: label counts, prediction
+ * counts, hits) and the mean of hits / label count over the classes labelled or predicted (NaN when one is never labelled, or
+ * without class_label).  V >= 1, K in 1..1024, V * K < INT_MAX, top_k >= 1.  Kernels, memsets and device copies only
+ * (graph-capturable); workspace about 25 bytes per (video, class). */
+size_t ssnb_video_metrics_workspace_bytes(int n_videos, int num_class);
+int ssnb_video_metrics(const void* scores, int scores_f64, int n_videos, int num_class, const int32_t* label_video, const int32_t* label,
+                       int64_t n_labels, const int32_t* class_label, int top_k, int32_t* hits, int32_t* label_count, int32_t* top_k_idx,
+                       double* top_k_accuracy, double* ap, double* mean_ap, int32_t* confusion, double* mean_class_accuracy,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- frame transforms: the PIL group transforms of the data pipeline (transforms.py:41-206) followed by Stack(roll=True),
  *      ToTorchFormatTensor(div=False) and GroupNormalize (transforms.py:67-80,256-288), bitwise equal to PIL 8-bit BILINEAR --
  * Modes (cfg->mode):
