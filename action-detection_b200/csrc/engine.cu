@@ -396,7 +396,8 @@ static const char* fused_name(const ssnb_engine* e, const FusedBlock& fb) {
   return t_fused_name.c_str();
 }
 
-static int run_fwd(ssnb_engine* e, const Op& o, float* feat, cudaStream_t s) {
+// the forward of op `o` over the first n frames (n = F but for ssnb_backbone_fwd_frames, which bn1_train engines refuse)
+static int run_fwd(ssnb_engine* e, const Op& o, float* feat, int n, cudaStream_t s) {
   tag_next(0, 0.0);
   if (o.kind == OP_CONV && o.umma.enabled) {
     // tensor-core convolution (EXACT_TC: reads the input's hi/lo planes, writes fp32 + the output's planes); conv1 runs as a
@@ -404,10 +405,10 @@ static int run_fwd(ssnb_engine* e, const Op& o, float* feat, cudaStream_t s) {
     if (o.conv == 0 && !e->s2d_ready) {
       const View in = e->view(o.in, false);
       __half* s2d = (__half*)(e->ws + e->s2d_off);
-      if (int rc = launch_nhwc_to_s2d(in, e->F, s2d, (long long)e->s2d_plane, e->Cs, s)) return rc;
+      if (int rc = launch_nhwc_to_s2d(in, n, s2d, (long long)e->s2d_plane, e->Cs, s)) return rc;
     }
-    tag_next(0, e->conv_flops(o), o.id.c_str());
-    return umma_conv_launch(e->umma_ctx, o.umma, s);
+    tag_next(0, e->conv_flops(o, n), o.id.c_str());
+    return umma_conv_launch(e->umma_ctx, o.umma, s, false, n);
   }
   if (o.kind == OP_BN1) {
     if (!e->bn1_gamma || !e->bn1_beta) { set_thread_error("bn1_train engine: call ssnb_set_bn1 first"); return SSNB_ESTATE; }
@@ -415,15 +416,15 @@ static int run_fwd(ssnb_engine* e, const Op& o, float* feat, cudaStream_t s) {
                                e->bn1_beta, e->bn1_eps, e->bn1_momentum, e->bn1_rmean, e->bn1_rvar, (float*)(e->ws + e->bn_stat_off),
                                (float*)(e->ws + e->bn_partial_off), 1200, s);
   }
-  if (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) return e->pool_fwd(o, s);     // EXACT_TC: and the output's operand planes
+  if (o.kind == OP_MAXPOOL || o.kind == OP_AVGPOOL) return e->pool_fwd(o, n, s);     // EXACT_TC: and the output's operand planes
   if (o.kind == OP_GPOOL) {
     if (!feat) return e->fail(SSNB_EINVAL, "global_pool needs the feat output pointer");
-    return e->gpool_fwd(o, feat, s);
+    return e->gpool_fwd(o, n, feat, s);
   }
   // SIMT convolution; the raw conv1 of a bn1_train engine has no ReLU
-  if (int rc = e->simt_conv_fwd(o, o.raw ? 0 : 1, s)) return rc;
+  if (int rc = e->simt_conv_fwd(o, o.raw ? 0 : 1, n, s)) return rc;
   if (!e->exact_tc() || !e->bufs[e->vals[o.out].buf].plane) return 0;     // EXACT_TC: the output's operand planes
-  return launch_split_view(e->view(o.out), e->F, 1.0f, e->planes(o.out), nullptr, s);
+  return launch_split_view(e->view(o.out), n, 1.0f, e->planes(o.out), nullptr, s);
 }
 
 // SIMT convolution backward (EXACT_FP32, and layers or passes without a tensor-core plan), reading the masked fp32 / fp16
@@ -437,7 +438,7 @@ static int simt_wgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   w.x = x.base; w.IH = x.H; w.IW = x.W; w.Cin = x.C; w.x_pitch = x.pitch; w.x_coff = x.coff;
   w.partial = partial; w.F = e->F; w.k = c.kh; w.stride = c.stride; w.pad = c.ph;
   w.rows_per_split = o.wrows; w.splits = o.wsplits;
-  tag_next(2, e->conv_flops(o), o.id.c_str());
+  tag_next(2, e->conv_flops(o, e->F), o.id.c_str());
   if (int rc = DISPATCH(e, launch_wgrad<float>(w, s), launch_wgrad<__half>(w, s))) return rc;
   const float out_scale = e->fast() ? 1.0f / e->cfg.grad_scale : 1.0f;      // FAST stores gradients times the loss scale
   return launch_wgrad_finalize(partial, o.wsplits, c.kh * c.kw, c.cout, c.cin, (const float*)(e->ws + e->packed[o.conv].scale), out_scale,
@@ -451,7 +452,7 @@ static int simt_dgrad(ssnb_engine* e, const Op& o, cudaStream_t s) {
   a.dst = dx.base; a.DH = dx.H; a.DW = dx.W; a.Cdst = dx.C; a.dst_pitch = dx.pitch; a.dst_coff = dx.coff;
   a.wgt = e->ws + e->packed[o.conv].wd; a.bias = nullptr;
   a.F = e->F; a.kh = a.kw = c.kh; a.stride = c.stride; a.pad_h = a.pad_w = c.ph; a.relu = 0; a.accumulate = o.grad_accumulate; a.dgrad = 1;
-  tag_next(1, e->conv_flops(o), o.id.c_str());
+  tag_next(1, e->conv_flops(o, e->F), o.id.c_str());
   return DISPATCH(e, launch_conv<float>(a, s), launch_conv<__half>(a, s));
 }
 
@@ -539,7 +540,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   if (tc_w) {
     float* partial = (float*)(e->ws + o.partial_off);
     float* bp = bias_w ? (float*)(e->ws + o.bias_partial_off) : nullptr;
-    tag_next(2, e->conv_flops(o), o.id.c_str());
+    tag_next(2, e->conv_flops(o, F), o.id.c_str());
     if ((rc = umma_wgrad_launch(e->umma_ctx, o.umma_wgrad, s, bp))) return rc;
     if (full && o.conv != 0) e->pending_finalize.push_back((int)(&o - e->ops.data()));
     else if (o.conv == 0) rc = launch_wgrad_finalize_s2d(partial, o.umma_wgrad.p.splits, c.cout, c.cin, e->Cs, scale, 1.0f / gst, us, e->dw[o.conv],
@@ -550,7 +551,7 @@ static int run_bwd(ssnb_engine* e, const Op& o, const float* dfeat, cudaStream_t
   } else if (want_w && (rc = simt_wgrad(e, o, s))) return rc;
   // 4. data gradient; as the last writer of d(in) the wgmma epilogue applies in's ReLU mask
   if (tc_x) {
-    tag_next(1, e->conv_flops(o), o.id.c_str());
+    tag_next(1, e->conv_flops(o, F), o.id.c_str());
     return umma_conv_launch(e->umma_ctx, o.umma_dgrad, s, full && e->fold_pools && o.dgrad_masks);
   }
   return want_x ? simt_dgrad(e, o, s) : 0;
@@ -862,15 +863,13 @@ int ssnb_set_bn1(ssnb_handle h, const float* gamma, const float* beta, float* ru
   return SSNB_OK;
 }
 
-int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void* stream) {
-  if (!h || !input_nchw || !feat) return h ? h->fail(SSNB_EINVAL, "null argument") : SSNB_EINVAL;
-  if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
-  cudaStream_t s = (cudaStream_t)stream;
+// the forward of frames [0, n) after the caller's checks
+static int backbone_fwd(ssnb_handle h, const float* input_nchw, int n, float* feat, cudaStream_t s) {
   const View d = h->view(h->val_by_name["data"], false);
   int rc;
   h->s2d_ready = h->tensor_cores() && h->ops[0].umma.enabled;
-  if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, h->F, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
-  else rc = h->value_write(h->val_by_name["data"], false, input_nchw, 1.0f, s);
+  if (h->s2d_ready) rc = launch_nchw_to_s2d(input_nchw, n, d.C, d.H, d.W, (__half*)(h->ws + h->s2d_off), (long long)h->s2d_plane, h->Cs, s);
+  else rc = h->value_write(h->val_by_name["data"], false, input_nchw, 1.0f, n, s);
   if (rc) { h->s2d_ready = false; return h->fail(rc, "input layout: " + ssnb::thread_error()); }
   for (size_t i = 0; i < h->ops.size(); ++i) {
     const Op& o = h->ops[i];
@@ -881,15 +880,31 @@ int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void*
     if (o.fuse_role == 1) {
       const FusedBlock& fb = h->fused[o.fuse_block];
       double fl = 0.0;
-      for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j]);
+      for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j], n);
       tag_next(0, fl, fused_name(h, fb));
-      r = umma_conv_launch(h->umma_ctx, fb.fwd, s);
-    } else r = run_fwd(h, o, feat, s);
+      r = umma_conv_launch(h->umma_ctx, fb.fwd, s, false, n);
+    } else r = run_fwd(h, o, feat, n, s);
     if (prof) cudaProfilerStop();
     if (r) { h->s2d_ready = false; return h->fail(r, "fwd " + o.id + ": " + ssnb::thread_error()); }
   }
   h->s2d_ready = false;
   return SSNB_OK;
+}
+
+int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void* stream) {
+  if (!h || !input_nchw || !feat) return h ? h->fail(SSNB_EINVAL, "null argument") : SSNB_EINVAL;
+  if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
+  return backbone_fwd(h, input_nchw, h->F, feat, (cudaStream_t)stream);
+}
+
+int ssnb_backbone_fwd_frames(ssnb_handle h, const float* input_nchw, int frames, float* feat, void* stream) {
+  if (!h || !input_nchw || !feat) return h ? h->fail(SSNB_EINVAL, "null argument") : SSNB_EINVAL;
+  if (frames < 1 || frames > h->F) return h->fail(SSNB_EINVAL, "backbone_fwd_frames: frames must be in 1 .. " + std::to_string(h->F));
+  // a training engine keeps the activations of all F frames for its backward; bn_mode='partial' takes batch statistics over F
+  if (h->cfg.training) return h->fail(SSNB_ESTATE, "backbone_fwd_frames: runs forward-only engines (training = 0)");
+  if (h->bn1_train) return h->fail(SSNB_ENOSUPPORT, "backbone_fwd_frames: bn1_train engines run their planned frame count only");
+  if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
+  return backbone_fwd(h, input_nchw, frames, feat, (cudaStream_t)stream);
 }
 
 int ssnb_bind_grads(ssnb_handle h, float* const* dw, float* const* db) {
@@ -920,7 +935,7 @@ int ssnb_backbone_bwd_range(ssnb_handle h, const float* dfeat, float* const* dw,
       if (!rc && o.fuse_role == 1) {                                   // ... one fused data gradient
         const FusedBlock& fb = h->fused[o.fuse_block];
         double fl = 0.0;
-        for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j]);
+        for (int j : {fb.op1, fb.op_r3, fb.op_rd}) if (j >= 0) fl += h->conv_flops(h->ops[j], h->F);
         tag_next(1, fl, fused_name(h, fb));
         rc = umma_conv_launch(h->umma_ctx, fb.dgrad, s, h->fold_pools && o.dgrad_masks);
       }
@@ -1002,7 +1017,7 @@ int ssnb_value_write(ssnb_handle h, const char* name, int grad, const float* src
   if (grad && !h->cfg.training) return h->fail(SSNB_ESTATE, "no gradient buffers");
   // a gradient is stored in the units of the last backward: times 2^k (FAST: and grad_scale)
   const float sc = grad ? (h->fast() ? h->cfg.grad_scale : 1.0f) * host_gscale(h, 0, (cudaStream_t)stream) : 1.0f;
-  const int rc = h->value_write(v, grad != 0, src_nchw, sc, (cudaStream_t)stream);
+  const int rc = h->value_write(v, grad != 0, src_nchw, sc, h->F, (cudaStream_t)stream);
   return rc ? h->fail(rc, ssnb::thread_error()) : SSNB_OK;
 }
 
@@ -1027,7 +1042,7 @@ int ssnb_run_op(ssnb_handle h, int op, int backward, void* stream) {
   if (!h->ws || !h->weights_ready) return h->fail(SSNB_ESTATE, "workspace/weights not set");
   const Op& o = h->ops[op];
   if (o.kind == OP_GPOOL) return h->fail(SSNB_ENOSUPPORT, "run_op: global_pool runs through backbone_fwd/bwd");
-  int rc = backward ? run_bwd(h, o, nullptr, (cudaStream_t)stream) : run_fwd(h, o, nullptr, (cudaStream_t)stream);
+  int rc = backward ? run_bwd(h, o, nullptr, (cudaStream_t)stream) : run_fwd(h, o, nullptr, h->F, (cudaStream_t)stream);
   return rc ? h->fail(rc, o.id + ": " + ssnb::thread_error()) : SSNB_OK;
 }
 

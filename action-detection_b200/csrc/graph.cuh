@@ -186,50 +186,52 @@ struct Graph {
   }
 
   // ---- forward of the ops that do not run on the tensor cores ----
-  // algorithmic FLOPs of convolution op `o` (timing tags)
-  double conv_flops(const GraphOp& o) const {
+  // The forward helpers below run the first n <= F frames of the plan: every launch covers frames [0, n) only, and a frame's
+  // arithmetic does not depend on n.
+  // algorithmic FLOPs of convolution op `o` over n frames (timing tags)
+  double conv_flops(const GraphOp& o, int n) const {
     const Conv& c = convs[o.conv];
     const View out = view(o.out);
-    return 2.0 * F * out.H * out.W * (double)c.cout * c.cin * c.kh * c.kw;
+    return 2.0 * n * out.H * out.W * (double)c.cout * c.cin * c.kh * c.kw;
   }
   // vectorised max pool / 3x3 average pool; EXACT_TC also writes the output's operand planes (the next convolution's A operand)
-  int pool_fwd(const GraphOp& o, cudaStream_t s) const {
+  int pool_fwd(const GraphOp& o, int n, cudaStream_t s) const {
     const View in = view(o.in), out = view(o.out);
     const View pl = exact_tc() && bufs[vals[o.out].buf].plane ? planes(o.out) : View();
     uint8_t* am = (uint8_t*)(ws + o.argmax_off);
     if (o.kind == OP_MAXPOOL)
-      return fast() ? launch_maxpool_fwd_vec<__half>(in, out, pl, F, o.k, o.stride, o.pad, am, s)
-                    : launch_maxpool_fwd_vec<float>(in, out, pl, F, o.k, o.stride, o.pad, am, s);
-    return fast() ? launch_avgpool3_vec<__half>(in, out, pl, F, 0, s) : launch_avgpool3_vec<float>(in, out, pl, F, 0, s);
+      return fast() ? launch_maxpool_fwd_vec<__half>(in, out, pl, n, o.k, o.stride, o.pad, am, s)
+                    : launch_maxpool_fwd_vec<float>(in, out, pl, n, o.k, o.stride, o.pad, am, s);
+    return fast() ? launch_avgpool3_vec<__half>(in, out, pl, n, 0, s) : launch_avgpool3_vec<float>(in, out, pl, n, 0, s);
   }
-  // global average pool of op `o`'s input into feat [F, C]
-  int gpool_fwd(const GraphOp& o, float* feat, cudaStream_t s) const {
-    return fast() ? launch_gpool_fwd<__half>(view(o.in), F, feat, s) : launch_gpool_fwd<float>(view(o.in), F, feat, s);
+  // global average pool of op `o`'s input into feat [n, C]
+  int gpool_fwd(const GraphOp& o, int n, float* feat, cudaStream_t s) const {
+    return fast() ? launch_gpool_fwd<__half>(view(o.in), n, feat, s) : launch_gpool_fwd<float>(view(o.in), n, feat, s);
   }
   // SIMT convolution forward of op `o` from the packed fp32 / fp16 weights; relu = 0 leaves the result un-clamped
-  int simt_conv_fwd(const GraphOp& o, int relu, cudaStream_t s) const {
+  int simt_conv_fwd(const GraphOp& o, int relu, int n, cudaStream_t s) const {
     const Conv& c = convs[o.conv];
     const View in = view(o.in), out = view(o.out);
     ConvArgs a;
     a.src = in.base; a.SH = in.H; a.SW = in.W; a.Csrc = in.C; a.src_pitch = in.pitch; a.src_coff = in.coff;
     a.dst = out.base; a.DH = out.H; a.DW = out.W; a.Cdst = out.C; a.dst_pitch = out.pitch; a.dst_coff = out.coff;
     a.wgt = ws + packed[o.conv].wf; a.bias = (const float*)(ws + packed[o.conv].bias);
-    a.F = F; a.kh = c.kh; a.kw = c.kw; a.stride = c.stride; a.pad_h = c.ph; a.pad_w = c.pw; a.relu = relu; a.accumulate = 0; a.dgrad = 0;
-    t_tag.phase = 0; t_tag.flop = conv_flops(o); t_tag.op = o.id.c_str();
+    a.F = n; a.kh = c.kh; a.kw = c.kw; a.stride = c.stride; a.pad_h = c.ph; a.pad_w = c.pw; a.relu = relu; a.accumulate = 0; a.dgrad = 0;
+    t_tag.phase = 0; t_tag.flop = conv_flops(o, n); t_tag.op = o.id.c_str();
     return fast() ? launch_conv<__half>(a, s) : launch_conv<float>(a, s);
   }
 
   // ---- value I/O (NCHW fp32 on the caller's side) ----
-  // the value's storage = src * scale; EXACT_TC refreshes an activation's operand planes (a padded input: every channel of
-  // the pixel, the padding included)
-  int value_write(int v, bool grad, const float* src, float scale, cudaStream_t s) const {
+  // frames [0, n) of the value's storage = src * scale; EXACT_TC refreshes an activation's operand planes (a padded input:
+  // every channel of the pixel, the padding included)
+  int value_write(int v, bool grad, const float* src, float scale, int n, cudaStream_t s) const {
     const View w = view(v, grad);
-    int rc = fast() ? launch_nchw_to_nhwc<__half>(src, F, w.C, w.H, w.W, w, scale, s)
-                    : launch_nchw_to_nhwc<float>(src, F, w.C, w.H, w.W, w, scale, s);
+    int rc = fast() ? launch_nchw_to_nhwc<__half>(src, n, w.C, w.H, w.W, w, scale, s)
+                    : launch_nchw_to_nhwc<float>(src, n, w.C, w.H, w.W, w, scale, s);
     if (!rc && exact_tc() && !grad && bufs[vals[v].buf].plane) {
       View x = w, xp = planes(v);
       if (w.C % 8) x.C = xp.C = w.pitch;
-      rc = launch_split_view(x, F, 1.0f, xp, nullptr, s);
+      rc = launch_split_view(x, n, 1.0f, xp, nullptr, s);
     }
     return rc;
   }

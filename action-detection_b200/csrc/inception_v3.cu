@@ -235,16 +235,39 @@ int bind_plans(ssnb_iv3* e) {
   return SSNB_OK;
 }
 
-int run_op(ssnb_iv3* e, const GraphOp& o, float* feat, cudaStream_t s) {
+// op `o` over the first n frames
+int run_op(ssnb_iv3* e, const GraphOp& o, float* feat, int n, cudaStream_t s) {
   if (o.kind == OP_CONV && e->tensor_cores()) {
-    t_tag.phase = 0; t_tag.flop = e->conv_flops(o); t_tag.op = o.id.c_str();
-    return umma_conv_launch(e->umma_ctx, e->plans[o.conv], s);
+    t_tag.phase = 0; t_tag.flop = e->conv_flops(o, n); t_tag.op = o.id.c_str();
+    return umma_conv_launch(e->umma_ctx, e->plans[o.conv], s, false, n);
   }
-  if (o.kind == OP_CONV) return e->simt_conv_fwd(o, 1, s);
+  if (o.kind == OP_CONV) return e->simt_conv_fwd(o, 1, n, s);
   t_tag.phase = 0; t_tag.flop = 0.0; t_tag.op = o.id.c_str();
-  if (o.kind != OP_GPOOL) return e->pool_fwd(o, s);
+  if (o.kind != OP_GPOOL) return e->pool_fwd(o, n, s);
   if (!feat) return fail(SSNB_EINVAL, "top_cls_pool needs the feat output pointer");
-  return e->gpool_fwd(o, feat, s);
+  return e->gpool_fwd(o, n, feat, s);
+}
+
+// the forward of frames [0, n) after the caller's checks
+int forward(ssnb_iv3* h, const float* input_nchw, int n, float* feat, cudaStream_t s) {
+  const int dv = h->val_by_name["data"];
+  const View d = h->view(dv);
+  int rc;
+  if (!h->tensor_cores()) {
+    rc = h->value_write(dv, false, input_nchw, 1.0f, n, s);
+  } else {      // every kStemK channels of a pixel written, the padding as zeros
+    rc = h->fast() ? launch_nchw_to_nhwc_pad<__half>(input_nchw, n, d.C, d.H * d.W, d.pitch, (__half*)d.base, s)
+                   : launch_nchw_to_nhwc_pad<float>(input_nchw, n, d.C, d.H * d.W, d.pitch, (float*)d.base, s);
+    if (!rc && h->exact_tc()) {
+      View x = d, xp = h->planes(dv);
+      x.C = xp.C = d.pitch;
+      rc = launch_split_view(x, n, 1.0f, xp, nullptr, s);
+    }
+  }
+  if (rc) return fail(rc, "input layout: " + thread_error());
+  for (const GraphOp& o : h->ops)
+    if (int rc = run_op(h, o, feat, n, s)) return fail(rc, o.id + ": " + thread_error());
+  return SSNB_OK;
 }
 
 // the graph of in_channels, planned for cfg
@@ -329,25 +352,14 @@ int ssnb_iv3_pack_weights(ssnb_iv3_handle h, const float* const* w, const float*
 int ssnb_iv3_forward(ssnb_iv3_handle h, const float* input_nchw, float* feat, void* stream) {
   if (!h || !input_nchw || !feat) return fail(SSNB_EINVAL, "ssnb_iv3_forward: null argument");
   if (!h->ws || !h->weights_ready) return fail(SSNB_ESTATE, "ssnb_iv3_forward: workspace / weights not set");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int dv = h->val_by_name["data"];
-  const View d = h->view(dv);
-  int rc;
-  if (!h->tensor_cores()) {
-    rc = h->value_write(dv, false, input_nchw, 1.0f, s);
-  } else {      // every kStemK channels of a pixel written, the padding as zeros
-    rc = h->fast() ? launch_nchw_to_nhwc_pad<__half>(input_nchw, h->F, d.C, d.H * d.W, d.pitch, (__half*)d.base, s)
-                   : launch_nchw_to_nhwc_pad<float>(input_nchw, h->F, d.C, d.H * d.W, d.pitch, (float*)d.base, s);
-    if (!rc && h->exact_tc()) {
-      View x = d, xp = h->planes(dv);
-      x.C = xp.C = d.pitch;
-      rc = launch_split_view(x, h->F, 1.0f, xp, nullptr, s);
-    }
-  }
-  if (rc) return fail(rc, "input layout: " + thread_error());
-  for (const GraphOp& o : h->ops)
-    if (int rc = run_op(h, o, feat, s)) return fail(rc, o.id + ": " + thread_error());
-  return SSNB_OK;
+  return forward(h, input_nchw, h->F, feat, (cudaStream_t)stream);
+}
+
+int ssnb_iv3_forward_frames(ssnb_iv3_handle h, const float* input_nchw, int frames, float* feat, void* stream) {
+  if (!h || !input_nchw || !feat) return fail(SSNB_EINVAL, "ssnb_iv3_forward_frames: null argument");
+  if (frames < 1 || frames > h->F) return fail(SSNB_EINVAL, "ssnb_iv3_forward_frames: frames must be in 1 .. " + std::to_string(h->F));
+  if (!h->ws || !h->weights_ready) return fail(SSNB_ESTATE, "ssnb_iv3_forward_frames: workspace / weights not set");
+  return forward(h, input_nchw, frames, feat, (cudaStream_t)stream);
 }
 
 int ssnb_iv3_num_ops(ssnb_iv3_handle h) { return h ? (int)h->ops.size() : 0; }
@@ -383,7 +395,7 @@ int ssnb_iv3_value_write(ssnb_iv3_handle h, const char* name, const float* src_n
   if (!h || !src_nchw || !h->ws) return fail(SSNB_EINVAL, "ssnb_iv3_value_write: null argument or no workspace");
   const int v = h->value_of(name);
   if (v < 0) return fail(SSNB_EINVAL, std::string("ssnb_iv3_value_write: unknown value ") + (name ? name : "(null)"));
-  const int rc = h->value_write(v, false, src_nchw, 1.0f, (cudaStream_t)stream);
+  const int rc = h->value_write(v, false, src_nchw, 1.0f, h->F, (cudaStream_t)stream);
   return rc ? fail(rc, thread_error()) : SSNB_OK;
 }
 
@@ -400,7 +412,7 @@ int ssnb_iv3_value_read(ssnb_iv3_handle h, const char* name, int planes, float* 
 int ssnb_iv3_run_op(ssnb_iv3_handle h, int op, float* feat, void* stream) {
   if (!h || op < 0 || op >= (int)h->ops.size()) return fail(SSNB_EINVAL, "ssnb_iv3_run_op: op out of range");
   if (!h->ws || !h->weights_ready) return fail(SSNB_ESTATE, "ssnb_iv3_run_op: workspace / weights not set");
-  if (int rc = run_op(h, h->ops[op], feat, (cudaStream_t)stream)) return fail(rc, h->ops[op].id + ": " + thread_error());
+  if (int rc = run_op(h, h->ops[op], feat, h->F, (cudaStream_t)stream)) return fail(rc, h->ops[op].id + ": " + thread_error());
   return SSNB_OK;
 }
 

@@ -95,16 +95,14 @@ __device__ __forceinline__ void ring_advance(uint32_t& stage, uint32_t& phase, i
   stage = s % (uint32_t)stages;
 }
 
-// BN = block_n: a multiple of 16, at most 128 (BN accumulators per consumer thread)
-template <int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2,
-                 const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_a_lo,
-                 const __grid_constant__ CUtensorMap tmap_a2_lo, const __grid_constant__ CUtensorMap tmap_b_lo,
-                 const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_o_hi,
-                 const __grid_constant__ CUtensorMap tmap_o_lo, const __grid_constant__ CUtensorMap tmap_o2,
-                 const __grid_constant__ CUtensorMap tmap_o2_hi, const __grid_constant__ CUtensorMap tmap_o2_lo,
-                 const __grid_constant__ UmmaConvParams p) {
+// BN = block_n: a multiple of 16, at most 128 (BN accumulators per consumer thread).  DIRECT: the launch has a frame box
+// that straddles its last frame below the maps' frame count (UmmaConvParams::f_direct)
+template <int BN, bool DIRECT>
+__device__ __forceinline__ void
+umma_conv_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_a2, const CUtensorMap& tmap_b, const CUtensorMap& tmap_a_lo,
+               const CUtensorMap& tmap_a2_lo, const CUtensorMap& tmap_b_lo, const CUtensorMap& tmap_o, const CUtensorMap& tmap_o_hi,
+               const CUtensorMap& tmap_o_lo, const CUtensorMap& tmap_o2, const CUtensorMap& tmap_o2_hi, const CUtensorMap& tmap_o2_lo,
+               const UmmaConvParams& p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operand tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -221,6 +219,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       // epilogue, one 16-column slice at a time, in the accumulators' fragment layout: thread (warp, lane) holds rows
       // 64 b + 16 warp + lane / 4 + 8 h and columns 8 k + 2 (lane % 4) + {0, 1} of the slice (b, h, k in {0, 1}).  The
       // results go to this warpgroup's staging in the output box layout, from which one thread stores them by TMA.
+      const bool direct = DIRECT && t.f0 >= p.f_direct;   // the partial last frame box of a launch of fewer frames than the maps'
       bool rv[2][2];                                   // the row is a pixel of the image (TMA clips the others)
       int rpix[2][2];                                  // its pixel index (f * H + h) * W + w
 #pragma unroll
@@ -395,7 +394,7 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         if (planes && p.flag && !(m <= 65504.f)) *p.flag = 1;
         fence_proxy_async_smem();
         named_bar_sync(EPI_BAR + cw, 128);
-        if (row == 0) {
+        if (row == 0 && !direct) {
           tma_store_4d(d1 ? &tmap_o : &tmap_o2, epi, cd, t.w0, t.h0, t.f0);
           if (planes) {
             tma_store_4d(d1 ? &tmap_o_hi : &tmap_o2_hi, epi + EPI_F32_BYTES, cd, t.w0, t.h0, t.f0);
@@ -403,11 +402,55 @@ umma_conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           }
           bulk_commit();
         }
+        if (direct) {
+          // the box straddles the launch's last frame below the maps' frame count, where the TMA store would also write the
+          // box's rows of frames >= F: each thread copies its staged row instead, when that row is a pixel of frames < F.
+          // The next slice's barrier keeps the staging until every thread has read it.
+          const int rw = row % p.bw, rh = (row / p.bw) % p.bh, rf = row / (p.bw * p.bh);
+          const int w = t.w0 + rw, y = t.h0 + rh, f = t.f0 + rf;
+          if (rf < p.bf && w < p.W && y < p.H && f < p.F) {
+            const long long po = ((long long)(f * p.H + y) * p.W + w) * opitch + ocoff + cd;
+            if (p.out_f32) {
+              float* o32 = (d1 ? p.out32 : p.out32_2) + po;
+#pragma unroll 1
+              for (int j = 0; j < EPI_COLS / 4; ++j)      // one 16-byte piece at a time: the accumulators of later slices are live
+                *reinterpret_cast<float4*>(o32 + 4 * j) = *reinterpret_cast<const float4*>(epi + sw64_off(row, 4 * j));
+            }
+            if (!p.out_f32 || planes) {
+              const uint8_t* st = epi + (p.out_f32 ? EPI_F32_BYTES : 0);
+              char* o16 = reinterpret_cast<char*>((d1 ? p.out : p.out2) + po);
+              const long long lo = d1 ? p.out_lo : p.out2_lo;
+#pragma unroll 1
+              for (int j = 0; j < EPI_COLS / 8; ++j) {
+                *reinterpret_cast<uint4*>(o16 + 16 * j) = *reinterpret_cast<const uint4*>(st + sw32_off(row, 8 * j));
+                if (planes) *reinterpret_cast<uint4*>(o16 + lo + 16 * j) = *reinterpret_cast<const uint4*>(st + EPI_F16_BYTES + sw32_off(row, 8 * j));
+              }
+            }
+          }
+        }
       }
     }
     if (row == 0) bulk_wait0();                        // the stores are complete before the CTA retires
   }
 }
+
+#define UMMA_CONV_PARAMS                                                                                                    \
+  const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_a2, const __grid_constant__ CUtensorMap tmap_b, \
+      const __grid_constant__ CUtensorMap tmap_a_lo, const __grid_constant__ CUtensorMap tmap_a2_lo,                               \
+      const __grid_constant__ CUtensorMap tmap_b_lo, const __grid_constant__ CUtensorMap tmap_o,                                   \
+      const __grid_constant__ CUtensorMap tmap_o_hi, const __grid_constant__ CUtensorMap tmap_o_lo,                                \
+      const __grid_constant__ CUtensorMap tmap_o2, const __grid_constant__ CUtensorMap tmap_o2_hi,                                 \
+      const __grid_constant__ CUtensorMap tmap_o2_lo, const __grid_constant__ UmmaConvParams p
+#define UMMA_CONV_ARGS tmap_a, tmap_a2, tmap_b, tmap_a_lo, tmap_a2_lo, tmap_b_lo, tmap_o, tmap_o_hi, tmap_o_lo, tmap_o2, tmap_o2_hi, tmap_o2_lo, p
+
+// every convolution launch
+template <int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) umma_conv_kernel(UMMA_CONV_PARAMS) { umma_conv_body<BN, false>(UMMA_CONV_ARGS); }
+// a forward launch of fewer frames than its plan whose last frame box straddles that count: the same body, whose epilogue
+// copies that box's rows of the launch's frames out of the staging instead of storing the box by TMA.  A kernel of its own,
+// so that the copy adds nothing to the epilogue of every other launch (inline, it made them 5-7 % slower on an H100).
+template <int BN>
+__global__ void __launch_bounds__(NUM_THREADS, 1) umma_conv_tail_kernel(UMMA_CONV_PARAMS) { umma_conv_body<BN, true>(UMMA_CONV_ARGS); }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -489,6 +532,7 @@ int bind_out(UmmaContext& ctx, UmmaConvPlan& plan, View o, float* out32, int n, 
   if (planes)
     if (int rc = encode_planes(ctx, mhi, mlo, p, reinterpret_cast<__half*>(o.base) + o.coff, o.lo_off, o.pitch, n)) return rc;
   (second ? p.planes2 : p.planes) = planes;
+  (second ? p.out2_lo : p.out_lo) = planes ? o.lo_off : 0;
   return 0;
 }
 
@@ -521,7 +565,7 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
     set_thread_error("umma conv: unsupported channel alignment"); return 1; }
   UmmaConvParams& p = plan.p;
   memset(&p, 0, sizeof(p));
-  p.W = a.W; p.H = a.H; p.F = F;
+  p.W = a.W; p.H = a.H; p.F = F; p.f_direct = 1 << 30;
   pick_box(a.W, p.bw, p.bh, p.bf);
   p.tiles_w = (a.W + p.bw - 1) / p.bw; p.tiles_h = (a.H + p.bh - 1) / p.bh; p.tiles_f = (F + p.bf - 1) / p.bf;
   // N split: equal tiles of block_n <= 128 (multiple of 16); the last tile may overhang N (TMA zero-fills the
@@ -565,7 +609,7 @@ int bind_common(UmmaContext& ctx, UmmaConvPlan& plan, View a, View o, int F, int
   if (tc && (!tc->out32 || !a.lo_off || !tc->w_lo_off)) { set_thread_error("umma conv: split-operand bind needs operand planes and an fp32 output"); return 1; }
   if (int rc = bind_out(ctx, plan, o, p.out32, N, false)) return rc;
   // second destination = the first unless a fused bind redirects it
-  p.out32_2 = p.out32; p.planes2 = p.planes;
+  p.out32_2 = p.out32; p.planes2 = p.planes; p.out2_lo = p.out_lo;
   plan.tmap_o2 = plan.tmap_o; plan.tmap_o2_hi = plan.tmap_o_hi; plan.tmap_o2_lo = plan.tmap_o_lo;
   plan.enabled = true;
   return 0;
@@ -698,10 +742,10 @@ int umma_conv_set_mask_tc(UmmaContext& ctx, UmmaConvPlan& plan, View y32, View d
 }
 
 namespace {
-template <int BN>
+template <int BN, bool DIRECT>
 int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, const CUtensorMap& o_hi, const CUtensorMap& o_lo, int grid, cudaStream_t s) {
   static bool attr_set[64] = {};          // function attributes are per device
-  auto kern = umma_conv_kernel<BN>;
+  auto kern = DIRECT ? umma_conv_tail_kernel<BN> : umma_conv_kernel<BN>;
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[dev]) {
@@ -711,14 +755,26 @@ int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, const CUtensorM
   }
   kern<<<grid, NUM_THREADS, SMEM_BYTES, s>>>(plan.tmap_a, plan.tmap_a2, plan.tmap_b, plan.tmap_a_lo, plan.tmap_a2_lo, plan.tmap_b_lo, plan.tmap_o, o_hi, o_lo,
                                              plan.tmap_o2, plan.tmap_o2_hi, plan.tmap_o2_lo, p);
-  SSNB_LAUNCH_CHECK("umma_conv_kernel");
+  SSNB_LAUNCH_CHECK("umma_conv_kernel");      // both kernels: the launch log names the convolution kernel
   return 0;
+}
+template <int BN>
+int launch_bn(const UmmaConvPlan& plan, const UmmaConvParams& p, const CUtensorMap& o_hi, const CUtensorMap& o_lo, int grid, cudaStream_t s) {
+  return p.f_direct < (1 << 30) ? launch_bn<BN, true>(plan, p, o_hi, o_lo, grid, s) : launch_bn<BN, false>(plan, p, o_hi, o_lo, grid, s);
 }
 }  // namespace
 
-int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask) {
+int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask, int frames) {
   if (!plan.enabled) { set_thread_error("umma conv: plan not bound"); return 3; }
   UmmaConvParams p = plan.p;
+  if (frames && frames != p.F) {
+    // n < F frames on the maps bound for F: frame boxes stay outermost in decode_tile, so the first ceil(n / bf) of them are
+    // the whole launch; the box that straddles n is stored row by row (f_direct)
+    if (frames < 1 || frames > p.F || mask || p.accumulate) { set_thread_error("umma conv: a frame count below the plan's runs forward plans only"); return 3; }
+    p.F = frames;
+    p.tiles_f = (frames + p.bf - 1) / p.bf;
+    if (frames % p.bf) p.f_direct = frames - frames % p.bf;
+  }
   if (mask && plan.mask_y) { p.mask_y = plan.mask_y; p.mask_pitch = plan.mask_pitch; p.mask_coff = plan.mask_coff; }
   const bool mplanes = mask && p.out_f32 && plan.mask32 && plan.mask_planes;
   if (mplanes) {

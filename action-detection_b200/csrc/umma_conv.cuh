@@ -22,9 +22,13 @@ struct UmmaContext {
 };
 
 struct UmmaConvParams {
-  int W, H, F;                    // spatial dims shared by input and output (stride-1 convolutions)
+  int W, H, F;                    // spatial dims shared by input and output (stride-1 convolutions); F: frames this launch computes
   int bw, bh, bf;                 // TMA box in pixels; bw*bh*bf <= 128 rows of the M tile
   int tiles_w, tiles_h, tiles_f;
+  // first frame of the tiles whose epilogue stores row by row instead of by TMA: a launch of fewer frames than the output
+  // maps were encoded for stores its last, partial frame box this way, so no row of a frame >= F is written (1 << 30: none)
+  int f_direct;
+  long long out_lo, out2_lo;      // byte distance of the LO operand plane from p.out / p.out2 (EXACT_TC planes, row-by-row stores)
   int n_tiles, block_n;           // N split of Cout into ceil(N/128) tiles; block_n is a multiple of 16, at most 128
   int stages, stage_bytes;        // smem pipeline depth / stride chosen from block_n
   int kchunks, ntaps, K;          // ceil(K/64), filter taps, reduction channels per tap
@@ -102,7 +106,9 @@ int umma_conv_bind_fused_fwd(UmmaContext& ctx, UmmaConvPlan& plan, View in, View
 // fused data gradient of sibling 1x1 convs: dx (+)= [dz1 | dz2] * W, weights [cin][pad64(k1) + k2]; dz1 may be empty (k1 = 0)
 int umma_conv_bind_fused_dgrad(UmmaContext& ctx, UmmaConvPlan& plan, View dz1, View dz2, View dx, int F, int cin, int k1, int k2,
                                const __half* w_n_k, int accumulate, const UmmaTcOpts* tc = nullptr);
-int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask = false);
+// frames = 0: the plan's frame count; 1 .. F (forward plans, mask = false): the first `frames` frames only, with that many
+// frames' tiles, the maps as bound and no store to a frame >= frames
+int umma_conv_launch(UmmaContext& ctx, const UmmaConvPlan& plan, cudaStream_t s, bool mask = false, int frames = 0);
 void umma_conv_set_mask(UmmaConvPlan& plan, View y);
 // EXACT_TC: y32 = fp32 activation of the output value, dplanes = that value's gradient operand planes (hi base + lo_off)
 int umma_conv_set_mask_tc(UmmaContext& ctx, UmmaConvPlan& plan, View y32, View dplanes, float plane_scale, int* flag);

@@ -57,9 +57,16 @@ class BNInception(EngineBackbone):
                                       "eval mode ('full' is listed as a next step in DESIGN.md)")
         return bool(bns[0].training)
 
+    @staticmethod
+    def _forward_only_key(key):
+        return not key[1] and not key[5]
+
     def engine_for(self, frames, training, device, bn1_train=False):
+        """the engine a call of `frames` frames runs on: planned for `frames`, or for the reserve_frames() count when it is a
+        forward-only (training=False, bn1_train=False) call"""
         if bn1_train and self.precision == _lib.FAST_FP16:
             raise NotImplementedError("bn_mode='partial' runs in EXACT_FP32 / EXACT_TC precision (fp32 activations), not FAST_FP16")
+        frames = self._planned_frames(frames, not training and not bn1_train)
         key = (frames, bool(training), self.precision, self.in_channels(), str(device), bool(bn1_train))
         return self._packed_engine(key, lambda: BackboneEngine(self.in_channels(), frames, self.precision, training, self.grad_scale,
                                                                device, bn1_train=bn1_train))

@@ -63,7 +63,13 @@ class InceptionV3(EngineBackbone):
             raise NotImplementedError("InceptionV3 runs with frozen BatchNorm2d layers (eval mode); " + FOLLOW_UP)
         return False
 
+    @staticmethod
+    def _forward_only_key(key):
+        return True
+
     def engine_for(self, frames, device):
+        """the engine a call of `frames` frames runs on: planned for `frames`, or for the reserve_frames() count"""
+        frames = self._planned_frames(frames, True)
         key = (frames, self.precision, self.in_channels(), str(device))
         return self._packed_engine(key, lambda: InceptionV3Engine(self.in_channels(), frames, self.precision, device))
 

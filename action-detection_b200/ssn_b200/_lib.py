@@ -103,6 +103,7 @@ SIGNATURES = {
     "ssnb_pack_weights": (_i, [_vp, _pp, _pp, _pp, _pp, _pp, _pp, _vp]),
     "ssnb_set_bn1": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _f, _f]),
     "ssnb_backbone_fwd": (_i, [_vp, _vp, _vp, _vp]),
+    "ssnb_backbone_fwd_frames": (_i, [_vp, _vp, _i, _vp, _vp]),
     "ssnb_backbone_bwd": (_i, [_vp, _vp, _pp, _pp, _vp]),
     "ssnb_backbone_bwd_range": (_i, [_vp, _vp, _pp, _pp, _i, _i, _vp]),
     "ssnb_bind_grads": (_i, [_vp, _pp, _pp]),
@@ -183,6 +184,7 @@ SIGNATURES = {
     "ssnb_iv3_set_workspace": (_i, [_vp, _vp, _sz]),
     "ssnb_iv3_pack_weights": (_i, [_vp, _pp, _pp, _pp, _pp, _pp, _pp, _vp]),
     "ssnb_iv3_forward": (_i, [_vp, _vp, _vp, _vp]),
+    "ssnb_iv3_forward_frames": (_i, [_vp, _vp, _i, _vp, _vp]),
     "ssnb_iv3_num_ops": (_i, [_vp]),
     "ssnb_iv3_op_info": (_i, [_vp, _i, C.c_char_p, _i, C.c_char_p, _i, C.c_char_p, _i, _ip, _ip, _ip, _ip]),
     "ssnb_iv3_value_info": (_i, [_vp, C.c_char_p, _ip, _ip, _ip, C.c_char_p, _i, _ip]),

@@ -64,18 +64,21 @@ class PlannedEngine:
 
 
 class BackboneEngine(PlannedEngine):
-    """One planned BNInception instance for a fixed frame count (ssnb_create .. ssnb_destroy)."""
+    """One planned BNInception instance for a fixed frame count (ssnb_create .. ssnb_destroy).  A forward-only engine
+    (training=False) also runs any smaller frame count on the same workspace.  device=None plans without allocating (the
+    plan needs no GPU)."""
     _set_workspace_fn, _pack_fn, _destroy_fn = "ssnb_set_workspace", "ssnb_pack_weights", "ssnb_destroy"
 
     def __init__(self, in_channels, frames, precision, training, grad_scale, device, bn1_train=False):
-        self.device = torch.device(device)
+        self.device = None if device is None else torch.device(device)
         self.frames, self.in_channels, self.precision, self.training = frames, in_channels, precision, training
         self.bn1_train = bool(bn1_train)
         cfg = _lib.Config(in_channels, frames, precision, 1 if training else 0, float(grad_scale), 1 if bn1_train else 0)
         self.h = C.c_void_p()
         check(lib.ssnb_create(C.byref(cfg), C.byref(self.h)), None, "ssnb_create")
         self.workspace_bytes = lib.ssnb_workspace_bytes(self.h)
-        self._set_workspace()
+        if self.device is not None:
+            self._set_workspace()
         self.packed_version = None
         self.generation = 0        # bumped by every forward: the saved activations belong to the latest one only
 
@@ -86,15 +89,21 @@ class BackboneEngine(PlannedEngine):
                                float(bn.momentum if bn.momentum is not None else 0.1), float(bn.eps)), self.h, "set_bn1")
 
     def forward(self, x):
+        """x [n, C, 224, 224] -> feat [n, 1024]; n < frames (forward-only engines) runs the first n frames of the plan"""
         _need_cuda(x, "input")
         x = x.contiguous().float()
-        assert x.shape[0] == self.frames and x.shape[1] == self.in_channels and tuple(x.shape[2:]) == (224, 224), \
-            "engine planned for [%d,%d,224,224], got %s" % (self.frames, self.in_channels, tuple(x.shape))
-        feat = torch.empty(self.frames, 1024, dtype=torch.float32, device=x.device)
+        n = x.shape[0]
+        assert 1 <= n <= self.frames and x.shape[1] == self.in_channels and tuple(x.shape[2:]) == (224, 224), \
+            "engine planned for [<=%d,%d,224,224], got %s" % (self.frames, self.in_channels, tuple(x.shape))
+        feat = torch.empty(n, 1024, dtype=torch.float32, device=x.device)
         self.generation += 1
         with torch.cuda.device(self.device):
-            check(lib.ssnb_backbone_fwd(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(feat.data_ptr()), _stream()),
-                  self.h, "backbone_fwd")
+            if n == self.frames:
+                check(lib.ssnb_backbone_fwd(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(feat.data_ptr()), _stream()),
+                      self.h, "backbone_fwd")
+            else:
+                check(lib.ssnb_backbone_fwd_frames(self.h, C.c_void_p(x.data_ptr()), n, C.c_void_p(feat.data_ptr()), _stream()),
+                      self.h, "backbone_fwd_frames")
         return feat
 
     def backward(self, dfeat, dw, db, accumulate=False, buckets=None, on_bucket=None):

@@ -23,8 +23,8 @@ def conv_table(in_channels):
 
 
 class InceptionV3Engine(PlannedEngine):
-    """One planned InceptionV3 forward for a fixed frame count (ssnb_iv3_create .. ssnb_iv3_destroy).  device=None plans
-    without allocating (the plan needs no GPU)."""
+    """One planned InceptionV3 forward for a fixed frame count (ssnb_iv3_create .. ssnb_iv3_destroy), which also runs any
+    smaller frame count on the same workspace.  device=None plans without allocating (the plan needs no GPU)."""
     _set_workspace_fn, _pack_fn, _destroy_fn = "ssnb_iv3_set_workspace", "ssnb_iv3_pack_weights", "ssnb_iv3_destroy"
     _errors_on_handle = False
 
@@ -40,13 +40,19 @@ class InceptionV3Engine(PlannedEngine):
             self._set_workspace()
 
     def forward(self, x):
+        """x [n, C, 299, 299] -> feat [n, 2048]; n < frames runs the first n frames of the plan"""
         _need_cuda(x, "input")
         x = x.contiguous().float()
-        assert tuple(x.shape) == (self.frames, self.in_channels, INPUT_SIZE, INPUT_SIZE), \
-            "engine planned for [%d,%d,299,299], got %s" % (self.frames, self.in_channels, tuple(x.shape))
-        feat = torch.empty(self.frames, FEAT_DIM, dtype=torch.float32, device=x.device)
+        n = x.shape[0]
+        assert 1 <= n <= self.frames and tuple(x.shape[1:]) == (self.in_channels, INPUT_SIZE, INPUT_SIZE), \
+            "engine planned for [<=%d,%d,299,299], got %s" % (self.frames, self.in_channels, tuple(x.shape))
+        feat = torch.empty(n, FEAT_DIM, dtype=torch.float32, device=x.device)
         with torch.cuda.device(self.device):
-            check(lib.ssnb_iv3_forward(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(feat.data_ptr()), _stream()), None, "iv3_forward")
+            if n == self.frames:
+                check(lib.ssnb_iv3_forward(self.h, C.c_void_p(x.data_ptr()), C.c_void_p(feat.data_ptr()), _stream()), None, "iv3_forward")
+            else:
+                check(lib.ssnb_iv3_forward_frames(self.h, C.c_void_p(x.data_ptr()), n, C.c_void_p(feat.data_ptr()), _stream()), None,
+                      "iv3_forward_frames")
         return feat
 
     # ---- introspection: the plan and the launch-by-launch tests ----

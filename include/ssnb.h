@@ -72,6 +72,12 @@ int ssnb_set_bn1(ssnb_handle h, const float* gamma, const float* beta, float* ru
 /* input [F, C, 224, 224] fp32 NCHW (the reference's frame tensor after input.view(-1, C, H, W),
  * ssn_models.py:266) -> feat [F, 1024] fp32 (global_pool output, fc replaced by Identity/Dropout) */
 int ssnb_backbone_fwd(ssnb_handle h, const float* input_nchw, float* feat, void* stream);
+/* The same forward over the first `frames` frames of the plan, 1 <= frames <= F: input [frames, C, 224, 224] -> feat
+ * [frames, 1024], rows bitwise those of an engine planned for `frames`, on this engine's workspace and with the launches of
+ * `frames` frames (no row of a frame >= frames is read from the input or written to feat).  frames == F is ssnb_backbone_fwd.
+ * Forward-only engines: SSNB_EINVAL for frames outside 1 .. F, SSNB_ESTATE for a training engine, SSNB_ENOSUPPORT for a
+ * bn1_train engine, each before any launch.  Binds nothing, so a call can be captured in a CUDA graph. */
+int ssnb_backbone_fwd_frames(ssnb_handle h, const float* input_nchw, int frames, float* feat, void* stream);
 /* dfeat [F,1024] fp32 -> dw[i] [cout,cin,k,k], db[i] [cout] fp32 in reference layout (what autograd
  * leaves in Conv2d.weight.grad / .bias.grad; BN params are frozen and get none).  Overwrites. */
 int ssnb_backbone_bwd(ssnb_handle h, const float* dfeat, float* const* dw, float* const* db, void* stream);
@@ -645,6 +651,10 @@ int ssnb_iv3_pack_weights(ssnb_iv3_handle h, const float* const* w, const float*
 /* input [F, C, 299, 299] fp32 NCHW -> feat [F, 2048] fp32 (top_cls_pool, the 8x8 average pool; top_cls_fc is replaced by
  * Identity / Dropout) */
 int ssnb_iv3_forward(ssnb_iv3_handle h, const float* input_nchw, float* feat, void* stream);
+/* the same forward over the first `frames` frames, 1 <= frames <= F (SSNB_EINVAL otherwise, before any launch): input
+ * [frames, C, 299, 299] -> feat [frames, 2048], rows bitwise those of an engine planned for `frames`, with that many frames'
+ * launches on this engine's workspace; graph-capturable.  frames == F is ssnb_iv3_forward. */
+int ssnb_iv3_forward_frames(ssnb_iv3_handle h, const float* input_nchw, int frames, float* feat, void* stream);
 /* introspection for the plan and the launch-by-launch tests: op kinds "conv" | "maxpool" | "avgpool" | "gpool", the names of the
  * values an op reads and writes (the yaml's blob names; the last op writes "top_cls_global_pool", the feat output), its
  * convolution index (-1 for pools) and a pool's window, stride and pad (0 / 1 / 0 for convolutions).  A value's shape, its buffer and its channel offset in that buffer. */
