@@ -84,11 +84,12 @@ class BinaryClassifier(_BNInceptionModel):
         return self.test_fc(base_out), base_out
 
     # ---- fused training step: backbone fwd -> pool + mask + segment mean -> classifier + CE (+grads) -> backbone bwd ------
-    def fused_step(self, input, target, loss_scale=1.0, grad_sync=None):
+    def fused_step(self, input, target, loss_scale=1.0, grad_sync=None, meters=None):
         """Same arithmetic as train_forward + torch.nn.CrossEntropyLoss() + loss.backward() (binary_train.py:153-169) in
         five library calls.  Accumulates into .grad like autograd and returns the mean loss as a device tensor [1].  Every
         gradient is multiplied by loss_scale (1/world for data parallel with equal rows per rank).  grad_sync
         (ssn_b200.dp.GradSync): exchange the gradients bucket by bucket while the backward of the lower layers is running.
+        meters (ssn_b200.meters.StepMeters('binary')): add this step's loss and accuracies to it, on the device.
         Keeps feat, course, logits and the dropout mask (None without dropout) of the step in self.last_fused."""
         self._require_trainable_backbone()
         if not input.is_cuda:
@@ -99,6 +100,32 @@ class BinaryClassifier(_BNInceptionModel):
         frames = self._frames(input)
         eng = self.base_model.engine_for(frames.shape[0], True, frames.device)
         x = frames.contiguous().float()
+        mask = None
+        if self.dropout != 0 and self.training:
+            keep = 1.0 - self.dropout
+            mask = torch.bernoulli(torch.full((x.shape[0], self.feature_dim), keep, device=x.device)) / keep
+        r = self._fused_forward(eng, x, target, mask, loss_scale)
+        if meters is not None:
+            meters.update_binary(r["loss"], r["logits"], r["target"], input.size(0))
+        n, S = r["course"].shape[0], self.course_segment
+        w, b = self.classifier_fc.weight, self.classifier_fc.bias
+        dft = torch.empty(x.shape[0], self.feature_dim, dtype=torch.float32, device=x.device)
+        with torch.cuda.device(x.device):
+            check(lib.ssnb_stpp_bwd(r["d_course"].data_ptr(), None, None, n, S, self.feature_dim, 0, None, None, None, None, 0, S,
+                                    dft.data_ptr(), _stream()), None, "stpp_bwd")
+        if mask is not None:
+            dft = dft * mask
+        if w.requires_grad:
+            self._accumulate_grad(w, r["dw"])
+        if b.requires_grad:
+            self._accumulate_grad(b, r["db"])
+        self._fused_backbone_backward(eng, dft, grad_sync)
+        self.last_fused = dict(feat=r["feat"], course=r["course"], logits=r["logits"], mask=mask)
+        return r["loss"]
+
+    def _fused_forward(self, eng, x, target, mask, loss_scale):
+        """backbone forward -> global pool (+ dropout mask) + segment mean -> classifier + cross-entropy (+ its gradients):
+        the forward half that fused_step and fused_eval share"""
         dev = x.device
         F_, S, D = x.shape[0], self.course_segment, self.feature_dim
         if F_ % S:
@@ -109,13 +136,9 @@ class BinaryClassifier(_BNInceptionModel):
             raise ValueError("%d targets for %d proposals" % (tg.numel(), n))
         f32 = dict(dtype=torch.float32, device=dev)
         feat, course = torch.empty(F_, D, **f32), torch.empty(n, D, **f32)
-        mask = None
-        if self.dropout != 0 and self.training:
-            keep = 1.0 - self.dropout
-            mask = torch.bernoulli(torch.full((F_, D), keep, device=dev)) / keep
         w, b = self.classifier_fc.weight, self.classifier_fc.bias
         logits, loss = torch.empty(n, K, **f32), torch.empty(1, **f32)
-        d_course, dw, db, dft = torch.empty(n, D, **f32), torch.empty_like(w), torch.empty_like(b), torch.empty(F_, D, **f32)
+        d_course, dw, db = torch.empty(n, D, **f32), torch.empty_like(w), torch.empty_like(b)
         ws = torch.empty(lib.ssnb_classifier_ce_workspace_bytes(n, K), dtype=torch.uint8, device=dev)
         with torch.cuda.device(dev):
             check(lib.ssnb_backbone_fwd(eng.h, x.data_ptr(), feat.data_ptr(), _stream()), eng.h, "backbone_fwd")
@@ -125,14 +148,26 @@ class BinaryClassifier(_BNInceptionModel):
             check(lib.ssnb_classifier_ce_fwd_bwd(course.data_ptr(), w.data_ptr(), b.data_ptr(), tg.data_ptr(), n, D, K,
                                                  float(loss_scale), logits.data_ptr(), loss.data_ptr(), d_course.data_ptr(),
                                                  dw.data_ptr(), db.data_ptr(), ws.data_ptr(), _stream()), None, "classifier_ce_fwd_bwd")
-            check(lib.ssnb_stpp_bwd(d_course.data_ptr(), None, None, n, S, D, 0, None, None, None, None, 0, S, dft.data_ptr(),
-                                    _stream()), None, "stpp_bwd")
-        if mask is not None:
-            dft = dft * mask
-        if w.requires_grad:
-            self._accumulate_grad(w, dw)
-        if b.requires_grad:
-            self._accumulate_grad(b, db)
-        self._fused_backbone_backward(eng, dft, grad_sync)
-        self.last_fused = dict(feat=feat, course=course, logits=logits, mask=mask)
-        return loss
+        return dict(feat=feat, course=course, logits=logits, loss=loss, target=tg, d_course=d_course, dw=dw, db=db)
+
+    def fused_eval(self, input, target, meters=None):
+        """The body of validate() (binary_train.py:219-243): the forward of a forward-only engine, global pool + segment mean,
+        classifier_fc and CrossEntropyLoss, without a backward.  The model must be in eval() (binary_train.py:225): no
+        dropout, no running-statistic update; no .grad changes.  Returns the mean loss [1] on the device, what fused_step's
+        forward half computes from the same features; meters (StepMeters('binary')) gets the loss and accuracies.  Keeps
+        feat, course and logits in self.last_eval."""
+        self._require_trainable_backbone()
+        if self.training:
+            raise RuntimeError("fused_eval runs validate()'s forward: call model.eval() first (binary_train.py:225)")
+        if not input.is_cuda:
+            raise RuntimeError("BinaryClassifier(H100).fused_eval needs CUDA tensors (libssn_b200 has no CPU path)")
+        frames = self._frames(input)
+        eng = self.base_model.engine_for(frames.shape[0], False, frames.device)
+        if eng.frames != frames.shape[0]:
+            raise ValueError("fused_eval pools the engine's whole plan: %d frames with %d reserved by reserve_frames(); "
+                             "call reserve_frames(None) or pass the reserved count" % (frames.shape[0], eng.frames))
+        r = self._fused_forward(eng, frames.contiguous().float(), target, None, 1.0)
+        if meters is not None:
+            meters.update_binary(r["loss"], r["logits"], r["target"], input.size(0))
+        self.last_eval = dict(feat=r["feat"], course=r["course"], logits=r["logits"])
+        return r["loss"]

@@ -773,19 +773,29 @@ __global__ void __launch_bounds__(HL_THREADS) heads_loss_kernel(HeadsArgs a) {
 // learning rate and weight decay (ssn_train.py:391-398 lr_mult / decay_mult); the segment of an element is found by
 // binary search over the cumulative ends staged in shared memory
 constexpr int SGD_MAX_SEG = 512;
-__global__ void sgd_groups_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ buf, long long n,
+// kClip: the gradient multiplier becomes gm * (float)c where c = max_norm / (*norm + 1e-6) < 1 (ssnb_grad_clip's rule), and
+// write_back stores the scaled gradient; otherwise the same expression with gm itself, so an unclipped step is bitwise
+// the plain one
+template <bool kClip>
+__global__ void sgd_groups_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ buf, long long n,
                                   const long long* __restrict__ seg_end, const float* __restrict__ seg_lr, const float* __restrict__ seg_wd,
-                                  int nseg, float mom, float gm) {
+                                  int nseg, float mom, float gm, const float* __restrict__ norm, float max_norm, int write_back) {
   __shared__ long long s_end[SGD_MAX_SEG];
   __shared__ float s_lr[SGD_MAX_SEG], s_wd[SGD_MAX_SEG];
   for (int i = threadIdx.x; i < nseg; i += blockDim.x) { s_end[i] = seg_end[i]; s_lr[i] = seg_lr[i]; s_wd[i] = seg_wd[i]; }
   __syncthreads();
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  if (kClip) {
+    const double c = (double)max_norm / ((double)*norm + 1e-6);
+    if (c < 1.0) gm = gm * (float)c;
+  }
   int lo = 0, hi = nseg - 1;                 // first segment whose end is > i
   while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_end[mid] > i) hi = mid; else lo = mid + 1; }
   const float w = p[i];
-  const float gr = g[i] * gm + s_wd[lo] * w;
+  const float gv = g[i];
+  const float gr = gv * gm + s_wd[lo] * w;
+  if (kClip && write_back) g[i] = __fmul_rn(gv, gm);   // its own rounding: gr keeps the plain kernel's contraction
   const float b = mom * buf[i] + gr;
   buf[i] = b;
   p[i] = w - s_lr[lo] * b;
@@ -807,7 +817,10 @@ int fill_parts(PartTable& pt, int n_parts, const int* lo, const int* hi, const i
 }  // namespace
 }  // namespace ssnb
 
-namespace ssnb { int engine_tail_view(ssnb_handle h, View* v, int* F, int* fp16); }
+namespace ssnb {
+int engine_tail_view(ssnb_handle h, View* v, int* F, int* fp16);
+int check_extra_grads(const ssnb_extra_grads* extra, const char* what);   // train_loop.cu
+}
 using namespace ssnb;
 
 extern "C" {
@@ -1118,9 +1131,27 @@ int ssnb_sgd_step_groups(float* param, const float* grad, float* momentum_buf, s
   cudaStream_t s = (cudaStream_t)stream;
   if (!param || !grad || !momentum_buf || !seg_end || !seg_lr || !seg_wd || n_seg < 1 || n_seg > SGD_MAX_SEG) { set_thread_error("sgd_groups: bad argument"); return SSNB_EINVAL; }
   if (n == 0) return SSNB_OK;
-  sgd_groups_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(param, grad, momentum_buf, (long long)n, (const long long*)seg_end, seg_lr, seg_wd, n_seg,
-                                                              momentum, grad_mult);
+  sgd_groups_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(param, const_cast<float*>(grad), momentum_buf, (long long)n,
+                                                                     (const long long*)seg_end, seg_lr, seg_wd, n_seg, momentum,
+                                                                     grad_mult, nullptr, 0.f, 0);
   SSNB_LAUNCH_CHECK("sgd_groups_kernel");
+  return SSNB_OK;
+}
+
+int ssnb_sgd_step_groups_clipped(float* param, float* grad, float* momentum_buf, size_t n, const int64_t* seg_end, const float* seg_lr,
+                                 const float* seg_wd, int n_seg, float momentum, float grad_mult, const float* norm, float max_norm,
+                                 int write_back, const ssnb_extra_grads* extra, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!param || !grad || !momentum_buf || !seg_end || !seg_lr || !seg_wd || n_seg < 1 || n_seg > SGD_MAX_SEG || !norm || !(max_norm >= 0.f)) {
+    set_thread_error("sgd_groups_clipped: bad argument"); return SSNB_EINVAL; }
+  if (int rc = check_extra_grads(extra, "sgd_groups_clipped")) return rc;
+  if (n > 0) {
+    sgd_groups_kernel<true><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(param, grad, momentum_buf, (long long)n, (const long long*)seg_end,
+                                                                       seg_lr, seg_wd, n_seg, momentum, grad_mult, norm, max_norm,
+                                                                       write_back);
+    SSNB_LAUNCH_CHECK("sgd_groups_clipped_kernel");
+  }
+  if (write_back && extra && extra->count > 0) return ssnb_grad_clip(norm, max_norm, nullptr, 0, extra, stream);
   return SSNB_OK;
 }
 

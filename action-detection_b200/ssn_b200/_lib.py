@@ -83,6 +83,14 @@ class ProposalTargetsCfg(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+GRAD_NORM_CTAS, MAX_EXTRA_GRADS = 512, 8
+
+
+class ExtraGrads(C.Structure):
+    _fields_ = [("count", C.c_int32), ("reserved", C.c_int32), ("grad", C.c_void_p * MAX_EXTRA_GRADS),
+                ("numel", C.c_int64 * MAX_EXTRA_GRADS)]
+
+
 PROPFRAMES_SECONDS, PROPFRAMES_NORMALISED, PROPFRAMES_AS_GIVEN = 0, 1, 2
 TAG_FG, TAG_INCOMPLETE, TAG_BACKGROUND = 1, 2, 4
 
@@ -192,6 +200,10 @@ SIGNATURES = {
     "ssnb_iv3_value_read": (_i, [_vp, C.c_char_p, _i, _vp, _vp]),
     "ssnb_iv3_run_op": (_i, [_vp, _i, _vp, _vp]),
     "ssnb_sgd_step_groups": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp]),
+    "ssnb_grad_norm": (_i, [_vp, _sz, _f, C.POINTER(ExtraGrads), _vp, _vp, _vp]),
+    "ssnb_grad_clip": (_i, [_vp, _f, _vp, _sz, C.POINTER(ExtraGrads), _vp]),
+    "ssnb_sgd_step_groups_clipped": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp, _f, _i, C.POINTER(ExtraGrads), _vp]),
+    "ssnb_train_meters": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, C.c_double, _vp, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -354,12 +354,13 @@ class SSN(_BNInceptionModel):
 
     # ---- fused training step: backbone fwd -> pool+STPP -> heads+loss(+grads) -> backbone bwd ---------
     def fused_step(self, input, aug_scaling, target, reg_target, prop_type, fg_per_video=1, comp_group=7,
-                   props_per_video=8, ohem_ratio=0.17, comp_w=0.1, reg_w=0.1, global_videos=None, loss_scale=1.0, grad_sync=None):
+                   props_per_video=8, ohem_ratio=0.17, comp_w=0.1, reg_w=0.1, global_videos=None, loss_scale=1.0, grad_sync=None,
+                   meters=None):
         """Same arithmetic as train_forward + the three criteria + loss.backward() of
         ssn_train.py:207-236, issued as ~4 library calls.  Accumulates into .grad like autograd and
         returns losses[4] = (act, comp, reg, total) as a device tensor.  grad_sync (ssn_b200.dp.GradSync): exchange the
-        gradients bucket by bucket while the backward of the lower layers is still running."""
-        import ctypes as C
+        gradients bucket by bucket while the backward of the lower layers is still running.  meters
+        (ssn_b200.meters.StepMeters('ssn')): add this step's losses and accuracies to it, on the device."""
         from ssn_b200.engine import _stream
         self._require_trainable_backbone()
         assert self.with_regression, "fused_step implements the regression configuration"
@@ -369,32 +370,20 @@ class SSN(_BNInceptionModel):
             raise NotImplementedError("fused_step implements bn_mode='frozen'; with bn_mode='partial' use the module path "
                                       "(model(...), criteria, loss.backward()), which runs the first BatchNorm2d in training mode")
         frames = self._frames(input)
-        bm = self.base_model
-        eng = bm.engine_for(frames.shape[0], True, frames.device)
+        eng = self.base_model.engine_for(frames.shape[0], True, frames.device)
         x = frames.contiguous().float()
-        dev = x.device
-        F_ = x.shape[0]
+        F_, D = x.shape[0], 1024
         n = F_ // self.num_segments
-        feat = torch.empty(F_, 1024, dtype=torch.float32, device=dev)
         mask = None
         if self.dropout != 0 and self.training:
             keep = 1.0 - self.dropout
-            mask = torch.bernoulli(torch.full((F_, 1024), keep, device=dev)) / keep
-        with torch.cuda.device(dev):
-            check(lib.ssnb_backbone_fwd(eng.h, x.data_ptr(), feat.data_ptr(), _stream()), eng.h, "backbone_fwd")
-            lo, hi, nm, col = self.stpp.part_table(self._seg_split())
-            D = 1024
-            course = torch.empty(n, D, dtype=torch.float32, device=dev)
-            stpp = torch.empty(n, len(lo) * D, dtype=torch.float32, device=dev)
-            sc = aug_scaling.contiguous().float().view(-1, 2)
-            check(lib.ssnb_gpool_stpp_fwd(eng.h, None if mask is None else mask.data_ptr(), sc.data_ptr(),
-                                          self.num_segments, len(lo), _lib.int_array(lo), _lib.int_array(hi),
-                                          _lib.int_array(nm), _lib.int_array(col), self.starting_segment,
-                                          self.starting_segment + self.course_segment, feat.data_ptr(),
-                                          course.data_ptr(), stpp.data_ptr(), _stream()), eng.h, "gpool_stpp_fwd")
-        out = heads_loss_fused(course, stpp, self.activity_fc, self.completeness_fc, self.regressor_fc, prop_type,
-                               target, reg_target, self.num_class, self.stpp.feat_multiplier, fg_per_video, comp_group,
-                               props_per_video, ohem_ratio, comp_w, reg_w, global_videos, loss_scale)
+            mask = torch.bernoulli(torch.full((F_, D), keep, device=x.device)) / keep
+        out, feat, course, stpp, sc, (lo, hi, nm, col) = self._fused_forward(
+            eng, x, mask, aug_scaling, target, reg_target, prop_type, fg_per_video, comp_group, props_per_video, ohem_ratio,
+            comp_w, reg_w, global_videos, loss_scale)
+        if meters is not None:
+            meters.update_ssn(out["losses"], out["raw_act"], target, prop_type, input.size(0))
+        dev = x.device
         dft = torch.empty(F_, D, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             check(lib.ssnb_stpp_bwd(out["d_course"].data_ptr(), out["d_stpp"].data_ptr(), sc.data_ptr(), n,
@@ -410,4 +399,54 @@ class SSN(_BNInceptionModel):
                 self._accumulate_grad(fc.bias, out["d_%s_b" % k])
         self._fused_backbone_backward(eng, dft, grad_sync)
         self.last_fused = dict(out, feat=feat, course=course, stpp=stpp, mask=mask)
+        return out["losses"]
+
+    def _fused_forward(self, eng, x, mask, aug_scaling, target, reg_target, prop_type, fg_per_video, comp_group, props_per_video,
+                       ohem_ratio, comp_w, reg_w, global_videos, loss_scale):
+        """backbone forward -> global pool (+ dropout mask) + STPP -> heads + losses (+ the head gradients, into the
+        returned dict): the forward half that fused_step and fused_eval share"""
+        from ssn_b200.engine import _stream
+        dev, F_, D = x.device, x.shape[0], 1024
+        n = F_ // self.num_segments
+        feat = torch.empty(F_, D, dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            check(lib.ssnb_backbone_fwd(eng.h, x.data_ptr(), feat.data_ptr(), _stream()), eng.h, "backbone_fwd")
+            lo, hi, nm, col = self.stpp.part_table(self._seg_split())
+            course = torch.empty(n, D, dtype=torch.float32, device=dev)
+            stpp = torch.empty(n, len(lo) * D, dtype=torch.float32, device=dev)
+            sc = aug_scaling.contiguous().float().view(-1, 2)
+            check(lib.ssnb_gpool_stpp_fwd(eng.h, None if mask is None else mask.data_ptr(), sc.data_ptr(),
+                                          self.num_segments, len(lo), _lib.int_array(lo), _lib.int_array(hi),
+                                          _lib.int_array(nm), _lib.int_array(col), self.starting_segment,
+                                          self.starting_segment + self.course_segment, feat.data_ptr(),
+                                          course.data_ptr(), stpp.data_ptr(), _stream()), eng.h, "gpool_stpp_fwd")
+        out = heads_loss_fused(course, stpp, self.activity_fc, self.completeness_fc, self.regressor_fc, prop_type,
+                               target, reg_target, self.num_class, self.stpp.feat_multiplier, fg_per_video, comp_group,
+                               props_per_video, ohem_ratio, comp_w, reg_w, global_videos, loss_scale)
+        return out, feat, course, stpp, sc, (lo, hi, nm, col)
+
+    def fused_eval(self, input, aug_scaling, target, reg_target, prop_type, fg_per_video=1, comp_group=7, props_per_video=8,
+                   ohem_ratio=0.17, comp_w=0.1, reg_w=0.1, meters=None):
+        """The body of validate() (ssn_train.py:278-364): the forward of a forward-only engine, global pool + STPP, the
+        heads and the three criteria, without a backward.  The model must be in eval() (ssn_train.py:289): no dropout, no
+        running-statistic update; no .grad changes.  Returns losses[4] = (act, comp, reg, total) on the device, what
+        fused_step's forward half computes from the same features; meters (StepMeters('ssn')) gets the step's losses and
+        accuracies.  Keeps feat, course, stpp and raw_act in self.last_eval."""
+        self._require_trainable_backbone()
+        assert self.with_regression, "fused_eval implements the regression configuration"
+        if self.training:
+            raise RuntimeError("fused_eval runs validate()'s forward: call model.eval() first (ssn_train.py:289)")
+        if not input.is_cuda:
+            raise RuntimeError("SSN(H100).fused_eval needs CUDA tensors (libssn_b200 has no CPU path)")
+        frames = self._frames(input)
+        eng = self.base_model.engine_for(frames.shape[0], False, frames.device)
+        if eng.frames != frames.shape[0]:
+            raise ValueError("fused_eval pools the engine's whole plan: %d frames with %d reserved by reserve_frames(); "
+                             "call reserve_frames(None) or pass the reserved count" % (frames.shape[0], eng.frames))
+        out, feat, course, stpp, _sc, _t = self._fused_forward(
+            eng, frames.contiguous().float(), None, aug_scaling, target, reg_target, prop_type, fg_per_video, comp_group,
+            props_per_video, ohem_ratio, comp_w, reg_w, None, 1.0)
+        if meters is not None:
+            meters.update_ssn(out["losses"], out["raw_act"], target, prop_type, input.size(0))
+        self.last_eval = dict(feat=feat, course=course, stpp=stpp, raw_act=out["raw_act"])
         return out["losses"]

@@ -677,6 +677,53 @@ int ssnb_iv3_run_op(ssnb_iv3_handle h, int op, float* feat, void* stream);
 int ssnb_sgd_step_groups(float* param, const float* grad, float* momentum_buf, size_t n, const int64_t* seg_end,
                          const float* seg_lr, const float* seg_wd, int n_seg, float momentum, float grad_mult, void* stream);
 
+/* ---- the rest of the training step between loss.backward() and optimizer.step(), and the loop's meters ----
+ * All four calls are graph-capturable: they neither synchronise the host nor allocate, and every argument is checked
+ * before any launch (SSNB_EINVAL).
+ *
+ * Extra gradients: tensors model.parameters() holds but no optimiser group does, so the flat buffers do not either (the
+ * first BatchNorm2d's weight and bias under bn_mode='partial': get_optim_policies leaves them out, ssn_models.py:203-251,
+ * while clip_grad_norm(model.parameters()) counts and scales them).  The struct is read on the host during the call. */
+enum { SSNB_GRAD_NORM_CTAS = 512, SSNB_MAX_EXTRA_GRADS = 8 };
+typedef struct {
+  int32_t count;                        /* 0 .. SSNB_MAX_EXTRA_GRADS */
+  int32_t reserved;
+  float* grad[SSNB_MAX_EXTRA_GRADS];    /* device fp32, may be NULL where numel is 0 */
+  int64_t numel[SSNB_MAX_EXTRA_GRADS];
+} ssnb_extra_grads;
+/* the total L2 norm of clip_grad_norm(model.parameters(), clip) (ssn_train.py:245-250, binary_train.py:192-197) after the
+ * iter_size division (ssn_train.py:238-243, binary_train.py:185-190): norm = sqrt(sum (grad[i]*grad_mult)^2 + sum extra^2)
+ * into the device fp32 scalar *norm.  The extras are not divided (the reference divides the optimiser groups only).  Two
+ * deterministic stages: fp64 partials of a fixed grid of SSNB_GRAD_NORM_CTAS CTAs (independent of the SM count) into
+ * `partials` (SSNB_GRAD_NORM_CTAS doubles of device scratch), then one CTA adds them in a fixed order.  Bitwise repeatable,
+ * and identical on every rank given identical gradients; a NaN or inf gradient gives a NaN or inf norm.  extra may be NULL. */
+int ssnb_grad_norm(const float* grad, size_t n, float grad_mult, const ssnb_extra_grads* extra, double* partials, float* norm,
+                   void* stream);
+/* the scaling half of clip_grad_norm (torch 0.3): c = max_norm / (*norm + 1e-6) in fp64; where c < 1 every gradient of the
+ * flat buffer (n elements, may be 0) and of the extras is multiplied by (float)c in place, else nothing changes (a NaN
+ * norm gives a NaN c, which is not < 1: no clipping, as in the reference).  *norm is read on the device. */
+int ssnb_grad_clip(const float* norm, float max_norm, float* grad, size_t n, const ssnb_extra_grads* extra, void* stream);
+/* ssnb_sgd_step_groups with the clip folded in: the gradient is multiplied by grad_mult * (float)c where c < 1 (c as in
+ * ssnb_grad_clip), else by grad_mult, so where no clipping happens the parameters and momentum are bitwise those of
+ * ssnb_sgd_step_groups.  write_back != 0 also stores that scaled gradient into grad and scales the extras by c (what the
+ * reference's .grad holds after the division and clip_grad_norm); write_back == 0 leaves grad and the extras untouched. */
+int ssnb_sgd_step_groups_clipped(float* param, float* grad, float* momentum_buf, size_t n, const int64_t* seg_end,
+                                 const float* seg_lr, const float* seg_wd, int n_seg, float momentum, float grad_mult,
+                                 const float* norm, float max_norm, int write_back, const ssnb_extra_grads* extra,
+                                 void* stream);
+/* the loop's AverageMeter updates of one step (ssn_train.py:213-233 with accuracy() :401-415 and AverageMeter :373-386;
+ * binary_train.py:170-180 with :288-321), from outputs already on the device.  scores [rows, cols] fp32 with targets
+ * [rows] int64: SSN's raw_act [n, K+1] of heads_loss_fused with prop_type [n] (the activity rows are those of type 0 or 2,
+ * in order: activity_out), BinaryClassifier's [n, 2] scores with prop_type NULL (every row).  meters: device fp64 (sum,
+ * count) pairs, n_losses + 3 of them: loss i gets sum += losses[i] * loss_n, count += loss_n (loss_n: out_frames.size(0));
+ * then top-1 accuracy in percent over all activity rows (n = their count m), over the even ones (fg, view(-1, 2, .)[:, 0],
+ * n = m / 2) and over the odd ones (bg, [:, 1], n = m / 2), each as the reference computes it:
+ * val = float(correct) * float(100.0 / n), sum += val * n, count += n; a meter with n = 0 is left alone.  top-1 takes the
+ * highest score, NaN above every number, and among equal scores the LOWEST class index (torch.topk leaves the order of
+ * ties unspecified).  A target outside [0, cols) is never correct.  One CTA; rows <= 65536. */
+int ssnb_train_meters(const float* scores, int rows, int cols, const int64_t* target, const int64_t* prop_type,
+                      const float* losses, int n_losses, double loss_n, double* meters, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
