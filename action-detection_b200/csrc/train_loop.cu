@@ -93,13 +93,17 @@ __device__ __forceinline__ bool beats(float a, int ia, float b, int ib) {
 }
 
 // one CTA: a warp per activity row takes its top-1 class and its rank among the activity rows (even rank: fg, odd: bg);
-// thread 0 then updates the meters in fp64 exactly as AverageMeter.update(val, n) does
+// thread 0 then updates the meters in fp64 exactly as AverageMeter.update(val, n) does.  An odd count of activity rows
+// leaves the last one without its bg partner (the reference's view(-1, 2) raises there): it counts in act_acc only, so
+// fg and bg both cover the same m / 2 pairs
 __global__ void __launch_bounds__(METER_THREADS) train_meters_kernel(const float* __restrict__ scores, int rows, int cols,
                                                                       const long long* __restrict__ target,
                                                                       const long long* __restrict__ ptype, const float* __restrict__ losses,
                                                                       int n_losses, double loss_n, double* __restrict__ meters) {
   __shared__ unsigned s_cnt[4];    // activity rows, correct over all, fg, bg
+  __shared__ unsigned s_last;      // (rank + 1) << 1 | correct, of the even-ranked activity row of the highest rank
   if (threadIdx.x < 4) s_cnt[threadIdx.x] = 0;
+  if (threadIdx.x == 0) s_last = 0;
   __syncthreads();
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   auto is_act = [&](int r) { return ptype == nullptr || ptype[r] == 0 || ptype[r] == 2; };
@@ -124,6 +128,7 @@ __global__ void __launch_bounds__(METER_THREADS) train_meters_kernel(const float
       atomicAdd(&s_cnt[0], 1u);
       atomicAdd(&s_cnt[1], ok);
       atomicAdd(&s_cnt[2 + (rank & 1)], ok);
+      if (!(rank & 1)) atomicMax(&s_last, ((unsigned)(rank + 1) << 1) | ok);
     }
   }
   __syncthreads();
@@ -133,6 +138,7 @@ __global__ void __launch_bounds__(METER_THREADS) train_meters_kernel(const float
     meters[2 * i + 1] += loss_n;
   }
   const unsigned m = s_cnt[0];
+  if (m & 1) s_cnt[2] -= s_last & 1;     // the unpaired last row (rank m - 1) leaves the fg count
   const unsigned nn[3] = {m, m / 2, m / 2};
   for (int k = 0; k < 3; ++k) {
     if (nn[k] == 0) continue;

@@ -62,7 +62,8 @@ class StepMeters:
     def update_ssn(self, losses, raw_act, target, prop_type, batch_size):
         """one SSN step: losses [4] (act, comp, reg, total) as fused_step returns them, raw_act [n, K+1] of every proposal
         (fused_step keeps it in last_fused), target and prop_type [n] (the activity rows are those of type 0 or 2), and the
-        reference's out_frames.size(0), the videos of the batch"""
+        reference's out_frames.size(0), the videos of the batch.  fg / bg accuracy pair the activity rows two by two; an
+        odd count (where the reference's view(-1, 2) raises) leaves the last one in act_acc only"""
         if self.kind != "ssn":
             raise ValueError("these are %s meters" % self.kind)
         self._update(losses, raw_act, target, prop_type, batch_size)

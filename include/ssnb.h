@@ -717,7 +717,9 @@ int ssnb_sgd_step_groups_clipped(float* param, float* grad, float* momentum_buf,
  * in order: activity_out), BinaryClassifier's [n, 2] scores with prop_type NULL (every row).  meters: device fp64 (sum,
  * count) pairs, n_losses + 3 of them: loss i gets sum += losses[i] * loss_n, count += loss_n (loss_n: out_frames.size(0));
  * then top-1 accuracy in percent over all activity rows (n = their count m), over the even ones (fg, view(-1, 2, .)[:, 0],
- * n = m / 2) and over the odd ones (bg, [:, 1], n = m / 2), each as the reference computes it:
+ * n = m / 2) and over the odd ones (bg, [:, 1], n = m / 2), each as the reference computes it.  An odd m (the reference's
+ * view(-1, 2) raises) leaves the last activity row unpaired: it counts in the accuracy over all rows only, and fg and bg
+ * cover the first m - 1 rows:
  * val = float(correct) * float(100.0 / n), sum += val * n, count += n; a meter with n = 0 is left alone.  top-1 takes the
  * highest score, NaN above every number, and among equal scores the LOWEST class index (torch.topk leaves the order of
  * ties unspecified).  A target outside [0, cols) is never correct.  One CTA; rows <= 65536. */
