@@ -154,6 +154,9 @@ SIGNATURES = {
     "ssnb_detection_ap_workspace_bytes": (_sz, [_i, _i, C.c_int64, C.c_int64, _i]),
     "ssnb_detection_ap": (_i, [_vp, _vp, _vp, _i, _i, C.c_int64, _vp, _vp, _vp, C.c_int64, C.POINTER(C.c_double), _i, _vp, _vp, _vp,
                                _vp, _sz, _vp]),
+    "ssnb_detection_ap_rows_workspace_bytes": (_sz, [C.c_int64, _i, _i, C.c_int64, _i]),
+    "ssnb_detection_ap_rows": (_i, [_vp, _vp, _vp, _vp, C.c_int64, _i, _i, _vp, _vp, _vp, C.c_int64, C.POINTER(C.c_double), _i, _vp, _vp,
+                                    _vp, _vp, _sz, _vp]),
     "ssnb_tag_proposals_workspace_bytes": (_sz, [_i, C.c_int64, _i, _i]),
     "ssnb_tag_proposals": (_i, [C.POINTER(TagProposalsCfg), _vp, _i, C.POINTER(C.c_int64), _vp, _i, _vp] + [_vp] * 10
                            + [_sz, _vp]),

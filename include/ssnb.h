@@ -306,6 +306,28 @@ int ssnb_detection_ap(const float* dets, const int32_t* counts, const int64_t* d
                       const int64_t* gt_offsets, const int32_t* gt_cls, const double* gt_seg, int64_t n_gt, const double* thresholds,
                       int n_thresholds, double* ap, int32_t* rank, uint8_t* tp, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- detection AP of an ActivityNet detection results file (anet_toolkit/Evaluation/eval_detection.py:11-158 ANETdetection,
+ *      :160-235 compute_average_precision_detection, utils.py:14-51 interpolated_prec_rec / segment_iou), every class and tIoU
+ *      threshold in one call --
+ * Predictions: `rows` rows in file order, video int32, label int32 (the class), seg double [rows, 2] (t0, t1), score double;
+ * a row whose video is outside [0, V) or whose label is outside [0, K) is in no class: ignored (not ranked, no trace).
+ * Ground truth: packed per video as for ssnb_detection_ap (gt_offsets device int64 [V+1], gt_cls int32, gt_seg double
+ * [n_gt, 2]; rows gt_offsets[V] .. n_gt-1 count in npos only); a video with no ground truth of the row's class makes the row a
+ * false positive at every threshold.  The rules of ssnb_detection_ap, in double: per class, rows ranked by descending double
+ * score (NaN first, -0 equal to +0, equal scores the later file row first: argsort(kind="stable")[::-1]); each matched in its
+ * own video and class to the unlocked ground truth of the highest double tIoU not below the threshold (NaN tIoU first; equal
+ * tIoU the larger ground-truth index first; segment_iou rounded operation by operation, as numpy computes it); ap by
+ * interpolated_prec_rec.  No ground truth and >= 1 row: NaN; no row: 0.  thresholds: host double [n_thr], 1..64, not NaN.
+ * ap: device double [K, n_thr].  Optional traces: rank [rows] int32 (a row's position in its class's ranking), tp [n_thr,
+ * rows] uint8 (1 = true positive), both written at ranked rows only.  Kernels only (graph-capturable): no host
+ * synchronisation, allocation or host copy, and no cap on the rows of a video or a class.  rows <= INT_MAX - 1,
+ * n_gt <= INT_MAX, 1 <= K <= 1024, K * V < INT_MAX; anything else returns SSNB_EINVAL before any launch. */
+size_t ssnb_detection_ap_rows_workspace_bytes(int64_t rows, int n_videos, int num_class, int64_t n_gt, int n_thresholds);
+int ssnb_detection_ap_rows(const int32_t* video, const int32_t* label, const double* seg, const double* score, int64_t rows, int n_videos,
+                           int num_class, const int64_t* gt_offsets, const int32_t* gt_cls, const double* gt_seg, int64_t n_gt,
+                           const double* thresholds, int n_thresholds, double* ap, int32_t* rank, uint8_t* tp, void* workspace,
+                           size_t workspace_bytes, void* stream);
+
 /* ---- TAG bottom-up proposals of many videos (gen_bottom_up_proposals.py:116-142, ops/sequence_funcs.py:11-34,71-136) ----
  * Per video v with T_v = offsets[v+1] - offsets[v] ticks of the merged crop-mean score f_score [T_v, num_cols] (rows
  * offsets[v] .. offsets[v+1]-1 of one packed fp32 [offsets[V], num_cols] array): softmax (ops/metrics.py:8-11), column
