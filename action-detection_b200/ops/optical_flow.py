@@ -1,0 +1,134 @@
+"""TV-L1 optical flow on the GPU: the Flow stream's x / y planes from RGB frames, many frame pairs per call (csrc/optical_flow.cu).
+
+The reference README ("Extract Frames and Optical Flow Images") makes these planes with DenseFlow, which runs OpenCV's CUDA
+OpticalFlowDual_TVL1 on one frame pair at a time and writes flow_{x,y}_%05d.jpg.  Here the same solver, with the rules
+oracle/tvl1_oracle.py writes down, runs on all pairs of many videos in one call:
+
+    frames = decode_jpeg(byte_groups, mode='RGB')               # uint8 [n, H, W, 3] per video, one size for all
+    flow = tvl1_flow(torch.cat(frames), offsets)                # fp32 [P, 2, H, W], pair k of a video = (frame k, frame k + 1)
+    planes = flow_planes(flow)                                  # uint8 [2P, H, W, 1]: x, y, x, y, ... as JpegBytesLoader keeps them
+    x = model.frame_transforms().oversample(planes[2 * k:2 * k + 2 * model.new_length])   # a Flow tick, as from decoded JPEGs
+    write_flow_jpegs(planes, video_dirs, offsets=offsets)      # or the files SSNDataSet reads
+
+No CPU path: the frames must be CUDA tensors.  Parity with a built DenseFlow or OpenCV CUDA is not checked by this project.
+"""
+import ctypes as C
+import os
+
+import numpy as np
+import torch
+
+from ssn_b200._lib import lib, check, TVL1Params
+
+DEFAULTS = dict(tau=0.25, lambda_=0.15, theta=0.3, nscales=5, warps=5, epsilon=0.01, iterations=300, scale_step=0.8, gamma=0.0,
+                fixed_iterations=False)
+
+
+def tvl1_params(**params):
+    """-> TVL1Params with OpenCV's defaults; 'lambda' may be given as lambda_ or as **{'lambda': ...}"""
+    if "lambda" in params:
+        params["lambda_"] = params.pop("lambda")
+    unknown = set(params) - set(DEFAULTS)
+    if unknown:
+        raise TypeError("unknown TV-L1 parameter(s): %s" % sorted(unknown))
+    q = dict(DEFAULTS, **params)
+    return TVL1Params(float(q["tau"]), float(q["lambda_"]), float(q["theta"]), float(q["epsilon"]), float(q["scale_step"]),
+                      float(q["gamma"]), int(q["nscales"]), int(q["warps"]), int(q["iterations"]), int(bool(q["fixed_iterations"])))
+
+
+def _stream():
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def pair_offsets(offsets):
+    """frame offsets [V + 1] -> pair offsets [V + 1]: video v's pairs are rows pairs[v] .. pairs[v + 1] - 1 of the flow"""
+    off = np.asarray(offsets, np.int64)
+    return off - np.arange(len(off), dtype=np.int64)
+
+
+class TVL1Plan:
+    """One call's shapes, parameters and workspace, so the solver can be run again (or captured in a CUDA graph) on new frames
+    of the same layout: plan.run(frames) writes plan.flow and plan.iterations."""
+
+    def __init__(self, offsets, height, width, device, **params):
+        self.prm = tvl1_params(**params)
+        self.offsets = np.ascontiguousarray(np.asarray(offsets, np.int64))
+        self.V, self.H, self.W = len(self.offsets) - 1, int(height), int(width)
+        self._off = self.offsets.ctypes.data_as(C.POINTER(C.c_int64))
+        ws = lib.ssnb_tvl1_workspace_bytes(self.prm, self._off, self.V, self.H, self.W)
+        if ws == 0:
+            check(lib.ssnb_tvl1_flow(self.prm, None, self._off, None, self.V, self.H, self.W, None, None, None, 0, None), None, "tvl1_flow")
+        self.levels = lib.ssnb_tvl1_levels(self.prm, self.H, self.W)
+        self.P = int(self.offsets[-1]) - self.V
+        dev = torch.device(device)
+        self.workspace = torch.empty(ws, dtype=torch.uint8, device=dev)
+        self.offsets_dev = torch.from_numpy(self.offsets).to(dev)
+        self.flow = torch.empty(self.P, 2, self.H, self.W, dtype=torch.float32, device=dev)
+        self.iterations = torch.empty(self.P, self.levels, self.prm.warps, dtype=torch.int32, device=dev)
+
+    def run(self, frames):
+        if not (torch.is_tensor(frames) and frames.is_cuda and frames.dtype == torch.uint8):
+            raise RuntimeError("tvl1_flow needs CUDA uint8 RGB frames [n, H, W, 3] (no CPU path)")
+        if tuple(frames.shape) != (int(self.offsets[-1]), self.H, self.W, 3):
+            raise ValueError("frames must be [%d, %d, %d, 3], got %s" % (int(self.offsets[-1]), self.H, self.W, tuple(frames.shape)))
+        frames = frames.contiguous()
+        with torch.cuda.device(self.flow.device):
+            check(lib.ssnb_tvl1_flow(self.prm, frames.data_ptr(), self._off, self.offsets_dev.data_ptr(), self.V, self.H, self.W,
+                                     self.flow.data_ptr(), self.iterations.data_ptr(), self.workspace.data_ptr(), self.workspace.numel(),
+                                     _stream()), None, "tvl1_flow")
+        return self.flow
+
+
+def tvl1_flow(frames, offsets=None, return_iterations=False, **params):
+    """uint8 RGB frames [sum N, H, W, 3] on the GPU (decode_jpeg's output, concatenated), frame offsets [V + 1] (default: one
+    video) -> fp32 flow [sum (N - 1), 2, H, W] on the device: pair k of video v is (frame k, frame k + 1), u then v in pixels.
+    params: tau, lambda (or lambda_), theta, nscales, warps, epsilon, iterations, scale_step, gamma, fixed_iterations, OpenCV's
+    defaults.  return_iterations: also the int32 [P, levels, warps] iterations each warp ran (level 0 the finest)."""
+    if not (torch.is_tensor(frames) and frames.is_cuda):
+        raise RuntimeError("tvl1_flow needs CUDA uint8 RGB frames [n, H, W, 3] (no CPU path)")
+    if frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError("frames must be uint8 [n, H, W, 3]")
+    if offsets is None:
+        offsets = [0, frames.shape[0]]
+    plan = TVL1Plan(offsets, frames.shape[1], frames.shape[2], frames.device, **params)
+    flow = plan.run(frames)
+    return (flow, plan.iterations) if return_iterations else flow
+
+
+def flow_planes(flow, bound=20.0):
+    """fp32 flow [P, 2, H, W] on the GPU -> uint8 planes [2P, H, W, 1] (x, y, x, y, ...), DenseFlow's convertFlowToImage with
+    this bound: what decode_jpeg(..., mode='L') returns for its flow_x / flow_y files, before the JPEG round trip."""
+    if not (torch.is_tensor(flow) and flow.is_cuda and flow.dtype == torch.float32):
+        raise RuntimeError("flow_planes needs a CUDA fp32 flow [P, 2, H, W]")
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise ValueError("flow must be [P, 2, H, W]")
+    flow = flow.contiguous()
+    P, _, H, W = flow.shape
+    out = torch.empty(2 * P, H, W, 1, dtype=torch.uint8, device=flow.device)
+    with torch.cuda.device(flow.device):
+        check(lib.ssnb_flow_planes(flow.data_ptr(), P, H, W, float(bound), out.data_ptr(), _stream()), None, "flow_planes")
+    return out
+
+
+def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
+    """Write flow_planes' output as DenseFlow does, one directory per video: {prefix}x_{:05d}.jpg and {prefix}y_{:05d}.jpg
+    numbered from 1 like img_{:05d}.jpg, through Pillow on the host.  dirs: one directory, or one per video with the frame
+    offsets the flow was computed with.  -> the paths written, x then y per pair."""
+    from PIL import Image
+    if isinstance(dirs, (str, os.PathLike)):
+        dirs = [dirs]
+    arr = planes.cpu().numpy() if torch.is_tensor(planes) else np.asarray(planes)
+    if arr.dtype != np.uint8 or arr.ndim != 4 or arr.shape[3] != 1 or arr.shape[0] % 2:
+        raise ValueError("planes must be uint8 [2P, H, W, 1]")
+    pairs = pair_offsets(offsets if offsets is not None else [0, arr.shape[0] // 2 + 1])
+    if len(pairs) != len(dirs) + 1 or pairs[-1] != arr.shape[0] // 2:
+        raise ValueError("one directory per video, and offsets that match the planes' %d pairs" % (arr.shape[0] // 2))
+    paths = []
+    for v, d in enumerate(dirs):
+        os.makedirs(d, exist_ok=True)
+        for k in range(int(pairs[v + 1] - pairs[v])):
+            for c, axis in enumerate("xy"):
+                path = os.path.join(d, "%s%s_%05d.jpg" % (prefix, axis, k + 1))
+                Image.fromarray(arr[2 * (pairs[v] + k) + c, :, :, 0]).save(path, quality=quality)
+                paths.append(path)
+    return paths

@@ -91,6 +91,13 @@ class ExtraGrads(C.Structure):
                 ("numel", C.c_int64 * MAX_EXTRA_GRADS)]
 
 
+class TVL1Params(C.Structure):
+    _fields_ = [("tau", C.c_double), ("lambda", C.c_double), ("theta", C.c_double), ("epsilon", C.c_double), ("scale_step", C.c_double),
+                ("gamma", C.c_double), ("nscales", C.c_int32), ("warps", C.c_int32), ("iterations", C.c_int32), ("fixed_iterations", C.c_int32)]
+
+
+TVL1_GREY, TVL1_RESIZE, TVL1_GRADIENT, TVL1_WARP, TVL1_PRIMAL, TVL1_DUAL = 0, 1, 2, 3, 4, 5
+
 PROPFRAMES_SECONDS, PROPFRAMES_NORMALISED, PROPFRAMES_AS_GIVEN = 0, 1, 2
 TAG_FG, TAG_INCOMPLETE, TAG_BACKGROUND = 1, 2, 4
 
@@ -207,6 +214,11 @@ SIGNATURES = {
     "ssnb_grad_clip": (_i, [_vp, _f, _vp, _sz, C.POINTER(ExtraGrads), _vp]),
     "ssnb_sgd_step_groups_clipped": (_i, [_vp, _vp, _vp, _sz, _vp, _vp, _vp, _i, _f, _f, _vp, _f, _i, C.POINTER(ExtraGrads), _vp]),
     "ssnb_train_meters": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, C.c_double, _vp, _vp]),
+    "ssnb_tvl1_levels": (_i, [C.POINTER(TVL1Params), _i, _i]),
+    "ssnb_tvl1_workspace_bytes": (_sz, [C.POINTER(TVL1Params), C.POINTER(C.c_int64), _i, _i, _i]),
+    "ssnb_tvl1_flow": (_i, [C.POINTER(TVL1Params), _vp, C.POINTER(C.c_int64), _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
+    "ssnb_tvl1_stage": (_i, [_i, C.POINTER(TVL1Params), _i, _i, _i, _i, _i, C.c_double, _pp, _pp, _vp]),
+    "ssnb_flow_planes": (_i, [_vp, C.c_int64, _i, _i, C.c_double, _vp, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

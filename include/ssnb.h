@@ -748,6 +748,45 @@ int ssnb_sgd_step_groups_clipped(float* param, float* grad, float* momentum_buf,
 int ssnb_train_meters(const float* scores, int rows, int cols, const int64_t* target, const int64_t* prop_type,
                       const float* losses, int n_losses, double loss_n, double* meters, void* stream);
 
+/* ---- TV-L1 optical flow (csrc/optical_flow.cu): the Flow stream's x / y planes from RGB frames.  Outside the reference's
+ * code: its README ("Extract Frames and Optical Flow Images") computes them with DenseFlow, which runs OpenCV's CUDA
+ * OpticalFlowDual_TVL1 one frame pair at a time.  This is that solver for many pairs per call, with the rules
+ * oracle/tvl1_oracle.py writes down (grey conversion, bilinear pyramid, bicubic warp, replicated borders, stopping rule).
+ * The defaults are OpenCV's: tau 0.25, lambda 0.15, theta 0.3, nscales 5, warps 5, epsilon 0.01, iterations 300,
+ * scale_step 0.8, gamma 0 (gamma != 0, the illumination term, is refused).  fixed_iterations != 0 runs every warp for
+ * `iterations` iterations; otherwise a warp of a pair stops after the first iteration whose summed squared primal update is
+ * <= epsilon^2 * level area (summed on the device in a fixed order; pairs that stopped launch CTAs that return at once). */
+typedef struct {
+  double tau, lambda, theta, epsilon, scale_step, gamma;
+  int32_t nscales, warps, iterations, fixed_iterations;
+} ssnb_tvl1_params;
+/* Pyramid levels of an height x width frame (level l + 1 = cvRound(level l * scale_step) per axis, stopping before the
+ * first level under 16 pixels on a side and after nscales); 0 for bad parameters or sizes. */
+int ssnb_tvl1_levels(const ssnb_tvl1_params* prm, int height, int width);
+/* Frames: uint8 RGB [offsets[n_videos], height, width, 3] (device), video v owning frames offsets[v] .. offsets[v+1]-1
+ * (each video at least one frame).  Pair k of video v is (frame k, frame k + 1): P = offsets[n_videos] - n_videos pairs,
+ * 1 <= P <= 32767 and at most 65535 frames.  offsets is the host copy (validation and launch shapes), offsets_dev the same values on the device.
+ * flow fp32 [P, 2, height, width] (u then v, in pixels); iterations (optional, NULL: not written) int32
+ * [P, levels, warps], level 0 the finest.  Nothing synchronises with the host and nothing is allocated, so the call can be
+ * captured in a CUDA graph; every launch covers all pairs, and a pair's result does not depend on the other pairs.
+ * Bad arguments return SSNB_EINVAL before any launch, and the workspace query returns 0 for them. */
+size_t ssnb_tvl1_workspace_bytes(const ssnb_tvl1_params* prm, const int64_t* offsets, int n_videos, int height, int width);
+int ssnb_tvl1_flow(const ssnb_tvl1_params* prm, const uint8_t* frames, const int64_t* offsets, const int64_t* offsets_dev, int n_videos,
+                   int height, int width, float* flow, int32_t* iterations, void* workspace, size_t workspace_bytes, void* stream);
+/* One stage of the solver on caller-given operands (n pairs or planes of height x width, fp32 unless stated), for tests:
+ *   GREY      in[0] uint8 RGB [n, h, w, 3]                                  -> out[0] [n, h, w]
+ *   RESIZE    in[0] [n, h, w]                                               -> out[0] [n, out_height, out_width], times mul
+ *   GRADIENT  in[0] I1 [n, h, w]                                            -> out[0] Ix, out[1] Iy
+ *   WARP      in[0] I0, in[1] I1, in[2] Ix, in[3] Iy, in[4] u [n, 2, h, w]  -> out[0] Ixw, out[1] Iyw, out[2] grad, out[3] rho_c
+ *   PRIMAL    in[0..3] Ixw, Iyw, grad, rho_c, in[4] p [n, 4, h, w], in[5] u -> out[0] u [n, 2, h, w]
+ *   DUAL      in[0] u [n, 2, h, w], in[1] p [n, 4, h, w]                    -> out[0] p [n, 4, h, w] */
+enum { SSNB_TVL1_GREY = 0, SSNB_TVL1_RESIZE = 1, SSNB_TVL1_GRADIENT = 2, SSNB_TVL1_WARP = 3, SSNB_TVL1_PRIMAL = 4, SSNB_TVL1_DUAL = 5 };
+int ssnb_tvl1_stage(int stage, const ssnb_tvl1_params* prm, int n, int height, int width, int out_height, int out_width, double mul,
+                    const void* const* in, void* const* out, void* stream);
+/* DenseFlow's convertFlowToImage: fp32 flow [pairs, 2, height, width] -> uint8 planes [2 pairs, height, width] (x, y, x, y, ...):
+ * v < -bound (or NaN) -> 0, v > bound -> 255, else cvRound(255 (v + bound) / (2 bound)) in double, half to even.  bound > 0. */
+int ssnb_flow_planes(const float* flow, int64_t pairs, int height, int width, double bound, uint8_t* planes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
