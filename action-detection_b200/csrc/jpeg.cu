@@ -27,6 +27,7 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
+#include "jpeg_common.cuh"
 
 namespace ssnb {
 namespace {
@@ -115,10 +116,6 @@ __device__ __forceinline__ int huff_decode(BitReader& br, const DevHuff* __restr
 }
 
 __device__ __forceinline__ int extend(int v, int s) { return v < (1 << (s - 1)) ? v + 1 - (1 << s) : v; }
-
-__constant__ uint8_t c_natural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
-                                      41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
-                                      30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
 __device__ __forceinline__ void zero_block(int16_t* blk) {
   int4* q = reinterpret_cast<int4*>(blk);
@@ -266,8 +263,6 @@ __global__ void __launch_bounds__(128) jpeg_idct_kernel(Tables t, int n_planes, 
 
 // ------------------------------------------------------------------------------------------------- upsample, colour, store
 
-__host__ __device__ constexpr int fix16(double x) { return (int)(x * 65536.0 + 0.5); }
-
 __device__ __forceinline__ int chroma(const uint8_t* __restrict__ p, int stride, int dw, int dh, int hs, int vs, int x, int y) {
   if (hs == 1) return p[(int64_t)y * stride + x];
   const int j = x >> 1, odd = x & 1;
@@ -340,10 +335,6 @@ struct Parsed {
   HuffSpec dc[4], ac[4];
   int64_t scan = 0;                // offset of the entropy-coded segment within the image
 };
-
-const uint8_t kNatural[64] = {0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
-                              41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
-                              30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63};
 
 const char* refused_sof(int m) {
   switch (m) {

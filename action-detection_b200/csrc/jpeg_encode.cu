@@ -1,0 +1,666 @@
+// JPEG encode on the GPU, byte for byte Image.save(f, quality=q) through libjpeg-turbo (and cv2.imencode at the same quality):
+// the img_%05d.jpg / flow_{x,y}_%05d.jpg files of DenseFlow's extraction step, many ragged images per call.  The stages are
+// those of oracle/jpeg_encode_oracle.py, which names the libjpeg-turbo function each one follows.  Device, in launch order:
+//
+//   enc_setup_kernel    one CTA: each image's MCU, bit-buffer word, chunk and output-slot offsets (exclusive scans of sizes
+//                       the host computes the same way, so the call needs no host round trip).
+//   enc_coef_kernel     one thread per 8x8 block (a warp per block position of the MCU, 32 MCUs per CTA): samples with edge
+//                       expansion, rgb_ycc_convert and h2v2 downsampling, islow FDCT, rounded quantisation, stored in zig-zag
+//                       order; and the bits of the block's AC codes.  Dummy blocks (past the luma plane's right / bottom edge
+//                       inside the last MCU) are zero with an EOB.
+//   enc_scan_kernel     one CTA per image: each block's bit length (its AC bits plus its DC difference's code), an exclusive
+//                       scan into bit offsets, the image's byte count; zeroes the image's bit buffer and sets the 1-bit padding.
+//   enc_pack_kernel     one thread per block: Huffman codes ORed into the bit buffer (32-bit words, most significant bit first).
+//   enc_count_kernel    one CTA per 4 KB chunk of an image's bytes: its 0xFF bytes.
+//   enc_finish_kernel   one CTA per image: an exclusive scan of the chunk counts into stuffing offsets, the header (with the
+//                       image's size in SOF0), EOI and the file's length.
+//   enc_scatter_kernel  one CTA per chunk: the bytes at their stuffed positions, 0x00 after every 0xFF.
+//
+// Grids are sized for each image's worst case (known from its size); CTAs past an image's actual bytes return at once.
+#include <cub/block/block_reduce.cuh>
+#include <cub/block/block_scan.cuh>
+
+#include <algorithm>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "../../include/ssnb.h"
+#include "common.cuh"
+#include "jpeg_common.cuh"
+
+namespace ssnb {
+namespace {
+
+constexpr int kMaxSide = 65500;                  // libjpeg's JPEG_MAX_DIMENSION
+constexpr int kMaxBlockBits = 22 + 63 * 26;      // a DC code of <= 11 bits + 11 value bits, 63 AC codes of <= 16 + 10 bits
+constexpr int kChunk = 4096, kChunkThreads = 256, kChunkBytesPerThread = kChunk / kChunkThreads;
+constexpr int kScanThreads = 1024, kMcusPerCta = 32;
+constexpr int kMaxHeader = 624;
+
+// ---------------------------------------------------------------------------------------------------------------- tables
+
+// Annex K.1, natural order
+constexpr uint8_t kStdQuant[2][64] = {
+    {16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51, 87, 80, 62,
+     18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100,
+     103, 99},
+    {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66, 99, 99, 99, 99, 99, 99,
+     99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99}};
+
+// Annex K.3: DC luminance, AC luminance, DC chrominance, AC chrominance (table t of class c is kHuff[2 t + c])
+struct HuffSpec {
+  uint8_t bits[16];
+  uint8_t vals[162];
+  int count;
+};
+constexpr HuffSpec kHuff[4] = {
+    {{0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0}, {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11}, 12},
+    {{0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7d},
+     {0x01, 0x02, 0x03, 0x00, 0x04, 0x11, 0x05, 0x12, 0x21, 0x31, 0x41, 0x06, 0x13, 0x51, 0x61, 0x07, 0x22, 0x71, 0x14, 0x32, 0x81,
+      0x91, 0xa1, 0x08, 0x23, 0x42, 0xb1, 0xc1, 0x15, 0x52, 0xd1, 0xf0, 0x24, 0x33, 0x62, 0x72, 0x82, 0x09, 0x0a, 0x16, 0x17, 0x18,
+      0x19, 0x1a, 0x25, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x34, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47, 0x48,
+      0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74, 0x75,
+      0x76, 0x77, 0x78, 0x79, 0x7a, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97, 0x98, 0x99,
+      0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba, 0xc2, 0xc3,
+      0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe1, 0xe2, 0xe3, 0xe4, 0xe5,
+      0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf1, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+     162},
+    {{0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0}, {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11}, 12},
+    {{0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77},
+     {0x00, 0x01, 0x02, 0x03, 0x11, 0x04, 0x05, 0x21, 0x31, 0x06, 0x12, 0x41, 0x51, 0x07, 0x61, 0x71, 0x13, 0x22, 0x32, 0x81, 0x08,
+      0x14, 0x42, 0x91, 0xa1, 0xb1, 0xc1, 0x09, 0x23, 0x33, 0x52, 0xf0, 0x15, 0x62, 0x72, 0xd1, 0x0a, 0x16, 0x24, 0x34, 0xe1, 0x25,
+      0xf1, 0x17, 0x18, 0x19, 0x1a, 0x26, 0x27, 0x28, 0x29, 0x2a, 0x35, 0x36, 0x37, 0x38, 0x39, 0x3a, 0x43, 0x44, 0x45, 0x46, 0x47,
+      0x48, 0x49, 0x4a, 0x53, 0x54, 0x55, 0x56, 0x57, 0x58, 0x59, 0x5a, 0x63, 0x64, 0x65, 0x66, 0x67, 0x68, 0x69, 0x6a, 0x73, 0x74,
+      0x75, 0x76, 0x77, 0x78, 0x79, 0x7a, 0x82, 0x83, 0x84, 0x85, 0x86, 0x87, 0x88, 0x89, 0x8a, 0x92, 0x93, 0x94, 0x95, 0x96, 0x97,
+      0x98, 0x99, 0x9a, 0xa2, 0xa3, 0xa4, 0xa5, 0xa6, 0xa7, 0xa8, 0xa9, 0xaa, 0xb2, 0xb3, 0xb4, 0xb5, 0xb6, 0xb7, 0xb8, 0xb9, 0xba,
+      0xc2, 0xc3, 0xc4, 0xc5, 0xc6, 0xc7, 0xc8, 0xc9, 0xca, 0xd2, 0xd3, 0xd4, 0xd5, 0xd6, 0xd7, 0xd8, 0xd9, 0xda, 0xe2, 0xe3, 0xe4,
+      0xe5, 0xe6, 0xe7, 0xe8, 0xe9, 0xea, 0xf2, 0xf3, 0xf4, 0xf5, 0xf6, 0xf7, 0xf8, 0xf9, 0xfa},
+     162}};
+
+// jchuff.c jpeg_make_c_derived_tbl: the canonical code and its length per symbol
+struct HuffEnc {
+  uint16_t code[256];
+  uint8_t size[256];
+};
+struct HuffSet {
+  HuffEnc t[4];
+};
+constexpr HuffSet make_huff() {
+  HuffSet h{};
+  for (int t = 0; t < 4; ++t) {
+    int code = 0, k = 0;
+    for (int l = 1; l <= 16; ++l) {
+      for (int i = 0; i < kHuff[t].bits[l - 1]; ++i, ++code, ++k) {
+        h.t[t].code[kHuff[t].vals[k]] = (uint16_t)code;
+        h.t[t].size[kHuff[t].vals[k]] = (uint8_t)l;
+      }
+      code <<= 1;
+    }
+  }
+  return h;
+}
+__device__ const HuffSet d_huff = make_huff();
+enum { kDC0 = 0, kAC0 = 1, kDC1 = 2, kAC1 = 3 };
+
+// the call's constants, passed by value: quantisation divisors and the header with SOF0's size left for each image
+struct EncConst {
+  int32_t div[2][64];              // quantval << 3 (the islow FDCT's output is scaled by 8), natural order
+  uint8_t header[kMaxHeader];
+  int32_t header_len, sof_size;    // sof_size: offset of SOF0's height (then width), big-endian 16-bit each
+  int32_t comps, bpm;              // components, blocks per MCU (1 or 6)
+};
+
+struct DevEnc {
+  int64_t src, out;                // the image's first byte in src, its output slot
+  int64_t mcu0, word0, chunk0;     // first MCU, bit-buffer word and byte chunk in the call's arrays
+  int64_t nbytes;                  // entropy-coded bytes before stuffing, padding included (enc_scan_kernel)
+  int32_t h, w, mcux, mcuy;
+};
+
+struct Geo {
+  int mcux, mcuy;
+  int64_t mcus, blocks, raw, words, chunks, capacity;
+};
+
+__host__ __device__ inline Geo geometry(int comps, int header_len, int h, int w) {
+  Geo g;
+  const int m = comps == 1 ? 8 : 16;
+  g.mcux = (w + m - 1) / m;
+  g.mcuy = (h + m - 1) / m;
+  g.mcus = (int64_t)g.mcux * g.mcuy;
+  g.blocks = g.mcus * (comps == 1 ? 1 : 6);
+  g.raw = (g.blocks * kMaxBlockBits + 7) / 8;
+  g.words = (g.raw + 3) / 4;
+  g.chunks = (g.raw + kChunk - 1) / kChunk;
+  g.capacity = header_len + 2 * g.raw + 2;
+  return g;
+}
+
+// ------------------------------------------------------------------------------------------------------------- setup
+
+__global__ void __launch_bounds__(kScanThreads) enc_setup_kernel(const ssnb_jpeg_encode_image* __restrict__ img, int n, int comps,
+                                                                  int header_len, DevEnc* __restrict__ t) {
+  using Scan = cub::BlockScan<long long, kScanThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  long long carry[4] = {0, 0, 0, 0};
+  for (int base = 0; base < n; base += kScanThreads) {
+    const int i = base + threadIdx.x;
+    ssnb_jpeg_encode_image e{};
+    Geo g{};
+    if (i < n) {
+      e = img[i];
+      g = geometry(comps, header_len, e.height, e.width);
+    }
+    const long long v[4] = {g.mcus, g.words, g.chunks, g.capacity};
+    long long o[4], tot[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      Scan(tmp).ExclusiveSum(v[k], o[k], tot[k]);
+      __syncthreads();
+    }
+    if (i < n) {
+      DevEnc d;
+      d.src = e.src_offset;
+      d.mcu0 = carry[0] + o[0];
+      d.word0 = carry[1] + o[1];
+      d.chunk0 = carry[2] + o[2];
+      d.out = carry[3] + o[3];
+      d.nbytes = 0;
+      d.h = e.height; d.w = e.width; d.mcux = g.mcux; d.mcuy = g.mcuy;
+      t[i] = d;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) carry[k] += tot[k];
+  }
+}
+
+// the image whose range of field F holds x (every image has at least one MCU and one chunk, so the starts increase)
+template <int64_t DevEnc::*F>
+__device__ __forceinline__ int find_image(const DevEnc* __restrict__ t, int n, int64_t x) {
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (t[mid].*F <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// ------------------------------------------------------------------------------------------------- samples, FDCT, quantise
+
+__device__ __forceinline__ int rgb_y(const uint8_t* p) {
+  return (fix16(0.29900) * p[0] + fix16(0.58700) * p[1] + fix16(0.11400) * p[2] + (1 << 15)) >> 16;
+}
+__device__ __forceinline__ int rgb_c(const uint8_t* p, int cr) {      // ONE_HALF - 1: never above 255
+  const int v = cr ? fix16(0.5) * p[0] - fix16(0.41869) * p[1] - fix16(0.08131) * p[2]
+                   : -fix16(0.16874) * p[0] - fix16(0.33126) * p[1] + fix16(0.5) * p[2];
+  return (v + (128 << 16) + (1 << 15) - 1) >> 16;
+}
+
+constexpr int CONST_BITS = 13, PASS1_BITS = 2;
+
+// one jfdctint.c pass over x[0], x[s], ... x[7 s]
+template <bool first>
+__device__ __forceinline__ void fdct8(int* x, int s) {
+  const int t0 = x[0] + x[7 * s], t7 = x[0] - x[7 * s], t1 = x[s] + x[6 * s], t6 = x[s] - x[6 * s];
+  const int t2 = x[2 * s] + x[5 * s], t5 = x[2 * s] - x[5 * s], t3 = x[3 * s] + x[4 * s], t4 = x[3 * s] - x[4 * s];
+  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
+  constexpr int sh = first ? CONST_BITS - PASS1_BITS : CONST_BITS + PASS1_BITS;
+  constexpr int r = 1 << (sh - 1);
+  if (first) {
+    x[0] = (t10 + t11) * (1 << PASS1_BITS);
+    x[4 * s] = (t10 - t11) * (1 << PASS1_BITS);
+  } else {
+    x[0] = (t10 + t11 + (1 << (PASS1_BITS - 1))) >> PASS1_BITS;
+    x[4 * s] = (t10 - t11 + (1 << (PASS1_BITS - 1))) >> PASS1_BITS;
+  }
+  int z1 = (t12 + t13) * 4433;
+  x[2 * s] = (z1 + t13 * 6270 + r) >> sh;
+  x[6 * s] = (z1 - t12 * 15137 + r) >> sh;
+  z1 = t4 + t7;
+  int z2 = t5 + t6, z3 = t4 + t6, z4 = t5 + t7;
+  const int z5 = (z3 + z4) * 9633;
+  const int a4 = t4 * 2446, a5 = t5 * 16819, a6 = t6 * 25172, a7 = t7 * 12299;
+  z1 *= -7373; z2 *= -20995; z3 = z3 * -16069 + z5; z4 = z4 * -3196 + z5;
+  x[7 * s] = (a4 + z1 + z3 + r) >> sh;
+  x[5 * s] = (a5 + z2 + z4 + r) >> sh;
+  x[3 * s] = (a6 + z2 + z3 + r) >> sh;
+  x[s] = (a7 + z1 + z4 + r) >> sh;
+}
+
+__device__ __forceinline__ int nbits(int v) { return 32 - __clz(abs(v)); }
+
+// position kb of the MCU at local index m: is it a dummy block (luma past the plane's right / bottom edge)?
+__device__ __forceinline__ bool is_dummy(const DevEnc& im, int bpm, int64_t lb) {
+  if (bpm == 1) return false;
+  const int kb = (int)(lb % 6);
+  if (kb >= 4) return false;
+  const int64_t m = lb / 6;
+  const int by = 2 * (int)(m / im.mcux) + (kb >> 1), bx = 2 * (int)(m % im.mcux) + (kb & 1);
+  return by * 8 >= im.h || bx * 8 >= im.w;
+}
+
+__global__ void __launch_bounds__(kMcusPerCta * 6) enc_coef_kernel(const DevEnc* __restrict__ t, int n, int64_t total_mcus, EncConst c,
+                                                                  const uint8_t* __restrict__ src, int16_t* __restrict__ coef,
+                                                                  int64_t* __restrict__ bits) {
+  const int64_t mcu = (int64_t)blockIdx.x * kMcusPerCta + (threadIdx.x & 31);
+  const int kb = threadIdx.x >> 5;
+  if (mcu >= total_mcus) return;
+  const DevEnc im = t[find_image<&DevEnc::mcu0>(t, n, mcu)];
+  const int64_t m = mcu - im.mcu0;
+  const int my = (int)(m / im.mcux), mx = (int)(m % im.mcux);
+  const int64_t b = mcu * c.bpm + kb;
+  const int H = im.h, W = im.w;
+  const uint8_t* __restrict__ px = src + im.src;
+  int4* dst = reinterpret_cast<int4*>(coef + b * 64);
+  int s[64];
+  const int comp = kb < 4 ? 0 : kb - 3;
+  if (c.comps == 1) {
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const uint8_t* row = px + (int64_t)min(my * 8 + r, H - 1) * W;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) s[r * 8 + q] = __ldg(row + min(mx * 8 + q, W - 1));
+    }
+  } else if (kb < 4) {
+    const int by = 2 * my + (kb >> 1), bx = 2 * mx + (kb & 1);
+    if (by * 8 >= H || bx * 8 >= W) {                   // dummy block: zero, coded as DC difference 0 and EOB
+#pragma unroll
+      for (int i = 0; i < 8; ++i) dst[i] = make_int4(0, 0, 0, 0);
+      bits[b] = d_huff.t[kAC0].size[0];
+      return;
+    }
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const uint8_t* row = px + (int64_t)min(by * 8 + r, H - 1) * W * 3;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) s[r * 8 + q] = rgb_y(row + 3 * min(bx * 8 + q, W - 1));
+    }
+  } else {                                              // h2v2: rows in pairs (the last one repeated), columns clamped
+    const int ch = (H + 1) / 2, cr = comp == 2;
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const int r0 = 2 * min(my * 8 + r, ch - 1), r1 = min(r0 + 1, H - 1);
+      const uint8_t* row0 = px + (int64_t)r0 * W * 3;
+      const uint8_t* row1 = px + (int64_t)r1 * W * 3;
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int c0 = 3 * min(2 * (mx * 8 + q), W - 1), c1 = 3 * min(2 * (mx * 8 + q) + 1, W - 1);
+        s[r * 8 + q] = (rgb_c(row0 + c0, cr) + rgb_c(row0 + c1, cr) + rgb_c(row1 + c0, cr) + rgb_c(row1 + c1, cr) + 1 + (q & 1)) >> 2;
+      }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 64; ++i) s[i] -= 128;
+#pragma unroll
+  for (int r = 0; r < 8; ++r) fdct8<true>(s + r * 8, 1);
+#pragma unroll
+  for (int q = 0; q < 8; ++q) fdct8<false>(s + q, 8);
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int d = comp ? c.div[1][i] : c.div[0][i], a = (abs(s[i]) + (d >> 1)) / d;
+    s[i] = s[i] < 0 ? -a : a;
+  }
+  constexpr NaturalOrder N = natural_order();
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    int u[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) u[j] = (int)(((uint32_t)s[N.v[8 * i + 2 * j]] & 0xFFFFu) | ((uint32_t)s[N.v[8 * i + 2 * j + 1]] << 16));
+    dst[i] = make_int4(u[0], u[1], u[2], u[3]);
+  }
+  const HuffEnc& ac = d_huff.t[comp ? kAC1 : kAC0];
+  int run = 0, total = 0;
+#pragma unroll
+  for (int k = 1; k < 64; ++k) {
+    const int v = s[N.v[k]];
+    if (v == 0) { ++run; continue; }
+    for (; run > 15; run -= 16) total += ac.size[0xF0];
+    const int nb = nbits(v);
+    total += ac.size[(run << 4) | nb] + nb;
+    run = 0;
+  }
+  if (run) total += ac.size[0];
+  bits[b] = total;
+}
+
+// ---------------------------------------------------------------------------------------------------- DC differences
+
+// the previous block of the same component in scan order (-1 before the image's first)
+__device__ __forceinline__ int64_t prev_same(int bpm, int64_t lb) {
+  if (bpm == 1) return lb - 1;
+  const int kb = (int)(lb % 6);
+  const int64_t p = kb == 0 ? lb - 3 : (kb < 4 ? lb - 1 : lb - 6);
+  return p < 0 ? -1 : p;
+}
+
+// the DC difference of block lb of an image whose blocks start at coef + b0 * 64.  A dummy block carries the DC of the block
+// before it (jccoefct.c), so its difference is 0 and the next block predicts from the last real block.
+__device__ int dc_diff(const DevEnc& im, int bpm, const int16_t* __restrict__ coef, int64_t b0, int64_t lb) {
+  if (is_dummy(im, bpm, lb)) return 0;
+  int64_t p = prev_same(bpm, lb);
+  while (p >= 0 && is_dummy(im, bpm, p)) p = prev_same(bpm, p);
+  return coef[(b0 + lb) * 64] - (p < 0 ? 0 : coef[(b0 + p) * 64]);
+}
+
+__device__ __forceinline__ bool chroma_block(int bpm, int64_t lb) { return bpm == 6 && lb % 6 >= 4; }
+
+__global__ void __launch_bounds__(kScanThreads) enc_scan_kernel(DevEnc* __restrict__ t, int bpm, const int16_t* __restrict__ coef,
+                                                                 int64_t* __restrict__ bits, uint32_t* __restrict__ words) {
+  using Scan = cub::BlockScan<long long, kScanThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  const DevEnc im = t[blockIdx.x];
+  const int64_t b0 = im.mcu0 * bpm, nb = (int64_t)im.mcux * im.mcuy * bpm;
+  long long carry = 0;
+  for (int64_t base = 0; base < nb; base += kScanThreads) {
+    const int64_t lb = base + threadIdx.x;
+    long long len = 0, off, tot;
+    if (lb < nb) {
+      const int d = dc_diff(im, bpm, coef, b0, lb), n = nbits(d);
+      len = bits[b0 + lb] + d_huff.t[chroma_block(bpm, lb) ? kDC1 : kDC0].size[n] + n;
+    }
+    Scan(tmp).ExclusiveSum(len, off, tot);
+    if (lb < nb) bits[b0 + lb] = carry + off;
+    carry += tot;
+    __syncthreads();
+  }
+  const int64_t nbytes = (carry + 7) >> 3, nwords = (nbytes + 3) >> 2;
+  uint32_t* w = words + im.word0;
+  for (int64_t j = threadIdx.x; j < nwords; j += blockDim.x) w[j] = 0;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (carry & 7) {                                    // jchuff.c flush_bits: pad the last byte with 1-bits
+      const int64_t e = nbytes * 8 - 1;
+      const int npad = (int)(e - carry + 1);
+      w[e >> 5] |= ((1u << npad) - 1) << (31 - (int)(e & 31));
+    }
+    t[blockIdx.x].nbytes = nbytes;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------ pack
+
+struct BitWriter {
+  uint32_t* w;
+  int64_t word;
+  uint64_t acc;                    // the pending bits, the last `n` of them valid
+  int n;
+
+  __device__ __forceinline__ void put(uint32_t v, int len) {          // len <= 27
+    acc = (acc << len) | v;
+    n += len;
+    if (n >= 32) {
+      n -= 32;
+      atomicOr(w + word, (uint32_t)(acc >> n));
+      ++word;
+      acc &= (1ull << n) - 1;
+    }
+  }
+  __device__ __forceinline__ void flush() {
+    if (n) atomicOr(w + word, (uint32_t)(acc << (32 - n)));
+  }
+};
+
+__global__ void __launch_bounds__(kMcusPerCta * 6) enc_pack_kernel(const DevEnc* __restrict__ t, int n, int64_t total_mcus, int bpm,
+                                                                  const int16_t* __restrict__ coef, const int64_t* __restrict__ bits,
+                                                                  uint32_t* __restrict__ words) {
+  const int64_t mcu = (int64_t)blockIdx.x * kMcusPerCta + (threadIdx.x & 31);
+  const int kb = threadIdx.x >> 5;
+  if (mcu >= total_mcus) return;
+  const DevEnc im = t[find_image<&DevEnc::mcu0>(t, n, mcu)];
+  const int64_t b0 = im.mcu0 * bpm, lb = (mcu - im.mcu0) * bpm + kb;
+  const bool chroma = kb >= 4;
+  const HuffEnc& dc = d_huff.t[chroma ? kDC1 : kDC0];
+  const HuffEnc& ac = d_huff.t[chroma ? kAC1 : kAC0];
+  const int64_t pos = bits[b0 + lb];
+  BitWriter bw{words + im.word0, pos >> 5, 0ull, (int)(pos & 31)};
+  const int d = dc_diff(im, bpm, coef, b0, lb), nd = nbits(d);
+  bw.put(((uint32_t)dc.code[nd] << nd) | ((uint32_t)(d - (d < 0)) & ((1u << nd) - 1)), dc.size[nd] + nd);
+  const int16_t* __restrict__ z = coef + (b0 + lb) * 64;
+  int run = 0;
+  for (int k = 1; k < 64; ++k) {
+    const int v = z[k];
+    if (v == 0) { ++run; continue; }
+    for (; run > 15; run -= 16) bw.put(ac.code[0xF0], ac.size[0xF0]);
+    const int nb = nbits(v), sym = (run << 4) | nb;
+    bw.put(((uint32_t)ac.code[sym] << nb) | ((uint32_t)(v - (v < 0)) & ((1u << nb) - 1)), ac.size[sym] + nb);
+    run = 0;
+  }
+  if (run) bw.put(ac.code[0], ac.size[0]);
+  bw.flush();
+}
+
+// ------------------------------------------------------------------------------------------------------------- stuffing
+
+// this thread's bytes of an image's entropy-coded data: [start, start + 16) clipped to nbytes; returns how many are 0xFF
+__device__ __forceinline__ int load_bytes(const uint32_t* __restrict__ w, int64_t start, int64_t nbytes, uint8_t (&b)[kChunkBytesPerThread]) {
+  int ff = 0;
+#pragma unroll
+  for (int q = 0; q < kChunkBytesPerThread / 4; ++q) {
+    const int64_t k = start + 4 * q;
+    const uint32_t v = k < nbytes ? w[k >> 2] : 0u;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      b[4 * q + j] = (uint8_t)(v >> (24 - 8 * j));
+      ff += (k + j < nbytes) && b[4 * q + j] == 0xFF;
+    }
+  }
+  return ff;
+}
+
+__global__ void __launch_bounds__(kChunkThreads) enc_count_kernel(const DevEnc* __restrict__ t, int n, const uint32_t* __restrict__ words,
+                                                                   int64_t* __restrict__ counts) {
+  using Reduce = cub::BlockReduce<int, kChunkThreads>;
+  __shared__ typename Reduce::TempStorage tmp;
+  const DevEnc im = t[find_image<&DevEnc::chunk0>(t, n, blockIdx.x)];
+  const int64_t first = ((int64_t)blockIdx.x - im.chunk0) * kChunk;
+  if (first >= im.nbytes) return;
+  uint8_t b[kChunkBytesPerThread];
+  const int ff = load_bytes(words + im.word0, first + threadIdx.x * kChunkBytesPerThread, im.nbytes, b);
+  const int total = Reduce(tmp).Sum(ff);
+  if (threadIdx.x == 0) counts[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kChunkThreads) enc_finish_kernel(const DevEnc* __restrict__ t, EncConst c, int64_t* __restrict__ counts,
+                                                                    uint8_t* __restrict__ out, int64_t* __restrict__ lengths) {
+  using Scan = cub::BlockScan<long long, kChunkThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  const DevEnc im = t[blockIdx.x];
+  const int64_t used = (im.nbytes + kChunk - 1) / kChunk;
+  int64_t* cc = counts + im.chunk0;
+  long long carry = 0;
+  for (int64_t base = 0; base < used; base += kChunkThreads) {
+    const int64_t j = base + threadIdx.x;
+    long long v = j < used ? cc[j] : 0, off, tot;
+    Scan(tmp).ExclusiveSum(v, off, tot);
+    if (j < used) cc[j] = carry + off;
+    carry += tot;
+    __syncthreads();
+  }
+  uint8_t* dst = out + im.out;
+  const uint8_t size[4] = {(uint8_t)(im.h >> 8), (uint8_t)im.h, (uint8_t)(im.w >> 8), (uint8_t)im.w};
+  for (int j = threadIdx.x; j < c.header_len; j += blockDim.x) {
+    const int k = j - c.sof_size;
+    dst[j] = k >= 0 && k < 4 ? size[k] : c.header[j];
+  }
+  if (threadIdx.x == 0) {
+    const int64_t e = c.header_len + im.nbytes + carry;
+    dst[e] = 0xFF;
+    dst[e + 1] = 0xD9;
+    lengths[blockIdx.x] = e + 2;
+  }
+}
+
+__global__ void __launch_bounds__(kChunkThreads) enc_scatter_kernel(const DevEnc* __restrict__ t, int n, int header_len,
+                                                                     const uint32_t* __restrict__ words, const int64_t* __restrict__ counts,
+                                                                     uint8_t* __restrict__ out) {
+  using Scan = cub::BlockScan<int, kChunkThreads>;
+  __shared__ typename Scan::TempStorage tmp;
+  const DevEnc im = t[find_image<&DevEnc::chunk0>(t, n, blockIdx.x)];
+  const int64_t first = ((int64_t)blockIdx.x - im.chunk0) * kChunk;
+  if (first >= im.nbytes) return;
+  const int64_t start = first + threadIdx.x * kChunkBytesPerThread;
+  uint8_t b[kChunkBytesPerThread];
+  const int ff = load_bytes(words + im.word0, start, im.nbytes, b);
+  int before;
+  Scan(tmp).ExclusiveSum(ff, before);
+  uint8_t* dst = out + im.out + header_len + start + counts[blockIdx.x] + before;
+#pragma unroll
+  for (int j = 0; j < kChunkBytesPerThread; ++j) {
+    if (start + j >= im.nbytes) break;
+    *dst++ = b[j];
+    if (b[j] == 0xFF) *dst++ = 0;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------- host
+
+size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+void put16(std::vector<uint8_t>& h, int v) {
+  h.push_back((uint8_t)(v >> 8));
+  h.push_back((uint8_t)v);
+}
+
+// jcparam.c jpeg_set_quality(quality, TRUE) and jcmarker.c's header (oracle/jpeg_encode_oracle.py quant_tables / header)
+EncConst make_const(int comps, int quality) {
+  EncConst c;
+  memset(&c, 0, sizeof c);
+  const int scale = quality < 50 ? 5000 / quality : 200 - 2 * quality;
+  int q[2][64];
+  for (int t = 0; t < 2; ++t)
+    for (int i = 0; i < 64; ++i) {
+      q[t][i] = std::min(std::max((kStdQuant[t][i] * scale + 50) / 100, 1), 255);
+      c.div[t][i] = q[t][i] << 3;
+    }
+  const int tables = comps == 1 ? 1 : 2;
+  std::vector<uint8_t> h = {0xFF, 0xD8, 0xFF, 0xE0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
+  for (int t = 0; t < tables; ++t) {
+    h.insert(h.end(), {0xFF, 0xDB, 0, 67, (uint8_t)t});
+    for (int k = 0; k < 64; ++k) h.push_back((uint8_t)q[t][kNatural[k]]);
+  }
+  h.insert(h.end(), {0xFF, 0xC0});
+  put16(h, 8 + 3 * comps);
+  h.push_back(8);
+  c.sof_size = (int)h.size();
+  h.insert(h.end(), {0, 0, 0, 0, (uint8_t)comps});
+  if (comps == 1) h.insert(h.end(), {1, 0x11, 0});
+  else h.insert(h.end(), {1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1});
+  for (int t = 0; t < tables; ++t)
+    for (int cls = 0; cls < 2; ++cls) {
+      const HuffSpec& s = kHuff[2 * t + cls];
+      h.insert(h.end(), {0xFF, 0xC4});
+      put16(h, 2 + 1 + 16 + s.count);
+      h.push_back((uint8_t)(cls << 4 | t));
+      h.insert(h.end(), s.bits, s.bits + 16);
+      h.insert(h.end(), s.vals, s.vals + s.count);
+    }
+  h.insert(h.end(), {0xFF, 0xDA});
+  put16(h, 6 + 2 * comps);
+  h.push_back((uint8_t)comps);
+  if (comps == 1) h.insert(h.end(), {1, 0x00});
+  else h.insert(h.end(), {1, 0x00, 2, 0x11, 3, 0x11});
+  h.insert(h.end(), {0, 63, 0});
+  memcpy(c.header, h.data(), h.size());
+  c.header_len = (int)h.size();
+  c.comps = comps;
+  c.bpm = comps == 1 ? 1 : 6;
+  return c;
+}
+
+int header_len(int comps) { return make_const(comps, 50).header_len; }
+
+struct Layout {
+  int64_t mcus = 0, blocks = 0, words = 0, chunks = 0, out_bytes = 0;
+  size_t off_coef = 0, off_bits = 0, off_words = 0, off_counts = 0, workspace = 0;
+};
+
+bool check_image_size(int h, int w) { return h >= 1 && w >= 1 && h <= kMaxSide && w <= kMaxSide; }
+
+// the call's sizes; an empty string when the arguments are acceptable, else the reason
+std::string plan(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, int64_t src_bytes, Layout& L) {
+  if (mode != SSNB_JPEG_ENC_L && mode != SSNB_JPEG_ENC_RGB) return "mode must be SSNB_JPEG_ENC_L (1) or SSNB_JPEG_ENC_RGB (3)";
+  if (quality < 1 || quality > 100) return "quality must be 1 .. 100";
+  if (n < 1 || !images) return "no image, or NULL images";
+  const int hl = header_len(mode);
+  for (int i = 0; i < n; ++i) {
+    const ssnb_jpeg_encode_image& e = images[i];
+    if (!check_image_size(e.height, e.width))
+      return "image " + std::to_string(i) + ": height and width must be 1 .. " + std::to_string(kMaxSide);
+    if (src_bytes >= 0 && (e.src_offset < 0 || e.src_offset + (int64_t)e.height * e.width * mode > src_bytes))
+      return "image " + std::to_string(i) + ": pixels outside src";
+    const Geo g = geometry(mode, hl, e.height, e.width);
+    L.mcus += g.mcus; L.blocks += g.blocks; L.words += g.words; L.chunks += g.chunks; L.out_bytes += g.capacity;
+  }
+  if ((L.mcus + kMcusPerCta - 1) / kMcusPerCta > INT32_MAX || L.chunks > INT32_MAX) return "too many blocks in one call";
+  size_t o = align256((size_t)n * sizeof(DevEnc));
+  L.off_coef = o; o = align256(o + (size_t)L.blocks * 128);
+  L.off_bits = o; o = align256(o + (size_t)L.blocks * 8);
+  L.off_words = o; o = align256(o + (size_t)L.words * 4);
+  L.off_counts = o; o = align256(o + (size_t)L.chunks * 8);
+  L.workspace = o;
+  return "";
+}
+
+}  // namespace
+}  // namespace ssnb
+
+using namespace ssnb;
+
+extern "C" {
+
+int64_t ssnb_jpeg_encode_capacity(int mode, int height, int width) {
+  if ((mode != SSNB_JPEG_ENC_L && mode != SSNB_JPEG_ENC_RGB) || !check_image_size(height, width)) return 0;
+  return geometry(mode, header_len(mode), height, width).capacity;
+}
+
+int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, size_t* workspace_bytes, int64_t* out_bytes) {
+  Layout L;
+  const std::string why = plan(mode, quality, images, n, -1, L);
+  if (!why.empty()) {
+    set_thread_error("jpeg_encode: " + why);
+    return SSNB_EINVAL;
+  }
+  if (workspace_bytes) *workspace_bytes = L.workspace;
+  if (out_bytes) *out_bytes = L.out_bytes;
+  return SSNB_OK;
+}
+
+int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
+                     const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  auto fail = [](const std::string& m) { set_thread_error("jpeg_encode: " + m); return (int)SSNB_EINVAL; };
+  Layout L;
+  const std::string why = plan(mode, quality, images, n, src_bytes, L);
+  if (!why.empty()) return fail(why);
+  if (!src || !images_dev || !out || !lengths || !workspace) return fail("NULL src, images_dev, out, lengths or workspace");
+  if ((uintptr_t)workspace % 256) return fail("workspace must be 256-byte aligned");
+  if (out_bytes < L.out_bytes) return fail("out holds fewer bytes than the images' slots (ssnb_jpeg_encode_sizes)");
+  if (workspace_bytes < L.workspace) return fail("workspace too small (ssnb_jpeg_encode_sizes)");
+  const EncConst c = make_const(mode, quality);
+  uint8_t* ws = (uint8_t*)workspace;
+  DevEnc* t = (DevEnc*)ws;
+  int16_t* coef = (int16_t*)(ws + L.off_coef);
+  int64_t* bits = (int64_t*)(ws + L.off_bits);
+  uint32_t* words = (uint32_t*)(ws + L.off_words);
+  int64_t* counts = (int64_t*)(ws + L.off_counts);
+  const unsigned mcu_ctas = (unsigned)((L.mcus + kMcusPerCta - 1) / kMcusPerCta);
+  enc_setup_kernel<<<1, kScanThreads, 0, s>>>(images_dev, n, mode, c.header_len, t);
+  SSNB_LAUNCH_CHECK("enc_setup_kernel");
+  enc_coef_kernel<<<mcu_ctas, kMcusPerCta * c.bpm, 0, s>>>(t, n, L.mcus, c, src, coef, bits);
+  SSNB_LAUNCH_CHECK("enc_coef_kernel");
+  enc_scan_kernel<<<n, kScanThreads, 0, s>>>(t, c.bpm, coef, bits, words);
+  SSNB_LAUNCH_CHECK("enc_scan_kernel");
+  enc_pack_kernel<<<mcu_ctas, kMcusPerCta * c.bpm, 0, s>>>(t, n, L.mcus, c.bpm, coef, bits, words);
+  SSNB_LAUNCH_CHECK("enc_pack_kernel");
+  enc_count_kernel<<<(unsigned)L.chunks, kChunkThreads, 0, s>>>(t, n, words, counts);
+  SSNB_LAUNCH_CHECK("enc_count_kernel");
+  enc_finish_kernel<<<n, kChunkThreads, 0, s>>>(t, c, counts, out, lengths);
+  SSNB_LAUNCH_CHECK("enc_finish_kernel");
+  enc_scatter_kernel<<<(unsigned)L.chunks, kChunkThreads, 0, s>>>(t, n, c.header_len, words, counts, out);
+  SSNB_LAUNCH_CHECK("enc_scatter_kernel");
+  return SSNB_OK;
+}
+
+}  // extern "C"

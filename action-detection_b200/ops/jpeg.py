@@ -12,6 +12,10 @@ ops.frame_transforms takes:
 Huffman-coded sequential 8-bit JPEG only (what video frame extractors write): grayscale or YCbCr at 4:4:4, 4:2:2 or 4:2:0, any
 size, with or without restart intervals.  Other streams are refused before anything runs on the GPU, with the image and the
 reason; there is no CPU fallback.
+
+encode_jpeg is the other direction, the files of the extraction step (DenseFlow's img_%05d.jpg and flow_{x,y}_%05d.jpg):
+CUDA uint8 images -> the bytes Pillow's Image.save(f, quality=q) writes, computed by csrc/jpeg_encode.cu.  JpegEncodePlan
+keeps one call's buffers so the encode can be repeated or captured in a CUDA graph.
 """
 import ctypes as C
 import os
@@ -19,7 +23,7 @@ import os
 import numpy as np
 import torch
 
-from ssn_b200._lib import lib, JpegInput, JpegImageInfo
+from ssn_b200._lib import lib, JpegInput, JpegImageInfo, JpegEncodeImage, JPEG_ENC_L, JPEG_ENC_RGB
 
 STATUS_TEXT = {1: "entropy-coded data truncated", 2: "invalid Huffman code", 3: "AC coefficient run past the end of the block",
                4: "restart marker missing or out of sequence"}
@@ -230,3 +234,117 @@ def collate_jpeg(batch):
     from torch.utils.data import default_collate
     rest = default_collate([b[1:] for b in batch])
     return [[b[0] for b in batch]] + list(rest)
+
+
+# ------------------------------------------------------------------------------------------------------------------ encode
+
+_ENC_MODES = {"L": (JPEG_ENC_L, 1), "RGB": (JPEG_ENC_RGB, 3)}
+
+
+def jpeg_encode_capacity(mode, height, width):
+    """the bytes the encoder reserves for one image's file (its worst case; 0 for a bad mode or size)"""
+    return int(lib.ssnb_jpeg_encode_capacity(_ENC_MODES[mode][0] if mode in _ENC_MODES else 0, int(height), int(width)))
+
+
+def _enc_mode(mode):
+    if mode not in _ENC_MODES:
+        raise ValueError("encode_jpeg: mode must be 'RGB' or 'L'")
+    return _ENC_MODES[mode]
+
+
+class JpegEncodePlan:
+    """One encode call's sizes, mode and quality with its device buffers: the image table, the workspace, the output slots
+    (image i's file starts at out[slots[i]]) and the int64 lengths.  plan.run(images) only enqueues, so it can be repeated
+    or captured in a CUDA graph on new pixels of the same sizes; plan.files() waits and returns one bytes object per image."""
+
+    def __init__(self, sizes, mode="RGB", quality=95, device=None):
+        self.mode, self.quality = mode, int(quality)
+        self._code, self.channels = _enc_mode(mode)
+        self.sizes = [(int(h), int(w)) for h, w in sizes]
+        n = len(self.sizes)
+        if n < 1:
+            raise ValueError("encode_jpeg: no image")
+        self.images = (JpegEncodeImage * n)()
+        off = 0
+        for e, (h, w) in zip(self.images, self.sizes):
+            e.src_offset, e.height, e.width = off, h, w
+            off += max(h, 0) * max(w, 0) * self.channels
+        self.src_bytes = off
+        ws, ob = C.c_size_t(), C.c_int64()
+        if lib.ssnb_jpeg_encode_sizes(self._code, self.quality, self.images, n, C.byref(ws), C.byref(ob)) != 0:
+            raise ValueError("encode_jpeg: " + (lib.ssnb_last_error(None) or b"").decode().split(": ", 1)[-1])
+        caps = [lib.ssnb_jpeg_encode_capacity(self._code, h, w) for h, w in self.sizes]
+        self.slots = np.concatenate([[0], np.cumsum(caps)[:-1]]).astype(np.int64)
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.images_dev = torch.frombuffer(bytearray(bytes(self.images)), dtype=torch.uint8).to(dev)
+        self.workspace = torch.empty(ws.value, dtype=torch.uint8, device=dev)
+        self.out = torch.empty(ob.value, dtype=torch.uint8, device=dev)
+        self.lengths = torch.zeros(n, dtype=torch.int64, device=dev)
+
+    def _pixels(self, images):
+        """CUDA uint8 [N, H, W, C] or a list of [H, W, C] of the plan's sizes -> one contiguous uint8 buffer"""
+        ts = [images] if torch.is_tensor(images) else list(images)
+        if not all(torch.is_tensor(t) and t.is_cuda for t in ts):
+            raise RuntimeError("encode_jpeg needs CUDA uint8 images (no CPU path)")
+        if any(t.dtype != torch.uint8 for t in ts):
+            raise ValueError("encode_jpeg: images must be uint8")
+        if torch.is_tensor(images):
+            if images.dim() != 4 or images.shape[3] != self.channels:
+                raise ValueError("encode_jpeg: images must be [N, H, W, %d] for mode %r" % (self.channels, self.mode))
+            shapes = [tuple(images.shape[1:3])] * images.shape[0]
+        else:
+            if any(t.dim() != 3 or t.shape[2] != self.channels for t in ts):
+                raise ValueError("encode_jpeg: each image must be [H, W, %d] for mode %r" % (self.channels, self.mode))
+            shapes = [tuple(t.shape[:2]) for t in ts]
+        if shapes != self.sizes:
+            raise ValueError("encode_jpeg: the images' sizes differ from the plan's")
+        if torch.is_tensor(images):
+            return images.contiguous().reshape(-1)
+        return torch.cat([t.reshape(-1) for t in ts])
+
+    def run(self, images):
+        """enqueue the encode of `images` on the current stream; returns (out, lengths) on the device"""
+        src = self._pixels(images)
+        if src.device != self.out.device:
+            raise ValueError("encode_jpeg: images on %s, plan on %s" % (src.device, self.out.device))
+        self._src = src                       # kept alive until the next run
+        with torch.cuda.device(self.out.device):
+            rc = lib.ssnb_jpeg_encode(self._code, self.quality, src.data_ptr(), src.numel(), self.images, self.images_dev.data_ptr(),
+                                      len(self.sizes), self.out.data_ptr(), self.out.numel(), self.lengths.data_ptr(),
+                                      self.workspace.data_ptr(), self.workspace.numel(), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        if rc != 0:
+            raise RuntimeError("libssn_b200 jpeg_encode failed (code %d): %s" % (rc, (lib.ssnb_last_error(None) or b"").decode()))
+        return self.out, self.lengths
+
+    def files(self):
+        """wait for the last run and return each image's file as bytes (one device-to-host copy of the files' bytes)"""
+        lens = self.lengths.cpu().numpy()
+        flat = torch.cat([self.out[int(o):int(o) + int(l)] for o, l in zip(self.slots, lens)]).cpu().numpy().tobytes()
+        ends = np.cumsum(lens)
+        return [flat[e - l:e] for e, l in zip(ends.tolist(), lens.tolist())]
+
+
+def encode_jpeg(images, mode="RGB", quality=95):
+    """Encode CUDA uint8 images on the GPU: [N, H, W, C] or a list of ragged [H, W, C], C = 3 for 'RGB' and 1 for 'L'.  Returns
+    one bytes object per image, equal to what Image.fromarray(img).save(f, format='JPEG', quality=quality) writes (Pillow over
+    libjpeg-turbo; cv2.imencode writes the same bytes): baseline, 4:2:0 for 'RGB', no optimize, no metadata.  quality 1 .. 100."""
+    if torch.is_tensor(images):
+        if not images.is_cuda:
+            raise RuntimeError("encode_jpeg needs CUDA uint8 images (no CPU path)")
+        if images.dim() != 4:
+            raise ValueError("encode_jpeg: images must be [N, H, W, C] or a list of [H, W, C]")
+        sizes, device = [tuple(images.shape[1:3])] * images.shape[0], images.device
+    else:
+        images = list(images)
+        if not images:
+            return []
+        if not all(torch.is_tensor(t) and t.is_cuda for t in images):
+            raise RuntimeError("encode_jpeg needs CUDA uint8 images (no CPU path)")
+        if any(t.dim() != 3 for t in images):
+            raise ValueError("encode_jpeg: images must be [N, H, W, C] or a list of [H, W, C]")
+        sizes, device = [tuple(t.shape[:2]) for t in images], images[0].device
+    if len(sizes) == 0:
+        return []
+    plan = JpegEncodePlan(sizes, mode, quality, device)
+    plan.run(images)
+    return plan.files()

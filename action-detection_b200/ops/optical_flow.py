@@ -8,7 +8,8 @@ oracle/tvl1_oracle.py writes down, runs on all pairs of many videos in one call:
     flow = tvl1_flow(torch.cat(frames), offsets)                # fp32 [P, 2, H, W], pair k of a video = (frame k, frame k + 1)
     planes = flow_planes(flow)                                  # uint8 [2P, H, W, 1]: x, y, x, y, ... as JpegBytesLoader keeps them
     x = model.frame_transforms().oversample(planes[2 * k:2 * k + 2 * model.new_length])   # a Flow tick, as from decoded JPEGs
-    write_flow_jpegs(planes, video_dirs, offsets=offsets)      # or the files SSNDataSet reads
+    write_flow_jpegs(planes, video_dirs, offsets=offsets)      # or the files SSNDataSet reads, encoded on the GPU
+    write_frame_jpegs(torch.cat(frames), video_dirs, offsets=offsets)   # and the RGB side, img_{:05d}.jpg
 
 No CPU path: the frames must be CUDA tensors.  Parity with a built DenseFlow or OpenCV CUDA is not checked by this project.
 """
@@ -110,25 +111,90 @@ def flow_planes(flow, bound=20.0):
     return out
 
 
-def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
-    """Write flow_planes' output as DenseFlow does, one directory per video: {prefix}x_{:05d}.jpg and {prefix}y_{:05d}.jpg
-    numbered from 1 like img_{:05d}.jpg, through Pillow on the host.  dirs: one directory, or one per video with the frame
-    offsets the flow was computed with.  -> the paths written, x then y per pair."""
-    from PIL import Image
+def _video_dirs(dirs, counts, what):
+    """one directory, or one per video whose item counts the offsets give -> a directory per video"""
     if isinstance(dirs, (str, os.PathLike)):
         dirs = [dirs]
-    arr = planes.cpu().numpy() if torch.is_tensor(planes) else np.asarray(planes)
-    if arr.dtype != np.uint8 or arr.ndim != 4 or arr.shape[3] != 1 or arr.shape[0] % 2:
-        raise ValueError("planes must be uint8 [2P, H, W, 1]")
-    pairs = pair_offsets(offsets if offsets is not None else [0, arr.shape[0] // 2 + 1])
-    if len(pairs) != len(dirs) + 1 or pairs[-1] != arr.shape[0] // 2:
-        raise ValueError("one directory per video, and offsets that match the planes' %d pairs" % (arr.shape[0] // 2))
+    dirs = list(dirs)
+    if len(dirs) != len(counts):
+        raise ValueError("one directory per video, and offsets that match the %s" % what)
+    return dirs
+
+
+def _encoded(images, mode, quality):
+    """CUDA uint8 [N, H, W, C] -> the files' bytes from the GPU encoder; anything else -> None (the Pillow path)"""
+    if torch.is_tensor(images) and images.is_cuda:
+        from ops.jpeg import encode_jpeg
+        return encode_jpeg(images, mode=mode, quality=quality)
+    return None
+
+
+def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
+    """Write flow_planes' output as DenseFlow does, one directory per video: {prefix}x_{:05d}.jpg and {prefix}y_{:05d}.jpg
+    numbered from 1 like img_{:05d}.jpg.  CUDA planes are encoded on the GPU (ops.jpeg.encode_jpeg, one call for all planes),
+    host planes through Pillow; the files are the same bytes either way.  dirs: one directory, or one per video with the
+    frame offsets the flow was computed with.  -> the paths written, x then y per pair."""
+    from PIL import Image
+    if torch.is_tensor(planes) and planes.is_cuda:
+        if planes.dtype != torch.uint8 or planes.dim() != 4 or planes.shape[3] != 1 or planes.shape[0] % 2:
+            raise ValueError("planes must be uint8 [2P, H, W, 1]")
+        n = planes.shape[0]
+    else:
+        arr = planes.cpu().numpy() if torch.is_tensor(planes) else np.asarray(planes)
+        if arr.dtype != np.uint8 or arr.ndim != 4 or arr.shape[3] != 1 or arr.shape[0] % 2:
+            raise ValueError("planes must be uint8 [2P, H, W, 1]")
+        n = arr.shape[0]
+    pairs = pair_offsets(offsets if offsets is not None else [0, n // 2 + 1])
+    if pairs[-1] != n // 2:
+        raise ValueError("one directory per video, and offsets that match the planes' %d pairs" % (n // 2))
+    dirs = _video_dirs(dirs, np.diff(pairs), "planes' %d pairs" % (n // 2))
+    files = _encoded(planes, "L", quality)
     paths = []
     for v, d in enumerate(dirs):
         os.makedirs(d, exist_ok=True)
         for k in range(int(pairs[v + 1] - pairs[v])):
             for c, axis in enumerate("xy"):
                 path = os.path.join(d, "%s%s_%05d.jpg" % (prefix, axis, k + 1))
-                Image.fromarray(arr[2 * (pairs[v] + k) + c, :, :, 0]).save(path, quality=quality)
+                i = 2 * (pairs[v] + k) + c
+                if files is not None:
+                    with open(path, "wb") as f:
+                        f.write(files[i])
+                else:
+                    Image.fromarray(arr[i, :, :, 0]).save(path, quality=quality)
                 paths.append(path)
+    return paths
+
+
+def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None):
+    """Write RGB frames as DenseFlow does, one directory per video: {prefix}{:05d}.jpg numbered from 1, the files SSNDataSet
+    reads for RGB.  frames uint8 [N, H, W, 3]: CUDA frames are encoded on the GPU in one call, host frames through Pillow,
+    the same bytes either way.  dirs: one directory, or one per video with the frame offsets [V + 1] (as tvl1_flow takes
+    them).  -> the paths written, in frame order."""
+    from PIL import Image
+    if torch.is_tensor(frames) and frames.is_cuda:
+        if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+            raise ValueError("frames must be uint8 [N, H, W, 3]")
+        n = frames.shape[0]
+    else:
+        arr = frames.cpu().numpy() if torch.is_tensor(frames) else np.asarray(frames)
+        if arr.dtype != np.uint8 or arr.ndim != 4 or arr.shape[3] != 3:
+            raise ValueError("frames must be uint8 [N, H, W, 3]")
+        n = arr.shape[0]
+    off = np.asarray(offsets if offsets is not None else [0, n], np.int64)
+    if off.ndim != 1 or len(off) < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
+        raise ValueError("one directory per video, and offsets that match the %d frames" % n)
+    dirs = _video_dirs(dirs, np.diff(off), "%d frames" % n)
+    files = _encoded(frames, "RGB", quality)
+    paths = []
+    for v, d in enumerate(dirs):
+        os.makedirs(d, exist_ok=True)
+        for k in range(int(off[v + 1] - off[v])):
+            path = os.path.join(d, "%s%05d.jpg" % (prefix, k + 1))
+            i = int(off[v]) + k
+            if files is not None:
+                with open(path, "wb") as f:
+                    f.write(files[i])
+            else:
+                Image.fromarray(arr[i]).save(path, quality=quality)
+            paths.append(path)
     return paths

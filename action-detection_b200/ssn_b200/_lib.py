@@ -77,6 +77,13 @@ class JpegImageInfo(C.Structure):
 JPEG_OK, JPEG_TRUNCATED, JPEG_BAD_CODE, JPEG_BAD_RUN, JPEG_BAD_RESTART = 0, 1, 2, 3, 4
 
 
+class JpegEncodeImage(C.Structure):
+    _fields_ = [("src_offset", C.c_int64), ("height", C.c_int32), ("width", C.c_int32)]
+
+
+JPEG_ENC_L, JPEG_ENC_RGB = 1, 3
+
+
 class ProposalTargetsCfg(C.Structure):
     _fields_ = [("fg_thresh", C.c_double), ("incomplete_iou_thresh", C.c_double), ("bg_iou_thresh", C.c_double),
                 ("bg_coverage_thresh", C.c_double), ("incomplete_overlap_thresh", C.c_double), ("exclude_empty", C.c_int32),
@@ -194,6 +201,9 @@ SIGNATURES = {
     "ssnb_jpeg_plan_image": (_i, [_vp, _i, C.POINTER(JpegImageInfo)]),
     "ssnb_jpeg_plan_write_table": (_i, [_vp, _vp, _sz]),
     "ssnb_jpeg_decode": (_i, [_vp, _vp, _vp, _sz, _vp, C.c_int64, _vp, _vp, _sz, _vp]),
+    "ssnb_jpeg_encode_capacity": (C.c_int64, [_i, _i, _i]),
+    "ssnb_jpeg_encode_sizes": (_i, [_i, _i, C.POINTER(JpegEncodeImage), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
+    "ssnb_jpeg_encode": (_i, [_i, _i, _vp, C.c_int64, C.POINTER(JpegEncodeImage), _vp, _i, _vp, C.c_int64, _vp, _vp, _sz, _vp]),
     "ssnb_iv3_num_convs": (_i, []),
     "ssnb_iv3_conv_info": (_i, [_i, _i, C.c_char_p, _i] + [_ip] * 7),
     "ssnb_iv3_create": (_i, [C.POINTER(IV3Config), C.POINTER(_vp)]),

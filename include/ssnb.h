@@ -642,6 +642,34 @@ int ssnb_jpeg_plan_write_table(ssnb_jpeg_plan plan, void* dst, size_t dst_bytes)
 int ssnb_jpeg_decode(ssnb_jpeg_plan plan, const void* table_dev, const uint8_t* src_dev, size_t src_bytes, uint8_t* out, int64_t out_bytes,
                      int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- JPEG encode (csrc/jpeg_encode.cu): the frame and flow-plane files of the reference README's extraction step
+ * (DenseFlow's img_%05d.jpg and flow_{x,y}_%05d.jpg), byte for byte what Pillow's Image.save(f, quality=q) writes through
+ * libjpeg-turbo, and what cv2.imencode writes at the same quality.  Baseline sequential 8-bit JPEG: mode SSNB_JPEG_ENC_L (one
+ * component) or SSNB_JPEG_ENC_RGB (YCbCr, luma 2x2 over 1x1 chroma); libjpeg's jpeg_set_quality(quality, force_baseline)
+ * tables; the Annex K Huffman tables; no restart interval, no metadata beyond the JFIF APP0.  The stages are those of
+ * oracle/jpeg_encode_oracle.py: rgb_ycc_convert, edge expansion, h2v2 downsampling, islow FDCT, rounded quantisation,
+ * Huffman coding with ZRL / EOB, 1-bit padding, 0xFF 0x00 stuffing.
+ *
+ * Image i is uint8 [height, width, components] (rows packed) at src + images[i].src_offset; its file is written at the
+ * start of its output slot, slots back to back in call order, each ssnb_jpeg_encode_capacity bytes: the header, every block
+ * at its largest Huffman code length (22 + 63 * 26 bits) plus 7 pad bits with every byte stuffed, and EOI.  lengths int64 [n]
+ * (device) gets each file's size.  images is the host copy (validation, sizes, launch shapes), images_dev the same values
+ * on the device.  Nothing synchronises with the host and nothing is allocated, so a call can be captured in a CUDA graph; a
+ * file's bytes do not depend on the other images of the call.  Bad arguments (mode, quality outside 1 .. 100, a side of 0
+ * or above 65500, src bytes outside src_bytes, out or workspace too small) return SSNB_EINVAL before any launch; the
+ * capacity and size queries return 0 / SSNB_EINVAL for them. */
+enum { SSNB_JPEG_ENC_L = 1, SSNB_JPEG_ENC_RGB = 3 };
+typedef struct {
+  int64_t src_offset;      /* the image's first byte in src */
+  int32_t height, width;
+} ssnb_jpeg_encode_image;
+int64_t ssnb_jpeg_encode_capacity(int mode, int height, int width);
+int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, size_t* workspace_bytes,
+                           int64_t* out_bytes);
+int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
+                     const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
+                     size_t workspace_bytes, void* stream);
+
 /* ---- InceptionV3 backbone at test time: replaces model_zoo.InceptionV3 (pytorch_load.py:64-67, inceptionv3.yaml) as used by
  *      SSN.test_forward and BinaryClassifier scoring with --arch InceptionV3 (ssn_models.py:133-139, binary_model.py:175-178) ----
  * Forward only, frozen BatchNorm folded into each convolution, in every precision: EXACT_FP32 (fp32 SIMT convolutions),
