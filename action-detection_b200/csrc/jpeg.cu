@@ -17,6 +17,8 @@
 //                        with its edge replication and alternating rounding bias; a plane at most 2 samples wide is
 //                        replicated, as libjpeg does), the fixed-point YCbCr -> RGB of jdcolor (16 fraction bits), and for
 //                        'L' PIL's (R 19595 + G 38470 + B 7471 + 0x8000) >> 16; a grayscale JPEG's 'RGB' repeats Y.
+//
+// The IDCT, the upsampling and the colour tables are jpeg_block.cuh's, which the round trip (jpeg_roundtrip.cu) calls too.
 #include <algorithm>
 #include <climits>
 #include <cstdio>
@@ -27,7 +29,7 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
-#include "jpeg_common.cuh"
+#include "jpeg_block.cuh"
 
 namespace ssnb {
 namespace {
@@ -180,31 +182,6 @@ __global__ void __launch_bounds__(32) jpeg_entropy_kernel(Tables t, int n_interv
 
 // ------------------------------------------------------------------------------------------------------------------- IDCT
 
-constexpr int CONST_BITS = 13, PASS1_BITS = 2;
-constexpr int F0298 = 2446, F0390 = 3196, F0541 = 4433, F0765 = 6270, F0899 = 7373, F1175 = 9633, F1501 = 12299, F1847 = 15137,
-              F1961 = 16069, F2053 = 16819, F2562 = 20995, F3072 = 25172;
-
-// one islow butterfly (jidctint.c); x[0..7] in, o[0..7] out descaled by `shift`
-template <int shift>
-__device__ __forceinline__ void idct8(const int* x, int* o) {
-  int z1 = (x[2] + x[6]) * F0541;
-  const int t2 = z1 - x[6] * F1847, t3 = z1 + x[2] * F0765;
-  const int t0 = (x[0] + x[4]) * (1 << CONST_BITS), t1 = (x[0] - x[4]) * (1 << CONST_BITS);
-  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
-  int o0 = x[7], o1 = x[5], o2 = x[3], o3 = x[1];
-  z1 = o0 + o3;
-  int z2 = o1 + o2, z3 = o0 + o2, z4 = o1 + o3;
-  const int z5 = (z3 + z4) * F1175;
-  o0 *= F0298; o1 *= F2053; o2 *= F3072; o3 *= F1501;
-  z1 *= -F0899; z2 *= -F2562; z3 = z3 * -F1961 + z5; z4 = z4 * -F0390 + z5;
-  o0 += z1 + z3; o1 += z2 + z4; o2 += z2 + z3; o3 += z1 + z4;
-  constexpr int r = 1 << (shift - 1);
-  o[0] = (t10 + o3 + r) >> shift; o[7] = (t10 - o3 + r) >> shift;
-  o[1] = (t11 + o2 + r) >> shift; o[6] = (t11 - o2 + r) >> shift;
-  o[2] = (t12 + o1 + r) >> shift; o[5] = (t12 - o1 + r) >> shift;
-  o[3] = (t13 + o0 + r) >> shift; o[4] = (t13 - o0 + r) >> shift;
-}
-
 __device__ __forceinline__ int plane_of(const DevPlane* __restrict__ p, int n, int64_t blk) {
   int lo = 0, hi = n - 1;
   while (lo < hi) {
@@ -222,62 +199,26 @@ __global__ void __launch_bounds__(128) jpeg_idct_kernel(Tables t, int n_planes, 
   const int64_t local = b - pl.block;
   const int by = (int)(local / pl.bw), bx = (int)(local - (int64_t)by * pl.bw);
   const int32_t* __restrict__ q = t.quant + pl.quant * 64;
-  int ws[64];
-  {
-    int v[64];
-    const int4* src = reinterpret_cast<const int4*>(coef + b * 64);
+  int v[64];
+  const int4* src = reinterpret_cast<const int4*>(coef + b * 64);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int4 w = __ldg(src + i);
-      const int u[4] = {w.x, w.y, w.z, w.w};
+  for (int i = 0; i < 8; ++i) {
+    const int4 w = __ldg(src + i);
+    const int u[4] = {w.x, w.y, w.z, w.w};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        v[i * 8 + 2 * j] = (int)(int16_t)(u[j] & 0xFFFF) * __ldg(q + i * 8 + 2 * j);
-        v[i * 8 + 2 * j + 1] = (u[j] >> 16) * __ldg(q + i * 8 + 2 * j + 1);
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {           // pass 1: columns
-      int x[8], o[8];
-#pragma unroll
-      for (int r = 0; r < 8; ++r) x[r] = v[r * 8 + c];
-      idct8<CONST_BITS - PASS1_BITS>(x, o);
-#pragma unroll
-      for (int r = 0; r < 8; ++r) ws[r * 8 + c] = o[r];
+    for (int j = 0; j < 4; ++j) {
+      v[i * 8 + 2 * j] = (int)(int16_t)(u[j] & 0xFFFF) * __ldg(q + i * 8 + 2 * j);
+      v[i * 8 + 2 * j + 1] = (u[j] >> 16) * __ldg(q + i * 8 + 2 * j + 1);
     }
   }
+  uint32_t px[16];
+  idct_block(v, px);
   uint8_t* out = pix + pl.pix + (int64_t)by * 8 * (pl.bw * 8) + bx * 8;
 #pragma unroll
-  for (int r = 0; r < 8; ++r) {             // pass 2: rows, then the range limit
-    int o[8];
-    idct8<CONST_BITS + PASS1_BITS + 3>(ws + r * 8, o);
-    uint32_t lo = 0, hi = 0;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      lo |= (uint32_t)(min(max(o[c], -128), 127) + 128) << (8 * c);
-      hi |= (uint32_t)(min(max(o[c + 4], -128), 127) + 128) << (8 * c);
-    }
-    *reinterpret_cast<uint2*>(out + (int64_t)r * pl.bw * 8) = make_uint2(lo, hi);
-  }
+  for (int r = 0; r < 8; ++r) *reinterpret_cast<uint2*>(out + (int64_t)r * pl.bw * 8) = make_uint2(px[2 * r], px[2 * r + 1]);
 }
 
 // ------------------------------------------------------------------------------------------------- upsample, colour, store
-
-__device__ __forceinline__ int chroma(const uint8_t* __restrict__ p, int stride, int dw, int dh, int hs, int vs, int x, int y) {
-  if (hs == 1) return p[(int64_t)y * stride + x];
-  const int j = x >> 1, odd = x & 1;
-  if (dw <= 2) return p[(int64_t)(vs == 2 ? y >> 1 : y) * stride + j];     // libjpeg replicates planes this narrow
-  const int jn = odd ? min(j + 1, dw - 1) : max(j - 1, 0);
-  if (vs == 1) {
-    const uint8_t* row = p + (int64_t)y * stride;
-    return (3 * row[j] + row[jn] + 1 + odd) >> 2;
-  }
-  const int i = y >> 1, in_ = (y & 1) ? min(i + 1, dh - 1) : max(i - 1, 0);
-  const uint8_t* r0 = p + (int64_t)i * stride;
-  const uint8_t* r1 = p + (int64_t)in_ * stride;
-  const int cs = 3 * r0[j] + r1[j], csn = 3 * r0[jn] + r1[jn];
-  return (3 * cs + csn + 8 - odd) >> 4;
-}
 
 __global__ void __launch_bounds__(256) jpeg_colour_kernel(Tables t, const uint8_t* __restrict__ pix, uint8_t* __restrict__ out) {
   const DevImage im = t.images[blockIdx.x];
@@ -304,13 +245,12 @@ __global__ void __launch_bounds__(256) jpeg_colour_kernel(Tables t, const uint8_
   for (int64_t i = (int64_t)blockIdx.y * blockDim.x + threadIdx.x; i < npx; i += (int64_t)gridDim.y * blockDim.x) {
     const int y = (int)(i / W), x = (int)(i - (int64_t)y * W);
     const int Y = y_pl[(int64_t)y * ys + x];
-    const int cb = chroma(cb_pl, cstride, dw, dh, hs, vs, x, y) - 128;
-    const int cr = chroma(cr_pl, cstride, dw, dh, hs, vs, x, y) - 128;
-    const int R = min(max(Y + ((fix16(1.40200) * cr + (1 << 15)) >> 16), 0), 255);
-    const int G = min(max(Y + ((-fix16(0.34414) * cb + (1 << 15) - fix16(0.71414) * cr) >> 16), 0), 255);
-    const int B = min(max(Y + ((fix16(1.77200) * cb + (1 << 15)) >> 16), 0), 255);
+    const int cb = chroma(cb_pl, cstride, 0, 0, dw, dh, hs, vs, x, y) - 128;
+    const int cr = chroma(cr_pl, cstride, 0, 0, dw, dh, hs, vs, x, y) - 128;
+    int R, G, B;
+    ycc_rgb(Y, cb, cr, R, G, B);
     if (im.channels == 3) { dst[i * 3] = (uint8_t)R; dst[i * 3 + 1] = (uint8_t)G; dst[i * 3 + 2] = (uint8_t)B; }
-    else dst[i] = (uint8_t)((R * 19595 + G * 38470 + B * 7471 + 0x8000) >> 16);
+    else dst[i] = (uint8_t)rgb_l(R, G, B);
   }
 }
 

@@ -1,4 +1,5 @@
-// What the JPEG decoder (jpeg.cu) and encoder (jpeg_encode.cu) share: the zig-zag order and libjpeg's 16-bit fixed point.
+// What the JPEG decoder (jpeg.cu) and encoder (jpeg_encode.cu) share: the zig-zag order and libjpeg's 16-bit fixed point
+// (jpeg_block.cuh has the per-block arithmetic).
 #pragma once
 #include <stdint.h>
 

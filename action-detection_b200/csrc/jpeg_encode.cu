@@ -16,7 +16,8 @@
 //                       image's size in SOF0), EOI and the file's length.
 //   enc_scatter_kernel  one CTA per chunk: the bytes at their stuffed positions, 0x00 after every 0xFF.
 //
-// Grids are sized for each image's worst case (known from its size); CTAs past an image's actual bytes return at once.
+// Grids are sized for each image's worst case (known from its size); CTAs past an image's actual bytes return at once.  The
+// per-block stages of enc_coef_kernel live in jpeg_block.cuh, which the round trip (jpeg_roundtrip.cu) calls too.
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
@@ -27,26 +28,17 @@
 
 #include "../../include/ssnb.h"
 #include "common.cuh"
-#include "jpeg_common.cuh"
+#include "jpeg_block.cuh"
 
 namespace ssnb {
 namespace {
 
-constexpr int kMaxSide = 65500;                  // libjpeg's JPEG_MAX_DIMENSION
 constexpr int kMaxBlockBits = 22 + 63 * 26;      // a DC code of <= 11 bits + 11 value bits, 63 AC codes of <= 16 + 10 bits
 constexpr int kChunk = 4096, kChunkThreads = 256, kChunkBytesPerThread = kChunk / kChunkThreads;
 constexpr int kScanThreads = 1024, kMcusPerCta = 32;
 constexpr int kMaxHeader = 624;
 
 // ---------------------------------------------------------------------------------------------------------------- tables
-
-// Annex K.1, natural order
-constexpr uint8_t kStdQuant[2][64] = {
-    {16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51, 87, 80, 62,
-     18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112, 100,
-     103, 99},
-    {17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66, 99, 99, 99, 99, 99, 99,
-     99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99, 99}};
 
 // Annex K.3: DC luminance, AC luminance, DC chrominance, AC chrominance (table t of class c is kHuff[2 t + c])
 struct HuffSpec {
@@ -188,46 +180,6 @@ __device__ __forceinline__ int find_image(const DevEnc* __restrict__ t, int n, i
 
 // ------------------------------------------------------------------------------------------------- samples, FDCT, quantise
 
-__device__ __forceinline__ int rgb_y(const uint8_t* p) {
-  return (fix16(0.29900) * p[0] + fix16(0.58700) * p[1] + fix16(0.11400) * p[2] + (1 << 15)) >> 16;
-}
-__device__ __forceinline__ int rgb_c(const uint8_t* p, int cr) {      // ONE_HALF - 1: never above 255
-  const int v = cr ? fix16(0.5) * p[0] - fix16(0.41869) * p[1] - fix16(0.08131) * p[2]
-                   : -fix16(0.16874) * p[0] - fix16(0.33126) * p[1] + fix16(0.5) * p[2];
-  return (v + (128 << 16) + (1 << 15) - 1) >> 16;
-}
-
-constexpr int CONST_BITS = 13, PASS1_BITS = 2;
-
-// one jfdctint.c pass over x[0], x[s], ... x[7 s]
-template <bool first>
-__device__ __forceinline__ void fdct8(int* x, int s) {
-  const int t0 = x[0] + x[7 * s], t7 = x[0] - x[7 * s], t1 = x[s] + x[6 * s], t6 = x[s] - x[6 * s];
-  const int t2 = x[2 * s] + x[5 * s], t5 = x[2 * s] - x[5 * s], t3 = x[3 * s] + x[4 * s], t4 = x[3 * s] - x[4 * s];
-  const int t10 = t0 + t3, t13 = t0 - t3, t11 = t1 + t2, t12 = t1 - t2;
-  constexpr int sh = first ? CONST_BITS - PASS1_BITS : CONST_BITS + PASS1_BITS;
-  constexpr int r = 1 << (sh - 1);
-  if (first) {
-    x[0] = (t10 + t11) * (1 << PASS1_BITS);
-    x[4 * s] = (t10 - t11) * (1 << PASS1_BITS);
-  } else {
-    x[0] = (t10 + t11 + (1 << (PASS1_BITS - 1))) >> PASS1_BITS;
-    x[4 * s] = (t10 - t11 + (1 << (PASS1_BITS - 1))) >> PASS1_BITS;
-  }
-  int z1 = (t12 + t13) * 4433;
-  x[2 * s] = (z1 + t13 * 6270 + r) >> sh;
-  x[6 * s] = (z1 - t12 * 15137 + r) >> sh;
-  z1 = t4 + t7;
-  int z2 = t5 + t6, z3 = t4 + t6, z4 = t5 + t7;
-  const int z5 = (z3 + z4) * 9633;
-  const int a4 = t4 * 2446, a5 = t5 * 16819, a6 = t6 * 25172, a7 = t7 * 12299;
-  z1 *= -7373; z2 *= -20995; z3 = z3 * -16069 + z5; z4 = z4 * -3196 + z5;
-  x[7 * s] = (a4 + z1 + z3 + r) >> sh;
-  x[5 * s] = (a5 + z2 + z4 + r) >> sh;
-  x[3 * s] = (a6 + z2 + z3 + r) >> sh;
-  x[s] = (a7 + z1 + z4 + r) >> sh;
-}
-
 __device__ __forceinline__ int nbits(int v) { return 32 - __clz(abs(v)); }
 
 // position kb of the MCU at local index m: is it a dummy block (luma past the plane's right / bottom edge)?
@@ -255,14 +207,7 @@ __global__ void __launch_bounds__(kMcusPerCta * 6) enc_coef_kernel(const DevEnc*
   int4* dst = reinterpret_cast<int4*>(coef + b * 64);
   int s[64];
   const int comp = kb < 4 ? 0 : kb - 3;
-  if (c.comps == 1) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const uint8_t* row = px + (int64_t)min(my * 8 + r, H - 1) * W;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) s[r * 8 + q] = __ldg(row + min(mx * 8 + q, W - 1));
-    }
-  } else if (kb < 4) {
+  if (c.comps == 3 && kb < 4) {
     const int by = 2 * my + (kb >> 1), bx = 2 * mx + (kb & 1);
     if (by * 8 >= H || bx * 8 >= W) {                   // dummy block: zero, coded as DC difference 0 and EOB
 #pragma unroll
@@ -270,37 +215,13 @@ __global__ void __launch_bounds__(kMcusPerCta * 6) enc_coef_kernel(const DevEnc*
       bits[b] = d_huff.t[kAC0].size[0];
       return;
     }
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const uint8_t* row = px + (int64_t)min(by * 8 + r, H - 1) * W * 3;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) s[r * 8 + q] = rgb_y(row + 3 * min(bx * 8 + q, W - 1));
-    }
-  } else {                                              // h2v2: rows in pairs (the last one repeated), columns clamped
-    const int ch = (H + 1) / 2, cr = comp == 2;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      const int r0 = 2 * min(my * 8 + r, ch - 1), r1 = min(r0 + 1, H - 1);
-      const uint8_t* row0 = px + (int64_t)r0 * W * 3;
-      const uint8_t* row1 = px + (int64_t)r1 * W * 3;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) {
-        const int c0 = 3 * min(2 * (mx * 8 + q), W - 1), c1 = 3 * min(2 * (mx * 8 + q) + 1, W - 1);
-        s[r * 8 + q] = (rgb_c(row0 + c0, cr) + rgb_c(row0 + c1, cr) + rgb_c(row1 + c0, cr) + rgb_c(row1 + c1, cr) + 1 + (q & 1)) >> 2;
-      }
-    }
+    block_samples(px, H, W, 3, 0, by, bx, s);
+  } else {
+    block_samples(px, H, W, c.comps, comp, my, mx, s);
   }
+  fdct_block(s);
 #pragma unroll
-  for (int i = 0; i < 64; ++i) s[i] -= 128;
-#pragma unroll
-  for (int r = 0; r < 8; ++r) fdct8<true>(s + r * 8, 1);
-#pragma unroll
-  for (int q = 0; q < 8; ++q) fdct8<false>(s + q, 8);
-#pragma unroll
-  for (int i = 0; i < 64; ++i) {
-    const int d = comp ? c.div[1][i] : c.div[0][i], a = (abs(s[i]) + (d >> 1)) / d;
-    s[i] = s[i] < 0 ? -a : a;
-  }
+  for (int i = 0; i < 64; ++i) s[i] = quantise(s[i], comp ? c.div[1][i] : c.div[0][i]);
   constexpr NaturalOrder N = natural_order();
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -526,13 +447,10 @@ void put16(std::vector<uint8_t>& h, int v) {
 EncConst make_const(int comps, int quality) {
   EncConst c;
   memset(&c, 0, sizeof c);
-  const int scale = quality < 50 ? 5000 / quality : 200 - 2 * quality;
   int q[2][64];
+  quant_tables(quality, q);
   for (int t = 0; t < 2; ++t)
-    for (int i = 0; i < 64; ++i) {
-      q[t][i] = std::min(std::max((kStdQuant[t][i] * scale + 50) / 100, 1), 255);
-      c.div[t][i] = q[t][i] << 3;
-    }
+    for (int i = 0; i < 64; ++i) c.div[t][i] = q[t][i] << 3;
   const int tables = comps == 1 ? 1 : 2;
   std::vector<uint8_t> h = {0xFF, 0xD8, 0xFF, 0xE0, 0, 16, 'J', 'F', 'I', 'F', 0, 1, 1, 0, 0, 1, 0, 1, 0, 0};
   for (int t = 0; t < tables; ++t) {
@@ -575,7 +493,7 @@ struct Layout {
   size_t off_coef = 0, off_bits = 0, off_words = 0, off_counts = 0, workspace = 0;
 };
 
-bool check_image_size(int h, int w) { return h >= 1 && w >= 1 && h <= kMaxSide && w <= kMaxSide; }
+bool check_image_size(int h, int w) { return h >= 1 && w >= 1 && h <= kJpegEncMaxSide && w <= kJpegEncMaxSide; }
 
 // the call's sizes; an empty string when the arguments are acceptable, else the reason
 std::string plan(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, int64_t src_bytes, Layout& L) {
@@ -586,7 +504,7 @@ std::string plan(int mode, int quality, const ssnb_jpeg_encode_image* images, in
   for (int i = 0; i < n; ++i) {
     const ssnb_jpeg_encode_image& e = images[i];
     if (!check_image_size(e.height, e.width))
-      return "image " + std::to_string(i) + ": height and width must be 1 .. " + std::to_string(kMaxSide);
+      return "image " + std::to_string(i) + ": height and width must be 1 .. " + std::to_string(kJpegEncMaxSide);
     if (src_bytes >= 0 && (e.src_offset < 0 || e.src_offset + (int64_t)e.height * e.width * mode > src_bytes))
       return "image " + std::to_string(i) + ": pixels outside src";
     const Geo g = geometry(mode, hl, e.height, e.width);

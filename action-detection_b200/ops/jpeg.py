@@ -16,6 +16,11 @@ reason; there is no CPU fallback.
 encode_jpeg is the other direction, the files of the extraction step (DenseFlow's img_%05d.jpg and flow_{x,y}_%05d.jpg):
 CUDA uint8 images -> the bytes Pillow's Image.save(f, quality=q) writes, computed by csrc/jpeg_encode.cu.  JpegEncodePlan
 keeps one call's buffers so the encode can be repeated or captured in a CUDA graph.
+
+jpeg_roundtrip joins the two without the files: CUDA uint8 images -> what decode_jpeg returns for the files encode_jpeg
+writes of them (csrc/jpeg_roundtrip.cu, no Huffman coding), so decoded video frames or flow planes become the exact inputs
+the data sets would read from the extraction step's files.  JpegRoundtripPlan keeps one call's buffers for repeats and
+CUDA graphs.
 """
 import ctypes as C
 import os
@@ -252,6 +257,28 @@ def _enc_mode(mode):
     return _ENC_MODES[mode]
 
 
+def _pixel_buffer(images, sizes, channels, mode, what):
+    """CUDA uint8 [N, H, W, C] or a list of [H, W, C] of the given sizes -> one contiguous uint8 buffer"""
+    ts = [images] if torch.is_tensor(images) else list(images)
+    if not all(torch.is_tensor(t) and t.is_cuda for t in ts):
+        raise RuntimeError("%s needs CUDA uint8 images (no CPU path)" % what)
+    if any(t.dtype != torch.uint8 for t in ts):
+        raise ValueError("%s: images must be uint8" % what)
+    if torch.is_tensor(images):
+        if images.dim() != 4 or images.shape[3] != channels:
+            raise ValueError("%s: images must be [N, H, W, %d] for mode %r" % (what, channels, mode))
+        shapes = [tuple(images.shape[1:3])] * images.shape[0]
+    else:
+        if any(t.dim() != 3 or t.shape[2] != channels for t in ts):
+            raise ValueError("%s: each image must be [H, W, %d] for mode %r" % (what, channels, mode))
+        shapes = [tuple(t.shape[:2]) for t in ts]
+    if shapes != sizes:
+        raise ValueError("%s: the images' sizes differ from the plan's" % what)
+    if torch.is_tensor(images):
+        return images.contiguous().reshape(-1)
+    return torch.cat([t.reshape(-1) for t in ts])
+
+
 class JpegEncodePlan:
     """One encode call's sizes, mode and quality with its device buffers: the image table, the workspace, the output slots
     (image i's file starts at out[slots[i]]) and the int64 lengths.  plan.run(images) only enqueues, so it can be repeated
@@ -283,24 +310,7 @@ class JpegEncodePlan:
 
     def _pixels(self, images):
         """CUDA uint8 [N, H, W, C] or a list of [H, W, C] of the plan's sizes -> one contiguous uint8 buffer"""
-        ts = [images] if torch.is_tensor(images) else list(images)
-        if not all(torch.is_tensor(t) and t.is_cuda for t in ts):
-            raise RuntimeError("encode_jpeg needs CUDA uint8 images (no CPU path)")
-        if any(t.dtype != torch.uint8 for t in ts):
-            raise ValueError("encode_jpeg: images must be uint8")
-        if torch.is_tensor(images):
-            if images.dim() != 4 or images.shape[3] != self.channels:
-                raise ValueError("encode_jpeg: images must be [N, H, W, %d] for mode %r" % (self.channels, self.mode))
-            shapes = [tuple(images.shape[1:3])] * images.shape[0]
-        else:
-            if any(t.dim() != 3 or t.shape[2] != self.channels for t in ts):
-                raise ValueError("encode_jpeg: each image must be [H, W, %d] for mode %r" % (self.channels, self.mode))
-            shapes = [tuple(t.shape[:2]) for t in ts]
-        if shapes != self.sizes:
-            raise ValueError("encode_jpeg: the images' sizes differ from the plan's")
-        if torch.is_tensor(images):
-            return images.contiguous().reshape(-1)
-        return torch.cat([t.reshape(-1) for t in ts])
+        return _pixel_buffer(images, self.sizes, self.channels, self.mode, "encode_jpeg")
 
     def run(self, images):
         """enqueue the encode of `images` on the current stream; returns (out, lengths) on the device"""
@@ -348,3 +358,79 @@ def encode_jpeg(images, mode="RGB", quality=95):
     plan = JpegEncodePlan(sizes, mode, quality, device)
     plan.run(images)
     return plan.files()
+
+
+# ------------------------------------------------------------------------------------------------------------- round trip
+
+def _sizes_of(images, what):
+    """[N, H, W, C] or a list of [H, W, C] CUDA tensors -> ([(H, W)] per image, device); CPU tensors raise"""
+    if torch.is_tensor(images):
+        if not images.is_cuda:
+            raise RuntimeError("%s needs CUDA uint8 images (no CPU path)" % what)
+        if images.dim() != 4:
+            raise ValueError("%s: images must be [N, H, W, C] or a list of [H, W, C]" % what)
+        return [tuple(images.shape[1:3])] * images.shape[0], images.device
+    if not all(torch.is_tensor(t) and t.is_cuda for t in images):
+        raise RuntimeError("%s needs CUDA uint8 images (no CPU path)" % what)
+    if any(t.dim() != 3 for t in images):
+        raise ValueError("%s: images must be [N, H, W, C] or a list of [H, W, C]" % what)
+    return [tuple(t.shape[:2]) for t in images], (images[0].device if images else None)
+
+
+class JpegRoundtripPlan:
+    """One round-trip call's sizes, mode and quality with its device image table and output buffer (image i's result at
+    out[offsets[i]:offsets[i + 1]], images back to back).  plan.run(images) only enqueues, so it can be repeated or captured
+    in a CUDA graph on new pixels of the same sizes; it returns the results as views of plan.out."""
+
+    def __init__(self, sizes, mode="RGB", quality=95, device=None):
+        if mode not in _ENC_MODES:
+            raise ValueError("jpeg_roundtrip: mode must be 'RGB' or 'L'")
+        self.mode, self.quality = mode, int(quality)
+        self._code, self.channels = _ENC_MODES[mode]
+        if not 1 <= self.quality <= 100:
+            raise ValueError("jpeg_roundtrip: quality must be 1 .. 100")
+        self.sizes = [(int(h), int(w)) for h, w in sizes]
+        n = len(self.sizes)
+        if n < 1:
+            raise ValueError("jpeg_roundtrip: no image")
+        if any(not (1 <= h <= 65500 and 1 <= w <= 65500) for h, w in self.sizes):
+            raise ValueError("jpeg_roundtrip: height and width must be 1 .. 65500")
+        self.images = (JpegEncodeImage * n)()
+        self.offsets = np.zeros(n + 1, np.int64)
+        for i, (e, (h, w)) in enumerate(zip(self.images, self.sizes)):
+            e.src_offset, e.height, e.width = int(self.offsets[i]), h, w
+            self.offsets[i + 1] = self.offsets[i] + h * w * self.channels
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.images_dev = torch.frombuffer(bytearray(bytes(self.images)), dtype=torch.uint8).to(dev)
+        self.out = torch.empty(int(self.offsets[-1]), dtype=torch.uint8, device=dev)
+
+    def run(self, images):
+        """enqueue the round trip of `images` ([N, H, W, C] or a list of [H, W, C] of the plan's sizes) on the current stream;
+        -> uint8 [N, H, W, C] for a tensor, else a list of [H, W, C], views of plan.out"""
+        src = _pixel_buffer(images, self.sizes, self.channels, self.mode, "jpeg_roundtrip")
+        if src.device != self.out.device:
+            raise ValueError("jpeg_roundtrip: images on %s, plan on %s" % (src.device, self.out.device))
+        self._src = src                       # kept alive until the next run
+        with torch.cuda.device(self.out.device):
+            rc = lib.ssnb_jpeg_roundtrip(self._code, self.quality, src.data_ptr(), src.numel(), self.images, self.images_dev.data_ptr(),
+                                         len(self.sizes), self.out.data_ptr(), self.out.numel(),
+                                         C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        if rc != 0:
+            raise RuntimeError("libssn_b200 jpeg_roundtrip failed (code %d): %s" % (rc, (lib.ssnb_last_error(None) or b"").decode()))
+        if torch.is_tensor(images):
+            return self.out.view(len(self.sizes), *self.sizes[0], self.channels)
+        return [self.out[int(a):int(b)].view(h, w, self.channels) for a, b, (h, w) in zip(self.offsets[:-1], self.offsets[1:], self.sizes)]
+
+
+def jpeg_roundtrip(images, mode="RGB", quality=95):
+    """The pixels the data sets' loaders read back from JPEG files of CUDA uint8 images, computed without the files: [N, H, W,
+    C] or a list of ragged [H, W, C], C = 3 for 'RGB' and 1 for 'L'.  Returns the same structure, uint8 on the same device,
+    bitwise equal to decode_jpeg(encode_jpeg(images, mode, quality), mode), i.e. to
+    np.asarray(Image.open(BytesIO(f)).convert(mode)) of the file f that Image.fromarray(img).save(f, format='JPEG',
+    quality=quality) writes: 4:2:0 for 'RGB'.  quality 1 .. 100.  Enqueued on the current stream; nothing waits."""
+    if not torch.is_tensor(images):
+        images = list(images)
+    sizes, device = _sizes_of(images, "jpeg_roundtrip")
+    if not sizes:
+        return images.new_empty(images.shape) if torch.is_tensor(images) else []
+    return JpegRoundtripPlan(sizes, mode, quality, device).run(images)

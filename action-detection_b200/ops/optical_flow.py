@@ -11,6 +11,11 @@ oracle/tvl1_oracle.py writes down, runs on all pairs of many videos in one call:
     write_flow_jpegs(planes, video_dirs, offsets=offsets)      # or the files SSNDataSet reads, encoded on the GPU
     write_frame_jpegs(torch.cat(frames), video_dirs, offsets=offsets)   # and the RGB side, img_{:05d}.jpg
 
+or, without the files, the pixels the data sets would read back from them (the JPEG round trip, computed on the GPU):
+
+    x = model.frame_transforms().oversample(flow_images(planes)[2 * k:2 * k + 2 * model.new_length])
+    rgb = frame_images(torch.cat(frames))                       # what decode_jpeg returns for img_{:05d}.jpg
+
 No CPU path: the frames must be CUDA tensors.  Parity with a built DenseFlow or OpenCV CUDA is not checked by this project.
 """
 import ctypes as C
@@ -198,3 +203,27 @@ def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None):
                 Image.fromarray(arr[i]).save(path, quality=quality)
             paths.append(path)
     return paths
+
+
+def flow_images(planes, quality=95):
+    """The in-memory counterpart of write_flow_jpegs: CUDA uint8 planes [2P, H, W, 1] (flow_planes' output, x then y per pair,
+    the order JpegBytesLoader keeps) -> uint8 [2P, H, W, 1] on the device, bitwise what decode_jpeg(..., mode='L') returns for
+    the flow_x / flow_y files write_flow_jpegs writes at this quality (ops.jpeg.jpeg_roundtrip; no file is written)."""
+    from ops.jpeg import jpeg_roundtrip
+    if not (torch.is_tensor(planes) and planes.is_cuda):
+        raise RuntimeError("flow_images needs CUDA uint8 planes [2P, H, W, 1] (no CPU path)")
+    if planes.dtype != torch.uint8 or planes.dim() != 4 or planes.shape[3] != 1 or planes.shape[0] % 2:
+        raise ValueError("planes must be uint8 [2P, H, W, 1]")
+    return jpeg_roundtrip(planes, mode="L", quality=quality)
+
+
+def frame_images(frames, quality=95):
+    """The in-memory counterpart of write_frame_jpegs: CUDA uint8 RGB frames [N, H, W, 3] -> uint8 [N, H, W, 3] on the device,
+    bitwise what decode_jpeg(..., mode='RGB') returns for the img_{:05d}.jpg files write_frame_jpegs writes at this quality
+    (ops.jpeg.jpeg_roundtrip; no file is written)."""
+    from ops.jpeg import jpeg_roundtrip
+    if not (torch.is_tensor(frames) and frames.is_cuda):
+        raise RuntimeError("frame_images needs CUDA uint8 frames [N, H, W, 3] (no CPU path)")
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
+        raise ValueError("frames must be uint8 [N, H, W, 3]")
+    return jpeg_roundtrip(frames, mode="RGB", quality=quality)

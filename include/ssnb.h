@@ -670,6 +670,23 @@ int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_byte
                      const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
                      size_t workspace_bytes, void* stream);
 
+/* ---- JPEG round trip (csrc/jpeg_roundtrip.cu): what the data sets' loaders read back from the frame and flow-plane files of
+ * the extraction step, straight from the frames: for uint8 images, np.asarray(Image.open(BytesIO(f)).convert(mode)) of the
+ * file f that Image.save(f, quality=q) writes, i.e. ssnb_jpeg_decode of ssnb_jpeg_encode's files, without writing, reading
+ * or Huffman-decoding them.  Per 8x8 block: the encoder's edge expansion, rgb_ycc_convert, h2v2 downsampling, islow FDCT and
+ * rounded quantisation, then the decoder's dequantisation, islow IDCT and range limit; then h2v2 fancy upsampling and the
+ * YCbCr -> RGB tables.  mode SSNB_JPEG_ENC_L (one component, the result [height, width, 1]) or SSNB_JPEG_ENC_RGB (YCbCr
+ * 4:2:0, the result [height, width, 3]); quality 1 .. 100 with libjpeg's scaling, as ssnb_jpeg_encode.
+ *
+ * Image i is uint8 [height, width, mode] (rows packed) at src + images[i].src_offset; its result is written at the same
+ * offset of out, so out mirrors src's layout.  out must not overlap src.  images is the host copy (validation, launch shapes),
+ * images_dev the same values on the device.  The call only enqueues kernels: no workspace, no allocation and no host
+ * synchronisation, so it can be captured in a CUDA graph; an image's result does not depend on the other images of the call.
+ * Bad arguments (mode, quality, no image, a side of 0 or above 65500, pixels outside src_bytes or out_bytes, NULL pointers,
+ * out overlapping src) return SSNB_EINVAL before any launch. */
+int ssnb_jpeg_roundtrip(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
+                        const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, void* stream);
+
 /* ---- InceptionV3 backbone at test time: replaces model_zoo.InceptionV3 (pytorch_load.py:64-67, inceptionv3.yaml) as used by
  *      SSN.test_forward and BinaryClassifier scoring with --arch InceptionV3 (ssn_models.py:133-139, binary_model.py:175-178) ----
  * Forward only, frozen BatchNorm folded into each convolution, in every precision: EXACT_FP32 (fp32 SIMT convolutions),
