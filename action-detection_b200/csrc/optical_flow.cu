@@ -113,14 +113,16 @@ __global__ void tvl1_warp_kernel(const float* __restrict__ I0, const float* __re
   const float* gx = Ix + p * A;
   const float* gy = Iy + p * A;
   const float u1 = u[2 * p * A + o], u2 = u[(2 * p + 1) * A + o];
-  const float wx = fminf(fmaxf((float)x + u1, -3.f), (float)w + 2.f), wy = fminf(fmaxf((float)y + u2, -3.f), (float)h + 2.f);
-  const int xmin = (int)ceilf(wx - 2.f), xmax = (int)floorf(wx + 2.f), ymin = (int)ceilf(wy - 2.f), ymax = (int)floorf(wy + 2.f);
+  // the sample point and each tap's offset in double, the offset rounded once to fp32: x + u1 in fp32 rounds to 2^-11 px near
+  // x = 8191 (to 3e-5 px near x = 300), and every tap weight would carry that
+  const double wx = fmin(fmax(x + (double)u1, -3.0), w + 2.0), wy = fmin(fmax(y + (double)u2, -3.0), h + 2.0);
+  const int xmin = (int)ceil(wx - 2.0), xmax = (int)floor(wx + 2.0), ymin = (int)ceil(wy - 2.0), ymax = (int)floor(wy + 2.0);
   float s = 0.f, sx = 0.f, sy = 0.f, ws = 0.f;
   for (int cy = ymin; cy <= ymax; ++cy) {
-    const float ky = cubic(wy - (float)cy);
+    const float ky = cubic((float)(wy - cy));
     const long long row = (long long)clampi(cy, 0, h - 1) * w;
     for (int cx = xmin; cx <= xmax; ++cx) {
-      const float k = ky * cubic(wx - (float)cx);
+      const float k = ky * cubic((float)(wx - cx));
       const long long q = row + clampi(cx, 0, w - 1);
       s += k * J[q];
       sx += k * gx[q];

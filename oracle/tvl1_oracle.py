@@ -160,9 +160,10 @@ def dual(u, p, tau=0.25, theta=0.3):
     return out
 
 
-def tvl1(g0, g1, counts=None, fixed_iterations=False, **params):
+def tvl1(g0, g1, counts=None, fixed_iterations=False, trace=None, **params):
     """R2 .. R8 for one pair of grey frames [H, W] -> (flow [2, H, W] float64, iterations int32 [levels, warps]).
-    counts [levels, warps] (level 0 the finest): run exactly that many iterations (replaying another run's stopping rule)."""
+    counts [levels, warps] (level 0 the finest): run exactly that many iterations (replaying another run's stopping rule).
+    trace: a dict that receives trace[(level, warp)] = [error of iteration 1, 2, ...], R8's error as computed (replayed or not)."""
     prm = dict(DEFAULTS, **params)
     if prm["gamma"] != 0:
         raise ValueError("gamma != 0 is not implemented")
@@ -179,9 +180,13 @@ def tvl1(g0, g1, counts=None, fixed_iterations=False, **params):
         for wp in range(W):
             Ixw, Iyw, grad, rho_c = warp(P0[lv], P1[lv], Ix, Iy, u)
             n = 0
+            errs = []
+            if trace is not None:
+                trace[(lv, wp)] = errs
             while True:
                 u, err = primal(Ixw, Iyw, grad, rho_c, p, u, prm["lambda_"], prm["theta"])
                 p = dual(u, p, prm["tau"], prm["theta"])
+                errs.append(err)
                 n += 1
                 if counts is not None:
                     if n >= counts[lv][wp]:

@@ -115,7 +115,7 @@ def _grey_np(frames):
 
 
 def test_whole_solver_replayed_against_oracle():
-    """two videos of 4 and 3 frames at 40 x 56 (three pyramid levels), default parameters: the oracle run for exactly the
+    """two videos of 4 and 3 frames at 40 x 56 (five pyramid levels), default parameters: the oracle run for exactly the
     GPU's iteration counts gives the GPU's flow within 1e-2 px and 1e-4 relative L2; the planes differ by one level at most,
     only next to a rounding tie"""
     from ops.optical_flow import tvl1_flow, flow_planes

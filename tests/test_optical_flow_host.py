@@ -37,6 +37,76 @@ def test_level_sizes_round_half_even_and_stop_under_16():
     assert O.level_sizes(256, 340, nscales=2) == [(256, 340), (205, 272)]
 
 
+def test_library_level_count_equals_oracle_for_every_size():
+    """ssnb_tvl1_levels against len(O.level_sizes(...)) for every h, w in 1 .. 600 at scale_step 0.8, 0.75 and 0.5 (odd sizes
+    at 0.5 are exact half ties of R2's round half to even).  The oracle's count at nscales 32 is the shorter of the two axes'
+    chains (R2 stops at the first axis under 16), checked against O.level_sizes itself on every seventh size; nscales 1 .. 32
+    on every seventh h and w."""
+    from ssn_b200._lib import lib
+    assert O.level_sizes(33, 33, 5, 0.5) == [(33, 33), (16, 16)]           # 16.5 -> 16 (even), still a level
+    assert O.level_sizes(35, 31, 5, 0.5) == [(35, 31), (18, 16)]           # 17.5 -> 18, 15.5 -> 16
+    assert O.level_sizes(34, 600, 5, 0.5) == [(34, 600), (17, 300)]
+    sizes = range(1, 601)
+    for step in (0.8, 0.75, 0.5):
+        axis = {n: len(O.level_sizes(n, 1 << 40, 32, step)) for n in sizes}
+        want = lambda h, w, ns=32: min(ns, axis[h], axis[w])
+        for h in sizes[::7]:
+            for w in sizes[::7]:
+                assert len(O.level_sizes(h, w, 32, step)) == want(h, w), (h, w, step)
+        prm = _params(scale_step=step, nscales=32)
+        bad = [(h, w) for h in sizes for w in sizes if lib.ssnb_tvl1_levels(prm, h, w) != want(h, w)]
+        assert not bad, (step, bad[:10])
+        for ns in range(1, 33):
+            prm = _params(scale_step=step, nscales=ns)
+            bad = [(h, w) for h in sizes[::7] for w in sizes[::7] if lib.ssnb_tvl1_levels(prm, h, w) != want(h, w, ns)]
+            assert not bad, (step, ns, bad[:10])
+            assert lib.ssnb_tvl1_levels(prm, 33, 33) == min(ns, 2 if step == 0.5 else 3 if step == 0.75 else 4)
+
+
+def test_oracle_trace_brackets_its_own_stopping_rule():
+    """trace= records R8's error per iteration: where the oracle's own rule stops a warp early, the last traced error is
+    <= epsilon^2 h_l w_l of that level and every earlier one above it; a warp that runs out of iterations never went under.
+    Replaying the counts traces the same errors."""
+    I0, I1, _ = O.moving_pair(40, 56, ("shift", 0.8, -0.45), seed=4)
+    tr = {}
+    _, its = O.tvl1(np.rint(I0), np.rint(I1), iterations=40, trace=tr)
+    sizes = O.level_sizes(40, 56)
+    assert sorted(tr) == [(l, w) for l in range(len(sizes)) for w in range(5)]
+    early = 0
+    for (l, w), errs in tr.items():
+        thr = 0.01 ** 2 * sizes[l][0] * sizes[l][1]
+        assert len(errs) == its[l, w]
+        assert all(e > thr for e in errs[:-1]), (l, w)
+        if its[l, w] < 40:
+            assert errs[-1] <= thr, (l, w)
+            early += 1
+        else:
+            assert errs[-1] > thr, (l, w)
+    assert early >= 10 and (its == 40).any()
+    tr2 = {}
+    O.tvl1(np.rint(I0), np.rint(I1), counts=its, trace=tr2)
+    assert tr2 == tr
+
+
+def test_single_frame_videos_in_offsets(tmp_path):
+    """videos of one frame (no pair) at the start, in the middle, back to back and at the end: pair_offsets gives them empty
+    ranges, and write_flow_jpegs (host planes) makes their directories and writes nothing in them"""
+    from ops.optical_flow import pair_offsets, write_flow_jpegs
+    off = [0, 1, 4, 5, 6, 9, 10]                           # 1, 3, 1, 1, 3, 1 frames
+    assert pair_offsets(off).tolist() == [0, 0, 2, 2, 2, 4, 4]
+    planes = np.arange(8, dtype=np.uint8).reshape(8, 1, 1, 1).repeat(8, 1).repeat(8, 2) * 30
+    dirs = [str(tmp_path / ("v%d" % v)) for v in range(6)]
+    paths = write_flow_jpegs(planes, dirs, offsets=off)
+    assert [os.path.relpath(p, tmp_path) for p in paths] == ["v1/flow_x_00001.jpg", "v1/flow_y_00001.jpg", "v1/flow_x_00002.jpg",
+                                                             "v1/flow_y_00002.jpg", "v4/flow_x_00001.jpg", "v4/flow_y_00001.jpg",
+                                                             "v4/flow_x_00002.jpg", "v4/flow_y_00002.jpg"]
+    assert all(os.path.isdir(d) for d in dirs) and not os.listdir(dirs[0]) and not os.listdir(dirs[5])
+    from PIL import Image
+    assert [int(np.asarray(Image.open(p)).mean().round()) for p in paths] == [0, 30, 60, 90, 120, 150, 180, 210]
+    with pytest.raises(ValueError):
+        write_flow_jpegs(planes, dirs, offsets=[0, 1, 4, 5, 6, 9, 11])
+
+
 @pytest.mark.parametrize("motion", [("shift", 0.37, -0.61), ("shift", 1.6, 0.85), ("shift", -2.3, 0.2), ("rotate", 2.0)])
 def test_oracle_recovers_known_motion(motion):
     """a seeded texture moved by a sub-pixel / two-pixel translation or a 2 degree rotation about the centre, rounded to
