@@ -6,6 +6,12 @@ oracle/tvl1_oracle.py writes down, runs on all pairs of many videos in one call:
 
     frames = decode_jpeg(byte_groups, mode='RGB')               # uint8 [n, H, W, 3] per video, one size for all
     flow = tvl1_flow(torch.cat(frames), offsets)                # fp32 [P, 2, H, W], pair k of a video = (frame k, frame k + 1)
+
+Videos of different sizes are first brought to one size as DenseFlow's extract_gpu --new_width 340 --new_height 256 does
+(cv::resize, INTER_LINEAR; bitwise cv2.resize, csrc/frame_resize.cu):
+
+    frames, offsets = resize_frames(decoded_videos)             # uint8 [sum n, 256, 340, 3], offsets [V + 1]
+    flow = tvl1_flow(frames, offsets)
     planes = flow_planes(flow)                                  # uint8 [2P, H, W, 1]: x, y, x, y, ... as JpegBytesLoader keeps them
     x = model.frame_transforms().oversample(planes[2 * k:2 * k + 2 * model.new_length])   # a Flow tick, as from decoded JPEGs
     write_flow_jpegs(planes, video_dirs, offsets=offsets)      # or the files SSNDataSet reads, encoded on the GPU
@@ -24,7 +30,7 @@ import os
 import numpy as np
 import torch
 
-from ssn_b200._lib import lib, check, TVL1Params
+from ssn_b200._lib import lib, check, TVL1Params, ResizeVideo
 
 DEFAULTS = dict(tau=0.25, lambda_=0.15, theta=0.3, nscales=5, warps=5, epsilon=0.01, iterations=300, scale_step=0.8, gamma=0.0,
                 fixed_iterations=False)
@@ -227,3 +233,75 @@ def frame_images(frames, quality=95):
     if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
         raise ValueError("frames must be uint8 [N, H, W, 3]")
     return jpeg_roundtrip(frames, mode="RGB", quality=quality)
+
+
+MAX_SIDE = 65500
+
+
+class ResizePlan:
+    """One resize call's table and buffers, so it can be run again (or captured in a CUDA graph) on new frames of the same
+    videos' sizes.  shapes: (frames, height, width) per video.  plan.inputs[v] is video v's uint8 [n_v, H_v, W_v, 3] view of
+    the packed source plan.src; plan.run(videos) copies the videos there first, plan.run() resizes what plan.src holds into
+    plan.frames, uint8 [sum n_v, height, width, 3].  plan.offsets are the frame offsets [V + 1] of tvl1_flow and write_*_jpegs."""
+
+    def __init__(self, shapes, width=340, height=256, device="cuda"):
+        shapes = [tuple(int(x) for x in s) for s in shapes]
+        if not shapes:
+            raise ValueError("resize_frames needs at least one video")
+        self.width, self.height = int(width), int(height)
+        if not (1 <= self.width <= MAX_SIDE and 1 <= self.height <= MAX_SIDE):
+            raise ValueError("destination height and width must be 1 .. %d" % MAX_SIDE)
+        self.table = (ResizeVideo * len(shapes))()
+        src_bytes, frames = 0, 0
+        for e, (n, h, w) in zip(self.table, shapes):
+            if n < 1:
+                raise ValueError("each video needs at least one frame")
+            if not (1 <= h <= MAX_SIDE and 1 <= w <= MAX_SIDE):
+                raise ValueError("frame height and width must be 1 .. %d" % MAX_SIDE)
+            e.src_offset, e.first_frame, e.height, e.width, e.frames = src_bytes, frames, h, w, n
+            src_bytes += n * h * w * 3
+            frames += n
+        self.shapes = shapes
+        self.offsets = np.cumsum([0] + [n for n, _, _ in shapes]).astype(np.int64)
+        dev = torch.device(device)
+        self.src = torch.empty(src_bytes, dtype=torch.uint8, device=dev)
+        self.inputs = [self.src[e.src_offset:e.src_offset + n * h * w * 3].view(n, h, w, 3) for e, (n, h, w) in zip(self.table, shapes)]
+        self.table_dev = torch.frombuffer(bytearray(bytes(self.table)), dtype=torch.uint8).to(dev)
+        self.frames = torch.empty(frames, self.height, self.width, 3, dtype=torch.uint8, device=dev)
+
+    def run(self, videos=None):
+        if videos is not None:
+            videos = list(videos)
+            if len(videos) != len(self.inputs):
+                raise ValueError("the plan has %d videos, got %d" % (len(self.inputs), len(videos)))
+            for v, (x, dst) in enumerate(zip(videos, self.inputs)):
+                if not (torch.is_tensor(x) and x.is_cuda and x.dtype == torch.uint8):
+                    raise RuntimeError("resize_frames needs CUDA uint8 RGB frames [n, H, W, 3] (no CPU path)")
+                if tuple(x.shape) != tuple(dst.shape):
+                    raise ValueError("video %d must be %s, got %s" % (v, tuple(dst.shape), tuple(x.shape)))
+                dst.copy_(x)
+        with torch.cuda.device(self.frames.device):
+            check(lib.ssnb_frame_resize(self.src.data_ptr(), self.src.numel(), self.table, self.table_dev.data_ptr(), len(self.table),
+                                        self.height, self.width, self.frames.data_ptr(), self.frames.numel(), _stream()),
+                  None, "frame_resize")
+        return self.frames
+
+
+def resize_frames(videos, width=340, height=256):
+    """DenseFlow's per-frame cv::resize(frame, image, Size(width, height)) (extract_gpu --new_width / --new_height), bitwise
+    cv2.resize(frame, (width, height), interpolation=cv2.INTER_LINEAR), for many videos of any sizes in one call.
+    videos: a list of CUDA uint8 [n_v, H_v, W_v, 3] (RGB or BGR alike; decode_jpeg's output) -> (frames uint8
+    [sum n_v, height, width, 3] on the device, frame offsets int64 [V + 1]), the frames and offsets tvl1_flow,
+    write_frame_jpegs and frame_images take."""
+    if torch.is_tensor(videos):
+        videos = [videos]
+    videos = list(videos)
+    for x in videos:
+        if not (torch.is_tensor(x) and x.is_cuda):
+            raise RuntimeError("resize_frames needs CUDA uint8 RGB frames [n, H, W, 3] (no CPU path)")
+        if x.dtype != torch.uint8 or x.dim() != 4 or x.shape[3] != 3:
+            raise ValueError("each video must be uint8 [n, H, W, 3]")
+    if not videos:
+        raise ValueError("resize_frames needs at least one video")
+    plan = ResizePlan([x.shape[:3] for x in videos], width, height, videos[0].device)
+    return plan.run(videos), plan.offsets

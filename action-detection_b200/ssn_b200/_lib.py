@@ -103,6 +103,11 @@ class TVL1Params(C.Structure):
                 ("gamma", C.c_double), ("nscales", C.c_int32), ("warps", C.c_int32), ("iterations", C.c_int32), ("fixed_iterations", C.c_int32)]
 
 
+class ResizeVideo(C.Structure):
+    _fields_ = [("src_offset", C.c_int64), ("first_frame", C.c_int64), ("height", C.c_int32), ("width", C.c_int32),
+                ("frames", C.c_int32), ("reserved", C.c_int32)]
+
+
 TVL1_GREY, TVL1_RESIZE, TVL1_GRADIENT, TVL1_WARP, TVL1_PRIMAL, TVL1_DUAL = 0, 1, 2, 3, 4, 5
 
 PROPFRAMES_SECONDS, PROPFRAMES_NORMALISED, PROPFRAMES_AS_GIVEN = 0, 1, 2
@@ -230,6 +235,7 @@ SIGNATURES = {
     "ssnb_tvl1_flow": (_i, [C.POINTER(TVL1Params), _vp, C.POINTER(C.c_int64), _vp, _i, _i, _i, _vp, _vp, _vp, _sz, _vp]),
     "ssnb_tvl1_stage": (_i, [_i, C.POINTER(TVL1Params), _i, _i, _i, _i, _i, C.c_double, _pp, _pp, _vp]),
     "ssnb_flow_planes": (_i, [_vp, C.c_int64, _i, _i, C.c_double, _vp, _vp]),
+    "ssnb_frame_resize": (_i, [_vp, C.c_int64, C.POINTER(ResizeVideo), _vp, _i, _i, _i, _vp, C.c_int64, _vp]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

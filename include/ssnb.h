@@ -832,6 +832,30 @@ int ssnb_tvl1_stage(int stage, const ssnb_tvl1_params* prm, int n, int height, i
  * v < -bound (or NaN) -> 0, v > bound -> 255, else cvRound(255 (v + bound) / (2 bound)) in double, half to even.  bound > 0. */
 int ssnb_flow_planes(const float* flow, int64_t pairs, int height, int width, double bound, uint8_t* planes, void* stream);
 
+/* ---- Frame resize (csrc/frame_resize.cu): DenseFlow's cv::resize(frame, image, Size(new_width, new_height)) of every
+ * decoded frame before the flow (extract_gpu --new_width 340 --new_height 256), bitwise equal to OpenCV 4's
+ * cv2.resize(frame, (dst_width, dst_height), interpolation=INTER_LINEAR) on uint8 3-channel frames, upscale, downscale,
+ * copy and the 2 x 2 area path alike, with the rules oracle/frame_resize_oracle.py writes down.  Channels are independent.
+ *
+ * Video v's frames are uint8 [frames, height, width, 3] (rows packed) at src + videos[v].src_offset; every frame of the call
+ * is resized to dst_height x dst_width and written to dst as uint8 [sum frames, dst_height, dst_width, 3], videos in table
+ * order, the layout ssnb_tvl1_flow and ssnb_jpeg_encode take.  videos[v].first_frame is the frames of the videos before v
+ * (the video's first output frame).  videos is the host copy (validation, launch shapes), videos_dev the same values on the
+ * device.  The call only enqueues kernels: no workspace, no allocation and no host synchronisation, so it can be captured
+ * in a CUDA graph and replayed on new pixels; a frame's output depends on its own pixels and its video's size only.  Bad
+ * arguments (no video, a side of 0 or above 65500, a video without frames, first_frame not the running frame count, pixels
+ * outside src_bytes, dst smaller than the call's frames, NULL pointers, dst overlapping src) return SSNB_EINVAL before any
+ * launch. */
+typedef struct {
+  int64_t src_offset;      /* bytes: the video's first frame in src */
+  int64_t first_frame;     /* frames of the videos before this one */
+  int32_t height, width;   /* 1 .. 65500 */
+  int32_t frames;          /* >= 1 */
+  int32_t reserved;
+} ssnb_resize_video;
+int ssnb_frame_resize(const uint8_t* src, int64_t src_bytes, const ssnb_resize_video* videos, const ssnb_resize_video* videos_dev,
+                      int n_videos, int dst_height, int dst_width, uint8_t* dst, int64_t dst_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
