@@ -1,23 +1,29 @@
 // JPEG encode on the GPU, byte for byte Image.save(f, quality=q) through libjpeg-turbo (and cv2.imencode at the same quality):
-// the img_%05d.jpg / flow_{x,y}_%05d.jpg files of DenseFlow's extraction step, many ragged images per call.  The stages are
-// those of oracle/jpeg_encode_oracle.py, which names the libjpeg-turbo function each one follows.  Device, in launch order:
+// the img_%05d.jpg / flow_{x,y}_%05d.jpg files of DenseFlow's extraction step, many ragged images per call, optionally with
+// Pillow's restart_marker_blocks / restart_marker_rows.  The stages are those of oracle/jpeg_encode_oracle.py, which names
+// the libjpeg-turbo function each one follows, and the restart rules those of oracle/jpeg_restart_oracle.py.  Device, in
+// launch order:
 //
 //   enc_setup_kernel    one CTA: each image's MCU, bit-buffer word, chunk and output-slot offsets (exclusive scans of sizes
-//                       the host computes the same way, so the call needs no host round trip).
+//                       the host computes the same way, so the call needs no host round trip) and its restart interval.
 //   enc_coef_kernel     one thread per 8x8 block (a warp per block position of the MCU, 32 MCUs per CTA): samples with edge
 //                       expansion, rgb_ycc_convert and h2v2 downsampling, islow FDCT, rounded quantisation, stored in zig-zag
 //                       order; and the bits of the block's AC codes.  Dummy blocks (past the luma plane's right / bottom edge
 //                       inside the last MCU) are zero with an EOB.
-//   enc_scan_kernel     one CTA per image: each block's bit length (its AC bits plus its DC difference's code), an exclusive
-//                       scan into bit offsets, the image's byte count; zeroes the image's bit buffer and sets the 1-bit padding.
-//   enc_pack_kernel     one thread per block: Huffman codes ORed into the bit buffer (32-bit words, most significant bit first).
-//   enc_count_kernel    one CTA per 4 KB chunk of an image's bytes: its 0xFF bytes.
-//   enc_finish_kernel   one CTA per image: an exclusive scan of the chunk counts into stuffing offsets, the header (with the
-//                       image's size in SOF0), EOI and the file's length.
-//   enc_scatter_kernel  one CTA per chunk: the bytes at their stuffed positions, 0x00 after every 0xFF.
+//   enc_scan_kernel     one CTA per image: each block's bit length (its AC bits plus its DC difference's code, the predictor
+//                       reset at each restart interval), a segmented scan into bit offsets in which every interval starts on
+//                       a byte, the image's byte count; zeroes the image's bit buffer and its interval-end bitmap.
+//   enc_pack_kernel     one thread per block: Huffman codes ORed into the bit buffer (32-bit words, most significant bit first);
+//                       the last block of each interval adds the 1-bit padding and marks the interval's last byte.
+//   enc_count_kernel    one CTA per 4 KB chunk of an image's bytes: its 0xFF bytes and interval ends.
+//   enc_finish_kernel   one CTA per image: an exclusive scan of the chunk counts into stuffing and marker offsets, the header
+//                       (with the image's size in SOF0 and its interval in DRI), EOI and the file's length.
+//   enc_scatter_kernel  one CTA per chunk: the bytes at their stuffed positions, 0x00 after every 0xFF, FF D0+k after the last
+//                       byte of interval k (mod 8) but the image's last.
 //
-// Grids are sized for each image's worst case (known from its size); CTAs past an image's actual bytes return at once.  The
-// per-block stages of enc_coef_kernel live in jpeg_block.cuh, which the round trip (jpeg_roundtrip.cu) calls too.
+// Without a restart interval an image is one interval: no marker, no DRI, the bytes of Image.save(f, quality=q).  Grids are
+// sized for each image's worst case (known from its size); CTAs past an image's actual bytes return at once.  The per-block
+// stages of enc_coef_kernel live in jpeg_block.cuh, which the round trip (jpeg_roundtrip.cu) calls too.
 #include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
@@ -36,7 +42,9 @@ namespace {
 constexpr int kMaxBlockBits = 22 + 63 * 26;      // a DC code of <= 11 bits + 11 value bits, 63 AC codes of <= 16 + 10 bits
 constexpr int kChunk = 4096, kChunkThreads = 256, kChunkBytesPerThread = kChunk / kChunkThreads;
 constexpr int kScanThreads = 1024, kMcusPerCta = 32;
-constexpr int kMaxHeader = 624;
+constexpr int kMaxHeader = 632;                   // RGB: 623 bytes, 629 with DRI
+constexpr int kMaxInterval = 65535;               // DRI's 16 bits (jcmaster.c clamps restart_in_rows * MCUs_per_row to it)
+constexpr int kMarkShift = 36;                    // a chunk count: its 0xFF bytes + (its interval ends << kMarkShift)
 
 // ---------------------------------------------------------------------------------------------------------------- tables
 
@@ -95,75 +103,90 @@ constexpr HuffSet make_huff() {
 __device__ const HuffSet d_huff = make_huff();
 enum { kDC0 = 0, kAC0 = 1, kDC1 = 2, kAC1 = 3 };
 
-// the call's constants, passed by value: quantisation divisors and the header with SOF0's size left for each image
+// the call's constants, passed by value: quantisation divisors and the header with SOF0's size and DRI's interval left for
+// each image
 struct EncConst {
   int32_t div[2][64];              // quantval << 3 (the islow FDCT's output is scaled by 8), natural order
   uint8_t header[kMaxHeader];
   int32_t header_len, sof_size;    // sof_size: offset of SOF0's height (then width), big-endian 16-bit each
+  int32_t dri;                     // offset of DRI's interval (big-endian 16-bit), 0 when the call writes no DRI
   int32_t comps, bpm;              // components, blocks per MCU (1 or 6)
 };
 
 struct DevEnc {
   int64_t src, out;                // the image's first byte in src, its output slot
   int64_t mcu0, word0, chunk0;     // first MCU, bit-buffer word and byte chunk in the call's arrays
+  int64_t mark0;                   // first word of the interval-end bitmap (bit j of word i: byte 32 i + j ends an interval)
   int64_t nbytes;                  // entropy-coded bytes before stuffing, padding included (enc_scan_kernel)
   int32_t h, w, mcux, mcuy;
+  int32_t rst, dri, intervals;     // MCUs per interval (the image's MCUs without one), DRI's value (0: none), intervals
 };
 
+// an image's sizes.  Interval k of K carries b_k bits, at most its blocks times kMaxBlockBits, padded to ceil(b_k / 8) <=
+// (b_k + 7) / 8 bytes, so raw = floor((blocks * kMaxBlockBits + 7 K) / 8) bounds the entropy-coded bytes; the slot holds the
+// header (with DRI when the call has an interval), raw bytes each stuffed, 2 marker bytes per interval but the first, EOI.
 struct Geo {
-  int mcux, mcuy;
-  int64_t mcus, blocks, raw, words, chunks, capacity;
+  int mcux, mcuy, dri;
+  int64_t mcus, blocks, intervals, raw, words, marks, chunks, capacity;
 };
 
-__host__ __device__ inline Geo geometry(int comps, int header_len, int h, int w) {
+__host__ __device__ inline Geo geometry(int comps, int header_len, int h, int w, int restart_blocks, int restart_rows) {
   Geo g;
   const int m = comps == 1 ? 8 : 16;
   g.mcux = (w + m - 1) / m;
   g.mcuy = (h + m - 1) / m;
   g.mcus = (int64_t)g.mcux * g.mcuy;
   g.blocks = g.mcus * (comps == 1 ? 1 : 6);
-  g.raw = (g.blocks * kMaxBlockBits + 7) / 8;
+  // jcmaster.c per_scan_setup: restart_in_rows * MCUs_per_row, clamped to 65535, per image
+  g.dri = restart_blocks ? restart_blocks : restart_rows ? (int)((int64_t)restart_rows * g.mcux < kMaxInterval ? (int64_t)restart_rows * g.mcux : kMaxInterval) : 0;
+  g.intervals = g.dri ? (g.mcus + g.dri - 1) / g.dri : 1;
+  g.raw = (g.blocks * kMaxBlockBits + 7 * g.intervals) / 8;
   g.words = (g.raw + 3) / 4;
+  g.marks = g.intervals > 1 ? (g.raw + 31) / 32 : 0;
   g.chunks = (g.raw + kChunk - 1) / kChunk;
-  g.capacity = header_len + 2 * g.raw + 2;
+  g.capacity = header_len + 2 * g.raw + 2 * (g.intervals - 1) + 2;
   return g;
 }
 
 // ------------------------------------------------------------------------------------------------------------- setup
 
 __global__ void __launch_bounds__(kScanThreads) enc_setup_kernel(const ssnb_jpeg_encode_image* __restrict__ img, int n, int comps,
-                                                                  int header_len, DevEnc* __restrict__ t) {
-  using Scan = cub::BlockScan<long long, kScanThreads>;
+                                                                  int header_len, int restart_blocks, int restart_rows,
+                                                                  DevEnc* __restrict__ t) {
+  using Scan = cub::BlockScan<long long, kScanThreads, cub::BLOCK_SCAN_WARP_SCANS>;
   __shared__ typename Scan::TempStorage tmp;
   long long carry[4] = {0, 0, 0, 0};
   for (int base = 0; base < n; base += kScanThreads) {
     const int i = base + threadIdx.x;
-    ssnb_jpeg_encode_image e{};
-    Geo g{};
-    if (i < n) {
-      e = img[i];
-      g = geometry(comps, header_len, e.height, e.width);
-    }
-    const long long v[4] = {g.mcus, g.words, g.chunks, g.capacity};
-    long long o[4], tot[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      Scan(tmp).ExclusiveSum(v[k], o[k], tot[k]);
-      __syncthreads();
-    }
-    if (i < n) {
+    long long v[4] = {0, 0, 0, 0}, words = 0;
+    if (i < n) {                                        // every field but the offsets; those follow each scan
+      const ssnb_jpeg_encode_image e = img[i];
+      const Geo g = geometry(comps, header_len, e.height, e.width, restart_blocks, restart_rows);
       DevEnc d;
       d.src = e.src_offset;
-      d.mcu0 = carry[0] + o[0];
-      d.word0 = carry[1] + o[1];
-      d.chunk0 = carry[2] + o[2];
-      d.out = carry[3] + o[3];
       d.nbytes = 0;
       d.h = e.height; d.w = e.width; d.mcux = g.mcux; d.mcuy = g.mcuy;
+      d.rst = g.dri ? g.dri : (int)g.mcus;
+      d.dri = g.dri;
+      d.intervals = (int)g.intervals;
       t[i] = d;
+      v[0] = g.mcus; v[1] = g.words + g.marks; v[2] = g.chunks; v[3] = g.capacity;
+      words = g.words;
     }
 #pragma unroll
-    for (int k = 0; k < 4; ++k) carry[k] += tot[k];
+    for (int k = 0; k < 4; ++k) {
+      long long o, tot;
+      Scan(tmp).ExclusiveSum(v[k], o, tot);
+      __syncthreads();
+      o += carry[k];
+      carry[k] += tot;
+      if (i < n) {
+        if (k == 0) t[i].mcu0 = o;
+        if (k == 1) { t[i].word0 = o; t[i].mark0 = o + words; }
+        if (k == 2) t[i].chunk0 = o;
+        if (k == 3) t[i].out = o;
+      }
+    }
   }
 }
 
@@ -256,47 +279,105 @@ __device__ __forceinline__ int64_t prev_same(int bpm, int64_t lb) {
 }
 
 // the DC difference of block lb of an image whose blocks start at coef + b0 * 64.  A dummy block carries the DC of the block
-// before it (jccoefct.c), so its difference is 0 and the next block predicts from the last real block.
+// before it (jccoefct.c), so its difference is 0 and the next block predicts from the last real block.  The predictors
+// restart at 0 with each interval (jchuff.c emit_restart), whose first block is an MCU's first luma block, never a dummy.
 __device__ int dc_diff(const DevEnc& im, int bpm, const int16_t* __restrict__ coef, int64_t b0, int64_t lb) {
   if (is_dummy(im, bpm, lb)) return 0;
+  int64_t first = 0;                                  // the interval's first block (an image's blocks fit 31 bits)
+  if (im.intervals > 1) {
+    const int m = bpm == 1 ? (int)lb : (int)lb / 6;
+    first = (int64_t)(m - m % im.rst) * bpm;
+  }
   int64_t p = prev_same(bpm, lb);
-  while (p >= 0 && is_dummy(im, bpm, p)) p = prev_same(bpm, p);
-  return coef[(b0 + lb) * 64] - (p < 0 ? 0 : coef[(b0 + p) * 64]);
+  while (p >= first && is_dummy(im, bpm, p)) p = prev_same(bpm, p);
+  return coef[(b0 + lb) * 64] - (p < first ? 0 : coef[(b0 + p) * 64]);
 }
 
 __device__ __forceinline__ bool chroma_block(int bpm, int64_t lb) { return bpm == 6 && lb % 6 >= 4; }
 
+// the bit offset after a run of blocks as a function of the offset before it: x + a when no interval starts inside the run,
+// else ceil8(x + a) + b (a: the bits before the first interval start, b: those after the last, intervals between whole
+// bytes).  Composition is associative, so a block scan of one element per block gives every block's offset with each
+// interval byte aligned.  Within one pass of kScanThreads blocks a and b stay below kScanThreads * (kMaxBlockBits + 7) <
+// 2^21, so the block scan runs on one 64-bit word per run (a, b and the flag packed); the carry between passes is a Seg.
+struct Seg {
+  long long a, b;
+  bool starts;                     // does an interval start in the run?
+};
+__device__ __forceinline__ long long ceil8(long long x) { return (x + 7) & ~7ll; }
+__device__ __forceinline__ Seg seg_then(const Seg& l, const Seg& r) {          // l, then r
+  if (!r.starts) return l.starts ? Seg{l.a, l.b + r.a, true} : Seg{l.a + r.a, 0, false};
+  return l.starts ? Seg{l.a, ceil8(l.b + r.a) + r.b, true} : Seg{l.a + r.a, r.b, true};
+}
+__device__ __forceinline__ long long seg_end(const Seg& f) { return f.starts ? ceil8(f.a) + f.b : f.a; }
+constexpr int kSegBits = 22;
+static_assert(kScanThreads * (kMaxBlockBits + 7) < (1 << kSegBits), "a pass's bits must fit a packed Seg field");
+__device__ __forceinline__ unsigned long long seg_pack(const Seg& f) {
+  return (unsigned long long)f.a | (unsigned long long)f.b << kSegBits | (unsigned long long)f.starts << (2 * kSegBits);
+}
+__device__ __forceinline__ Seg seg_unpack(unsigned long long v) {
+  constexpr unsigned long long m = (1ull << kSegBits) - 1;
+  return Seg{(long long)(v & m), (long long)(v >> kSegBits & m), (bool)(v >> (2 * kSegBits))};
+}
+struct PackedSegThen {
+  __device__ __forceinline__ unsigned long long operator()(unsigned long long l, unsigned long long r) const {
+    return seg_pack(seg_then(seg_unpack(l), seg_unpack(r)));
+  }
+};
+
+// block lb's bit length: its AC bits (enc_coef_kernel) and its DC difference's code
+__device__ __forceinline__ long long block_bits(const DevEnc& im, int bpm, const int16_t* __restrict__ coef,
+                                                const int64_t* __restrict__ bits, int64_t b0, int64_t lb) {
+  const int d = dc_diff(im, bpm, coef, b0, lb), n = nbits(d);
+  return bits[b0 + lb] + d_huff.t[chroma_block(bpm, lb) ? kDC1 : kDC0].size[n] + n;
+}
+
 __global__ void __launch_bounds__(kScanThreads) enc_scan_kernel(DevEnc* __restrict__ t, int bpm, const int16_t* __restrict__ coef,
                                                                  int64_t* __restrict__ bits, uint32_t* __restrict__ words) {
-  using Scan = cub::BlockScan<long long, kScanThreads>;
-  __shared__ typename Scan::TempStorage tmp;
+  using Sum = cub::BlockScan<long long, kScanThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+  using SegScan = cub::BlockScan<unsigned long long, kScanThreads, cub::BLOCK_SCAN_WARP_SCANS>;
+  __shared__ union {
+    typename Sum::TempStorage sum;
+    typename SegScan::TempStorage seg;
+  } tmp;
   const DevEnc im = t[blockIdx.x];
   const int64_t b0 = im.mcu0 * bpm, nb = (int64_t)im.mcux * im.mcuy * bpm;
-  long long carry = 0;
-  for (int64_t base = 0; base < nb; base += kScanThreads) {
-    const int64_t lb = base + threadIdx.x;
-    long long len = 0, off, tot;
-    if (lb < nb) {
-      const int d = dc_diff(im, bpm, coef, b0, lb), n = nbits(d);
-      len = bits[b0 + lb] + d_huff.t[chroma_block(bpm, lb) ? kDC1 : kDC0].size[n] + n;
+  long long end = 0;                                    // the image's bits, each interval padded to a byte but the last
+  if (im.intervals == 1) {                              // one interval: a sum of the block lengths
+    for (int64_t base = 0; base < nb; base += kScanThreads) {
+      const int64_t lb = base + threadIdx.x;
+      long long len = 0, off, tot;
+      if (lb < nb) len = block_bits(im, bpm, coef, bits, b0, lb);
+      Sum(tmp.sum).ExclusiveSum(len, off, tot);
+      if (lb < nb) bits[b0 + lb] = end + off;
+      end += tot;
+      __syncthreads();
     }
-    Scan(tmp).ExclusiveSum(len, off, tot);
-    if (lb < nb) bits[b0 + lb] = carry + off;
-    carry += tot;
-    __syncthreads();
+  } else {
+    Seg carry{0, 0, false};
+    for (int64_t base = 0; base < nb; base += kScanThreads) {
+      const int64_t lb = base + threadIdx.x;
+      long long len = 0;
+      unsigned long long v = 0, inc, tot;
+      if (lb < nb) {
+        len = block_bits(im, bpm, coef, bits, b0, lb);
+        const int m = bpm == 1 ? (int)lb : (int)lb / 6;
+        const bool starts = lb > 0 && m * bpm == lb && m % im.rst == 0;
+        v = seg_pack(starts ? Seg{0, len, true} : Seg{len, 0, false});
+      }
+      SegScan(tmp.seg).InclusiveScan(v, inc, PackedSegThen(), tot);
+      if (lb < nb) bits[b0 + lb] = seg_end(seg_then(carry, seg_unpack(inc))) - len;
+      carry = seg_then(carry, seg_unpack(tot));
+      __syncthreads();
+    }
+    end = seg_end(carry);
   }
-  const int64_t nbytes = (carry + 7) >> 3, nwords = (nbytes + 3) >> 2;
+  const int64_t nbytes = (end + 7) >> 3, nwords = (nbytes + 3) >> 2;
+  const int64_t nmarks = im.intervals > 1 ? (nbytes + 31) >> 5 : 0;
   uint32_t* w = words + im.word0;
   for (int64_t j = threadIdx.x; j < nwords; j += blockDim.x) w[j] = 0;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    if (carry & 7) {                                    // jchuff.c flush_bits: pad the last byte with 1-bits
-      const int64_t e = nbytes * 8 - 1;
-      const int npad = (int)(e - carry + 1);
-      w[e >> 5] |= ((1u << npad) - 1) << (31 - (int)(e & 31));
-    }
-    t[blockIdx.x].nbytes = nbytes;
-  }
+  for (int64_t j = threadIdx.x; j < nmarks; j += blockDim.x) words[im.mark0 + j] = 0;
+  if (threadIdx.x == 0) t[blockIdx.x].nbytes = nbytes;
 }
 
 // ------------------------------------------------------------------------------------------------------------------ pack
@@ -320,6 +401,7 @@ struct BitWriter {
   __device__ __forceinline__ void flush() {
     if (n) atomicOr(w + word, (uint32_t)(acc << (32 - n)));
   }
+  __device__ __forceinline__ int64_t pos() const { return word * 32 + n; }
 };
 
 __global__ void __launch_bounds__(kMcusPerCta * 6) enc_pack_kernel(const DevEnc* __restrict__ t, int n, int64_t total_mcus, int bpm,
@@ -348,6 +430,15 @@ __global__ void __launch_bounds__(kMcusPerCta * 6) enc_pack_kernel(const DevEnc*
     run = 0;
   }
   if (run) bw.put(ac.code[0], ac.size[0]);
+  const int m = (int)(mcu - im.mcu0);
+  if (kb == bpm - 1 && (m + 1 == im.mcux * im.mcuy || (im.intervals > 1 && (m + 1) % im.rst == 0))) {
+    const int npad = (int)(-bw.pos() & 7);             // jchuff.c flush_bits: the interval's last byte padded with 1-bits
+    bw.put((1u << npad) - 1, npad);
+    if (m + 1 < im.mcux * im.mcuy) {                    // an RST follows this byte
+      const int64_t last = (bw.pos() >> 3) - 1;
+      atomicOr(words + im.mark0 + (last >> 5), 1u << (last & 31));
+    }
+  }
   bw.flush();
 }
 
@@ -369,6 +460,12 @@ __device__ __forceinline__ int load_bytes(const uint32_t* __restrict__ w, int64_
   return ff;
 }
 
+// which of this thread's bytes [start, start + 16) end an interval that an RST follows: bit j for byte start + j
+__device__ __forceinline__ uint32_t load_marks(const DevEnc& im, const uint32_t* __restrict__ words, int64_t start) {
+  if (im.intervals == 1 || start >= im.nbytes) return 0u;
+  return (words[im.mark0 + (start >> 5)] >> (start & 31)) & 0xFFFFu;
+}
+
 __global__ void __launch_bounds__(kChunkThreads) enc_count_kernel(const DevEnc* __restrict__ t, int n, const uint32_t* __restrict__ words,
                                                                    int64_t* __restrict__ counts) {
   using Reduce = cub::BlockReduce<int, kChunkThreads>;
@@ -376,10 +473,11 @@ __global__ void __launch_bounds__(kChunkThreads) enc_count_kernel(const DevEnc* 
   const DevEnc im = t[find_image<&DevEnc::chunk0>(t, n, blockIdx.x)];
   const int64_t first = ((int64_t)blockIdx.x - im.chunk0) * kChunk;
   if (first >= im.nbytes) return;
+  const int64_t start = first + threadIdx.x * kChunkBytesPerThread;
   uint8_t b[kChunkBytesPerThread];
-  const int ff = load_bytes(words + im.word0, first + threadIdx.x * kChunkBytesPerThread, im.nbytes, b);
-  const int total = Reduce(tmp).Sum(ff);
-  if (threadIdx.x == 0) counts[blockIdx.x] = total;
+  const int ff = load_bytes(words + im.word0, start, im.nbytes, b);
+  const int total = Reduce(tmp).Sum(ff | __popc(load_marks(im, words, start)) << 16);    // each <= 4096 per chunk
+  if (threadIdx.x == 0) counts[blockIdx.x] = (total & 0xFFFF) | (int64_t)(total >> 16) << kMarkShift;
 }
 
 __global__ void __launch_bounds__(kChunkThreads) enc_finish_kernel(const DevEnc* __restrict__ t, EncConst c, int64_t* __restrict__ counts,
@@ -401,11 +499,11 @@ __global__ void __launch_bounds__(kChunkThreads) enc_finish_kernel(const DevEnc*
   uint8_t* dst = out + im.out;
   const uint8_t size[4] = {(uint8_t)(im.h >> 8), (uint8_t)im.h, (uint8_t)(im.w >> 8), (uint8_t)im.w};
   for (int j = threadIdx.x; j < c.header_len; j += blockDim.x) {
-    const int k = j - c.sof_size;
-    dst[j] = k >= 0 && k < 4 ? size[k] : c.header[j];
+    const int k = j - c.sof_size, r = j - c.dri;
+    dst[j] = k >= 0 && k < 4 ? size[k] : c.dri && r >= 0 && r < 2 ? (uint8_t)(im.dri >> (8 - 8 * r)) : c.header[j];
   }
   if (threadIdx.x == 0) {
-    const int64_t e = c.header_len + im.nbytes + carry;
+    const int64_t e = c.header_len + im.nbytes + (carry & ((1ll << kMarkShift) - 1)) + 2 * (carry >> kMarkShift);
     dst[e] = 0xFF;
     dst[e + 1] = 0xD9;
     lengths[blockIdx.x] = e + 2;
@@ -423,14 +521,23 @@ __global__ void __launch_bounds__(kChunkThreads) enc_scatter_kernel(const DevEnc
   const int64_t start = first + threadIdx.x * kChunkBytesPerThread;
   uint8_t b[kChunkBytesPerThread];
   const int ff = load_bytes(words + im.word0, start, im.nbytes, b);
+  const uint32_t mk = load_marks(im, words, start);
   int before;
-  Scan(tmp).ExclusiveSum(ff, before);
-  uint8_t* dst = out + im.out + header_len + start + counts[blockIdx.x] + before;
+  Scan(tmp).ExclusiveSum(ff | __popc(mk) << 16, before);
+  const int64_t c = counts[blockIdx.x];
+  const int64_t ff_before = (c & ((1ll << kMarkShift) - 1)) + (before & 0xFFFF), rst_before = (c >> kMarkShift) + (before >> 16);
+  uint8_t* dst = out + im.out + header_len + start + ff_before + 2 * rst_before;
+  int rst = (int)(rst_before & 7);
 #pragma unroll
   for (int j = 0; j < kChunkBytesPerThread; ++j) {
     if (start + j >= im.nbytes) break;
     *dst++ = b[j];
     if (b[j] == 0xFF) *dst++ = 0;
+    if (mk >> j & 1) {                                  // jchuff.c emit_restart: RSTk after the interval's padded last byte
+      *dst++ = 0xFF;
+      *dst++ = (uint8_t)(0xD0 + rst);
+      rst = (rst + 1) & 7;
+    }
   }
 }
 
@@ -443,8 +550,9 @@ void put16(std::vector<uint8_t>& h, int v) {
   h.push_back((uint8_t)v);
 }
 
-// jcparam.c jpeg_set_quality(quality, TRUE) and jcmarker.c's header (oracle/jpeg_encode_oracle.py quant_tables / header)
-EncConst make_const(int comps, int quality) {
+// jcparam.c jpeg_set_quality(quality, TRUE) and jcmarker.c's header (oracle/jpeg_encode_oracle.py quant_tables / header), with
+// write_scan_header's DRI before SOS when the call has a restart interval (oracle/jpeg_restart_oracle.py header)
+EncConst make_const(int comps, int quality, bool restart) {
   EncConst c;
   memset(&c, 0, sizeof c);
   int q[2][64];
@@ -473,6 +581,11 @@ EncConst make_const(int comps, int quality) {
       h.insert(h.end(), s.bits, s.bits + 16);
       h.insert(h.end(), s.vals, s.vals + s.count);
     }
+  if (restart) {
+    h.insert(h.end(), {0xFF, 0xDD, 0, 4});
+    c.dri = (int)h.size();
+    h.insert(h.end(), {0, 0});
+  }
   h.insert(h.end(), {0xFF, 0xDA});
   put16(h, 6 + 2 * comps);
   h.push_back((uint8_t)comps);
@@ -486,7 +599,7 @@ EncConst make_const(int comps, int quality) {
   return c;
 }
 
-int header_len(int comps) { return make_const(comps, 50).header_len; }
+int header_len(int comps, bool restart) { return make_const(comps, 50, restart).header_len; }
 
 struct Layout {
   int64_t mcus = 0, blocks = 0, words = 0, chunks = 0, out_bytes = 0;
@@ -495,20 +608,31 @@ struct Layout {
 
 bool check_image_size(int h, int w) { return h >= 1 && w >= 1 && h <= kJpegEncMaxSide && w <= kJpegEncMaxSide; }
 
+// an empty string when the restart options are acceptable, else the reason
+std::string check_restart(int restart_blocks, int restart_rows) {
+  if (restart_blocks < 0 || restart_rows < 0) return "restart_blocks and restart_rows must be >= 0";
+  if (restart_blocks && restart_rows) return "restart_blocks and restart_rows cannot both be set";
+  if (restart_blocks > kMaxInterval) return "restart_blocks must be <= " + std::to_string(kMaxInterval);
+  return "";
+}
+
 // the call's sizes; an empty string when the arguments are acceptable, else the reason
-std::string plan(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, int64_t src_bytes, Layout& L) {
+std::string plan(int mode, int quality, int restart_blocks, int restart_rows, const ssnb_jpeg_encode_image* images, int n,
+                 int64_t src_bytes, Layout& L) {
   if (mode != SSNB_JPEG_ENC_L && mode != SSNB_JPEG_ENC_RGB) return "mode must be SSNB_JPEG_ENC_L (1) or SSNB_JPEG_ENC_RGB (3)";
   if (quality < 1 || quality > 100) return "quality must be 1 .. 100";
+  const std::string why = check_restart(restart_blocks, restart_rows);
+  if (!why.empty()) return why;
   if (n < 1 || !images) return "no image, or NULL images";
-  const int hl = header_len(mode);
+  const int hl = header_len(mode, restart_blocks || restart_rows);
   for (int i = 0; i < n; ++i) {
     const ssnb_jpeg_encode_image& e = images[i];
     if (!check_image_size(e.height, e.width))
       return "image " + std::to_string(i) + ": height and width must be 1 .. " + std::to_string(kJpegEncMaxSide);
     if (src_bytes >= 0 && (e.src_offset < 0 || e.src_offset + (int64_t)e.height * e.width * mode > src_bytes))
       return "image " + std::to_string(i) + ": pixels outside src";
-    const Geo g = geometry(mode, hl, e.height, e.width);
-    L.mcus += g.mcus; L.blocks += g.blocks; L.words += g.words; L.chunks += g.chunks; L.out_bytes += g.capacity;
+    const Geo g = geometry(mode, hl, e.height, e.width, restart_blocks, restart_rows);
+    L.mcus += g.mcus; L.blocks += g.blocks; L.words += g.words + g.marks; L.chunks += g.chunks; L.out_bytes += g.capacity;
   }
   if ((L.mcus + kMcusPerCta - 1) / kMcusPerCta > INT32_MAX || L.chunks > INT32_MAX) return "too many blocks in one call";
   size_t o = align256((size_t)n * sizeof(DevEnc));
@@ -527,14 +651,19 @@ using namespace ssnb;
 
 extern "C" {
 
-int64_t ssnb_jpeg_encode_capacity(int mode, int height, int width) {
-  if ((mode != SSNB_JPEG_ENC_L && mode != SSNB_JPEG_ENC_RGB) || !check_image_size(height, width)) return 0;
-  return geometry(mode, header_len(mode), height, width).capacity;
+int64_t ssnb_jpeg_encode_restart_capacity(int mode, int height, int width, int restart_blocks, int restart_rows) {
+  if ((mode != SSNB_JPEG_ENC_L && mode != SSNB_JPEG_ENC_RGB) || !check_image_size(height, width) ||
+      !check_restart(restart_blocks, restart_rows).empty())
+    return 0;
+  return geometry(mode, header_len(mode, restart_blocks || restart_rows), height, width, restart_blocks, restart_rows).capacity;
 }
 
-int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, size_t* workspace_bytes, int64_t* out_bytes) {
+int64_t ssnb_jpeg_encode_capacity(int mode, int height, int width) { return ssnb_jpeg_encode_restart_capacity(mode, height, width, 0, 0); }
+
+int ssnb_jpeg_encode_restart_sizes(int mode, int quality, int restart_blocks, int restart_rows, const ssnb_jpeg_encode_image* images, int n,
+                                   size_t* workspace_bytes, int64_t* out_bytes) {
   Layout L;
-  const std::string why = plan(mode, quality, images, n, -1, L);
+  const std::string why = plan(mode, quality, restart_blocks, restart_rows, images, n, -1, L);
   if (!why.empty()) {
     set_thread_error("jpeg_encode: " + why);
     return SSNB_EINVAL;
@@ -544,19 +673,23 @@ int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* 
   return SSNB_OK;
 }
 
-int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
-                     const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
-                     size_t workspace_bytes, void* stream) {
+int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* images, int n, size_t* workspace_bytes, int64_t* out_bytes) {
+  return ssnb_jpeg_encode_restart_sizes(mode, quality, 0, 0, images, n, workspace_bytes, out_bytes);
+}
+
+int ssnb_jpeg_encode_restart(int mode, int quality, int restart_blocks, int restart_rows, const uint8_t* src, int64_t src_bytes,
+                             const ssnb_jpeg_encode_image* images, const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out,
+                             int64_t out_bytes, int64_t* lengths, void* workspace, size_t workspace_bytes, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   auto fail = [](const std::string& m) { set_thread_error("jpeg_encode: " + m); return (int)SSNB_EINVAL; };
   Layout L;
-  const std::string why = plan(mode, quality, images, n, src_bytes, L);
+  const std::string why = plan(mode, quality, restart_blocks, restart_rows, images, n, src_bytes, L);
   if (!why.empty()) return fail(why);
   if (!src || !images_dev || !out || !lengths || !workspace) return fail("NULL src, images_dev, out, lengths or workspace");
   if ((uintptr_t)workspace % 256) return fail("workspace must be 256-byte aligned");
   if (out_bytes < L.out_bytes) return fail("out holds fewer bytes than the images' slots (ssnb_jpeg_encode_sizes)");
   if (workspace_bytes < L.workspace) return fail("workspace too small (ssnb_jpeg_encode_sizes)");
-  const EncConst c = make_const(mode, quality);
+  const EncConst c = make_const(mode, quality, restart_blocks || restart_rows);
   uint8_t* ws = (uint8_t*)workspace;
   DevEnc* t = (DevEnc*)ws;
   int16_t* coef = (int16_t*)(ws + L.off_coef);
@@ -564,7 +697,7 @@ int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_byte
   uint32_t* words = (uint32_t*)(ws + L.off_words);
   int64_t* counts = (int64_t*)(ws + L.off_counts);
   const unsigned mcu_ctas = (unsigned)((L.mcus + kMcusPerCta - 1) / kMcusPerCta);
-  enc_setup_kernel<<<1, kScanThreads, 0, s>>>(images_dev, n, mode, c.header_len, t);
+  enc_setup_kernel<<<1, kScanThreads, 0, s>>>(images_dev, n, mode, c.header_len, restart_blocks, restart_rows, t);
   SSNB_LAUNCH_CHECK("enc_setup_kernel");
   enc_coef_kernel<<<mcu_ctas, kMcusPerCta * c.bpm, 0, s>>>(t, n, L.mcus, c, src, coef, bits);
   SSNB_LAUNCH_CHECK("enc_coef_kernel");
@@ -579,6 +712,13 @@ int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_byte
   enc_scatter_kernel<<<(unsigned)L.chunks, kChunkThreads, 0, s>>>(t, n, c.header_len, words, counts, out);
   SSNB_LAUNCH_CHECK("enc_scatter_kernel");
   return SSNB_OK;
+}
+
+int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
+                     const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  return ssnb_jpeg_encode_restart(mode, quality, 0, 0, src, src_bytes, images, images_dev, n, out, out_bytes, lengths, workspace,
+                                  workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -15,7 +15,10 @@ reason; there is no CPU fallback.
 
 encode_jpeg is the other direction, the files of the extraction step (DenseFlow's img_%05d.jpg and flow_{x,y}_%05d.jpg):
 CUDA uint8 images -> the bytes Pillow's Image.save(f, quality=q) writes, computed by csrc/jpeg_encode.cu.  JpegEncodePlan
-keeps one call's buffers so the encode can be repeated or captured in a CUDA graph.
+keeps one call's buffers so the encode can be repeated or captured in a CUDA graph.  restart_marker_blocks /
+restart_marker_rows write Pillow's restart intervals, so that decode_jpeg splits each file into independent intervals:
+
+    files = encode_jpeg(frames, mode='RGB', quality=95, restart_marker_rows=1)    # 16 intervals per 340 x 256 frame
 
 jpeg_roundtrip joins the two without the files: CUDA uint8 images -> what decode_jpeg returns for the files encode_jpeg
 writes of them (csrc/jpeg_roundtrip.cu, no Huffman coding), so decoded video frames or flow planes become the exact inputs
@@ -246,15 +249,28 @@ def collate_jpeg(batch):
 _ENC_MODES = {"L": (JPEG_ENC_L, 1), "RGB": (JPEG_ENC_RGB, 3)}
 
 
-def jpeg_encode_capacity(mode, height, width):
-    """the bytes the encoder reserves for one image's file (its worst case; 0 for a bad mode or size)"""
-    return int(lib.ssnb_jpeg_encode_capacity(_ENC_MODES[mode][0] if mode in _ENC_MODES else 0, int(height), int(width)))
+def jpeg_encode_capacity(mode, height, width, restart_marker_blocks=0, restart_marker_rows=0):
+    """the bytes the encoder reserves for one image's file (its worst case; 0 for a bad mode, size or restart option)"""
+    return int(lib.ssnb_jpeg_encode_restart_capacity(_ENC_MODES[mode][0] if mode in _ENC_MODES else 0, int(height), int(width),
+                                                     int(restart_marker_blocks), int(restart_marker_rows)))
 
 
 def _enc_mode(mode):
     if mode not in _ENC_MODES:
         raise ValueError("encode_jpeg: mode must be 'RGB' or 'L'")
     return _ENC_MODES[mode]
+
+
+def _enc_restart(restart_marker_blocks, restart_marker_rows):
+    """the restart options as ints; ValueError for those the library refuses (both set, negative, blocks above 65535)"""
+    b, r = int(restart_marker_blocks), int(restart_marker_rows)
+    if b < 0 or r < 0:
+        raise ValueError("encode_jpeg: restart_marker_blocks and restart_marker_rows must be >= 0")
+    if b and r:
+        raise ValueError("encode_jpeg: restart_marker_blocks and restart_marker_rows cannot both be set")
+    if b > 65535:
+        raise ValueError("encode_jpeg: restart_marker_blocks must be <= 65535 (DRI's 16 bits)")
+    return b, r
 
 
 def _pixel_buffer(images, sizes, channels, mode, what):
@@ -280,13 +296,16 @@ def _pixel_buffer(images, sizes, channels, mode, what):
 
 
 class JpegEncodePlan:
-    """One encode call's sizes, mode and quality with its device buffers: the image table, the workspace, the output slots
-    (image i's file starts at out[slots[i]]) and the int64 lengths.  plan.run(images) only enqueues, so it can be repeated
-    or captured in a CUDA graph on new pixels of the same sizes; plan.files() waits and returns one bytes object per image."""
+    """One encode call's sizes, mode, quality and restart option with its device buffers: the image table, the workspace, the
+    output slots (image i's file starts at out[slots[i]]) and the int64 lengths.  plan.run(images) only enqueues, so it can be
+    repeated or captured in a CUDA graph on new pixels of the same sizes; plan.files() waits and returns one bytes object per
+    image."""
 
-    def __init__(self, sizes, mode="RGB", quality=95, device=None):
+    def __init__(self, sizes, mode="RGB", quality=95, device=None, restart_marker_blocks=0, restart_marker_rows=0):
         self.mode, self.quality = mode, int(quality)
         self._code, self.channels = _enc_mode(mode)
+        self.restart_marker_blocks, self.restart_marker_rows = _enc_restart(restart_marker_blocks, restart_marker_rows)
+        rst = (self.restart_marker_blocks, self.restart_marker_rows)
         self.sizes = [(int(h), int(w)) for h, w in sizes]
         n = len(self.sizes)
         if n < 1:
@@ -298,9 +317,9 @@ class JpegEncodePlan:
             off += max(h, 0) * max(w, 0) * self.channels
         self.src_bytes = off
         ws, ob = C.c_size_t(), C.c_int64()
-        if lib.ssnb_jpeg_encode_sizes(self._code, self.quality, self.images, n, C.byref(ws), C.byref(ob)) != 0:
+        if lib.ssnb_jpeg_encode_restart_sizes(self._code, self.quality, *rst, self.images, n, C.byref(ws), C.byref(ob)) != 0:
             raise ValueError("encode_jpeg: " + (lib.ssnb_last_error(None) or b"").decode().split(": ", 1)[-1])
-        caps = [lib.ssnb_jpeg_encode_capacity(self._code, h, w) for h, w in self.sizes]
+        caps = [lib.ssnb_jpeg_encode_restart_capacity(self._code, h, w, *rst) for h, w in self.sizes]
         self.slots = np.concatenate([[0], np.cumsum(caps)[:-1]]).astype(np.int64)
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.images_dev = torch.frombuffer(bytearray(bytes(self.images)), dtype=torch.uint8).to(dev)
@@ -319,9 +338,10 @@ class JpegEncodePlan:
             raise ValueError("encode_jpeg: images on %s, plan on %s" % (src.device, self.out.device))
         self._src = src                       # kept alive until the next run
         with torch.cuda.device(self.out.device):
-            rc = lib.ssnb_jpeg_encode(self._code, self.quality, src.data_ptr(), src.numel(), self.images, self.images_dev.data_ptr(),
-                                      len(self.sizes), self.out.data_ptr(), self.out.numel(), self.lengths.data_ptr(),
-                                      self.workspace.data_ptr(), self.workspace.numel(), C.c_void_p(torch.cuda.current_stream().cuda_stream))
+            rc = lib.ssnb_jpeg_encode_restart(self._code, self.quality, self.restart_marker_blocks, self.restart_marker_rows, src.data_ptr(),
+                                              src.numel(), self.images, self.images_dev.data_ptr(), len(self.sizes), self.out.data_ptr(),
+                                              self.out.numel(), self.lengths.data_ptr(), self.workspace.data_ptr(), self.workspace.numel(),
+                                              C.c_void_p(torch.cuda.current_stream().cuda_stream))
         if rc != 0:
             raise RuntimeError("libssn_b200 jpeg_encode failed (code %d): %s" % (rc, (lib.ssnb_last_error(None) or b"").decode()))
         return self.out, self.lengths
@@ -334,10 +354,16 @@ class JpegEncodePlan:
         return [flat[e - l:e] for e, l in zip(ends.tolist(), lens.tolist())]
 
 
-def encode_jpeg(images, mode="RGB", quality=95):
+def encode_jpeg(images, mode="RGB", quality=95, restart_marker_blocks=0, restart_marker_rows=0):
     """Encode CUDA uint8 images on the GPU: [N, H, W, C] or a list of ragged [H, W, C], C = 3 for 'RGB' and 1 for 'L'.  Returns
     one bytes object per image, equal to what Image.fromarray(img).save(f, format='JPEG', quality=quality) writes (Pillow over
-    libjpeg-turbo; cv2.imencode writes the same bytes): baseline, 4:2:0 for 'RGB', no optimize, no metadata.  quality 1 .. 100."""
+    libjpeg-turbo; cv2.imencode writes the same bytes): baseline, 4:2:0 for 'RGB', no optimize, no metadata.  quality 1 .. 100.
+
+    restart_marker_blocks = n (a restart interval of n MCUs, 1 .. 65535; cv2's IMWRITE_JPEG_RST_INTERVAL) or
+    restart_marker_rows = r (r MCU rows per interval, min(r * MCUs per row, 65535) MCUs per image) give the bytes of Pillow's
+    save with the same keyword.  The decoded pixels are those of the file without markers; decode_jpeg decodes each interval
+    in a thread of its own.  Setting both, or a negative value, raises ValueError."""
+    restart = _enc_restart(restart_marker_blocks, restart_marker_rows)
     if torch.is_tensor(images):
         if not images.is_cuda:
             raise RuntimeError("encode_jpeg needs CUDA uint8 images (no CPU path)")
@@ -355,7 +381,7 @@ def encode_jpeg(images, mode="RGB", quality=95):
         sizes, device = [tuple(t.shape[:2]) for t in images], images[0].device
     if len(sizes) == 0:
         return []
-    plan = JpegEncodePlan(sizes, mode, quality, device)
+    plan = JpegEncodePlan(sizes, mode, quality, device, *restart)
     plan.run(images)
     return plan.files()
 

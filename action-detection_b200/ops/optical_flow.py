@@ -132,19 +132,23 @@ def _video_dirs(dirs, counts, what):
     return dirs
 
 
-def _encoded(images, mode, quality):
-    """CUDA uint8 [N, H, W, C] -> the files' bytes from the GPU encoder; anything else -> None (the Pillow path)"""
+def _encoded(images, mode, quality, restart):
+    """CUDA uint8 [N, H, W, C] -> the files' bytes from the GPU encoder; anything else -> None (the Pillow path).  restart:
+    the restart keywords, as encode_jpeg and Image.save take them (checked here for both paths)."""
+    from ops.jpeg import encode_jpeg, _enc_restart
+    _enc_restart(restart["restart_marker_blocks"], restart["restart_marker_rows"])
     if torch.is_tensor(images) and images.is_cuda:
-        from ops.jpeg import encode_jpeg
-        return encode_jpeg(images, mode=mode, quality=quality)
+        return encode_jpeg(images, mode=mode, quality=quality, **restart)
     return None
 
 
-def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
+def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None, restart_marker_blocks=0, restart_marker_rows=0):
     """Write flow_planes' output as DenseFlow does, one directory per video: {prefix}x_{:05d}.jpg and {prefix}y_{:05d}.jpg
     numbered from 1 like img_{:05d}.jpg.  CUDA planes are encoded on the GPU (ops.jpeg.encode_jpeg, one call for all planes),
     host planes through Pillow; the files are the same bytes either way.  dirs: one directory, or one per video with the
-    frame offsets the flow was computed with.  -> the paths written, x then y per pair."""
+    frame offsets the flow was computed with.  restart_marker_blocks / restart_marker_rows: Pillow's restart intervals
+    (encode_jpeg), which let decode_jpeg split each file; the decoded planes do not change.  -> the paths written, x then y
+    per pair."""
     from PIL import Image
     if torch.is_tensor(planes) and planes.is_cuda:
         if planes.dtype != torch.uint8 or planes.dim() != 4 or planes.shape[3] != 1 or planes.shape[0] % 2:
@@ -159,7 +163,8 @@ def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
     if pairs[-1] != n // 2:
         raise ValueError("one directory per video, and offsets that match the planes' %d pairs" % (n // 2))
     dirs = _video_dirs(dirs, np.diff(pairs), "planes' %d pairs" % (n // 2))
-    files = _encoded(planes, "L", quality)
+    restart = dict(restart_marker_blocks=int(restart_marker_blocks), restart_marker_rows=int(restart_marker_rows))
+    files = _encoded(planes, "L", quality, restart)
     paths = []
     for v, d in enumerate(dirs):
         os.makedirs(d, exist_ok=True)
@@ -171,16 +176,17 @@ def write_flow_jpegs(planes, dirs, prefix="flow_", quality=95, offsets=None):
                     with open(path, "wb") as f:
                         f.write(files[i])
                 else:
-                    Image.fromarray(arr[i, :, :, 0]).save(path, quality=quality)
+                    Image.fromarray(arr[i, :, :, 0]).save(path, quality=quality, **restart)
                 paths.append(path)
     return paths
 
 
-def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None):
+def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None, restart_marker_blocks=0, restart_marker_rows=0):
     """Write RGB frames as DenseFlow does, one directory per video: {prefix}{:05d}.jpg numbered from 1, the files SSNDataSet
     reads for RGB.  frames uint8 [N, H, W, 3]: CUDA frames are encoded on the GPU in one call, host frames through Pillow,
     the same bytes either way.  dirs: one directory, or one per video with the frame offsets [V + 1] (as tvl1_flow takes
-    them).  -> the paths written, in frame order."""
+    them).  restart_marker_blocks / restart_marker_rows: Pillow's restart intervals (encode_jpeg), which let decode_jpeg
+    split each file; the decoded frames do not change.  -> the paths written, in frame order."""
     from PIL import Image
     if torch.is_tensor(frames) and frames.is_cuda:
         if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[3] != 3:
@@ -195,7 +201,8 @@ def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None):
     if off.ndim != 1 or len(off) < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
         raise ValueError("one directory per video, and offsets that match the %d frames" % n)
     dirs = _video_dirs(dirs, np.diff(off), "%d frames" % n)
-    files = _encoded(frames, "RGB", quality)
+    restart = dict(restart_marker_blocks=int(restart_marker_blocks), restart_marker_rows=int(restart_marker_rows))
+    files = _encoded(frames, "RGB", quality, restart)
     paths = []
     for v, d in enumerate(dirs):
         os.makedirs(d, exist_ok=True)
@@ -206,7 +213,7 @@ def write_frame_jpegs(frames, dirs, prefix="img_", quality=95, offsets=None):
                 with open(path, "wb") as f:
                     f.write(files[i])
             else:
-                Image.fromarray(arr[i]).save(path, quality=quality)
+                Image.fromarray(arr[i]).save(path, quality=quality, **restart)
             paths.append(path)
     return paths
 

@@ -209,6 +209,10 @@ SIGNATURES = {
     "ssnb_jpeg_encode_capacity": (C.c_int64, [_i, _i, _i]),
     "ssnb_jpeg_encode_sizes": (_i, [_i, _i, C.POINTER(JpegEncodeImage), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
     "ssnb_jpeg_encode": (_i, [_i, _i, _vp, C.c_int64, C.POINTER(JpegEncodeImage), _vp, _i, _vp, C.c_int64, _vp, _vp, _sz, _vp]),
+    "ssnb_jpeg_encode_restart_capacity": (C.c_int64, [_i, _i, _i, _i, _i]),
+    "ssnb_jpeg_encode_restart_sizes": (_i, [_i, _i, _i, _i, C.POINTER(JpegEncodeImage), _i, C.POINTER(_sz), C.POINTER(C.c_int64)]),
+    "ssnb_jpeg_encode_restart": (_i, [_i, _i, _i, _i, _vp, C.c_int64, C.POINTER(JpegEncodeImage), _vp, _i, _vp, C.c_int64, _vp, _vp, _sz,
+                                      _vp]),
     "ssnb_jpeg_roundtrip": (_i, [_i, _i, _vp, C.c_int64, C.POINTER(JpegEncodeImage), _vp, _i, _vp, C.c_int64, _vp]),
     "ssnb_iv3_num_convs": (_i, []),
     "ssnb_iv3_conv_info": (_i, [_i, _i, C.c_char_p, _i] + [_ip] * 7),

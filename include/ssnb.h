@@ -646,9 +646,9 @@ int ssnb_jpeg_decode(ssnb_jpeg_plan plan, const void* table_dev, const uint8_t* 
  * (DenseFlow's img_%05d.jpg and flow_{x,y}_%05d.jpg), byte for byte what Pillow's Image.save(f, quality=q) writes through
  * libjpeg-turbo, and what cv2.imencode writes at the same quality.  Baseline sequential 8-bit JPEG: mode SSNB_JPEG_ENC_L (one
  * component) or SSNB_JPEG_ENC_RGB (YCbCr, luma 2x2 over 1x1 chroma); libjpeg's jpeg_set_quality(quality, force_baseline)
- * tables; the Annex K Huffman tables; no restart interval, no metadata beyond the JFIF APP0.  The stages are those of
+ * tables; the Annex K Huffman tables; no metadata beyond the JFIF APP0.  The stages are those of
  * oracle/jpeg_encode_oracle.py: rgb_ycc_convert, edge expansion, h2v2 downsampling, islow FDCT, rounded quantisation,
- * Huffman coding with ZRL / EOB, 1-bit padding, 0xFF 0x00 stuffing.
+ * Huffman coding with ZRL / EOB, 1-bit padding, 0xFF 0x00 stuffing.  ssnb_jpeg_encode writes no restart interval.
  *
  * Image i is uint8 [height, width, components] (rows packed) at src + images[i].src_offset; its file is written at the
  * start of its output slot, slots back to back in call order, each ssnb_jpeg_encode_capacity bytes: the header, every block
@@ -669,6 +669,24 @@ int ssnb_jpeg_encode_sizes(int mode, int quality, const ssnb_jpeg_encode_image* 
 int ssnb_jpeg_encode(int mode, int quality, const uint8_t* src, int64_t src_bytes, const ssnb_jpeg_encode_image* images,
                      const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out, int64_t out_bytes, int64_t* lengths, void* workspace,
                      size_t workspace_bytes, void* stream);
+
+/* The same encode with restart intervals, byte for byte Image.save(f, quality=q, restart_marker_blocks=restart_blocks) or
+ * Image.save(f, quality=q, restart_marker_rows=restart_rows) (oracle/jpeg_restart_oracle.py), so that a decoder can split
+ * each file's scan into independent intervals (ssnb_jpeg_decode runs one thread per interval).  restart_blocks = n gives
+ * an interval of n MCUs (libjpeg's restart_interval, cv2's IMWRITE_JPEG_RST_INTERVAL); restart_rows = r gives
+ * min(r * MCUs per row, 65535) MCUs, per image from its own width.  The file gets a DRI segment before SOS, and before
+ * every interval but the first the previous one is padded to a byte with 1-bits, FF D0+(k mod 8) follows and the DC
+ * predictors restart at 0; the quantised coefficients, and so the decoded pixels, are those without markers.  Both 0 is
+ * ssnb_jpeg_encode's file, which the three entries above are.  Each slot (ssnb_jpeg_encode_restart_capacity) holds the
+ * header with DRI, the entropy-coded bytes' bound floor((blocks * (22 + 63 * 26) + 7 * intervals) / 8) with every byte
+ * stuffed, 2 bytes per RST and EOI.  Both options non-zero, a negative one or restart_blocks above 65535 return
+ * SSNB_EINVAL before any launch (0 from the capacity query); everything else is as ssnb_jpeg_encode. */
+int64_t ssnb_jpeg_encode_restart_capacity(int mode, int height, int width, int restart_blocks, int restart_rows);
+int ssnb_jpeg_encode_restart_sizes(int mode, int quality, int restart_blocks, int restart_rows, const ssnb_jpeg_encode_image* images,
+                                   int n, size_t* workspace_bytes, int64_t* out_bytes);
+int ssnb_jpeg_encode_restart(int mode, int quality, int restart_blocks, int restart_rows, const uint8_t* src, int64_t src_bytes,
+                             const ssnb_jpeg_encode_image* images, const ssnb_jpeg_encode_image* images_dev, int n, uint8_t* out,
+                             int64_t out_bytes, int64_t* lengths, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- JPEG round trip (csrc/jpeg_roundtrip.cu): what the data sets' loaders read back from the frame and flow-plane files of
  * the extraction step, straight from the frames: for uint8 images, np.asarray(Image.open(BytesIO(f)).convert(mode)) of the
